@@ -3,15 +3,15 @@
 host-posted and host-staged baselines measured in the same process (BASELINE.md section 3: B1 / B2 / P1).
 
 Contract (driver): ``python bench.py --gpus N --steps K --warmup W`` (torchrun for N > 1) prints ONE JSON line from
-rank 0.  One *step* = ONE launch of the sm_100a poster kernel, which builds ``msgs_per_step`` RDMA WRITE work requests
-of ``--msg-bytes`` (default 256 MiB, larger than the 126 MB L2, rotating over 4 distinct buffers), rings the doorbell
+rank 0.  One *step* = ONE launch of the sm_90a poster kernel, which builds ``msgs_per_step`` RDMA WRITE work requests
+of ``--msg-bytes`` (default 256 MiB, larger than the 50 MB L2 of an H100, rotating over 4 distinct buffers), rings the doorbell
 for each and polls the completion queue on the device (window 8).  ``msgs_per_step`` is fixed before the timed region
 from a calibration run so that the K timed steps last >= ``--min-seconds`` (default 1.2 s): long enough for the clock
 record to mean something.  ``value`` is the whole-job aggregate GB/s, device-timed with CUDA events, max over ranks.
 
 Wire (``--wire auto``): a ConnectX through libibverbs / mlx5dv when one is reachable (real /dev/infiniband + rdma-core;
 then the same code measures BASELINE configs 1-3 on the NIC), else the software HCA: mlx5-format queues in HBM and a
-persistent sm_100a DMA engine on ``--engine-ctas`` SMs (default 32: the engine stands in for a NIC and is deliberately
+persistent sm_90a DMA engine on ``--engine-ctas`` SMs (default 32: the engine stands in for a NIC and is deliberately
 NOT given the whole GPU; ``extras.engine_128_ctas`` records what it reaches with 128).  This sandbox exposes no
 /dev/infiniband, so the numbers the driver records are software-HCA numbers (``config.wire`` says so), and BASELINE.md
 publishes no reference figure, hence ``vs_baseline: null``.
@@ -48,14 +48,31 @@ def emit(obj):
 
 
 def reference_arm():
-    # `pip install --no-index ... /root/reference` fails: the reference is a Linux kernel module for
+    # `pip install` of the reference fails: it is a Linux kernel module for
     # AMD KFD + MLNX_OFED 3.2 (no setup.py / pyproject, no userspace, needs amd_rdma.h); see DESIGN.md.
     if int(os.environ.get("RANK", "0")) != 0:      # launched like our own arm (torchrun for N > 1): one line, from rank 0
         return 0
     emit({"impl": "reference",
           "unavailable": "reference is an AMD-KFD/MLNX_OFED kernel module (amdp2p.ko): not pip-installable, "
-                         "no userspace entry point, cannot build or load on a B200 box"})
+                         "no userspace entry point, cannot build or load on an NVIDIA GPU box"})
     return 0
+
+
+def dump_outputs(d, dst, msg, nslots, last, counters, mps):
+    """What the timed path hands its caller: the destination buffer the RDMA writes filled (a fixed, seeded sample of
+    2 Mi of its bytes per slot, as float32, with the sampled offsets: 48 MiB in all) and whether the last poster launch
+    completed every message without an error CQE.  The inputs are seeded and the sample does not depend on how many messages
+    a step carries, so two builds run with the same arguments must write the same arrays."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    g = torch.Generator(device="cpu").manual_seed(1234)
+    idx = torch.randint(0, msg, (2 << 20,), generator=g).to(dst.device)
+    sample = torch.stack([dst[i * msg:(i + 1) * msg][idx] for i in range(nslots)]).float().cpu().numpy()
+    np.save(os.path.join(d, "dst_sample.npy"), sample)
+    np.save(os.path.join(d, "dst_sample_index.npy"), idx.cpu().double().numpy())
+    np.save(os.path.join(d, "last_step_completions.npy"),
+            np.array([float(last.ok and last.done == [mps]), float(counters["n_err"])], dtype=np.float64))
 
 
 def main():
@@ -71,6 +88,8 @@ def main():
     ap.add_argument("--min-seconds", type=float, default=2.0, help="lower bound on the timed region (msgs_per_step is sized for it)")
     ap.add_argument("--msgs-per-step", type=int, default=0, help="0 = calibrate")
     ap.add_argument("--extras", type=int, default=1, help="also run baselines' siblings: ring, fused pack, small messages, GEMM, mock NIC")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last step delivered as DIR/<name>.npy (to compare two builds)")
     args = ap.parse_args()
     if args.impl == "reference":
         return reference_arm()
@@ -94,7 +113,7 @@ def main():
         # the GPU-initiated path has no CPU fallback by design: say so in one line instead of a traceback
         if rank == 0:
             emit({"metric": "rdma_write_gbps_gpu_hbm_device_timed", "value": None, "impl": "ours",
-                  "unavailable": "no CUDA device visible: the data path is sm_100a kernels only"})
+                  "unavailable": "no CUDA device visible: the data path is sm_90a kernels only"})
         return 2
     torch.cuda.set_device(local_rank)
     from rocnrdma_b200.utils.affinity import bind_to_gpu
@@ -114,10 +133,11 @@ def main():
     nslots = 4
     window = max(1, min(args.window, 16))
     dev = torch.device("cuda", local_rank)
+    n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
     peaks = R.measured_peaks()
     ctx = rn.Context(device=local_rank, wire=wire)
     softhca = ctx.wire == "softhca"
-    wire_desc = ("softhca: mlx5-format queues in HBM, persistent sm_100a DMA engine on %d SMs (no /dev/infiniband in this container; "
+    wire_desc = ("softhca: mlx5-format queues in HBM, persistent sm_90a DMA engine on %d SMs (no /dev/infiniband in this container; "
                  "the ConnectX backend is compiled in and selected automatically when a NIC is reachable)" % args.engine_ctas) if softhca else \
                 ("verbs: %s through libibverbs/mlx5dv%s, GPU-posted into the NIC's own send queue" % (ctx.nic, " (MOCK provider)" if ctx.nic_is_mock else ""))
 
@@ -218,6 +238,8 @@ def main():
     assert last.ok and last.done == [mps], (last.status, last.done)
     counters = qp.counters()
     engine_off()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dst, msg, nslots, last, counters, mps)
     # byte verification: every destination slot equals its source slot
     n_bad = sum(ops.compare(src[i * msg:(i + 1) * msg], dst[i * msg:(i + 1) * msg]) for i in range(nslots))
 
@@ -351,7 +373,7 @@ def main():
             extras["small_msg"] = {"error": str(e)[:160]}
         try:   # K4 fused: panels RDMA-written from the GEMM epilogue vs GEMM-then-send, the engine holding its SMs
             gs = {}
-            grid = 148 - args.engine_ctas if softhca else 0
+            grid = n_sms - args.engine_ctas if softhca else 0
             for (M, Nn, K), (a, b, c, d, cm, dm) in gemm_bufs.items():
                 ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=dm, signal_every=4, grid=grid)
                 f = min((ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=dm, signal_every=4, grid=grid) for _ in range(3)), key=lambda r: r.device_ns)
@@ -365,7 +387,7 @@ def main():
                         ev[3].record()
                     ev[3].synchronize()
                     unf_us = min(unf_us, ev[2].elapsed_time(ev[3]) * 1e3)
-                gs[f"{M}x{Nn}x{K}"] = {"gemm_ctas": grid or 148, "fused_gemm_send_us": round(f.device_ns / 1e3, 1), "fused_tflops": round(f.tflops, 1),
+                gs[f"{M}x{Nn}x{K}"] = {"gemm_ctas": grid or n_sms, "fused_gemm_send_us": round(f.device_ns / 1e3, 1), "fused_tflops": round(f.tflops, 1),
                                        "gemm_then_send_us": round(unf_us, 1), "fused_speedup": round(unf_us / (f.device_ns / 1e3), 3),
                                        "fused_verified": fused_ok}
             extras["gemm_send"] = gs
@@ -406,8 +428,8 @@ def main():
                 good = bool(torch.allclose(c[:256].float(), ref, rtol=2e-2, atol=2.0))
                 row = extras.setdefault("gemm_send", {}).setdefault(f"{M}x{Nn}x{K}", {})
                 row.update({"cublas_tflops": round(cublas, 1), "ours_tflops": round(ours, 1), "ours_best_single_launch_tflops": round(best, 1),
-                            "vs_cublas": round(ours / cublas, 3), "frac_of_sustained_peak": round(ours / sustained, 3) if sustained else None,
-                            "kernel": {1: "single CTA (128x256)", 2: "CTA pair (256x256 per pair)", 3: "wide CTA pair (512x256 per pair)"}.get(singles[0].variant, "?"),
+                            "vs_cublas": round(ours / cublas, 3), "frac_of_bf16_peak": round(ours / sustained, 3) if sustained else None,
+                            "kernel": {1: "single CTA (128x256)", 2: "CTA pair (256x256 per pair)", 3: "CTA pair on the stream-K schedule (256x256 per pair)"}.get(singles[0].variant, "?"),
                             "timing": "10 back-to-back launches between CUDA events, both libraries", "numerics_ok": good})
                 if (M, Nn, K) not in gemm_bufs:
                     continue
@@ -438,7 +460,7 @@ def main():
                 r128 = post(64)
                 ctx.engine_stop()
                 extras["engine_128_ctas"] = {"gbps": round(r128.gbps, 1), "ok": r128.ok,
-                                             "frac_of_measured_copy_peak": round(r128.gbps / R.copy_roofline_gbps(peaks), 3)}
+                                             "frac_of_copy_peak": round(r128.gbps / R.copy_roofline_gbps(peaks), 3), "peaks_source": peaks.get("_source")}
             except Exception as e:
                 extras["engine_128_ctas"] = {"error": str(e)[:160]}
     torch.cuda.synchronize()
@@ -458,7 +480,7 @@ def main():
                         "gemm_then_write_us": round(r4.unfused_us, 1), "fused_speedup": round(r4.unfused_us / r4.fused_us, 3),
                         "tflops_incl_delivery": round(r4.tflops, 1), "wire_gbps": round(r4.wire_gbps, 1), "panels": r4.panels,
                         "engine_ctas": r4.engine_ctas,
-                        "limiter": ("NVLink store burstiness: all GEMM CTAs reach their epilogue together (~450 GB/s of SM-issued stores)"
+                        "limiter": ("NVLink store burstiness: all GEMM CTAs reach their epilogue together "
                                     if r4.mode == "direct" else "the 32 SMs the engine takes from the GEMM")}
                 # the same wire fused into BOTH GEMMs: GPU0's epilogue sends fp8 panel records, GPU1's block-scaled GEMM starts tiles on arrival
                 ch = SG.run_chain(8192, 8192, 2048, 8192, gpus=(local_rank, local_rank + 1), reps=3)
@@ -467,7 +489,7 @@ def main():
                     "sequential_us": round(ch["sequential_us"], 1) if ch["sequential_us"] else None,
                     "fused_speedup": round(ch["speedup"], 3) if ch["speedup"] else None, "wire_bytes": ch["wire_bytes"],
                     "timing": "host wall clock, launch to completion on both GPUs (no common device clock), best of 3",
-                    "what": ch["what"], "limiter": "GEMM 2 cannot finish before GEMM 1's last panel arrives; GEMM 1 runs on 116 SMs next to the engine"}
+                    "what": ch["what"], "limiter": f"GEMM 2 cannot finish before GEMM 1's last panel arrives; GEMM 1 runs on {n_sms - args.engine_ctas} SMs next to the engine"}
                 extras["config4_gemm_send_recv_nvlink"] = res
             except Exception as e:
                 extras["config4_gemm_send_recv_nvlink"] = {"error": str(e)[:200]}
@@ -512,14 +534,14 @@ def main():
                        "seq_len": msg, "parallelism": f"{world}x(GPU+own HCA), loopback per GPU (BASELINE config 5 shape)",
                        "wire": wire_desc, "engine_ctas": args.engine_ctas if softhca else None, "window": window,
                        "step": f"one poster-kernel launch = {mps} GPU-built RDMA WRITE WQEs of {msg >> 20} MiB (doorbell per WQE, device-polled CQ, window {window})",
-                       "poster": "sm_100a kernel: WQE + doorbell record + doorbell register + device CQ poll, queue state in registers",
+                       "poster": "sm_90a kernel: WQE + doorbell record + doorbell register + device CQ poll, queue state in registers",
                        "l2_policy": f"inputs larger than L2: {msg >> 20} MiB messages rotating over {nslots} buffers",
                        "timing": "CUDA events on the posting stream around exactly `steps` launches, max over ranks",
                        "timed_region_s": round(dev_ms_max / 1e3, 3), "wall_s": round(time.time() - t_wall0, 1)},
             "roofline": {"bound_gbps_per_gpu": round(R.copy_roofline_gbps(peaks), 1),
-                         "frac_of_measured_copy_peak": round(per_gpu / R.copy_roofline_gbps(peaks), 3),
+                         "frac_of_copy_peak": round(per_gpu / R.copy_roofline_gbps(peaks), 3),
                          "peaks_source": peaks.get("_source"),
-                         "limiter": "softhca: the DMA engine's SM count (~38 GB/s per engine CTA; 32 of 148 SMs by choice)" if softhca else "NIC line rate / PCIe Gen5 x16"},
+                         "limiter": f"softhca: the DMA engine's SM count ({args.engine_ctas} of {n_sms} SMs by choice)" if softhca else "NIC line rate / PCIe Gen5 x16"},
             "baselines": base,
             "e2e": {"value": round(e2e_value, 2), "unit": "GB/s", "h2d_bytes_per_step": msg, "d2h_bytes_per_step": 64, "steps": e2e_steps,
                     "step": "one message: H2D of its input from pinned host memory, one GPU-posted RDMA WRITE, status words read back on the host; two messages in flight (copy of i overlaps the write of i-1)",

@@ -65,7 +65,7 @@ def main():
                             aggregate_gbps=round(world * r["bytes"] * r["iters"] / ns, 1)))
             print(json.dumps(out[-1]), flush=True)
         res = dict(world=world, engine_ctas=a.engine_ctas, verified=t.tolist()[-1] == 0.0, rows=out,
-                   roofline_per_gpu_gbps=770.0, note="NVLink 5 peer copy measured 770 GB/s per direction per GPU (B200_PROFILING.md)")
+                   roofline_per_gpu_gbps=450.0, note="H100 SXM NVLink 4: 450 GB/s per direction per GPU (data sheet, not measured)")
         os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
         json.dump(res, open(a.out, "w"), indent=1)
         print("verified", res["verified"])

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Message-size sweep, 1 KB - 1 GB (BASELINE.json configs 1, 2, 3, 5 on one GPU):
 
-  gpu_posted      P1  sm_100a kernel posts WQEs + polls the CQ on the device (device-timed, %globaltimer)
+  gpu_posted      P1  sm_90a kernel posts WQEs + polls the CQ on the device (device-timed, %globaltimer)
   gpu_posted_read P1  same, RDMA READ
   host_posted     B2  CPU posts on host-resident rings and polls (the ib_write_bw-on-a-peermem-MR shape; host-timed)
   host_dram       B0  host MR -> host MR write, host-posted (plumbing check, no GPU memory)

@@ -1,4 +1,4 @@
-"""The README quick start as a runnable script (one B200)."""
+"""The README quick start as a runnable script (one H100)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, rocnrdma_b200 as rn
@@ -23,7 +23,7 @@ r = ops.rdma_stream(qp, W.OP_RDMA_WRITE, ms, md, 65536, iters=4096, window=128, 
 print(r.us_per_msg, "us per message")
 ctx.engine_stop(); ctx.engine_start(ctas=64)
 ops.pack_fp8_write(ctx, x, stg, qp=qp, dst_mr=md, chunk_elems=1 << 22)         # bf16 -> fp8 pack fused with the post
-ctx.engine_stop(); ctx.engine_start(ctas=32)                                   # leave 116 SMs to the GEMM
-g = ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=md, signal_every=4, grid=116)   # tcgen05 GEMM, one RDMA write per finished 128-row panel
+ctx.engine_stop(); ctx.engine_start(ctas=32)                                   # leave 100 of 132 SMs to the GEMM
+g = ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=md, signal_every=4, grid=100)   # wgmma GEMM, one RDMA write per finished 128-row panel
 print(g.tflops, "TFLOP/s including delivery")
 ctx.engine_stop()

@@ -1,7 +1,7 @@
 """Send side: a bf16 activation matrix is packed to block-scaled fp8 (one UE8M0 scale per 32 values) by the kernel that
 also posts the RDMA writes (K3).  Receive side: the delivered records are the A operand of a tensor-core GEMM as they
-stand (K7, tcgen05.mma.kind::mxf8f6f4.block_scale) -- no unpack pass, half the bytes of bf16 on the wire and in HBM,
-and the product comes out faster than a bf16 GEMM of the same shape.  Loopback wire on one B200."""
+stand (K7, e4m3 wgmma with the block scales applied in registers) -- no unpack pass, half the bytes of bf16 on the wire and in
+HBM.  Loopback wire on one H100."""
 import os
 import sys
 

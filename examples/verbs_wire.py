@@ -1,5 +1,5 @@
 """The ConnectX code path end to end: ``Context(wire="verbs")`` -- HBM registered with the HCA (dma-buf first, peer-memory
-client second), the QP's mlx5dv send queue / doorbell / CQ mapped into the GPU, an sm_100a kernel posting RDMA writes into
+client second), the QP's mlx5dv send queue / doorbell / CQ mapped into the GPU, an sm_90a kernel posting RDMA writes into
 them, and the two host-side baselines on the same MRs.
 
 On a box with a ConnectX and rdma-core this runs against the NIC (loopback on one port).  Without one it uses the

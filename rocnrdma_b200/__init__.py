@@ -1,12 +1,12 @@
-"""rocnrdma_b200 -- a Blackwell-native GPU<->NIC zero-copy RDMA stack.
+"""rocnrdma_b200 -- a Hopper-native (H100) GPU<->NIC zero-copy RDMA stack.
 
 Capability-for-capability rebuild of AMD's ``amdp2p`` PeerDirect bridge
-(rocmarchive/ROCnRDMA) for NVIDIA B200: registration of GPU HBM for RDMA
+(rocmarchive/ROCnRDMA) for NVIDIA H100: registration of GPU HBM for RDMA
 (kernel ``peer_memory_client`` on nv-p2p + userspace dma-buf exporter), the
 ``amdp2ptest`` harness (ioctl ABI, kernel module, userspace twin, CLI), and --
-new here -- a GPU-initiated data path: sm_100a kernels build mlx5 WQEs, ring the
+new here -- a GPU-initiated data path: sm_90a kernels build mlx5 WQEs, ring the
 doorbell and poll the CQ on the device, fused with a bf16->fp8 block-scaled pack
-or a tcgen05/TMEM GEMM that produces the send tile.
+or a wgmma/TMA GEMM that produces the send tile.
 """
 from . import wire  # noqa: F401
 from .wire import (ACC_ALL, ACC_LOCAL_WRITE, ACC_REMOTE_READ, ACC_REMOTE_WRITE, MEM_DEVICE,  # noqa: F401

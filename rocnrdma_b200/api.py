@@ -11,7 +11,7 @@
 
 Two wires sit under the same objects (``Context(wire=...)``):
 
-* ``softhca`` -- the software HCA: queues in GPU or pinned memory, a persistent sm_100a kernel moves
+* ``softhca`` -- the software HCA: queues in GPU or pinned memory, a persistent sm_90a kernel moves
   the bytes.  What runs when the box exposes no NIC.
 * ``verbs``   -- a ConnectX through libibverbs / mlx5dv (``csrc/verbs/verbs_dl.cc``): ``reg_mr`` is
   ``ibv_reg_dmabuf_mr`` / ``ibv_reg_mr`` on the GPU pointer, host-posted verbs are ``ibv_post_send``,
@@ -524,7 +524,7 @@ class Context:
 
         Kernels that post to, or wait on, the engine MUST run on a non-blocking stream:
         a kernel launched on the legacy default stream is serialised behind the
-        persistent engine kernel by the driver (measured on B200, driver 580: the poster
+        persistent engine kernel by the driver (observed with driver 580: the poster
         started 95 us after the engine's watchdog exit).  ``ops.*`` default to this
         stream; wrap torch work that must overlap the engine in
         ``with torch.cuda.stream(ctx.stream):``.

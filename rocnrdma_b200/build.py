@@ -1,4 +1,4 @@
-"""In-tree native build: nvcc -> rocnrdma_b200/lib/librocnrdma_b200.so (sm_100a only).
+"""In-tree native build: nvcc -> rocnrdma_b200/lib/librocnrdma_b200.so (sm_90a only: H100).
 
 The shared object exports a flat C ABI (``rn_*``) that ``rocnrdma_b200._native``
 loads with ctypes; keeping torch's C++ headers out of the build keeps a full
@@ -40,7 +40,7 @@ MOCK_VERBS = MOCKDIR / "libibverbs.so.1"
 MOCK_MLX5 = MOCKDIR / "libmlx5.so.1"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function",
     "--expt-relaxed-constexpr",
@@ -89,7 +89,7 @@ def build_mock() -> Path:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every native source for sm_100a and link the shared object."""
+    """Compile every native source for sm_90a and link the shared object."""
     cu, cc = sources()
     headers = list(CSRC.rglob("*.h")) + list(CSRC.rglob("*.cuh"))
     mock_srcs = sorted((CSRC / "mockverbs").glob("*.cc"))
@@ -129,7 +129,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     # register / shared-memory / spill summary per kernel (tracked: it is evidence); compile times are noise
     keep = lambda v: "\n".join(l for l in v.splitlines() if "Compile time" not in l)
     (LIBDIR / "ptxas_info.txt").write_text("\n".join(f"=== {k}\n{keep(v)}" for k, v in logs.items()))
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs),
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs),
             "-Xcompiler", "-fPIC", "-ldl", "-lpthread"]
     subprocess.run(link, check=True)
     build_mock()

@@ -1,4 +1,4 @@
-// The softhca DMA engine: a persistent sm_100a kernel that plays the HCA.
+// The softhca DMA engine: a persistent sm_90a kernel that plays the HCA.
 //
 // Pipeline per QP (every stage can be on a different CTA, many WQEs in flight):
 //   claim    one CAS on the claim head hands WQE w -- or, with a backlog visible, up to 16 WQEs -- to a

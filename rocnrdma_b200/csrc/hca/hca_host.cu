@@ -146,7 +146,7 @@ bool legal_transition(uint32_t from, uint32_t to) {
 // default lazy module loading the first launch of a kernel loads it, and that load is
 // serialised behind a resident persistent kernel -- a poster launched for the first
 // time while the engine runs would only start after the engine's watchdog exit
-// (observed on B200 / driver 580.159; see DESIGN.md "engine residency rules").
+// (observed with driver 580.159; see DESIGN.md "engine residency rules").
 extern "C" {
 uint64_t rn_gemm_workspace_bytes() __attribute__((weak));
 void rn_gemm_set_workspace(int dev, uint64_t ptr) __attribute__((weak));

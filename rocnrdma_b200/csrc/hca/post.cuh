@@ -1,6 +1,6 @@
 // GPU-initiated posting: reserve an SQ slot, write the 64-byte WQE, publish the
 // doorbell record, ring the doorbell, poll the completion queue -- all from an
-// sm_100a thread, no host in the loop (SURVEY.md N3, kernels K1/K2).
+// GPU thread, no host in the loop (SURVEY.md N3, kernels K1/K2).
 //
 // Ordering contract (what a ConnectX requires, and what the softhca engine checks
 // and counts violations of in QpDev::n_db_order_violations):
@@ -465,4 +465,11 @@ __device__ __forceinline__ long long recv_wait(QpDev* qp, uint32_t* imm, unsigne
 }
 
 }  // namespace dev
+
+// SM count of the current device (launch sizing of the persistent and grid-stride kernels)
+static inline int device_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+  return n;
+}
 }  // namespace rn

@@ -2,59 +2,50 @@
 //
 //   C[M,N] (bf16) = dequant(A) * dequant(B)^T,   A = (A_q [M,K] e4m3, A_s [M,K/32] UE8M0),  B likewise [N,K]
 //
-// with the dequantisation done by the tensor core: tcgen05.mma.kind::mxf8f6f4.block_scale multiplies every
-// 32-element block of K by 2^(scale - 127) for its row of A and its row of B while it accumulates in fp32.  The
-// operands are exactly the self-contained records the send side produces -- pack_fp8.cu chunk records
+// The operands are exactly the self-contained records the send side produces -- pack_fp8.cu chunk records
 // ([elems fp8][elems/32 scales]) and gemm_send.cu panel records ([128 x N fp8][128 x N/32 scales]) -- so a receiver
-// can multiply straight out of its registered receive buffer: no dequantisation pass, half the HBM bytes of bf16
-// operands, and (nominally) twice the tensor rate.  Round 1 had an fp8 EPILOGUE only; its records could be produced
-// but never consumed by a GEMM (VERDICT item 8b).
+// can multiply straight out of its registered receive buffer: no dequantisation pass and half the HBM bytes of bf16
+// operands.  Hopper's tensor cores multiply e4m3 but do not apply block scales, so the scaling happens in registers:
+// per 32-deep MX block of K one wgmma.m64n128k32 (e4m3 x e4m3 -> fp32) produces that block's partial product, and the
+// warpgroup adds it into the fp32 accumulator multiplied by 2^(scale_a - 127) * 2^(scale_b - 127) of its row and column.
+// Two partial register sets alternate, so the MMA of block k + 1 runs while block k is being scaled.
 //
-// Two kernels.  gemm_mxfp8_pair_kernel (further down; the default for M > 128): a CTA pair per 256 x 256 tile, scale factors
-// written into TMEM by the loader warps, TMA-store epilogue, optional per-panel arrival words (receive-side fusion).
-// gemm_mxfp8_kernel (first; small M, and the reference the pair kernel is tested against): one CTA per 128 x 128 tile,
-// persistent, 320 threads:
-//   warp 0      TMA producer: 3-D tensor maps (K, rows-in-record, record) so an operand may live inside records;
-//               128 x 128-byte boxes, SWIZZLE_128B, out-of-bounds rows / K filled with zeros (ragged shapes)
-//   warp 1      MMA issuer: per 128-deep k-block two tcgen05.cp 32x128b.warpx4 copy the block's scale factors from
-//               shared memory into TMEM (4 columns each for A and B), then four K=32 MMAs read them by scale-factor
-//               id; accumulators double-buffered in TMEM columns 0-255, scale factors ring through columns 256+
-//   warps 2-5   epilogue: tcgen05.ld 32x32b.x32 -> bf16 -> bounds-checked row stores
-//   warps 6-9   scale loaders: each thread owns one row of the A tile and one of the B tile and lays their four
-//               scale bytes of the k-block into the 512-byte chunk layout the hardware expects
-//               (byte (r % 32) * 16 + (r / 32) * 4 + k: 32 rows of 16 bytes, replicated to the four lane quarters)
-// Layout facts (instruction-descriptor bits, scale-factor chunk, UTCCP shape) were read off the CUTLASS headers
-// vendored in the image (cute/arch/mma_sm100_desc.hpp, cutlass/detail/sm100_blockscaled_layout.hpp); no CUTLASS code
-// is compiled in.  No counterpart in the reference.
+// Persistent, one CTA (384 threads) per SM, 128 x 128 tile per CTA:
+//   warpgroup 0    loaders: one thread issues the TMA loads (3-D tensor maps (K, rows-in-record, record), so an operand
+//                  may live inside records; 128-byte boxes, SWIZZLE_128B, out-of-bounds rows / K zero-filled); every
+//                  thread fetches the four scale bytes of one row of A and one row of B per 128-deep k-block into
+//                  shared memory (layout [MX block][row])
+//   warpgroups 1-2 each owns 64 rows of the tile: MMA, scaling, then bounds-checked bf16 stores from registers
+// gemm_mxfp8_kernel runs one CTA per tile; gemm_mxfp8_pair_kernel a 2-CTA cluster per 256 x 128 tile, each CTA loading
+// half of the B tile and multicasting it to both (half the B traffic per FLOP).
+// No counterpart in the reference.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../hca/post.cuh"
+#include "sm90.cuh"
 
 using namespace rn;
 using namespace rn::dev;
+using namespace rn::sm90;
 
 #define RN_API extern "C" __attribute__((visibility("default")))
 
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 128, UMMA_K = 32, STAGES = 4;
+constexpr int BM = 128, BN = 128, BK = 128, STAGES = 4;
 constexpr int A_STAGE = BM * BK, B_STAGE = BN * BK;            // 16 KiB each (one byte per element)
-constexpr int SF_STAGE = 512;                                  // 128 rows x 4 scale bytes, chunk layout
-constexpr int kThreads = 320;
-constexpr uint32_t kTmemCols = 512;
-constexpr uint32_t kSfCol0 = 256;                              // scale factors live above the two 128-column accumulators
+constexpr int kThreads = 384;
 constexpr unsigned long long kWaitNs = 2000000000ull;
 
 struct alignas(1024) Smem {
   uint8_t a[STAGES][A_STAGE];
   uint8_t b[STAGES][B_STAGE];
-  alignas(128) uint8_t sfa[STAGES][SF_STAGE];
-  alignas(128) uint8_t sfb[STAGES][SF_STAGE];
-  alignas(8) uint64_t full[STAGES], empty[STAGES], tfull[2], tempty[2];
-  uint32_t tmem_base;
+  uint8_t sfa[STAGES][4][BM];                                  // scale bytes of the stage's four MX blocks, [block][row]
+  uint8_t sfb[STAGES][4][BN];
+  alignas(8) uint64_t full[STAGES], empty[STAGES];
   volatile int abort;
 };
 
@@ -67,7 +58,6 @@ struct MxArgs {
   uint32_t M, N, K;
   unsigned long long* out;   // [status, t_start, t_end, tiles, 0...]: mapped pinned HOST memory -- written by the last CTA only
   unsigned int* done;        // device scratch (zeroed, self-cleaning): CTAs finished
-  uint32_t tma_store;        // pair kernel: C rows are 16-byte multiples -> epilogue through staged TMA tensor stores
   // Receive-side fusion ("the panel arrives -> its tiles start"): one word per 128-row panel of A, nonzero once the panel's
   // record has landed in this GPU's memory (recv_consume_kernel stamps it when the panel's receive completion shows up).
   // nullptr: A is complete before the launch.  The TMA producer and the scale loaders wait for the word of the panel
@@ -94,7 +84,7 @@ __device__ __forceinline__ bool wait_panel(const unsigned long long* ready, uint
   return true;
 }
 // Result words live in host memory: one atomic per CTA there (the first version's atomicMax of the end time) is a PCIe
-// round trip each -- 148 of them serialised cost ~150 us per launch, more than a 4096^3 product.  Count in device memory,
+// round trip each -- one per CTA, serialised, cost ~150 us per launch, more than a 4096^3 product.  Count in device memory,
 // let the last CTA write.
 __device__ __forceinline__ void mx_finish(const MxArgs& g, bool aborted, unsigned long long t_start, uint32_t n_tiles, uint32_t variant) {
   if (aborted) g.out[0] = (unsigned long long)(long long)WAIT_TIMEOUT;
@@ -104,85 +94,6 @@ __device__ __forceinline__ void mx_finish(const MxArgs& g, bool aborted, unsigne
   g.out[2] = globaltimer_ns();
   *g.done = 0;
 }
-
-__device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t n) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(b)), "r"(n)); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s32(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s32(b)) : "memory"); }
-__device__ __forceinline__ bool mbar_try(uint64_t* b, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(s32(b)), "r"(parity) : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ bool mbar_wait(Smem& s, uint64_t* b, uint32_t parity) {
-  if (mbar_try(b, parity)) return true;
-  unsigned long long t0 = globaltimer_ns();
-  unsigned n = 0;
-  while (!mbar_try(b, parity)) {
-    if ((++n & 255) == 0) {
-      if (s.abort) return false;
-      if (globaltimer_ns() - t0 > kWaitNs) { s.abort = 1; return false; }
-    }
-  }
-  return true;
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(s32(smem_dst)), "l"(map), "r"(s32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s32(bar)) : "memory");
-}
-// K-major, SWIZZLE_128B operand tile of one-byte elements: 128-byte rows (128 elements), 8-row groups 1024 bytes apart.
-__device__ __forceinline__ uint64_t smem_desc_sw128(const void* p) {
-  uint64_t d = (uint64_t)((s32(p) & 0x3ffff) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Scale-factor chunk for tcgen05.cp 32x128b: 32 rows of 16 bytes, no swizzle; 8-row core matrices 128 bytes apart.
-__device__ __forceinline__ uint64_t smem_desc_sf(const void* p) {
-  uint64_t d = (uint64_t)((s32(p) & 0x3ffff) >> 4);
-  d |= (uint64_t)(16 >> 4) << 16;                          // leading-dimension byte offset (one core matrix wide: unused)
-  d |= (uint64_t)(128 >> 4) << 32;                         // stride between 8-row core matrices
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-__device__ __forceinline__ void utccp_32x128b_warpx4(uint32_t tmem_dst, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(tmem_dst), "l"(sdesc) : "memory");
-}
-// kind::mxf8f6f4 block-scaled instruction descriptor: A = B = e4m3 (format 0), both K-major, UE8M0 scales,
-// N at [17,23) in units of 8, M at [24,29) in units of 16, scale-factor ids at [4,6) (B) and [29,31) (A), K = 32.
-__device__ __forceinline__ uint32_t mx_idesc(uint32_t sf_id) {
-  return (sf_id << 4) | ((uint32_t)(BN >> 3) << 17) | (1u << 23) | ((uint32_t)(BM >> 4) << 24) | (sf_id << 29);
-}
-__device__ __forceinline__ void umma_mxf8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t tsfa, uint32_t tsfb, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}"
-               ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(tsfa), "r"(tsfb) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                 "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-                 "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-                 "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ uint32_t pack_bf16(uint32_t lo, uint32_t hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(__uint_as_float(lo), __uint_as_float(hi));
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-
 // the four UE8M0 bytes of k-block kb for global row `row` of an operand (127 = 2^0 beyond the matrix: the data
 // there is zero-filled by TMA, so any finite scale gives 0)
 __device__ __forceinline__ uint32_t load_scales(const uint8_t* base, uint64_t rec_stride, uint32_t rows_per_rec, uint32_t rows, uint32_t ks,
@@ -196,522 +107,144 @@ __device__ __forceinline__ uint32_t load_scales(const uint8_t* base, uint64_t re
   return v;
 }
 
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, MxArgs g) {
+__device__ __forceinline__ float ue8m0(uint32_t e) { return e ? __uint_as_float(e << 23) : __uint_as_float(0x00400000u); }   // 2^(e - 127)
+
+template <int CTAS>
+__device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const MxArgs& g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t rank = CTAS == 2 ? cluster_rank() : 0u;
   const unsigned long long t_start = globaltimer_ns();
-  const uint32_t m_blks = (g.M + BM - 1) / BM, n_blks = (g.N + BN - 1) / BN, k_blks = (g.K + BK - 1) / BK;
-  const uint32_t n_tiles = m_blks * n_blks, ks = g.K / 32;
+  const uint32_t m_tiles = (g.M + CTAS * BM - 1) / (CTAS * BM), n_blks = (g.N + BN - 1) / BN, k_blks = (g.K + BK - 1) / BK;
+  const uint32_t n_tiles = m_tiles * n_blks, n_units = gridDim.x / CTAS, unit = blockIdx.x / CTAS;
+  const uint32_t ks = g.K / 32;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&s.full[i], 1 + 4); mbar_init(&s.empty[i], 1); }   // TMA transaction + 4 scale-loader warps
-    for (int i = 0; i < 2; ++i) { mbar_init(&s.tfull[i], 1); mbar_init(&s.tempty[i], 4); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&s.full[i], 1 + 128); mbar_init(&s.empty[i], 2 * CTAS); }
     s.abort = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(&s.tmem_base)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s.tmem_base;
+  if constexpr (CTAS == 2) cluster_sync_all();
 
-  if (warp == 0) {
-    // ===================== TMA producer
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (uint32_t tile = blockIdx.x; tile < n_tiles && !s.abort; tile += gridDim.x) {
-        const uint32_t m_blk = tile / n_blks, n_blk = tile % n_blks;
-        const uint32_t ar = m_blk * BM, br = n_blk * BN;
-        if (!wait_panel(g.a_ready, m_blk, g.ready_timeout_ns, &s.abort)) goto producer_done;
-        for (uint32_t kb = 0; kb < k_blks; ++kb) {
-          if (!mbar_wait(s, &s.empty[stage], phase ^ 1)) goto producer_done;
-          mbar_expect_tx(&s.full[stage], A_STAGE + B_STAGE);
-          // rows of a tile never straddle records (rows_per_rec is a multiple of 128, or the operand is one record)
-          tma_load_3d(s.a[stage], &tmap_a, &s.full[stage], (int)(kb * BK), (int)(ar % g.a_rows_per_rec), (int)(ar / g.a_rows_per_rec));
-          tma_load_3d(s.b[stage], &tmap_b, &s.full[stage], (int)(kb * BK), (int)(br % g.b_rows_per_rec), (int)(br / g.b_rows_per_rec));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  producer_done:
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (uint32_t tile = blockIdx.x; tile < n_tiles && !s.abort; tile += gridDim.x) {
-        if (!mbar_wait(s, &s.tempty[acc], acc_phase ^ 1)) goto mma_done;
-        tc_fence_after();
-        const uint32_t d = tmem_base + acc * BN;
-        for (uint32_t kb = 0; kb < k_blks; ++kb) {
-          if (!mbar_wait(s, &s.full[stage], phase)) goto mma_done;             // A, B landed and the scale chunks are written
-          tc_fence_after();
-          const uint32_t tsfa = tmem_base + kSfCol0 + stage * 8, tsfb = tsfa + 4;
-          utccp_32x128b_warpx4(tsfa, smem_desc_sf(s.sfa[stage]));              // copies and MMAs execute in issue order
-          utccp_32x128b_warpx4(tsfb, smem_desc_sf(s.sfb[stage]));
-          const uint64_t da = smem_desc_sw128(s.a[stage]), db = smem_desc_sw128(s.b[stage]);
-#pragma unroll
-          for (uint32_t k = 0; k < BK / UMMA_K; ++k)                            // +32 bytes along K = +2 in the address field
-            umma_mxf8(d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), mx_idesc(k), tsfa | (k << 30), tsfb | (k << 30), (kb | k) != 0);
-          tc_commit(&s.empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        tc_commit(&s.tfull[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  mma_done:
-    __syncwarp();
-  } else if (warp < 6) {
-    // ===================== epilogue
-    const uint32_t q = warp & 3;                                               // TMEM lane quarter this warp may read
-    uint32_t acc = 0, acc_phase = 0;
-    for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const uint32_t m_blk = tile / n_blks, n_blk = tile % n_blks;
-      if (!mbar_wait(s, &s.tfull[acc], acc_phase)) break;
-      tc_fence_after();
-      const uint32_t row = m_blk * BM + q * 32 + lane;
-      const uint32_t taddr = tmem_base + ((q * 32u) << 16) + acc * BN;
-      __nv_bfloat16* crow = g.c + (size_t)row * g.N + (size_t)n_blk * BN;
-#pragma unroll 2
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld32(taddr + c * 32, r);
-        tmem_ld_wait();
-        const uint32_t col0 = n_blk * BN + c * 32;
-        if (row < g.M && col0 < g.N) {
-          if (col0 + 32 <= g.N && (g.N & 7) == 0) {
-            uint4* dst = reinterpret_cast<uint4*>(crow + c * 32);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              dst[j] = make_uint4(pack_bf16(r[8 * j], r[8 * j + 1]), pack_bf16(r[8 * j + 2], r[8 * j + 3]), pack_bf16(r[8 * j + 4], r[8 * j + 5]),
-                                  pack_bf16(r[8 * j + 6], r[8 * j + 7]));
-          } else {
-            for (int j = 0; j < 32 && col0 + j < g.N; ++j) crow[c * 32 + j] = __float2bfloat16_rn(__uint_as_float(r[j]));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s.tempty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else {
-    // ===================== scale loaders (warps 6-9): thread (w, lane) owns tile row w * 32 + lane of A and of B
-    // One 16-byte load per operand row covers FOUR k-blocks, and the next group's loads are issued before this
-    // group is handed over: a k-block's MMAs take ~256 cycles, a global load ~1000, so loading block by block made
-    // the scale path -- not the tensor core -- the limiter of the first version (530 TFLOP/s at 4096^3).
-    const uint32_t w = warp - 6;
+  if (warp < 4) {
+    // ===================== loaders: thread t fetches the scales of tile row t of A and of B; thread 0 also issues the TMA
+    reg_dealloc<40>();
+    const uint32_t t = threadIdx.x;
     uint32_t stage = 0, phase = 0;
-    auto ld16 = [&](const uint8_t* base, uint64_t rec_stride, uint32_t rows_per_rec, uint32_t rows, uint32_t row, uint32_t kb) -> uint4 {
-      if (row < rows && kb * 4 + 16 <= ks) {
-        const uint8_t* p = base + (uint64_t)(row / rows_per_rec) * rec_stride + (uint64_t)(row % rows_per_rec) * ks + (uint64_t)kb * 4;
-        if (((uintptr_t)p & 15) == 0) return g.a_ready ? __ldcg(reinterpret_cast<const uint4*>(p)) : __ldg(reinterpret_cast<const uint4*>(p));
-      }
-      return make_uint4(load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb), load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb + 1),
-                        load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb + 2), load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb + 3));
-    };
-    for (uint32_t tile = blockIdx.x; tile < n_tiles && !s.abort; tile += gridDim.x) {
-      const uint32_t m_blk = tile / n_blks, n_blk = tile % n_blks;
-      const uint32_t arow = m_blk * BM + w * 32 + lane, brow = n_blk * BN + w * 32 + lane;
-      if (!wait_panel(g.a_ready, m_blk, g.ready_timeout_ns, &s.abort)) goto loader_done;      // the scales travel in the same record
-      uint4 ca = ld16(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, arow, 0), cb = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, brow, 0);
-      for (uint32_t kb0 = 0; kb0 < k_blks; kb0 += 4) {
-        uint4 na = ca, nb = cb;
-        if (kb0 + 4 < k_blks) {
-          na = ld16(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, arow, kb0 + 4);
-          nb = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, brow, kb0 + 4);
-        }
-        const uint32_t wa[4] = {ca.x, ca.y, ca.z, ca.w}, wb[4] = {cb.x, cb.y, cb.z, cb.w};
-#pragma unroll
-        for (uint32_t j = 0; j < 4; ++j) {
-          if (kb0 + j >= k_blks) break;
-          if (!mbar_wait(s, &s.empty[stage], phase ^ 1)) goto loader_done;
-          *reinterpret_cast<uint32_t*>(&s.sfa[stage][lane * 16 + w * 4]) = wa[j];
-          *reinterpret_cast<uint32_t*>(&s.sfb[stage][lane * 16 + w * 4]) = wb[j];
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // generic-proxy writes -> visible to tcgen05.cp
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&s.full[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ca = na; cb = nb;
-      }
-    }
-  loader_done:
-    __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-  }
-  if (threadIdx.x == 64) mx_finish(g, s.abort != 0, t_start, n_tiles, 1u);
-}
-
-
-// ==================================================================== CTA-pair variant (cta_group::2)
-// The single-CTA kernel above moves 32 KiB of operands per 4.2 MFLOP: at fp8 rates that is L2-bandwidth-bound (measured:
-// 1.28 PFLOP/s at 8192^3 = 10 TB/s of L2 -> SM traffic).  Here two CTAs of a cluster compute a 256 x 256 tile: each loads its
-// 128 rows of A and HALF of B (32 KiB per 8.4 MFLOP per CTA: half the traffic per FLOP), the leader issues ONE
-// M = 256, N = 256, K = 32 MMA per k32.
-//   * N = 256 matters at fp8 rates: a first version with two N = 128 MMAs per k32 (two accumulator halves, handed back
-//     separately) ran every MMA at half speed -- the issuer's own clock showed ~125 cycles per instruction where 64 were
-//     due.  Each N = 128 instruction re-reads the CTA's 4 KiB of A for 4 KiB of B: 8 KiB per 64 cycles is the whole
-//     128 B/cycle shared-memory port, with TMA writing into it at the same time.  N = 256 reads 12 KiB per 128 cycles.
-//   * TMEM: one 256-column accumulator (single-buffered: 512 columns do not hold two of them plus the scale factors).
-//     The epilogue releases it the moment its last values are in registers; what stays exposed is the TMEM drain
-//     (~1.5 k cycles per tile, see gemm_send.cu).
-//   * Scale factors are written into TMEM by the LOADER warps (tcgen05.st), not copied by the tensor pipe: each CTA needs
-//     the A scales of its own 128 rows and the B scales of all 256 columns (three 128-row chunks = 4 TMEM columns each,
-//     replicated in the four lane quarters).  The four loader warps exchange their rows' words through shared memory and
-//     each writes the complete chunks into the lane quarter it may access.  (The first version staged chunks in shared
-//     memory and had the issuer copy them with tcgen05.cp.cta_group::2 -- which does copy, in each CTA, that CTA's own
-//     chunk into its own TMEM -- but the copies execute in the tensor pipe, in order with the MMAs: ~48 cycles each, three
-//     per k-block, 144 of the 730 cycles a k-block took.)  The partner's TMEM must be ready before the leader issues: its
-//     loader warps meet at a named barrier and one thread rings a 16-byte shared::cta -> shared::cluster bulk copy whose
-//     completion is counted on the LEADER's full barrier -- a hardware signal, no release-scoped remote arrive on
-//     anybody's critical path (that pattern halved the bf16 pair kernel once).
-constexpr int STAGES2 = 6;
-constexpr int BN2 = 256;
-struct alignas(1024) Smem2 {
-  uint8_t a[STAGES2][A_STAGE];                 // this CTA's 128 rows of A
-  uint8_t b[STAGES2][B_STAGE];                 // this CTA's 128 of the tile's 256 B rows (leader: columns 0-127, partner: 128-255)
-  alignas(128) uint8_t sfa[STAGES2][SF_STAGE];   // scale words: exchange buffers of the loader warps (chunk layout), per stage
-  alignas(128) uint8_t sfb[STAGES2][2][SF_STAGE];
-  alignas(1024) uint8_t stage_c[4][4096];      // epilogue staging: per warp one 32-row x 64-column bf16 box (SWIZZLE_128B)
-  alignas(16) uint8_t bell[STAGES2][16];       // landing pad of the partner's "chunks written" doorbell copy (leader only)
-  alignas(8) uint64_t full[STAGES2], empty[STAGES2], tfull, tempty;
-  uint32_t tmem_base;
-  volatile int abort;
-};
-constexpr uint32_t kSfCol0_2 = 256;            // scale factors above the 256 accumulator columns: 16 columns per stage
-
-__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa(uint32_t cta_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(cta_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(s32(smem_dst)), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(s32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ uint32_t mx_idesc2(uint32_t sf_id) {    // M = 256 (both CTAs), N = 256
-  return (sf_id << 4) | ((uint32_t)(256 >> 3) << 17) | (1u << 23) | ((uint32_t)(256 >> 4) << 24) | (sf_id << 29);
-}
-__device__ __forceinline__ void umma_mxf8_2sm(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t tsfa, uint32_t tsfb, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::2.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}"
-               ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(tsfa), "r"(tsfb) : "memory");
-}
-// 16 bytes of this CTA's shared memory -> the leader's, completion counted (in bytes) on the leader's barrier
-__device__ __forceinline__ void ring_bell(uint32_t dst_cluster, const void* src_cta, uint32_t bar_cluster) {
-  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], 16, [%2];"
-               ::"r"(dst_cluster), "r"(s32(src_cta)), "r"(bar_cluster) : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(s32(smem_src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint4 v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-template <typename S>
-__device__ __forceinline__ bool mbar_wait_t(S& s, uint64_t* b, uint32_t parity) {
-  if (mbar_try(b, parity)) return true;
-  unsigned long long t0 = globaltimer_ns();
-  unsigned n = 0;
-  while (!mbar_try(b, parity)) {
-    if ((++n & 255) == 0) {
-      if (s.abort) return false;
-      if (globaltimer_ns() - t0 > kWaitNs) { s.abort = 1; return false; }
-    }
-  }
-  return true;
-}
-// grouped rasterisation (as gemm_send.cu): `group` M tiles advance together across N so concurrent clusters share B in L2
-__device__ __forceinline__ void tile_coords2(uint32_t t, uint32_t m_tiles, uint32_t n_tiles_n, uint32_t group, uint32_t* m, uint32_t* n) {
-  const uint32_t per_group = group * n_tiles_n;
-  const uint32_t grp = t / per_group, r = t % per_group;
-  const uint32_t m0 = grp * group;
-  const uint32_t gm = min(group, m_tiles - m0);
-  *m = m0 + r % gm;
-  *n = r / gm;
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_mxfp8_pair_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
-                       const __grid_constant__ MxArgs g) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  Smem2& s = *reinterpret_cast<Smem2*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const bool leader = rank == 0;
-  const unsigned long long t_start = globaltimer_ns();
-  const uint32_t m_tiles = (g.M + 2 * BM - 1) / (2 * BM), n_tiles_n = (g.N + BN2 - 1) / BN2, k_blks = (g.K + BK - 1) / BK;
-  const uint32_t n_tiles = m_tiles * n_tiles_n, ks = g.K / 32;
-  const uint32_t n_units = gridDim.x / 2, unit = blockIdx.x / 2;
-  constexpr uint32_t kGroup = 8;
-
-  if (threadIdx.x == 0) {
-    // full: the producer's expect_tx arrive + the LEADER's four loader warps; the partner's loaders are the 16 doorbell bytes
-    for (int i = 0; i < STAGES2; ++i) { mbar_init(&s.full[i], 1 + 4); mbar_init(&s.empty[i], 1); }
-    mbar_init(&s.tfull, 1);
-    mbar_init(&s.tempty, 8);
-    s.abort = 0;
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(&s.tmem_base)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = s.tmem_base;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs)
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (uint32_t tile = unit; tile < n_tiles && !s.abort; tile += n_units) {
-        uint32_t mt, nt;
-        tile_coords2(tile, m_tiles, n_tiles_n, kGroup, &mt, &nt);
-        const uint32_t ar = (mt * 2 + rank) * BM;
-        if (!wait_panel(g.a_ready, mt * 2 + rank, g.ready_timeout_ns, &s.abort)) goto producer2_done;   // this CTA's 128 rows are one panel
-        for (uint32_t kb = 0; kb < k_blks; ++kb) {
-          if (!mbar_wait_t(s, &s.empty[stage], phase ^ 1)) goto producer2_done;
-          const uint32_t lbar = mapa(s32(&s.full[stage]), 0);
-          if (leader) mbar_expect_tx(&s.full[stage], 2 * (A_STAGE + B_STAGE) + 16);
-          tma_load_3d_2sm(s.a[stage], &tmap_a, lbar, (int)(kb * BK), (int)(ar % g.a_rows_per_rec), (int)(ar / g.a_rows_per_rec));
-          const uint32_t br = nt * BN2 + rank * 128;                        // 128-row boxes never straddle records (rows_per_rec % 128 == 0)
-          tma_load_3d_2sm(s.b[stage], &tmap_b, lbar, (int)(kb * BK), (int)(br % g.b_rows_per_rec), (int)(br / g.b_rows_per_rec));
-          if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  producer2_done:
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader only)
-    if (leader && lane == 0) {
-      uint32_t stage = 0, phase = 0, tphase = 0;
-      auto sf_cols = [&](uint32_t st) { return tmem_base + kSfCol0_2 + st * 16; };
-      // where the issuer's time goes (cluster 0 reports it in out[7], as the bf16 wide kernel does): cycles waiting for
-      // operands + scale chunks / for TMEM / in the loop
-      long long w_full = 0, w_tmem = 0;
-      const long long t_loop = clock64();
-      for (uint32_t tile = unit; tile < n_tiles && !s.abort; tile += n_units) {
-        long long t0 = clock64();
-        if (!mbar_wait_t(s, &s.tempty, tphase ^ 1)) goto mma2_done;             // both CTAs' epilogues have the previous tile in registers
-        w_tmem += clock64() - t0;
-        tc_fence_after();
-        for (uint32_t kb = 0; kb < k_blks; ++kb) {
-          t0 = clock64();
-          if (!mbar_wait_t(s, &s.full[stage], phase)) goto mma2_done;
-          w_full += clock64() - t0;
-          tc_fence_after();
-          const uint64_t da = smem_desc_sw128(s.a[stage]), db = smem_desc_sw128(s.b[stage]);   // the stage's scale factors are already in TMEM (loaders)
-          const uint32_t tsfa = sf_cols(stage), tsfb = tsfa + 4;
-#pragma unroll
-          for (uint32_t k = 0; k < BK / UMMA_K; ++k)
-            umma_mxf8_2sm(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), mx_idesc2(k), tsfa | (k << 30), tsfb | (k << 30), (kb | k) != 0);
-          tc_commit_2sm(&s.empty[stage]);
-          if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_2sm(&s.tfull);
-        tphase ^= 1;
-      }
-      if (unit == 0) {
-        const unsigned long long tot = (unsigned long long)(clock64() - t_loop);
-        g.out[7] = (((unsigned long long)w_full >> 4) & 0x1fffffull) | ((((unsigned long long)w_tmem >> 4) & 0x1fffffull) << 21) | ((tot >> 4) << 42);
-      }
-    }
-  mma2_done:
-    __syncwarp();
-  } else if (warp < 6) {
-    // ===================== epilogue (both CTAs: their own 128 rows)
-    const uint32_t q = warp & 3;
-    uint32_t tphase = 0;
-    for (uint32_t tile = unit; tile < n_tiles; tile += n_units) {
-      uint32_t mt, nt;
-      tile_coords2(tile, m_tiles, n_tiles_n, kGroup, &mt, &nt);
-      if (!mbar_wait_t(s, &s.tfull, tphase)) break;
-      tphase ^= 1;
-      tc_fence_after();
-      const uint32_t row = (mt * 2 + rank) * BM + q * 32 + lane;
-      __nv_bfloat16* crow = g.c + (size_t)row * g.N + (size_t)nt * BN2;
-      const uint32_t taddr = tmem_base + ((q * 32u) << 16);
-      auto release = [&]() {                                                   // the accumulator is in registers: hand it back before storing
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (leader) mbar_arrive(&s.tempty);
-          else mbar_arrive_remote(mapa(s32(&s.tempty), 0));
-        }
-      };
-      if (g.tma_store) {
-        // as gemm_send.cu: bf16 rows staged in the SWIZZLE_128B pattern, one lane stores the 32 x 64 box (TMA clips at the edges).
-        // With per-thread row stores in this loop the LSU back-pressure sat between the TMEM loads: the issuer waited ~10 k
-        // cycles per tile for TMEM; staged, the drain is the TMEM read itself.
-        const uint32_t buf = s32(s.stage_c[q]), rowp = buf + lane * 128;
-#pragma unroll 1
-        for (int c = 0; c < BN2 / 64; ++c) {
-          uint32_t r[64];
-          tmem_ld32(taddr + c * 64, r);
-          tmem_ld32(taddr + c * 64 + 32, r + 32);
-          tmem_ld_wait();
-          if (c == BN2 / 64 - 1) release();
-          if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous store has read the box
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            st_shared_v4(rowp + ((uint32_t)(j ^ (lane & 7)) << 4), pack_bf16(r[8 * j], r[8 * j + 1]), pack_bf16(r[8 * j + 2], r[8 * j + 3]),
-                         pack_bf16(r[8 * j + 4], r[8 * j + 5]), pack_bf16(r[8 * j + 6], r[8 * j + 7]));
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&tmap_c, s.stage_c[q], (int)(nt * BN2 + c * 64), (int)((mt * 2 + rank) * BM + q * 32));
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < BN2 / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld32(taddr + c * 32, r);
-          tmem_ld_wait();
-          if (c == BN2 / 32 - 1) release();
-          const uint32_t col0 = nt * BN2 + c * 32;
-          if (row < g.M && col0 < g.N) {
-            __nv_bfloat16* dstp = crow + c * 32;
-            for (int j = 0; j < 32 && col0 + j < g.N; ++j) dstp[j] = __float2bfloat16_rn(__uint_as_float(r[j]));
-          }
-        }
-      }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");       // staged rows have left shared memory and are written
-  } else {
-    // ===================== scale loaders (warps 6-9, both CTAs): thread (w, lane) owns row w * 32 + lane of this CTA's A rows and
-    // of each 128-column half of the tile's B rows (every CTA needs the scales of all 256 columns)
-    const uint32_t w = warp - 6;
-    uint32_t stage = 0, phase = 0;
-    auto ld16 = [&](const uint8_t* base, uint64_t rec_stride, uint32_t rows_per_rec, uint32_t rows, uint32_t row, uint32_t kb) -> uint4 {
-      if (row < rows && kb * 4 + 16 <= ks) {
-        const uint8_t* p = base + (uint64_t)(row / rows_per_rec) * rec_stride + (uint64_t)(row % rows_per_rec) * ks + (uint64_t)kb * 4;
-        if (((uintptr_t)p & 15) == 0) return g.a_ready ? __ldcg(reinterpret_cast<const uint4*>(p)) : __ldg(reinterpret_cast<const uint4*>(p));
-      }
-      return make_uint4(load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb), load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb + 1),
-                        load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb + 2), load_scales(base, rec_stride, rows_per_rec, rows, ks, row, kb + 3));
-    };
-    const uint32_t bell_dst = mapa(s32(&s.bell[0][0]), 0);
-    const uint32_t tq = tmem_base + (((uint32_t)(warp & 3) * 32u) << 16);     // the TMEM lane quarter this warp may write
-    // rows this thread serves for a tile, and the first group (k-blocks 0-3) of their scales
-    struct Rows { uint32_t a, b0, b1; };
-    auto rows_of = [&](uint32_t tile) -> Rows {
-      uint32_t mt, nt;
-      tile_coords2(tile, m_tiles, n_tiles_n, kGroup, &mt, &nt);
-      const uint32_t b0 = nt * BN2 + w * 32 + lane;
-      return Rows{(mt * 2 + rank) * BM + w * 32 + lane, b0, b0 + 128};
-    };
-    uint4 ca = make_uint4(0, 0, 0, 0), cb0 = ca, cb1 = ca;
-    if (unit < n_tiles) {
-      const Rows r0 = rows_of(unit);
-      if (!wait_panel(g.a_ready, r0.a / BM, g.ready_timeout_ns, &s.abort)) goto loader2_done;
-      ca = ld16(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, r0.a, 0);
-      cb0 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, r0.b0, 0);
-      cb1 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, r0.b1, 0);
-    }
     for (uint32_t tile = unit; tile < n_tiles && !s.abort; tile += n_units) {
-      const Rows rw = rows_of(tile);
-      if (g.a_ready && tile != unit) {
-        if (!wait_panel(g.a_ready, rw.a / BM, g.ready_timeout_ns, &s.abort)) goto loader2_done;
-        ca = ld16(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, rw.a, 0);
-        cb0 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, rw.b0, 0);
-        cb1 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, rw.b1, 0);
-      }
-      for (uint32_t kb0 = 0; kb0 < k_blks; kb0 += 4) {
-        // the next group's loads are in flight while this one is handed over -- at the end of a tile that is the NEXT TILE's
-        // first group (a blocking load there put ~1 us per tile on the issuer's critical path)
-        uint4 na = ca, nb0 = cb0, nb1 = cb1;
-        if (kb0 + 4 < k_blks) {
-          na = ld16(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, rw.a, kb0 + 4);
-          nb0 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, rw.b0, kb0 + 4);
-          nb1 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, rw.b1, kb0 + 4);
-        } else if (tile + n_units < n_tiles && !g.a_ready) {                  // (with arrival words the next tile's loads wait for its panel: below)
-          const Rows rn = rows_of(tile + n_units);
-          na = ld16(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, rn.a, 0);
-          nb0 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, rn.b0, 0);
-          nb1 = ld16(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, rn.b1, 0);
-        }
-        const uint32_t wa[4] = {ca.x, ca.y, ca.z, ca.w}, wb0[4] = {cb0.x, cb0.y, cb0.z, cb0.w}, wb1[4] = {cb1.x, cb1.y, cb1.z, cb1.w};
-#pragma unroll
-        for (uint32_t j = 0; j < 4; ++j) {
-          if (kb0 + j >= k_blks) break;
-          if (!mbar_wait_t(s, &s.empty[stage], phase ^ 1)) goto loader2_done;
-          *reinterpret_cast<uint32_t*>(&s.sfa[stage][lane * 16 + w * 4]) = wa[j];
-          *reinterpret_cast<uint32_t*>(&s.sfb[stage][0][lane * 16 + w * 4]) = wb0[j];
-          *reinterpret_cast<uint32_t*>(&s.sfb[stage][1][lane * 16 + w * 4]) = wb1[j];
-          asm volatile("bar.sync 2, 128;" ::: "memory");                      // the four warps' words of every chunk are in the exchange buffer
-          {
-            // chunk row `lane` = the scale words of tile rows lane, lane + 32, lane + 64, lane + 96: four TMEM columns of lane
-            // `lane` in every lane quarter; this warp writes the quarter it may access
-            const uint4 va = *reinterpret_cast<const uint4*>(&s.sfa[stage][lane * 16]);
-            const uint4 vb0 = *reinterpret_cast<const uint4*>(&s.sfb[stage][0][lane * 16]);
-            const uint4 vb1 = *reinterpret_cast<const uint4*>(&s.sfb[stage][1][lane * 16]);
-            const uint32_t t = tq + kSfCol0_2 + stage * 16;
-            tmem_st4(t, va); tmem_st4(t + 4, vb0); tmem_st4(t + 8, vb1);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-          }
-          if (leader) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s.full[stage]);
+      const uint32_t m_blk = (tile / n_blks) * CTAS + rank, n_blk = tile % n_blks;
+      if (!wait_panel(g.a_ready, m_blk, g.ready_timeout_ns, &s.abort)) break;   // the scales travel in the same record
+      const uint32_t ar = m_blk * BM, br = n_blk * BN;                       // rows of a tile never straddle records
+      for (uint32_t kb = 0; kb < k_blks; ++kb) {
+        const uint32_t sa = load_scales(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, ks, ar + t, kb);
+        const uint32_t sb = load_scales(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, ks, br + t, kb);
+        if (!mbar_wait(&s.abort, &s.empty[stage], phase ^ 1, kWaitNs)) goto loader_done;
+        if (t == 0) {
+          mbar_expect_tx(&s.full[stage], A_STAGE + B_STAGE);
+          tma_load_3d(s.a[stage], &tmap_a, &s.full[stage], (int)(kb * BK), (int)(ar % g.a_rows_per_rec), (int)(ar / g.a_rows_per_rec));
+          if constexpr (CTAS == 2) {
+            const uint32_t bh = br + rank * (BN / 2);
+            tma_load_3d_mc(s.b[stage] + rank * (B_STAGE / 2), &tmap_b, &s.full[stage], (int)(kb * BK), (int)(bh % g.b_rows_per_rec),
+                           (int)(bh / g.b_rows_per_rec), (uint16_t)3);
           } else {
-            asm volatile("bar.sync 3, 128;" ::: "memory");                    // all four lane quarters of this CTA's TMEM hold the stage's scales
-            if (threadIdx.x == 6 * 32) ring_bell(bell_dst + stage * 16, s.sfa[stage], mapa(s32(&s.full[stage]), 0));
+            tma_load_3d(s.b[stage], &tmap_b, &s.full[stage], (int)(kb * BK), (int)(br % g.b_rows_per_rec), (int)(br / g.b_rows_per_rec));
           }
-          if (++stage == STAGES2) { stage = 0; phase ^= 1; }
         }
-        ca = na; cb0 = nb0; cb1 = nb1;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { s.sfa[stage][k][t] = (uint8_t)(sa >> (8 * k)); s.sfb[stage][k][t] = (uint8_t)(sb >> (8 * k)); }
+        mbar_arrive(&s.full[stage]);                                           // release: the scale bytes before the arrival
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  loader2_done:
-    __syncwarp();
+  loader_done:;
+  } else {
+    // ===================== MMA + scaling + epilogue: warpgroup wg owns rows wg * 64 .. wg * 64 + 63 of the tile
+    reg_alloc<232>();
+    const uint32_t wg = (uint32_t)(warp - 4) >> 2, t = threadIdx.x - 128 * (1 + wg), wq = t >> 5;
+    const uint32_t rl0 = wg * 64 + wq * 16 + (lane >> 2);                    // fragment rows rl0, rl0 + 8 of the tile
+    const bool even = (g.N % 2 == 0) && ((uintptr_t)g.c & 3) == 0;
+    uint32_t stage = 0, phase = 0;
+    float acc[64], p0[64], p1[64];
+    for (uint32_t tile = unit; tile < n_tiles; tile += n_units) {
+      const uint32_t m_blk = (tile / n_blks) * CTAS + rank, n_blk = tile % n_blks;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      bool ok = true;
+      for (uint32_t kb = 0; kb < k_blks; ++kb) {
+        if (named_sync_or(2 + wg, 128, !mbar_wait(&s.abort, &s.full[stage], phase, kWaitNs))) { ok = false; break; }
+        const uint64_t da = wg_desc(s.a[stage] + wg * 64 * BK), db = wg_desc(s.b[stage]);
+        wg_fence();
+        wgmma_e4m3_n128(p0, da, db, 0u);
+        wg_commit();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float* p = (k & 1) ? p1 : p0;
+          if (k < 3) {
+            wg_fence();
+            wgmma_e4m3_n128((k & 1) ? p0 : p1, da + (uint64_t)(2 * (k + 1)), db + (uint64_t)(2 * (k + 1)), 0u);
+            wg_commit();
+            wg_wait<1>();
+          } else {
+            wg_wait<0>();
+          }
+          reg_fence<64>(p);
+          const float sa0 = ue8m0(s.sfa[stage][k][rl0]), sa1 = ue8m0(s.sfa[stage][k][rl0 + 8]);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const uint32_t col = 8 * j + 2 * (lane & 3);
+            const uint16_t sb = *reinterpret_cast<const uint16_t*>(&s.sfb[stage][k][col]);
+            const float sb0 = ue8m0(sb & 0xff), sb1 = ue8m0(sb >> 8);
+            acc[4 * j] = fmaf(p[4 * j], sa0 * sb0, acc[4 * j]);
+            acc[4 * j + 1] = fmaf(p[4 * j + 1], sa0 * sb1, acc[4 * j + 1]);
+            acc[4 * j + 2] = fmaf(p[4 * j + 2], sa1 * sb0, acc[4 * j + 2]);
+            acc[4 * j + 3] = fmaf(p[4 * j + 3], sa1 * sb1, acc[4 * j + 3]);
+          }
+        }
+        // every warp of the warpgroup has read this stage's scale bytes (wgmma.wait_group orders only the warp's own MMAs,
+        // and the loaders rewrite the scales the moment the stage is released)
+        named_sync(2 + wg, 128);
+        if (t == 0) {                                                          // operands and scales of this stage are consumed
+          if constexpr (CTAS == 2) { mbar_arrive_cluster(&s.empty[stage], 0); mbar_arrive_cluster(&s.empty[stage], 1); }
+          else mbar_arrive(&s.empty[stage]);
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      if (!ok) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t row = m_blk * BM + rl0 + 8 * h;
+        if (row >= g.M) continue;
+        __nv_bfloat16* crow = g.c + (size_t)row * g.N;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const uint32_t col = n_blk * BN + 8 * j + 2 * (lane & 3);
+          const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (even && col + 1 < g.N) {
+            __nv_bfloat162 v = __floats2bfloat162_rn(v0, v1);
+            *reinterpret_cast<__nv_bfloat162*>(crow + col) = v;
+          } else {
+            if (col < g.N) crow[col] = __float2bfloat16_rn(v0);
+            if (col + 1 < g.N) crow[col + 1] = __float2bfloat16_rn(v1);
+          }
+        }
+      }
+    }
   }
 
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-  }
-  if (threadIdx.x == 64) mx_finish(g, s.abort != 0, t_start, n_tiles, 2u);
+  if constexpr (CTAS == 2) cluster_sync_all();      // no CTA exits while its partner may still multicast into it or arrive on it
+  if (threadIdx.x == 128) mx_finish(g, s.abort != 0, t_start, n_tiles, (uint32_t)CTAS);
+}
+
+__global__ void __launch_bounds__(kThreads, 1) gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                                                                 const __grid_constant__ MxArgs g) {
+  mx_body<1>(tmap_a, tmap_b, g);
+}
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
+gemm_mxfp8_pair_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ MxArgs g) {
+  mx_body<2>(tmap_a, tmap_b, g);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -760,49 +293,40 @@ RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s
   if (b_rows_per_rec >= N) b_rec_stride = (uint64_t)N * K;
   CUtensorMap ma, mb;
   int rc = make_map3(&ma, (const void*)a_q, M, K, a_rows_per_rec, a_rec_stride >= 16 ? (a_rec_stride + 15) / 16 * 16 : 16);
-  if (!rc) rc = make_map3(&mb, (const void*)b_q, N, K, b_rows_per_rec, b_rec_stride >= 16 ? (b_rec_stride + 15) / 16 * 16 : 16);
   if (rc) return rc;
   MxArgs g;
   g.a_s = (const uint8_t*)a_s; g.b_s = (const uint8_t*)b_s;
   g.a_rec_stride = a_rec_stride; g.b_rec_stride = b_rec_stride; g.a_rows_per_rec = a_rows_per_rec; g.b_rows_per_rec = b_rows_per_rec;
-  g.c = (__nv_bfloat16*)c; g.M = M; g.N = N; g.K = K; g.tma_store = 0;
+  g.c = (__nv_bfloat16*)c; g.M = M; g.N = N; g.K = K;
   g.a_ready = (const unsigned long long*)a_ready_dev; g.ready_timeout_ns = (ready_timeout_ms ? ready_timeout_ms : 2000) * 1000000ull;
   g.out = (unsigned long long*)out_dev;
   g.done = (unsigned int*)done_dev;
   if (!done_dev) return -22;
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
-  if (grid <= 0) grid = 148;
-  // cta_group: 2 = CTA-pair kernel (256 x 256 per pair), 1 = single-CTA kernel (128 x 128), 0 = pair when the matrix has more
-  // than one 128-row block (a pair tile hanging over the last rows computes zeros: correct, wasted)
+  // persistent kernels, one CTA per SM
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return -19;
+  if (grid <= 0 || grid > sms) grid = sms;
+  const size_t smem = sizeof(Smem) + 1024;
+  // cta_group: 2 = 2-CTA cluster per 256 x 128 tile, 1 = one CTA per 128 x 128 tile, 0 = the cluster when the matrix has more
+  // than one 128-row block (a cluster tile hanging over the last rows computes zeros: correct, wasted)
   if ((cta_group == 2 || (cta_group == 0 && M > BM)) && grid >= 2) {
-    rc = make_map3(&mb, (const void*)b_q, N, K, b_rows_per_rec, b_rec_stride >= 16 ? (b_rec_stride + 15) / 16 * 16 : 16, 128);
+    rc = make_map3(&mb, (const void*)b_q, N, K, b_rows_per_rec, b_rec_stride >= 16 ? (b_rec_stride + 15) / 16 * 16 : 16, BN / 2);
     if (rc) return rc;
-    CUtensorMap mc;
-    g.tma_store = (N % 8 == 0 && (c & 15) == 0) ? 1u : 0u;
-    if (g.tma_store) {
-      EncodeTiledFn fn = encode_tiled();
-      cuuint64_t dims[2] = {N, M};
-      cuuint64_t strides[1] = {(cuuint64_t)N * 2};
-      cuuint32_t box[2] = {64, 32};
-      cuuint32_t estr[2] = {1, 1};
-      if (!fn || fn(&mc, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)c, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        g.tma_store = 0;
-    }
-    if (!g.tma_store) mc = ma;                                       // never dereferenced
-    const uint32_t n_tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN2 - 1) / BN2);
+    const uint32_t n_tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN);
     grid &= ~1;
     if ((uint32_t)grid > 2 * n_tiles) grid = (int)(2 * n_tiles);
-    const size_t smem = sizeof(Smem2) + 1024;
     cudaError_t e = cudaFuncSetAttribute(gemm_mxfp8_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return -(int)e - 1000;
-    gemm_mxfp8_pair_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(ma, mb, mc, g);
+    gemm_mxfp8_pair_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(ma, mb, g);
     return (int)cudaGetLastError();
   }
+  rc = make_map3(&mb, (const void*)b_q, N, K, b_rows_per_rec, b_rec_stride >= 16 ? (b_rec_stride + 15) / 16 * 16 : 16);
+  if (rc) return rc;
   const uint32_t n_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
   if ((uint32_t)grid > n_tiles) grid = (int)n_tiles;
-  const size_t smem = sizeof(Smem) + 1024;
   cudaError_t e = cudaFuncSetAttribute(gemm_mxfp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return -(int)e - 1000;
   gemm_mxfp8_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(ma, mb, g);
@@ -814,6 +338,6 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_gemm_mx() {
   cudaFuncGetAttributes(&at, gemm_mxfp8_kernel);
   cudaFuncSetAttribute(gemm_mxfp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Smem) + 1024));
   cudaFuncGetAttributes(&at, gemm_mxfp8_pair_kernel);
-  cudaFuncSetAttribute(gemm_mxfp8_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Smem2) + 1024));
+  cudaFuncSetAttribute(gemm_mxfp8_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Smem) + 1024));
   encode_tiled();
 }

@@ -196,14 +196,14 @@ __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a
   }
 }
 
-// 256-bit streaming global accesses (sm_100: LDG / STG .256): a thread's 32 bytes of fp8 in, and its 64 bytes of bf16 out as two
-// whole 32-byte sectors -- with four 16-byte stores per thread every store instruction of a warp touched half sectors
+// 32 contiguous bytes per thread, streaming (evict-first): a thread's 32 bytes of fp8 in, and its 64 bytes of bf16 out as two
+// whole 32-byte sectors.  Hopper's widest global access is 128 bits, so each is a pair of adjacent 16-byte accesses.
 __device__ __forceinline__ void ld256_cs(const void* p, uint32_t* r) {
-  asm volatile("ld.global.cs.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.cs.v4.b32 {%0,%1,%2,%3}, [%8];\n\tld.global.cs.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p));
 }
 __device__ __forceinline__ void st256_cs(void* p, const uint32_t* r) {
-  asm volatile("st.global.cs.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
+  asm volatile("st.global.cs.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.cs.v4.b32 [%0+16], {%5,%6,%7,%8};"
                ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
 }
 
@@ -355,7 +355,7 @@ RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
   uint64_t n_tiles = n_elems / kTileElems;
-  if (grid <= 0) grid = 148 * 4;
+  if (grid <= 0) grid = device_sms() * 4;
   if ((uint64_t)grid > n_tiles) grid = (int)n_tiles;
   pack_fp8_write_kernel<<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -373,9 +373,8 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
   a.out = (unsigned long long*)out_dev; a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
-  uint32_t tiles_per_chunk = chunk_elems / kTileElems;
   // waiting for arrivals the kernel shares the GPU with whatever produces them (a pack kernel, an engine): one CTA per SM then
-  if (grid <= 0) grid = qp_dev ? 148 : 148 * 4;
+  if (grid <= 0) grid = qp_dev ? device_sms() : device_sms() * 4;
   {
     const uint64_t total_tiles = n_elems / kTileElems;
     if ((uint64_t)grid > total_tiles) grid = (int)total_tiles;

@@ -285,14 +285,14 @@ RN_API int rn_k_fill_random(uint64_t stream, uint64_t ptr, uint64_t bytes, uint6
   size_t n64 = bytes / 8;
   uint32_t ntail = (uint32_t)(bytes % 8);
   int grid = (int)((n64 + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > device_sms() * 16) grid = device_sms() * 16;
   if (grid < 1) grid = 1;
   fill_random_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint64_t*)ptr, n64, (uint8_t*)ptr + n64 * 8, ntail, seed);
   return (int)cudaGetLastError();
 }
 RN_API int rn_k_fill_bf16(uint64_t stream, uint64_t ptr, uint64_t n, uint64_t seed, float scale) {
   int grid = (int)((n + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > device_sms() * 16) grid = device_sms() * 16;
   if (grid < 1) grid = 1;
   fill_bf16_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint16_t*)ptr, n, seed, scale);
   return (int)cudaGetLastError();
@@ -301,7 +301,7 @@ RN_API int rn_k_checksum(uint64_t stream, uint64_t ptr, uint64_t bytes, uint64_t
   size_t n64 = bytes / 8;
   uint32_t ntail = (uint32_t)(bytes % 8);
   int grid = (int)((n64 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > device_sms() * 8) grid = device_sms() * 8;
   if (grid < 1) grid = 1;
   cudaMemsetAsync((void*)out_dev, 0, 8, (cudaStream_t)stream);
   checksum_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint64_t*)ptr, n64, (const uint8_t*)ptr + n64 * 8, ntail,
@@ -310,7 +310,7 @@ RN_API int rn_k_checksum(uint64_t stream, uint64_t ptr, uint64_t bytes, uint64_t
 }
 RN_API int rn_k_compare(uint64_t stream, uint64_t a, uint64_t b, uint64_t bytes, uint64_t out_dev) {
   int grid = (int)((bytes / 16 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > device_sms() * 8) grid = device_sms() * 8;
   if (grid < 1) grid = 1;
   cudaMemsetAsync((void*)out_dev, 0, 8, (cudaStream_t)stream);
   compare_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t*)a, (const uint8_t*)b, bytes,
@@ -318,14 +318,14 @@ RN_API int rn_k_compare(uint64_t stream, uint64_t a, uint64_t b, uint64_t bytes,
   return (int)cudaGetLastError();
 }
 
-// L2 flush between timed iterations: stream a buffer larger than the 126 MB L2.
+// L2 flush between timed iterations: stream a buffer larger than the L2 (50 MB on H100).
 __global__ void l2_flush_kernel(uint4* p, size_t n4, uint32_t v) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t step = (size_t)gridDim.x * blockDim.x;
   for (; i < n4; i += step) p[i] = make_uint4(v, v, v, v);
 }
 RN_API int rn_k_l2_flush(uint64_t stream, uint64_t ptr, uint64_t bytes, uint32_t v) {
-  l2_flush_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>((uint4*)ptr, bytes / 16, v);
+  l2_flush_kernel<<<device_sms() * 8, 256, 0, (cudaStream_t)stream>>>((uint4*)ptr, bytes / 16, v);
   return (int)cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-"""BASELINE configs 2, 3 and 5: one B200 driving its own HCA in loopback.
+"""BASELINE configs 2, 3 and 5: one H100 driving its own HCA in loopback.
 
     wl = Loopback(device=0, pool_bytes=1 << 30)
     wl.start(engine_ctas=128)

@@ -1,4 +1,4 @@
-"""BASELINE config 4: 2xB200 send/recv, GPU0 -> wire -> GPU1, overlapped with the tcgen05 GEMM that
+"""BASELINE config 4: 2xH100 send/recv, GPU0 -> wire -> GPU1, overlapped with the wgmma GEMM that
 produces the send tile.
 
 Two HCA contexts, one per GPU, connected QP to QP exactly as two nodes would be (the responder's MKey
@@ -40,9 +40,9 @@ def run(M: int = 8192, N: int = 8192, K: int = 2048, engine_ctas: int = 0, gpus=
     per-panel completion signal (zero-length RDMA_WRITE_IMM) goes through the queue pair.
     mode="auto": direct for compute-heavy shapes (K >= 4096), engine otherwise."""
     if mode == "auto":
-        # direct stores top out near 450 GB/s (bursty: all CTAs reach their epilogue together and only one TMEM
-        # buffer of slack absorbs it), the engine streams at NVLink rate but costs 32 SMs: measured crossover
-        # is where a tile's compute time covers its 64 KiB leaving the SM at that rate, about K >= 4096
+        # direct stores leave the SMs in bursts (all CTAs reach their epilogue together), the engine streams at NVLink
+        # rate but costs 32 SMs: direct pays off once a tile's compute time covers its 64 KiB of output leaving the SM.
+        # K >= 4096 is that point by estimate; the crossover has not been measured on H100 (it needs two GPUs)
         mode = "direct" if K >= 4096 else "engine"
     g0, g1 = gpus
     d0, d1 = torch.device("cuda", g0), torch.device("cuda", g1)
@@ -68,7 +68,7 @@ def run(M: int = 8192, N: int = 8192, K: int = 2048, engine_ctas: int = 0, gpus=
     if direct:
         d_local = tx.reg_mr(d)                     # GPU1's buffer, registered with GPU0's HCA: peer mapping over NVLink
     tx.engine_start(ctas=engine_ctas, idle_timeout_ms=5000)
-    grid = 148 - engine_ctas
+    grid = torch.cuda.get_device_properties(d0).multi_processor_count - engine_ctas
     best = None
     try:
         for rep in range(reps):
@@ -143,7 +143,7 @@ def run_chain(M: int = 8192, N1: int = 8192, K1: int = 2048, N2: int = 8192, gpu
     a_op, b_op = MX.MxOperand.from_panel_records(rcv, M, N1), MX.MxOperand.from_tensors(wq, ws)
     torch.cuda.synchronize(d0); torch.cuda.synchronize(d1)
     tx.engine_start(ctas=engine_ctas, idle_timeout_ms=5000)
-    grid1 = 148 - engine_ctas
+    grid1 = torch.cuda.get_device_properties(d0).multi_processor_count - engine_ctas
     best = {"fused": None, "sequential": None}
     try:
         for mode in ("sequential", "fused", "sequential", "fused") * max(1, (reps + 1) // 2):

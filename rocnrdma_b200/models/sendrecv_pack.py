@@ -1,4 +1,4 @@
-"""2xB200: a bf16 tensor on GPU0 leaves as block-scaled fp8 records and is bf16 again on GPU1, with no host step in between.
+"""2xH100: a bf16 tensor on GPU0 leaves as block-scaled fp8 records and is bf16 again on GPU1, with no host step in between.
 
 GPU0 runs ``pack_fp8_write`` (K3); GPU1 runs ``unpack_fp8`` (K5), which waits on its receive CQ from the device and
 unpacks every record the moment its RDMA_WRITE_IMM completion shows up.  Two data planes under the same control

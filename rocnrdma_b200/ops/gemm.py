@@ -1,4 +1,4 @@
-"""K4 wrapper: tcgen05/TMEM/TMA bf16 GEMM whose epilogue RDMA-writes finished 128-row panels."""
+"""K4 wrapper: Hopper wgmma/TMA bf16 GEMM whose epilogue RDMA-writes finished 128-row panels."""
 from __future__ import annotations
 
 import os
@@ -25,8 +25,8 @@ class GemmResult:
     M: int
     N: int
     K: int
-    issuer_cycles: dict | None = None
-    variant: int = 0          # kernel that ran: 1 = single CTA, 2 = CTA pair, 3 = wide CTA pair
+    variant: int = 0          # kernel that ran: 1 = single CTA, 2 = CTA pair, 3 = CTA pair with the stream-K tail
+    stream_k: bool = False    # the last, partial wave of tiles was split along K
 
     @property
     def ok(self) -> bool:
@@ -79,7 +79,7 @@ def dequant_fp8_panels(rec: torch.Tensor, M: int, Nn: int) -> torch.Tensor:
 def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None, qp=None, dst_mr=None,
               signal_every: int = 1, with_imm: bool = False, out_fp8: bool = False, cta_group: int = 0, group_m: int = 0, direct: bool = False, plain_stores: bool = False, grid: int = 0, timeout_ms: int = 2000, stream=None, sync: bool = True, post_only: bool = False, stream_k: bool = False,
               scratch_slot: int = 2):
-    """``c[M,N] = a[M,K] @ b[N,K].T`` (bf16 in/out, fp32 accumulate on the 5th-gen tensor cores).
+    """``c[M,N] = a[M,K] @ b[N,K].T`` (bf16 in/out, fp32 accumulate: wgmma on the H100 tensor cores).
 
     With ``qp``/``c_mr``/``dst_mr`` every finished 128-row panel of ``c`` is RDMA-written to the same
     offset of ``dst_mr`` from inside the kernel; the call returns when the last panel has landed.
@@ -91,12 +91,11 @@ def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None,
     peer region as seen locally, ``dst_mr``).
     ``plain_stores``: bf16 epilogue with per-thread row stores instead of staged TMA tensor stores (A/B switch).
     ``group_m``: M blocks that advance together across N (L2 reuse of B; 0 = 8 for compute only, 4 when sending).
-    ``cta_group``: 3 = wide CTA-pair kernel (512x256 per pair, 256 rows of A per CTA, the shape cuBLAS's nvjet
-    kernels use), 2 = CTA-pair kernel (256x256 per pair), 1 = single-CTA 128x256 kernel, 0 (default) = the widest
-    the shape allows (M % 512 and K >= 6144, else M % 256).
-    ``stream_k`` (wide kernel only): split the tiles of the last, partial wave along K over all CTA pairs and fold the
-    fp32 partials back in the owner's epilogue.  Correct and tested, but a measured loss on this box (the partial write +
-    read-back and the serialised extra epilogue cost more than the idle pairs: -9 % at 4096^3), so it is off by default.
+    ``cta_group``: 2 = CTA-pair kernel (a 2-CTA cluster per 256x256 tile, B multicast to both CTAs), 1 = single-CTA
+    128x256 kernel, 3 = the pair kernel with the stream-K tail available, 0 (default) = the pair kernel when M % 256 == 0,
+    else the single-CTA kernel.
+    ``stream_k`` (cta_group 3 only): split the tiles of the last, partial wave along K over all CTA pairs and fold the
+    fp32 partials back in the owner's epilogue.  Off by default; its speed on H100 has not been measured.
     """
     for t in (a, b):
         assert t.dtype == torch.bfloat16 and t.is_contiguous()
@@ -115,12 +114,7 @@ def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None,
     if qp is not None and (c_mr is None or dst_mr is None):
         raise ValueError("sending needs c_mr (registration of c) and dst_mr")
     if cta_group == 0:
-        # measured against cuBLAS on the same box (profiles/README.md): the wide kernel moves a quarter less operand traffic
-        # and wins at K = 8192 (0.96-0.97x cuBLAS at 8192^3 where the pair kernel is 0.92-0.93x); its TMEM is single-buffered
-        # and reading an accumulator half out of TMEM takes ~1.5 k cycles whatever the number of epilogue warps, so with
-        # shorter K loops (4096^3: 0.91-0.96 vs 0.95-0.97) the double-buffered pair kernel is the better choice
-        wide_ok = M % (4 * BM) == 0 and K >= 6144 and not direct and not plain_stores and not os.environ.get("RN_GEMM_DENSE_PROBE")
-        cta_group = 3 if wide_ok else (2 if M % (2 * BM) == 0 else 1)
+        cta_group = 2 if M % (2 * BM) == 0 else 1
     if os.environ.get("RN_GEMM_CTA_GROUP"):            # A/B switch for benchmarks
         cta_group = int(os.environ["RN_GEMM_CTA_GROUP"])
     if group_m == 0:
@@ -147,8 +141,6 @@ def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None,
 def parse(view, M, Nn, K) -> GemmResult:
     w = (C.c_int64 * 8).from_buffer(view)
     r = GemmResult(WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2], w[3], w[4], w[5], M, Nn, K)
-    # wide kernel only: the MMA issuer of cluster 0 reports (cycles waiting for operands, for TMEM, in its loop)
     r.variant = int(w[6])
-    u = w[7] & 0xFFFFFFFFFFFFFFFF
-    r.issuer_cycles = {"wait_operands": (u & 0x1FFFFF) << 4, "wait_tmem": ((u >> 21) & 0x1FFFFF) << 4, "loop": (u >> 42) << 4} if u else None
+    r.stream_k = bool(w[7])
     return r

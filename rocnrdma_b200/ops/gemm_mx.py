@@ -1,4 +1,4 @@
-"""K7 wrapper: block-scaled fp8 GEMM (``tcgen05.mma.kind::mxf8f6f4.block_scale``) whose operands are the records
+"""K7 wrapper: block-scaled fp8 GEMM (e4m3 ``wgmma`` per 32-deep MX block, scales applied in registers) whose operands are the records
 the send side produces -- so a receiver multiplies straight out of its receive buffer."""
 from __future__ import annotations
 
@@ -58,7 +58,6 @@ class MxResult:
     N: int
     K: int
     variant: int = 0                       # 1 = single-CTA kernel, 2 = CTA-pair kernel
-    issuer_cycles: dict | None = None      # pair kernel, cluster 0: cycles the MMA issuer waited for operands+scales / for TMEM / in its loop
 
     @property
     def ok(self) -> bool:
@@ -73,7 +72,7 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
                cta_group: int = 0, a_ready=None, timeout_ms: int = 2000):
     """``c[M,N] (bf16) = dequant(a)[M,K] @ dequant(b)[N,K].T`` with the block scales applied by the tensor core.
     Any M and N; K a multiple of 32 (one MX block) and of 16 bytes.
-    ``cta_group``: 2 = CTA-pair kernel (256 x 256 per pair, half the operand traffic per FLOP), 1 = single-CTA kernel
+    ``cta_group``: 2 = CTA-pair kernel (256 x 128 per 2-CTA cluster, B multicast: half the B traffic per FLOP), 1 = single-CTA kernel
     (128 x 128), 0 = pair for M > 128.  ``RN_MX_CTA_GROUP`` overrides (A/B switch).
     ``a_ready``: receive-side fusion.  An int64 tensor with one word per 128-row panel of ``a`` (``a`` living in panel or chunk
     records of a registered receive buffer); the kernel starts a tile only once the word of the panel it reads is nonzero --
@@ -101,9 +100,6 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
     ws.synchronize()
     w = (C.c_int64 * 8).from_buffer(out_view)
     r = MxResult(WAIT_STATUS.get(w[0], str(w[0])), w[2] - w[1], M, Nn, K, variant=int(w[6]))
-    u = w[7] & 0xFFFFFFFFFFFFFFFF
-    if u:
-        r.issuer_cycles = {"wait_operands": (u & 0x1FFFFF) << 4, "wait_tmem": ((u >> 21) & 0x1FFFFF) << 4, "loop": (u >> 42) << 4}
     return r
 
 

@@ -11,6 +11,7 @@ box: no /dev/infiniband, no libibverbs), and a CPU-only dev box.
 from __future__ import annotations
 
 import ctypes.util
+import functools
 import glob
 import json
 import os
@@ -174,6 +175,24 @@ def capabilities() -> dict:
     }
     caps["has_verbs"] = caps["has_uverbs_dev"] and caps["has_libibverbs"]
     return caps
+
+
+@functools.lru_cache(maxsize=None)
+def dmabuf_export_works(device: int = 0) -> bool:
+    """Whether the CUDA driver exports device memory as a dma-buf here (cuMemGetHandleForAddressRange).  The device
+    attribute is not enough: a driver can report support and still refuse the export."""
+    import ctypes as C
+    import torch
+    from . import _native as N
+    lib = N.load()
+    lib.rn_set_device(device)
+    t = torch.empty(4 << 20, dtype=torch.uint8, device=f"cuda:{device}")
+    cu = C.c_int(0)
+    fd = lib.rn_dmabuf_export((t.data_ptr() + 65535) & ~65535, 1 << 20, C.byref(cu))
+    if fd < 0:
+        return False
+    lib.rn_dmabuf_close(fd)
+    return True
 
 
 def choose_wire(caps: dict, n_gpus: int) -> dict:

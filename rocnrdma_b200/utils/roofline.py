@@ -1,13 +1,15 @@
-"""Roofline arithmetic against the driver-measured peaks (MEASURED_PEAKS.json)."""
+"""Roofline arithmetic against measured peaks (MEASURED_PEAKS.json, when a run has written one) or the H100 SXM data sheet."""
 from __future__ import annotations
 
 import json
 from pathlib import Path
 
-FALLBACK = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "_source": "fallback"}
+# NVIDIA H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16.  Not measured: a card run at a lower
+# power limit reaches less.
+FALLBACK = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "_source": "fallback"}
 NIC_LINE_RATE_GBS = 50.0          # ConnectX-7, 400 Gb/s per direction
 PCIE_GEN5_X16_GBS = 63.0          # raw, per direction
-NVLINK_PEER_GBS = 770.0           # measured peer copy per direction (B200_PROFILING.md)
+NVLINK_PEER_GBS = 450.0           # H100 SXM NVLink 4, per direction (data sheet: 900 GB/s total)
 
 
 def measured_peaks(repo_root=None) -> dict:

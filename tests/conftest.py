@@ -32,7 +32,7 @@ _private_kmod_sim()
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with `-m gpu` on a GPU machine)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 GPUs")
 
 

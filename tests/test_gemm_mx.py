@@ -1,4 +1,4 @@
-"""K7: the block-scaled fp8 GEMM (tcgen05.mma.kind::mxf8f6f4.block_scale) against a PyTorch fp32 reference of the
+"""K7: the block-scaled fp8 GEMM (e4m3 wgmma, block scales applied in registers) against a PyTorch fp32 reference of the
 same op: dequantise both operands (e4m3 * 2^(scale - 127) per 32-element block), multiply in fp32.  The kernel's
 only rounding beyond that is fp32 accumulation order and the bf16 store."""
 import pytest

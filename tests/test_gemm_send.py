@@ -1,4 +1,4 @@
-"""K4: tcgen05 GEMM + fused RDMA write of finished panels, vs a plain fp32 PyTorch reference."""
+"""K4: wgmma GEMM + fused RDMA write of finished panels, vs a plain fp32 PyTorch reference."""
 import pytest
 import torch
 
@@ -253,7 +253,7 @@ def test_gemm_epilogue_variants_agree_bit_for_bit(ctx, cta_group):
 
 @pytest.mark.parametrize("M,N,K", [(512, 256, 64), (512, 512, 256), (1024, 768, 320), (2048, 1024, 1024)])
 def test_gemm_wide_pair_kernel_matches_fp32_reference(ctx, M, N, K):
-    """cta_group=3: 256 rows of A per CTA, two M=256 pair-MMAs per k16 into the two halves of TMEM."""
+    """cta_group=3: the CTA-pair kernel on the schedule that can split the last wave along K (stream-K)."""
     a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
     b = torch.randn(N, K, device="cuda").to(torch.bfloat16)
     c = torch.zeros(M, N, device="cuda", dtype=torch.bfloat16)
@@ -264,12 +264,12 @@ def test_gemm_wide_pair_kernel_matches_fp32_reference(ctx, M, N, K):
 
 
 def test_gemm_wide_identity_layout(ctx):
-    """B = I: C must equal A exactly -- every row of every half of every CTA lands where it belongs."""
+    """B = I: C must equal A exactly -- every row of both CTAs of every cluster lands where it belongs."""
     M = N = K = 1024
     a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
     b = torch.eye(N, K, device="cuda").to(torch.bfloat16)
     c = torch.zeros(M, N, device="cuda", dtype=torch.bfloat16)
-    assert ops.gemm_send(ctx, a, b, c, cta_group=3, grid=6).ok          # 3 clusters over 8 tiles: uneven, several tiles per cluster
+    assert ops.gemm_send(ctx, a, b, c, cta_group=3, grid=6).ok          # 3 clusters over 16 tiles: uneven, several tiles per cluster
     assert torch.equal(c, a)
 
 
@@ -298,29 +298,37 @@ def test_gemm_wide_send_panels(ctx, out_fp8):
         assert torch.allclose(d.float(), ref, rtol=2e-2, atol=0.5)
 
 
-@pytest.mark.parametrize("M,N,K,grid", [(1024, 1024, 512, 6), (1536, 768, 1024, 10), (2560, 2048, 2048, 60), (512, 768, 4096, 4), (4096, 4096, 1024, 148)])
+@pytest.mark.parametrize("M,N,K,grid", [(1024, 1024, 512, 6), (1536, 768, 1024, 10), (2560, 2048, 2048, 60), (512, 768, 4096, 4),
+                                        (512, 768, 4096, 8), (4096, 4096, 1024, 148)])
 def test_gemm_wide_stream_k_matches_fp32_reference(ctx, M, N, K, grid):
-    """Tiles do not divide evenly among the clusters: some are split along K between neighbouring clusters and folded
-    back together through the fp32 workspace.  Same answer as the unsplit schedule, bit for bit is not required
-    (different summation order), fp32-reference accuracy is."""
+    """Where the 256x256 cluster tiles do not divide evenly among the clusters, the last wave is split along K between
+    neighbouring clusters and folded back together through the fp32 workspace: same answer as the unsplit schedule (bit
+    for bit is not required: different summation order), fp32-reference accuracy.  Where they do divide evenly (512 x 768
+    over 2 clusters), stream-K must not split anything and the result equals the plain schedule's exactly.  The grid is
+    clamped to the SM count, so 148 runs as many clusters as the GPU holds."""
     a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
     b = torch.randn(N, K, device="cuda").to(torch.bfloat16)
     c = torch.zeros(M, N, device="cuda", dtype=torch.bfloat16)
     c2 = torch.zeros_like(c)
-    n_tiles = (M // 512) * (N // 256)
-    assert n_tiles % min(grid // 2, n_tiles) != 0, "pick a grid that leaves a partial wave"
+    n_tiles = -(-M // 256) * -(-N // 256)
+    clusters = min(grid, torch.cuda.get_device_properties(0).multi_processor_count, 2 * n_tiles) // 2
+    partial_wave = n_tiles % clusters != 0
     for _ in range(2):                                               # twice: the epoch-stamped flags need no reset
         r = ops.gemm_send(ctx, a, b, c, cta_group=3, grid=grid, stream_k=True)
         assert r.ok, r.status
-    assert ops.gemm_send(ctx, a, b, c2, cta_group=3, grid=grid, stream_k=False).ok
+        assert r.stream_k == partial_wave, (n_tiles, clusters)
+    r2 = ops.gemm_send(ctx, a, b, c2, cta_group=3, grid=grid, stream_k=False)
+    assert r2.ok and not r2.stream_k
     ref = a.float() @ b.float().T
     tol = 0.5 * (K / 256) ** 0.5
     assert torch.allclose(c.float(), ref, rtol=2e-2, atol=tol)
     assert torch.allclose(c.float(), c2.float(), rtol=2e-2, atol=tol)
+    if not partial_wave:
+        assert torch.equal(c, c2)
 
 
 def test_gemm_wide_stream_k_send_and_fp8(ctx):
-    M, N, K = 1024, 768, 1024                                        # 6 tiles over 4 clusters
+    M, N, K = 1024, 768, 1024                                        # 12 tiles over 5 clusters: the last 2 are split along K
     a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
     b = torch.randn(N, K, device="cuda").to(torch.bfloat16)
     nb = (M // 128) * ops.gemm.panel_record_bytes(N)
@@ -329,8 +337,8 @@ def test_gemm_wide_stream_k_send_and_fp8(ctx):
     cm, dm = ctx.reg_mr(c), ctx.reg_mr(d)
     qp = ctx.loopback_qp(depth=64)
     ctx.engine_start(ctas=8, idle_timeout_ms=3000)
-    r = ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=dm, cta_group=3, out_fp8=True, grid=8, stream_k=True)
+    r = ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=dm, cta_group=3, out_fp8=True, grid=10, stream_k=True)
     ctx.engine_stop()
-    assert r.ok and r.panels_posted == M // 128 and torch.equal(c, d)
+    assert r.ok and r.stream_k and r.panels_posted == M // 128 and torch.equal(c, d)
     ref = a.float() @ b.float().T
     assert torch.allclose(ops.gemm.dequant_fp8_panels(d, M, N), ref, rtol=0.08, atol=1.0)

@@ -1,4 +1,4 @@
-"""N1 userspace registration on a real B200: dma-buf export, the harness twin, MR modes."""
+"""N1 userspace registration on a real H100: dma-buf export, the harness twin, MR modes."""
 import pytest
 import torch
 
@@ -8,9 +8,19 @@ pytestmark = pytest.mark.gpu
 PAGE = 1 << 16
 
 
+def _require_dmabuf():
+    from rocnrdma_b200 import probe
+    if not probe.dmabuf_export_works():
+        pytest.skip("the CUDA driver on this machine does not export device memory as a dma-buf")
+
+
 def _buf(n):
-    # cudaMalloc-backed, 2 MiB aligned: the caching allocator's large blocks
-    t = torch.zeros(max(n, 4 << 20), dtype=torch.uint8, device="cuda:0")
+    # cudaMalloc-backed, starting on a GPU page: the caching allocator hands out blocks inside cached segments at any
+    # 512-byte offset, so take the first page boundary of a block one page longer
+    n = max(n, 4 << 20)
+    raw = torch.zeros(n + PAGE, dtype=torch.uint8, device="cuda:0")
+    off = -raw.data_ptr() % PAGE
+    t = raw[off:off + n]
     assert t.data_ptr() % PAGE == 0
     return t
 
@@ -28,6 +38,7 @@ def test_twin_classifies_addresses_and_page_size():
 
 
 def test_twin_pin_multi_pin_and_cpu_window():
+    _require_dmabuf()
     be = H.UserBackend()
     t = _buf(8 * PAGE)
     va = t.data_ptr()
@@ -57,6 +68,7 @@ def test_twin_cpu_mapping_of_the_pin_is_attempted_and_reported():
     only handle on a pin is its dma-buf: mmap() of that fd is the same window where the exporter implements it.  Either it
     maps -- then peek / poke are CPU accesses through the BAR and must agree with the GPU's view -- or the attempt fails
     cleanly with the driver's errno (driver 580: ENOTSUPP, 524) and the twin says it is on the cudaMemcpy fallback."""
+    _require_dmabuf()
     be = H.UserBackend()
     t = _buf(2 * PAGE)
     va = t.data_ptr()
@@ -86,6 +98,7 @@ def test_twin_rejects_misaligned_and_host_ranges():
 
 
 def test_reg_mr_dmabuf_mode_holds_a_pin(ctx):
+    _require_dmabuf()
     import os
     t = _buf(1 << 20)
     mr = ctx.reg_mr(t, nbytes=1 << 20, mode="dmabuf")

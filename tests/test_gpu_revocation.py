@@ -2,9 +2,7 @@
 free_callback when pinned memory goes away, and the MR is invalidated).  In userspace the same event is observed
 through the CUDA driver's allocation identity: free the memory under a live registration, and the next post must
 complete with a protection error -- never touch the address."""
-import json
 import os
-from pathlib import Path
 
 import pytest
 import torch
@@ -14,6 +12,12 @@ from rocnrdma_b200 import ops, wire as W
 
 pytestmark = pytest.mark.gpu
 BIG = 64 << 20          # its own caching-allocator segment, so empty_cache() really returns it to the driver
+
+
+def _require_dmabuf():
+    from rocnrdma_b200 import probe
+    if not probe.dmabuf_export_works():
+        pytest.skip("the CUDA driver on this machine does not export device memory as a dma-buf")
 
 
 def _victim():
@@ -33,6 +37,8 @@ def test_tensor_registration_pins_its_storage(ctx):
 
 @pytest.mark.parametrize("mode", ["direct", "dmabuf"])
 def test_free_under_a_live_registration_revokes_it(ctx, mode):
+    if mode == "dmabuf":
+        _require_dmabuf()
     src = torch.full((4096,), 3, dtype=torch.uint8, device="cuda:0")
     ms = ctx.reg_mr(src)
     x = _victim()
@@ -43,19 +49,11 @@ def test_free_under_a_live_registration_revokes_it(ctx, mode):
     qp.post_write(ms, mr, 4096)
     assert qp.scq.wait(1)[0].status == "OK"
     ctx.engine_stop()
-    record = {"mode": mode, "driver": torch.version.cuda}
     if mode == "dmabuf":
         assert mr.dmabuf_fd >= 0
-        record["fd_size_before_free"] = ctx._lib.rn_dmabuf_size(mr.dmabuf_fd)
     fd = mr.dmabuf_fd
     del x
     torch.cuda.empty_cache()                                        # cudaFree of the segment while the MR (and the fd) is live
-    if mode == "dmabuf":
-        # what driver 580 does to the exported dma-buf when its backing allocation is freed
-        record["fd_size_after_free"] = ctx._lib.rn_dmabuf_size(fd)
-        record["fd_still_open"] = os.path.exists(f"/proc/self/fd/{fd}")
-        idn = rn.api.C.c_uint64()
-        record["driver_still_knows_pointer"] = ctx._lib.rn_buffer_id(ptr, rn.api.C.byref(idn)) == 0
     assert ctx.sweep_revoked() == 1
     assert mr.state == "REVOKED" and mr.driver_revoked
     assert ctx.sweep_revoked() == 0                                 # idempotent
@@ -71,9 +69,6 @@ def test_free_under_a_live_registration_revokes_it(ctx, mode):
     assert mr.state == "FREE"
     if mode == "dmabuf":
         assert not os.path.exists(f"/proc/self/fd/{fd}") or os.readlink(f"/proc/self/fd/{fd}").find("dmabuf") < 0
-        out = Path("gpurun_out")
-        out.mkdir(exist_ok=True)
-        (out / "dmabuf_after_free.json").write_text(json.dumps(record, indent=1))
 
 
 def test_gpu_posted_write_to_freed_memory_is_refused(ctx):

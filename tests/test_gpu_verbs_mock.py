@@ -1,6 +1,6 @@
-"""GPU tier: the verbs wire on a real B200 against the mock provider -- HBM registered with the (mock) HCA the
+"""GPU tier: the verbs wire on a real H100 against the mock provider -- HBM registered with the (mock) HCA the
 three ways, host-posted baselines on GPU MRs, and the product path: the mlx5dv queues of a QP mapped into the GPU
-and driven by the SAME sm_100a kernels that drive the software HCA (rdma_stream_kernel, pack_fp8_write_kernel,
+and driven by the SAME sm_90a kernels that drive the software HCA (rdma_stream_kernel, pack_fp8_write_kernel,
 gemm_send2_kernel), directly and through the CPU doorbell proxy.  The NIC here is a host thread that DMAs with
 cuMemcpyAsync; nothing else about the path differs from a ConnectX."""
 import os
@@ -30,13 +30,24 @@ def _bufs(n):
     return src, dst
 
 
+def _require_dmabuf():
+    from rocnrdma_b200 import probe
+    if not probe.dmabuf_export_works():
+        pytest.skip("the CUDA driver on this machine does not export device memory as a dma-buf")
+
+
 @pytest.mark.parametrize("mode", ["peermem", "dmabuf", "auto"])
 def test_host_posted_write_on_hbm_mrs(vctx, mode):
-    """BASELINE config 2 shape: cudaMalloc HBM registered with the HCA, host-posted RDMA write, CPU-polled CQ."""
+    """BASELINE config 2 shape: cudaMalloc HBM registered with the HCA, host-posted RDMA write, CPU-polled CQ.  ``auto``
+    takes the dma-buf route where the driver exports device memory and falls back to the peer-memory client where not."""
+    from rocnrdma_b200 import probe
+    if mode == "dmabuf":
+        _require_dmabuf()
     n = 1 << 20
     src, dst = _bufs(n)
     ms, md = vctx.reg_mr(src, mode=mode), vctx.reg_mr(dst, mode=mode)
-    assert ms.mode == ("dmabuf" if mode in ("dmabuf", "auto") else "peermem")
+    via_dmabuf = mode == "dmabuf" or (mode == "auto" and probe.dmabuf_export_works())
+    assert ms.mode == md.mode == ("dmabuf" if via_dmabuf else "peermem")
     assert (ms.dmabuf_fd >= 0) == (ms.mode == "dmabuf")
     qp = vctx.loopback_qp(depth=16, mem=W.MEM_HOST_PINNED)
     assert not qp.on_gpu

@@ -5,7 +5,7 @@ lib = os.path.join(root, "rocnrdma_b200", "lib", "librocnrdma_b200.so")
 out = os.path.join(root, "profiles", "sass")
 os.makedirs(out, exist_ok=True)
 txt = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
-want = ["engine_kernel", "gemm_send3_kernel", "gemm_mxfp8_pair_kernel", "gemm_mxfp8_kernel", "gemm_send2_kernel", "gemm_send_kernel", "pack_fp8_write_kernel", "unpack_fp8_kernel",
+want = ["engine_kernel", "gemm_mxfp8_pair_kernel", "gemm_mxfp8_kernel", "gemm_send2_kernel", "gemm_send_kernel", "pack_fp8_write_kernel", "unpack_fp8_kernel",
         "rdma_stream_kernel", "shared_post_stress_kernel", "recv_consume_kernel"]
 summary = {}
 for m in re.finditer(r"\t\tFunction : (\S+)\n(.*?)(?=\n\t\tFunction : |\Z)", txt, re.S):
@@ -21,11 +21,11 @@ for m in re.finditer(r"\t\tFunction : (\S+)\n(.*?)(?=\n\t\tFunction : |\Z)", txt
         if mm:
             ops[mm.group(1)] += 1
             full[mm.group(1) + mm.group(2)] += 1
-    blackwell = {k: v for k, v in full.items() if k.split(".")[0] in ("UTCHMMA", "UTMALDG", "UTMASTG", "UTCBAR", "LDTM", "UTCATOMSWS", "UBLKCP", "SYNCS", "UTMACMDFLUSH", "F2FP", "UTCQMMA", "UTCCP", "STTM")}
-    summary[name] = {"mangled": mangled, "instructions": sum(ops.values()), "blackwell": dict(sorted(blackwell.items())), "mnemonics": dict(ops.most_common())}
+    hopper = {k: v for k, v in full.items() if k.split(".")[0] in ("HGMMA", "QGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "UTMACMDFLUSH", "F2FP")}
+    summary[name] = {"mangled": mangled, "instructions": sum(ops.values()), "hopper": dict(sorted(hopper.items())), "mnemonics": dict(ops.most_common())}
 json.dump(summary, open(os.path.join(out, "summary.json"), "w"), indent=1)
 for k, v in summary.items():
-    print(k, v["instructions"], v["blackwell"])
+    print(k, v["instructions"], v["hopper"])
 
 # the register / spill / shared-memory report of the same build, next to the listings (the build writes it into the
 # git-ignored lib directory)

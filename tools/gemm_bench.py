@@ -1,4 +1,4 @@
-"""K4 bench: tcgen05 GEMM (compute only) vs cuBLAS, and GEMM+send fused vs GEMM-then-send."""
+"""K4 bench: wgmma GEMM (compute only) vs cuBLAS, and GEMM+send fused vs GEMM-then-send."""
 import json, sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -36,7 +36,7 @@ for (M, N, K) in shapes:
     by_ctas = {}
     for ectas in [16, 32]:
         ctx.engine_start(ctas=ectas, idle_timeout_ms=3000)
-        grid = 148 - ectas
+        grid = torch.cuda.get_device_properties(0).multi_processor_count - ectas
         ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=dm, signal_every=4, grid=grid)
         f = min((ops.gemm_send(ctx, a, b, c, c_mr=cm, qp=qp, dst_mr=dm, signal_every=4, grid=grid) for _ in range(3)), key=lambda r: r.device_ns)
         # unfused: GEMM (compute only, same grid), then one GPU-posted write of C; best of 3

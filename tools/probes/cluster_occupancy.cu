@@ -1,5 +1,5 @@
 // How many thread-block clusters of size 1/2/4/8 with one ~200 KiB CTA per SM can be resident at once on this GPU?
-// (GPC sizes decide: a cluster never spans GPCs.)  nvcc -arch=sm_100a -o cluster_occupancy cluster_occupancy.cu
+// (GPC sizes decide: a cluster never spans GPCs.)  nvcc -arch=sm_90a -o cluster_occupancy cluster_occupancy.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k(int* p) { extern __shared__ char s[]; if (p && threadIdx.x == 9999) p[0] = s[0]; }

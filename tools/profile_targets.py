@@ -1,6 +1,6 @@
 """Short, profiler-friendly runs of each hot kernel (used under ncu; one GPU).
 
-  gemm     tcgen05 GEMM, compute only, 4096^3
+  gemm     wgmma GEMM, compute only, 4096^3
   pack     bf16 -> fp8 block-scaled pack, 256 Mi elements (pack only: the post needs a resident engine)
   engine   the DMA engine in one-shot mode: 4 host-posted 256 MiB RDMA writes, then it exits
   poster   K1 posting kernel against a resident engine is NOT profilable under ncu (kernel
