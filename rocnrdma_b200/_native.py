@@ -94,6 +94,8 @@ _SIGS = {
     "rn_qp_query": (i32, [vp, C.POINTER(RnQpCounters)]),
     "rn_post_send": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, C.POINTER(u64)]),
     "rn_post_recv": (i32, [vp, u64, u32, u32]),
+    "rn_post_atomic": (i32, [vp, u32, u64, u32, u64, u32, u64, u64, u32, C.POINTER(u64)]),
+    "rn_hca_host_native_atomics": (i32, [vp]),
     "rn_host_stream": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, u64, u32, u64, C.POINTER(u64), C.POINTER(u32)]),
     "rn_host_staged_stream": (i32, [vp, u64, u64, u64, u32, u64, u32, u32, u32, u64, u32, u64, C.POINTER(u64)]),
     "rn_engine_running": (i32, [vp]),
@@ -127,6 +129,11 @@ _SIGS = {
     "rn_stream_clamp": (None, [u32, C.POINTER(u32), C.POINTER(u32)]),
     "rn_wire_build_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, u64, u32, u32, u32, u32]),
     "rn_wire_decode_cqe": (i32, [C.POINTER(u8), C.POINTER(RnWc)]),
+    "rn_wire_build_atomic_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, u64, u32, u64, u64, u32]),
+    "rn_wire_decode_wqe": (i32, [C.POINTER(u8), C.POINTER(u64)]),
+    "rn_k_atomic_stream": (i32, [u64, C.POINTER(u64), u32, u32, u32, u64, u32, u64, u64, u32, u64, u64, u64, u32, u32, u32, u32, u64, u64]),
+    "rn_k_put_signal": (i32, [u64, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32, u32, u64, u64]),
+    "rn_k_signal_wait": (i32, [u64, u64, u64, u64, u64, u64, u64, u64, u64, u64]),
     "rn_gpu_page_size": (u64, []),
     "rn_dmabuf_export": (i32, [u64, u64, C.POINTER(i32)]),
     "rn_dmabuf_close": (i32, [i32]),
@@ -181,6 +188,7 @@ _SIGS = {
     "rn_verbs_set_state": (i32, [vp, u32]),
     "rn_verbs_post_send": (i32, [vp, u32, u64, u32, u64, u32, u32, i32, u32, C.POINTER(u64)]),
     "rn_verbs_post_recv": (i32, [vp, u64, u32, u32, C.POINTER(u64)]),
+    "rn_verbs_post_atomic": (i32, [vp, u32, u64, u32, u64, u32, u64, u64, i32, C.POINTER(u64)]),
     "rn_verbs_poll": (i32, [vp, i32, C.POINTER(RnVWc)]),
     "rn_verbs_host_stream": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, u64, u32, u64, C.POINTER(u64), C.POINTER(u32)]),
     "rn_verbs_host_staged_stream": (i32, [vp, u64, u64, u64, u32, u64, u32, u32, u32, u64, u32, u64, C.POINTER(u64)]),

@@ -259,6 +259,28 @@ class QueuePair:
         """Post a WQE with arbitrary fields (error-path tests: bad keys, bad opcodes, NOP)."""
         return self._post(opcode, laddr, lkey, raddr, rkey, nbytes, signaled, imm)
 
+    def _post_atomic(self, opcode, local, remote, swap_add, compare, local_off, remote_off, signaled) -> int:
+        idx = C.c_uint64()
+        self.ctx.sweep_revoked()
+        N.check(self.ctx._lib.rn_post_atomic(self._q, opcode, local.addr + local_off, local.lkey, remote.addr + remote_off,
+                                             remote.rkey, swap_add & 0xFFFFFFFFFFFFFFFF, compare & 0xFFFFFFFFFFFFFFFF,
+                                             W.CTRL_CQ_UPDATE if signaled else 0, C.byref(idx)), "post_atomic")
+        return idx.value
+
+    def post_fetch_add(self, local: MemoryRegion, remote: MemoryRegion, add: int, local_off=0, remote_off=0,
+                       signaled=True) -> int:
+        """Host-posted 8-byte FETCH_AND_ADD: adds ``add`` to the u64 at ``remote.addr + remote_off`` (8-byte aligned,
+        registered with ``ACC_REMOTE_ATOMIC``) and writes its original value to the 8 bytes at ``local.addr + local_off``.
+        Executes after every earlier work request of this QP.  Returns the WQE index."""
+        return self._post_atomic(W.OP_ATOMIC_FA, local, remote, add, 0, local_off, remote_off, signaled)
+
+    def post_cmp_swap(self, local: MemoryRegion, remote: MemoryRegion, compare: int, swap: int, local_off=0, remote_off=0,
+                      signaled=True) -> int:
+        """Host-posted 8-byte COMPARE_AND_SWAP: the remote u64 becomes ``swap`` if it equals ``compare``; its original
+        value lands in the local 8 bytes either way (equal to ``compare`` exactly when the swap happened).  Returns the
+        WQE index."""
+        return self._post_atomic(W.OP_ATOMIC_CS, local, remote, swap, compare, local_off, remote_off, signaled)
+
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
         """Post one receive buffer (consumed in order by SEND / WRITE_WITH_IMM)."""
         n = dst.length - off if nbytes is None else nbytes
@@ -383,6 +405,14 @@ class VerbsQueuePair(QueuePair):
         wr = C.c_uint64()
         self._vcheck(self.ctx._lib.rn_verbs_post_send(self._vq, opcode, laddr, lkey, raddr, rkey, nbytes, int(bool(signaled)), imm,
                                                       C.byref(wr)), "post_send")
+        return wr.value
+
+    def _post_atomic(self, opcode, local, remote, swap_add, compare, local_off, remote_off, signaled) -> int:
+        wr = C.c_uint64()
+        self._vcheck(self.ctx._lib.rn_verbs_post_atomic(self._vq, opcode, local.addr + local_off, local.lkey,
+                                                        remote.addr + remote_off, remote.rkey, swap_add & 0xFFFFFFFFFFFFFFFF,
+                                                        compare & 0xFFFFFFFFFFFFFFFF, int(bool(signaled)), C.byref(wr)),
+                     "post_atomic")
         return wr.value
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
@@ -726,6 +756,13 @@ class Context:
         s = N.RnEngineStats()
         N.check(self._lib.rn_engine_stats(self._h, C.byref(s)), "engine_stats")
         return {k: getattr(s, k) for k, _ in s._fields_}
+
+    @property
+    def host_native_atomics(self) -> bool:
+        """``cudaDevAttrHostNativeAtomicSupported`` of this context's GPU.  The software HCA executes an RDMA atomic
+        whose target is pinned host memory only when this is true (a GPU atomic on host memory is otherwise not atomic
+        with respect to the CPU); such an atomic completes with ``REMOTE_OP_ERR`` instead."""
+        return bool(self._h) and bool(self._lib.rn_hca_host_native_atomics(self._h))
 
     def mkey_table_ptr(self) -> int:
         """Device address of this HCA's MKey table (what a peer's engine translates rkeys with)."""

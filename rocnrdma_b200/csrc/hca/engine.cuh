@@ -221,8 +221,29 @@ struct Parsed {
   uint8_t syn;
 };
 
+// Atomic (CS / FA): both keys are checked here, nothing is moved; the retirer executes it in WQE order
+// (retire_atomics).  On success src = target word, dst = local fetch buffer, v.imm = RESOLVED_ATOMIC_* flags
+// and v.bytes = 0 (no chunks).
+__device__ __forceinline__ void parse_atomic(const EngineCtl* ctl, const QpDev* qp, Parsed* p) {
+  WqeView& v = p->v;
+  const MKeyRaw lk = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey), rk = mkey_load(qp->r.rkeys, qp->r.n_rkeys, v.rkey);
+  if (v.bytes != 8) {
+    p->syn = SYN_LOCAL_LENGTH_ERR;
+  } else {
+    p->dst = mkey_check(lk, v.lkey, v.laddr, 8, ACC_LOCAL_WRITE, false, &p->syn);
+    if (p->dst && (v.raddr & 7)) p->syn = SYN_REMOTE_INVAL_REQ_ERR;
+    else if (p->dst) p->src = mkey_check(rk, v.rkey, v.raddr, 8, ACC_REMOTE_ATOMIC, true, &p->syn);
+    // A GPU atomic on pinned host memory is only atomic with respect to the CPU where the platform says so.
+    if (p->src && rk.c.y == MEM_HOST_PINNED && !ctl->host_native_atomics) p->syn = SYN_REMOTE_OP_ERR;
+    const bool sys = rk.c.y != MEM_DEVICE || lk.c.y != MEM_DEVICE || qp->sys_scope != 0;
+    v.imm = sys ? RESOLVED_ATOMIC_SYS : 0u;
+  }
+  if (p->syn != SYN_OK) p->src = p->dst = 0;
+  v.bytes = 0;
+}
+
 // Parallel part: runs concurrently for neighbouring WQEs of the same QP.
-__device__ __forceinline__ void parse_wqe(QpDev* qp, unsigned long long w, Parsed* p) {
+__device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsigned long long w, Parsed* p) {
   const uint32_t mask = (1u << qp->sq_log) - 1;
   const uint8_t* slot = qp->sq + ((w & mask) << 6);
   Wqe64 wqe;
@@ -259,6 +280,8 @@ __device__ __forceinline__ void parse_wqe(QpDev* qp, unsigned long long w, Parse
       case OP_SEND_IMM:
         p->src = translate(qp->lkeys, qp->n_lkeys, v.lkey, v.laddr, v.bytes, 0, false, &p->syn);
         break;
+      case OP_ATOMIC_CS:
+      case OP_ATOMIC_FA: parse_atomic(ctl, qp, p); break;
       default: p->syn = SYN_LOCAL_QP_OP_ERR;
     }
   }
@@ -284,15 +307,17 @@ __device__ __forceinline__ uint32_t write_resolved(QpDev* qp, unsigned long long
     if (want > chunk) chunk = want;
   }
   uint32_t nchunks = (syn == SYN_OK && v.bytes > 0) ? (v.bytes + chunk - 1) / chunk : 1;
-  r->chunk = chunk;
+  // a clean atomic keeps its operands where a chunked copy / a receive keeps its bookkeeping (hca_types.h)
+  const bool atom = syn == SYN_OK && is_atomic(v.opcode);
+  r->chunk = atom ? (uint32_t)(v.compare >> 32) : chunk;
   if (chunk_out) *chunk_out = chunk;
   r->src = src; r->dst = dst;
   r->bytes = (syn == SYN_OK) ? v.bytes : 0;
   r->nchunks = nchunks;
   r->imm = v.imm;
   r->opcode = v.opcode; r->fm_ce_se = v.fm_ce_se; r->syndrome = syn; r->rq_consumed = rq_taken;
-  r->rq_idx = rq_idx;
-  r->done = 0;
+  r->rq_idx = atom ? v.swap_add : rq_idx;
+  r->done = atom ? (uint32_t)v.compare : 0u;
   *(volatile unsigned long long*)&r->state = (w << 2) | 1ull;
   return nchunks;
 }
@@ -364,6 +389,37 @@ __device__ __forceinline__ bool cq_would_overrun(CqDev* cq, unsigned int end_pi,
   return end_pi - ci > depth;
 }
 
+// Warp-collective part of retire for a run that holds atomics (amask: the lanes whose WQE is a clean CS / FA).
+// They execute one at a time in WQE order.  Each takes the fence a CQE owner bit takes -- cumulative over the
+// payload of every earlier WQE of the QP, observed through their "finished" state words (the __syncwarp carries
+// the other lanes' observations to the executing lane) -- then one 64-bit atom on the target, then stores the
+// original value to the local fetch buffer.  The caller publishes the run's CQEs afterwards, behind its own
+// fence, so a completion implies both the atomic and its fetched value.
+__device__ __forceinline__ void retire_atomics(const Resolved* r, bool mine, uint32_t amask, uint32_t lane, uint8_t opc,
+                                               uint32_t flags) {
+  uint4 a = make_uint4(0, 0, 0, 0), o = make_uint4(0, 0, 0, 0);
+  if (mine) {
+    a = ld_v4_volatile(r);                                         // target | fetch buffer
+    o = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r) + 32);  // compare (done | chunk) | swap_add (rq_idx)
+  }
+  __syncwarp();
+  for (uint32_t m = amask; m; m &= m - 1) {
+    if ((int)lane == __ffs((int)m) - 1) {
+      unsigned long long* tgt = reinterpret_cast<unsigned long long*>(((uint64_t)a.y << 32) | a.x);
+      uint8_t* fetch = reinterpret_cast<uint8_t*>(((uint64_t)a.w << 32) | a.z);
+      const unsigned long long cmp = ((unsigned long long)o.y << 32) | o.x, swp = ((unsigned long long)o.w << 32) | o.z;
+      const bool sys = (flags & RESOLVED_ATOMIC_SYS) != 0;
+      fence_scope(sys);
+      unsigned long long old;
+      if (opc == OP_ATOMIC_FA) old = sys ? atomicAdd_system(tgt, swp) : atomicAdd(tgt, swp);
+      else old = sys ? atomicCAS_system(tgt, cmp, swp) : atomicCAS(tgt, cmp, swp);
+      if (((uintptr_t)fetch & 7) == 0) *reinterpret_cast<volatile unsigned long long*>(fetch) = old;
+      else for (int i = 0; i < 8; ++i) reinterpret_cast<volatile uint8_t*>(fetch)[i] = (uint8_t)(old >> (8 * i));
+    }
+    __syncwarp();
+  }
+}
+
 __device__ __forceinline__ void retire(QpDev* qp, uint32_t lane, unsigned long long w_finished) {
   const uint32_t mask = (1u << qp->sq_log) - 1;
   const bool sys = qp->sys_scope != 0;
@@ -406,6 +462,13 @@ __device__ __forceinline__ void retire(QpDev* qp, uint32_t lane, unsigned long l
         want_recv = rqc && qp->r.rcq;
         want_send = syn != SYN_OK || (fm & CTRL_CQ_UPDATE);
         if (want_recv) rq_idx = ld_u64_volatile(&r->rq_idx);
+      }
+      // ---- atomics of the run execute here, in WQE order, before any CQE of the run is published
+      const bool atom = active && syn == SYN_OK && is_atomic(opc);
+      const uint32_t amask = __ballot_sync(0xffffffffu, atom);
+      if (amask) {
+        retire_atomics(r, atom, amask, lane, opc, imm);
+        if (atom) bytes = 8;
       }
       const bool err = active && syn != SYN_OK;
       const uint32_t smask = __ballot_sync(0xffffffffu, want_send), rmask = __ballot_sync(0xffffffffu, want_recv);
@@ -543,7 +606,7 @@ __device__ __forceinline__ int try_claim(EngineCtl* ctl, QpDev* qp, Work* out, b
         atomicAdd(&qp->n_db_order_violations, 1ull);
       // ---- parallel part
       Parsed p;
-      parse_wqe(qp, w, &p);
+      parse_wqe(ctl, qp, w, &p);
       const bool recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
       uint32_t n = 1, chunk_sz = 0;
       uint64_t fsrc = p.src, fdst = p.dst;
@@ -641,7 +704,7 @@ __device__ __forceinline__ void claim_batch(EngineCtl* ctl, QpDev* qp, unsigned 
   bool recv = false;
   if (lane < k) {
     trace_stamp(qp, w, TR_CLAIM);
-    parse_wqe(qp, w, &p);
+    parse_wqe(ctl, qp, w, &p);
     recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
     if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0);
   }

@@ -99,6 +99,7 @@ struct Hca {
   int engine_ctas = 0;
   bool engine_launched = false;
   int oneshot = 0;
+  int host_native_atomics = 0;         // cudaDevAttrHostNativeAtomicSupported of `dev`
   uint64_t idle_timeout_ns = 5ull * 1000000000ull, rnr_timeout_ns = 500ull * 1000000ull;
   std::mutex mu;
 };
@@ -185,6 +186,10 @@ RN_API int rn_hca_open(int dev, uint32_t max_mkeys, uint32_t max_qps, uint64_t a
   CU_OK(cudaSetDevice(dev));
   Hca* h = new Hca();
   h->dev = dev;
+  if (cudaDeviceGetAttribute(&h->host_native_atomics, cudaDevAttrHostNativeAtomicSupported, dev) != cudaSuccess) {
+    h->host_native_atomics = 0;
+    cudaGetLastError();
+  }
   int lo, hi;
   CU_OK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
   CU_OK(cudaStreamCreateWithPriority(&h->ctl, cudaStreamNonBlocking, hi));
@@ -258,6 +263,10 @@ RN_API uint64_t rn_hca_dev_scratch(void* hca, uint64_t* size) {
 }
 // Let this HCA's GPU (its engine, its posters) reach memory of `peer_dev` over NVLink: MKey tables,
 // receive rings and CQs of a peer HCA live there when two GPUs are connected.
+// 1 when a GPU atomic on pinned host memory is atomic with respect to the CPU too (the engine executes RDMA
+// atomics that target host memory only then, and completes them with REMOTE_OP_ERR otherwise).
+RN_API int rn_hca_host_native_atomics(void* hca) { return ((Hca*)hca)->host_native_atomics ? 1 : 0; }
+
 RN_API int rn_hca_enable_peer(void* hca, int peer_dev) {
   Hca* h = (Hca*)hca;
   CU_OK(cudaSetDevice(h->dev));
@@ -817,10 +826,9 @@ static int host_store(Qp* q, void* dst, const void* src, size_t n) {
   return push(q->hca, dst, src, n);
 }
 
-RN_API int rn_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
-                        uint32_t bytes, uint32_t flags, uint32_t imm, uint64_t* idx_out) {
-  Qp* q = (Qp*)qp;
-  if (q->adopted) return fail(-95, "post_send: adopted QPs are posted to by device kernels only");
+// Room for one more WQE on a host-posted QP: returns 0 and its index, or fails with "queue full".
+static int host_sq_slot(Qp* q, const char* what, uint64_t* idx_out) {
+  if (q->adopted) return fail(-95, "%s: adopted QPs are posted to by device kernels only", what);
   cudaSetDevice(q->hca->dev);
   uint64_t idx = q->h_sq_pi;
   const uint64_t depth = 1ull << q->h.sq_log;
@@ -829,25 +837,15 @@ RN_API int rn_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey
     unsigned long long rh = 0;
     if (!pull(q->hca, &rh, &q->d->retire_head, 8) && rh > q->h_sq_done && rh <= idx) q->h_sq_done = rh;
     if (idx - q->h_sq_done >= depth)
-      return fail(-12, "post_send: send queue full (%llu posted, %llu complete, depth %llu): poll the CQ first",
+      return fail(-12, "%s: send queue full (%llu posted, %llu complete, depth %llu): poll the CQ first", what,
                   (unsigned long long)idx, (unsigned long long)q->h_sq_done, (unsigned long long)depth);
   }
-  Wqe64 w;
-  memset(&w, 0, sizeof w);
-  switch (opcode) {
-    case OP_RDMA_WRITE: case OP_RDMA_WRITE_IMM: case OP_RDMA_READ:
-      build_rdma_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, raddr, rkey, bytes, (uint8_t)flags, imm);
-      break;
-    case OP_SEND: case OP_SEND_IMM:
-      build_send_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, bytes, (uint8_t)flags, imm);
-      break;
-    case OP_NOP:
-      encode_ctrl(&w.ctrl, OP_NOP, (uint16_t)idx, q->h.qpn, 1, (uint8_t)flags, 0);
-      break;
-    default:
-      // deliberately still posted: lets tests drive the engine's bad-opcode path
-      encode_ctrl(&w.ctrl, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, 1, (uint8_t)flags, 0);
-  }
+  *idx_out = idx;
+  return 0;
+}
+
+// Store WQE `idx`, then the doorbell record, then the doorbell register.
+static int host_sq_publish(Qp* q, const Wqe64& w, uint64_t idx, uint64_t* idx_out) {
   uint8_t* slot = q->h.sq + ((idx & ((1ull << q->h.sq_log) - 1)) << 6);
   int rc = host_store(q, slot, &w, 64);
   if (rc) return rc;
@@ -862,6 +860,49 @@ RN_API int rn_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey
   q->h_sq_pi = idx + 1;
   if (idx_out) *idx_out = idx;
   return 0;
+}
+
+RN_API int rn_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
+                        uint32_t bytes, uint32_t flags, uint32_t imm, uint64_t* idx_out) {
+  Qp* q = (Qp*)qp;
+  uint64_t idx = 0;
+  int rc = host_sq_slot(q, "post_send", &idx);
+  if (rc) return rc;
+  Wqe64 w;
+  memset(&w, 0, sizeof w);
+  switch (opcode) {
+    case OP_RDMA_WRITE: case OP_RDMA_WRITE_IMM: case OP_RDMA_READ:
+      build_rdma_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, raddr, rkey, bytes, (uint8_t)flags, imm);
+      break;
+    case OP_SEND: case OP_SEND_IMM:
+      build_send_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, bytes, (uint8_t)flags, imm);
+      break;
+    case OP_ATOMIC_CS: case OP_ATOMIC_FA:
+      // zero operands, data length as given (rn_post_atomic is the real entry point; this one drives error paths)
+      build_atomic_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, raddr, rkey, 0, 0, (uint8_t)flags, bytes);
+      break;
+    case OP_NOP:
+      encode_ctrl(&w.ctrl, OP_NOP, (uint16_t)idx, q->h.qpn, 1, (uint8_t)flags, 0);
+      break;
+    default:
+      // deliberately still posted: lets tests drive the engine's bad-opcode path
+      encode_ctrl(&w.ctrl, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, 1, (uint8_t)flags, 0);
+  }
+  return host_sq_publish(q, w, idx, idx_out);
+}
+
+// Host-posted 8-byte atomic (opcode OP_ATOMIC_FA: add = swap_add; OP_ATOMIC_CS: swap = swap_add, compare):
+// the original value of the remote word at raddr lands in the 8 local bytes at laddr.
+RN_API int rn_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
+                          uint64_t swap_add, uint64_t compare, uint32_t flags, uint64_t* idx_out) {
+  Qp* q = (Qp*)qp;
+  if (opcode != OP_ATOMIC_CS && opcode != OP_ATOMIC_FA) return fail(-22, "post_atomic: opcode 0x%x is not CS / FA", opcode);
+  uint64_t idx = 0;
+  int rc = host_sq_slot(q, "post_atomic", &idx);
+  if (rc) return rc;
+  Wqe64 w;
+  build_atomic_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, raddr, rkey, swap_add, compare, (uint8_t)flags);
+  return host_sq_publish(q, w, idx, idx_out);
 }
 
 RN_API int rn_post_recv(void* qp, uint64_t addr, uint32_t lkey, uint32_t bytes) {
@@ -941,6 +982,7 @@ RN_API int rn_engine_start(void* hca, int n_ctas, uint64_t idle_timeout_ms, uint
   c.stop = h->h_stop; c.qps = h->d_qptab; c.n_qps = nq; c.max_qps = h->max_qps;
   c.idle_timeout_ns = h->idle_timeout_ns; c.rnr_timeout_ns = h->rnr_timeout_ns;
   c.oneshot = h->oneshot;
+  c.host_native_atomics = h->host_native_atomics ? 1u : 0u;
   {
     const char* e = getenv("RN_ENGINE_STORES_IN_FLIGHT");
     int v = e ? atoi(e) : 0;
@@ -994,6 +1036,25 @@ RN_API void rn_wire_build_wqe(uint8_t* out64, uint32_t opcode, uint32_t idx, uin
   else
     build_rdma_wqe(&w, (uint8_t)opcode, (uint16_t)idx, qpn, laddr, lkey, raddr, rkey, bytes, (uint8_t)flags, imm);
   memcpy(out64, &w, 64);
+}
+RN_API void rn_wire_build_atomic_wqe(uint8_t* out64, uint32_t opcode, uint32_t idx, uint32_t qpn, uint64_t laddr,
+                                     uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add, uint64_t compare,
+                                     uint32_t flags) {
+  Wqe64 w;
+  build_atomic_wqe(&w, (uint8_t)opcode, (uint16_t)idx, qpn, laddr, lkey, raddr, rkey, swap_add, compare, (uint8_t)flags);
+  memcpy(out64, &w, 64);
+}
+// Decode a WQE with the engine's decoder: returns 1 if it is well formed.  out[] = opcode, wqe_idx, qpn, ds,
+// fm_ce_se, imm, raddr, rkey, laddr, lkey, bytes, swap_add, compare.
+RN_API int rn_wire_decode_wqe(const uint8_t* wqe64, uint64_t* out13) {
+  Wqe64 w;
+  memcpy(&w, wqe64, 64);
+  WqeView v;
+  const bool ok = decode_wqe(&w, &v);
+  const uint64_t f[13] = {v.opcode, v.wqe_idx, v.qpn, v.ds, v.fm_ce_se, v.imm, v.raddr, v.rkey, v.laddr, v.lkey, v.bytes,
+                          v.swap_add, v.compare};
+  memcpy(out13, f, sizeof f);
+  return ok ? 1 : 0;
 }
 RN_API int rn_wire_decode_cqe(const uint8_t* cqe64, RnWc* out) {
   Cqe64 c;

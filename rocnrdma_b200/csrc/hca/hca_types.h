@@ -12,6 +12,7 @@
 // Reference parity: amd_mem_context (amdp2p.c:73-85) is the per-registration
 // record there; MKeyEntry is its analogue here (VA, size, owner, pin handle).
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 #include "../wire/mlx5_wire.h"
 
@@ -59,6 +60,11 @@ struct CqDev {
 
 // Per-SQ-slot record written by the WQE prologue (address translation, checks)
 // and shared by every engine CTA that copies a chunk of that WQE.
+// An atomic (CS / FA) that parsed cleanly moves no chunks (bytes = 0, nchunks = 1) and is executed by the
+// retirer, so the fields a chunk copy or a receive would use carry its operands instead (a union in effect):
+//   src = target word, dst = local fetch buffer (both translated), imm = RESOLVED_ATOMIC_* flags,
+//   done | chunk = compare (low | high 32 bits), rq_idx = swap_add.
+// done | chunk | rq_idx are then one 16-byte load at offset 32.
 struct alignas(64) Resolved {
   uint64_t src, dst;
   uint32_t bytes, nchunks;
@@ -71,6 +77,9 @@ struct alignas(64) Resolved {
   unsigned long long ticket;  // [63:40] next chunk | [39:20] wqe_index mod 2^20 | [19:0] nchunks
 };
 static_assert(sizeof(Resolved) == 64, "Resolved is one cache-line pair slot");
+static_assert(offsetof(Resolved, done) == 32 && offsetof(Resolved, chunk) == 36 && offsetof(Resolved, rq_idx) == 40,
+              "atomic operands are read back as one 16-byte load at offset 32");
+enum : uint32_t { RESOLVED_ATOMIC_SYS = 1u };   // Resolved::imm of an atomic: execute (and fence) at system scope
 
 // What a requester's engine needs to know about the connected responder QP.  All
 // pointers are already translated into the engine GPU's address space.
@@ -145,6 +154,7 @@ struct EngineCtl {
   unsigned int quit_all;           // the host-doorbell watcher found the engine idle / drained: everybody leaves
   unsigned int stores_in_flight;   // smem ring split: this many TMA stores may still be reading smem, the rest of the ring holds loads (4, 6 or 8)
   unsigned int oneshot;            // exit as soon as every queue is drained (profiling under ncu: kernels are serialised there)
+  unsigned int host_native_atomics;  // cudaDevAttrHostNativeAtomicSupported: a GPU atomic on pinned host memory is atomic there
   unsigned long long n_bulk_chunks;     // chunks moved through the TMA bulk path
   unsigned long long t_start, t_exit;   // %globaltimer of engine start / exit (CTA 0)
 };

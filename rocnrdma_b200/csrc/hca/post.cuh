@@ -123,6 +123,25 @@ __device__ __forceinline__ void write_send_wqe(QpDev* qp, unsigned long long idx
   st_v4(slot + 48, 0u, 0u, 0u, 0u);
 }
 
+// 8-byte atomic (ds = 4): ctrl | raddr | atomic (swap_add, compare) | data (the local 8 bytes that receive the
+// original remote value).  FA: swap_add = addend, compare unused (0); CS: swap_add = swap, compare = compare.
+__device__ __forceinline__ void atomic_wqe_stores(uint8_t* slot, uint32_t w0, uint32_t w1, uint8_t opcode, uint64_t laddr,
+                                                  uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add,
+                                                  uint64_t compare, uint8_t fm_ce_se) {
+  if (opcode != OP_ATOMIC_CS) compare = 0;
+  st_v4(slot + 0, w0, w1, (uint32_t)fm_ce_se << 24, 0u);
+  st_v4(slot + 16, be32((uint32_t)(raddr >> 32)), be32((uint32_t)raddr), be32(rkey), 0u);
+  st_v4(slot + 32, be32((uint32_t)(swap_add >> 32)), be32((uint32_t)swap_add), be32((uint32_t)(compare >> 32)), be32((uint32_t)compare));
+  st_v4(slot + 48, be32(8u), be32(lkey), be32((uint32_t)(laddr >> 32)), be32((uint32_t)laddr));
+}
+__device__ __forceinline__ void write_atomic_wqe(QpDev* qp, unsigned long long idx, uint8_t opcode, uint64_t laddr,
+                                                 uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add,
+                                                 uint64_t compare, uint8_t fm_ce_se) {
+  uint8_t* slot = qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6);
+  atomic_wqe_stores(slot, ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(qp->qpn, 4), opcode, laddr, lkey, raddr, rkey,
+                    swap_add, compare, fm_ce_se);
+}
+
 // -------------------------------------------------------------- doorbell
 // Publish WQEs [idx, idx+n): in index order, update the doorbell record, then ring
 // the doorbell register with the first 8 bytes of the last WQE's ctrl segment.
@@ -384,6 +403,12 @@ __device__ __forceinline__ void poster_build_send(const Poster& p, unsigned long
   st_v4(slot + 32, 0u, 0u, 0u, 0u);
   st_v4(slot + 48, 0u, 0u, 0u, 0u);
 }
+__device__ __forceinline__ void poster_build_atomic(const Poster& p, unsigned long long idx, uint8_t opcode, uint64_t laddr,
+                                                    uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add,
+                                                    uint64_t compare, uint8_t fm_ce_se) {
+  atomic_wqe_stores(poster_slot(p, idx), ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(p.qpn, 4), opcode, laddr, lkey, raddr,
+                    rkey, swap_add, compare, fm_ce_se);
+}
 // Ring ONE doorbell for everything built in [p.head, to): record, release, register.
 __device__ __forceinline__ void poster_ring(Poster& p, unsigned long long to) {
   const unsigned long long last = to - 1;
@@ -421,6 +446,27 @@ __device__ __forceinline__ unsigned long long rdma_send(QpDev* qp, uint64_t ladd
   if (idx == ~0ull) return idx;
   write_send_wqe(qp, idx, with_imm ? OP_SEND_IMM : OP_SEND, laddr, lkey, bytes,
                  signaled ? CTRL_CQ_UPDATE : 0, imm);
+  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
+  return idx;
+}
+
+// Remote 8-byte atomics through the shared submit: any thread of any kernel may call them (a producer signalling
+// "data landed" after its RDMA WRITEs: the engine executes the atomic only after every earlier WQE of the QP).
+// The original remote value lands in the 8 local bytes at laddr.
+__device__ __forceinline__ unsigned long long rdma_fetch_add(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr,
+                                                             uint32_t rkey, uint64_t add, bool signaled = true) {
+  unsigned long long idx = sq_reserve(qp, 1);
+  if (idx == ~0ull) return idx;
+  write_atomic_wqe(qp, idx, OP_ATOMIC_FA, laddr, lkey, raddr, rkey, add, 0, signaled ? CTRL_CQ_UPDATE : 0);
+  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
+  return idx;
+}
+__device__ __forceinline__ unsigned long long rdma_cmp_swap(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr,
+                                                            uint32_t rkey, uint64_t compare, uint64_t swap,
+                                                            bool signaled = true) {
+  unsigned long long idx = sq_reserve(qp, 1);
+  if (idx == ~0ull) return idx;
+  write_atomic_wqe(qp, idx, OP_ATOMIC_CS, laddr, lkey, raddr, rkey, swap, compare, signaled ? CTRL_CQ_UPDATE : 0);
   if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
   return idx;
 }

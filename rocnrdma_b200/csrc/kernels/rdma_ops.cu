@@ -220,6 +220,263 @@ RN_API int rn_k_recv_consume(uint64_t stream, uint64_t qp_dev, uint32_t n, uint3
   return (int)cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- remote atomics (device-posted)
+// One warp per QP, posting CS / FA work requests with the exclusive Poster exactly like rdma_stream_kernel: bursts
+// share one reservation and one doorbell, the window bounds the outstanding WQEs.  Op i of CTA c targets the word at
+// target + c * target_stride and has its fetched (original) value written to fetch + (c * iters + i) * 8, so every
+// value an atomic returned can be checked afterwards (exactly-once under contention, in-order execution of a chain).
+struct AtomicArgs {
+  QpDev* qps[kMaxStreamQps];
+  uint32_t opcode;           // OP_ATOMIC_FA / OP_ATOMIC_CS
+  uint32_t chain;            // CS only: op i is CS(compare = i, swap = i + 1)
+  uint64_t target, target_stride, fetch;
+  uint32_t rkey, lkey;
+  uint64_t add, compare, swap;
+  uint32_t iters, window, signal_every, burst;
+  uint64_t timeout_ns;
+  unsigned long long* out;   // per CTA: [status, t_start, t_end, done, first_idx, last_idx, cons, 0]
+};
+
+__global__ void __launch_bounds__(32, 1) atomic_stream_kernel(AtomicArgs a) {
+  const uint32_t lane = threadIdx.x;
+  QpDev* qp = a.qps[blockIdx.x];
+  unsigned long long* out = a.out + (size_t)blockIdx.x * 8;
+  const uint64_t tgt = a.target + blockIdx.x * a.target_stride;
+  const uint64_t fbase = a.fetch + (uint64_t)blockIdx.x * a.iters * 8;
+  int status = WAIT_OK;
+  unsigned long long first = ~0ull, last = 0;
+  uint32_t done = 0;
+  Poster p = poster_open(qp);
+  if (qp->state == QPS_ERR) status = WAIT_QP_ERROR;
+  const unsigned long long t0 = globaltimer_ns();
+  while (done < a.iters && status != WAIT_QP_ERROR) {
+    const uint32_t n = min(a.burst, a.iters - done);
+    unsigned long long idx = 0;
+    int rc = WAIT_OK;
+    if (lane == 0) {
+      if (a.window && done + n > a.window) rc = poster_wait(p, last + n - a.window, a.timeout_ns);
+      if (rc != WAIT_TIMEOUT) {
+        idx = poster_reserve(p, n, a.timeout_ns);
+        if (idx == ~0ull) rc = WAIT_TIMEOUT;
+      }
+    }
+    rc = __shfl_sync(0xffffffffu, rc, 0);
+    idx = __shfl_sync(0xffffffffu, idx, 0);
+    if (rc != WAIT_OK) status = rc;
+    if (rc == WAIT_TIMEOUT) break;
+    if (first == ~0ull) first = idx;
+    if (lane < n) {
+      const uint32_t i = done + lane;
+      const bool sig = (a.signal_every <= 1) || ((i + 1) % a.signal_every == 0) || (i + 1 == a.iters);
+      const uint64_t cmp = a.chain ? (uint64_t)i : a.compare, swp = a.chain ? (uint64_t)i + 1 : a.swap;
+      poster_build_atomic(p, idx + lane, (uint8_t)a.opcode, fbase + (uint64_t)i * 8, a.lkey, tgt, a.rkey,
+                          a.opcode == OP_ATOMIC_FA ? a.add : swp, cmp, sig ? CTRL_CQ_UPDATE : 0);
+    }
+    if (n > 1) __syncwarp();
+    if (lane == 0) {
+      const bool outstanding = p.head > p.cons;
+      uint4 tail = make_uint4(0, 0, 0, 0);
+      if (outstanding) tail = poster_peek(p);
+      poster_ring(p, idx + n);
+      if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
+    }
+    last = idx + n - 1;
+    done += n;
+  }
+  if (lane != 0) return;
+  if (done) {
+    const int rc = poster_wait(p, last, a.timeout_ns);
+    if (rc != WAIT_OK) status = rc;
+  }
+  const unsigned long long t1 = globaltimer_ns();
+  poster_close(p);
+  out[0] = (unsigned long long)(long long)status;
+  out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
+  out[6] = p.cons;
+  out[7] = 0;
+}
+
+RN_API int rn_k_atomic_stream(uint64_t stream, const uint64_t* qps_host, uint32_t nqp, uint32_t opcode, uint32_t chain,
+                              uint64_t target, uint32_t rkey, uint64_t target_stride, uint64_t fetch, uint32_t lkey,
+                              uint64_t add, uint64_t compare, uint64_t swap, uint32_t iters, uint32_t window,
+                              uint32_t signal_every, uint32_t burst, uint64_t timeout_ms, uint64_t out_dev) {
+  AtomicArgs a;
+  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps) return -22;
+  if (opcode != OP_ATOMIC_FA && opcode != OP_ATOMIC_CS) return -22;
+  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
+  a.opcode = opcode; a.chain = chain && opcode == OP_ATOMIC_CS;
+  a.target = target; a.target_stride = target_stride; a.fetch = fetch; a.rkey = rkey; a.lkey = lkey;
+  a.add = add; a.compare = compare; a.swap = swap;
+  a.iters = iters; a.window = window;
+  rn_stream_clamp(window, &burst, &signal_every);
+  a.signal_every = signal_every; a.burst = burst;
+  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.out = (unsigned long long*)out_dev;
+  atomic_stream_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------- put-with-signal
+// Each message is an RDMA WRITE of `nbytes` (unsignaled) followed by a fetch-and-add of `add` on the remote signal
+// word (signaled), built by lanes 0 and 1 and published with ONE doorbell.  The engine executes the atomic only once
+// the WRITE before it on the QP has landed, so a receiver that sees the signal reach k may read messages 0..k-1.
+// Message i writes slot (i % nslots) * slot_stride; its fetched value goes to fetch + (i % fetch_slots) * 8.
+struct PutSignalArgs {
+  QpDev* qp;
+  uint64_t src, dst;
+  uint32_t lkey, rkey, nbytes, nslots;
+  uint64_t slot_stride;
+  uint64_t sig;
+  uint32_t sig_rkey, fetch_lkey;
+  uint64_t fetch;
+  uint32_t fetch_slots, iters, window, pad;
+  uint64_t add;
+  uint64_t timeout_ns;
+  unsigned long long* out;   // [status, t_start, t_end, done, first_idx, last_idx, cons, 0]
+};
+
+__global__ void __launch_bounds__(32, 1) put_signal_kernel(PutSignalArgs a) {
+  const uint32_t lane = threadIdx.x;
+  int status = WAIT_OK;
+  unsigned long long first = ~0ull, last = 0;
+  uint32_t done = 0;
+  Poster p = poster_open(a.qp);
+  if (a.qp->state == QPS_ERR) status = WAIT_QP_ERROR;
+  const unsigned long long t0 = globaltimer_ns();
+  for (; done < a.iters && status != WAIT_QP_ERROR; ++done) {
+    unsigned long long idx = 0;
+    int rc = WAIT_OK;
+    if (lane == 0) {
+      // window counts messages: the FA of message done - window (2 WQEs per message) must have completed
+      if (a.window && done >= a.window) rc = poster_wait(p, first + 2ull * (done - a.window) + 1, a.timeout_ns);
+      if (rc != WAIT_TIMEOUT) {
+        idx = poster_reserve(p, 2, a.timeout_ns);
+        if (idx == ~0ull) rc = WAIT_TIMEOUT;
+      }
+    }
+    rc = __shfl_sync(0xffffffffu, rc, 0);
+    idx = __shfl_sync(0xffffffffu, idx, 0);
+    if (rc != WAIT_OK) status = rc;
+    if (rc == WAIT_TIMEOUT) break;
+    if (first == ~0ull) first = idx;
+    const uint64_t off = (uint64_t)(done % a.nslots) * a.slot_stride;
+    if (lane == 0) poster_build_rdma(p, idx, OP_RDMA_WRITE, a.src + off, a.lkey, a.dst + off, a.rkey, a.nbytes, 0);
+    if (lane == 1)
+      poster_build_atomic(p, idx + 1, OP_ATOMIC_FA, a.fetch + (uint64_t)(done % a.fetch_slots) * 8, a.fetch_lkey, a.sig,
+                          a.sig_rkey, a.add, 0, CTRL_CQ_UPDATE);
+    __syncwarp();
+    if (lane == 0) {
+      const bool outstanding = p.head > p.cons;
+      uint4 tail = make_uint4(0, 0, 0, 0);
+      if (outstanding) tail = poster_peek(p);
+      poster_ring(p, idx + 2);
+      if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
+    }
+    last = idx + 1;
+  }
+  if (lane != 0) return;
+  if (done) {
+    const int rc = poster_wait(p, last, a.timeout_ns);
+    if (rc != WAIT_OK) status = rc;
+  }
+  const unsigned long long t1 = globaltimer_ns();
+  poster_close(p);
+  unsigned long long* out = a.out;
+  out[0] = (unsigned long long)(long long)status;
+  out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
+  out[6] = p.cons;
+  out[7] = 0;
+}
+
+RN_API int rn_k_put_signal(uint64_t stream, uint64_t qp_dev, uint64_t src, uint32_t lkey, uint64_t dst, uint32_t rkey,
+                           uint32_t nbytes, uint64_t slot_stride, uint32_t nslots, uint64_t sig, uint32_t sig_rkey,
+                           uint64_t fetch, uint32_t fetch_lkey, uint32_t fetch_slots, uint64_t add, uint32_t iters,
+                           uint32_t window, uint64_t timeout_ms, uint64_t out_dev) {
+  PutSignalArgs a;
+  a.qp = (QpDev*)qp_dev;
+  a.src = src; a.dst = dst; a.lkey = lkey; a.rkey = rkey; a.nbytes = nbytes;
+  a.nslots = nslots ? nslots : 1; a.slot_stride = slot_stride;
+  a.sig = sig; a.sig_rkey = sig_rkey; a.fetch = fetch; a.fetch_lkey = fetch_lkey; a.fetch_slots = fetch_slots ? fetch_slots : 1;
+  a.iters = iters; a.window = window; a.pad = 0; a.add = add;
+  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.out = (unsigned long long*)out_dev;
+  put_signal_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------- signal wait (receiver side)
+// Runs on the GPU that holds the signal word.  Thread 0 polls it with system-scope acquire loads until it reaches
+// `until`; every value 1..until is stamped (%globaltimer) when first seen.  Each wait for the next arrival is bounded
+// by timeout_ns.  With check_bytes != 0, as soon as the signal covers message k the whole CTA compares slot k of
+// check_dst with check_src (slot k at k * check_stride, check_bytes long) and counts mismatching 16-byte words.
+// out: [status, t_start, t_end, last value seen, mismatches, 0, 0, 0]
+constexpr int kSignalWaitThreads = 1024;
+__global__ void __launch_bounds__(kSignalWaitThreads, 1) signal_wait_kernel(const unsigned long long* signal, uint64_t until,
+                                                                            unsigned long long* stamps, unsigned long long* out,
+                                                                            unsigned long long timeout_ns, const uint8_t* check_dst,
+                                                                            const uint8_t* check_src, uint64_t check_bytes,
+                                                                            uint64_t check_stride) {
+  __shared__ unsigned long long s_seen, s_bad;
+  __shared__ int s_status;
+  unsigned long long seen = 0, bad = 0;
+  const unsigned long long t0 = globaltimer_ns();
+  if (threadIdx.x == 0) { s_seen = 0; s_bad = 0; s_status = WAIT_OK; }
+  __syncthreads();
+  while (seen < until) {
+    if (threadIdx.x == 0) {
+      unsigned long long v = ld_u64_acquire(signal), tw = globaltimer_ns();
+      while (v <= seen) {
+        const unsigned long long now = globaltimer_ns();
+        if (now - tw > timeout_ns) { s_status = WAIT_TIMEOUT; break; }
+        __nanosleep(64);
+        v = ld_u64_acquire(signal);
+      }
+      if (v > seen) {
+        const unsigned long long now = globaltimer_ns();
+        if (stamps)
+          for (unsigned long long k = seen; k < v && k < until; ++k) stamps[k] = now;
+        s_seen = v;
+      }
+    }
+    __syncthreads();   // thread 0's acquire, then the barrier: every thread's loads below see the messages it covers
+    const unsigned long long v = s_seen;
+    const int st = s_status;
+    if (check_bytes) {
+      const unsigned long long hi = v < until ? v : until;
+      for (unsigned long long k = seen; k < hi; ++k) {
+        const uint8_t* d = check_dst + k * check_stride;
+        const uint8_t* s = check_src + k * check_stride;
+        for (uint64_t o = (uint64_t)threadIdx.x * 16; o + 16 <= check_bytes; o += (uint64_t)kSignalWaitThreads * 16) {
+          const uint4 x = ld_v4_volatile(d + o), y = ld_v4_volatile(s + o);
+          if (x.x != y.x || x.y != y.y || x.z != y.z || x.w != y.w) ++bad;
+        }
+      }
+    }
+    seen = v;
+    __syncthreads();
+    if (st != WAIT_OK) break;
+  }
+  for (int o = 16; o; o >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, o);
+  if ((threadIdx.x & 31) == 0 && bad) atomicAdd(&s_bad, bad);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    out[0] = (unsigned long long)(long long)s_status;
+    out[1] = t0; out[2] = globaltimer_ns(); out[3] = s_seen; out[4] = s_bad;
+  }
+}
+
+RN_API int rn_k_signal_wait(uint64_t stream, uint64_t signal, uint64_t until, uint64_t stamps_dev, uint64_t out_dev,
+                            uint64_t timeout_ms, uint64_t check_dst, uint64_t check_src, uint64_t check_bytes,
+                            uint64_t check_stride) {
+  if (check_bytes & 15) return -22;
+  unsigned long long* o = (unsigned long long*)out_dev;
+  for (int i = 0; i < 8; ++i) o[i] = 0;
+  signal_wait_kernel<<<1, kSignalWaitThreads, 0, (cudaStream_t)stream>>>(
+      (const unsigned long long*)signal, until, (unsigned long long*)stamps_dev, o, (timeout_ms ? timeout_ms : 2000) * 1000000ull,
+      (const uint8_t*)check_dst, (const uint8_t*)check_src, check_bytes, check_stride);
+  return (int)cudaGetLastError();
+}
+
 // ---------------------------------------------------------------- K6: verification
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x += 0x9e3779b97f4a7c15ull;
@@ -334,6 +591,9 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncGetAttributes(&a, rdma_stream_kernel);
   cudaFuncGetAttributes(&a, recv_consume_kernel);
   cudaFuncGetAttributes(&a, shared_post_stress_kernel);
+  cudaFuncGetAttributes(&a, atomic_stream_kernel);
+  cudaFuncGetAttributes(&a, put_signal_kernel);
+  cudaFuncGetAttributes(&a, signal_wait_kernel);
   cudaFuncGetAttributes(&a, fill_random_kernel);
   cudaFuncGetAttributes(&a, fill_bf16_kernel);
   cudaFuncGetAttributes(&a, checksum_kernel);

@@ -348,6 +348,30 @@ bool dma_copy(uint64_t dst, MockMr* dmr, uint64_t src, MockMr* smr, uint64_t n) 
   return c.stream_sync(st) == 0;
 }
 
+// 8-byte atomic on the responder's memory; *old = the value before.  Host memory: a __atomic builtin.  CUDA memory:
+// read-modify-write through the DMA stream.  That is atomic with respect to this NIC only -- the NIC thread executes
+// one WQE at a time -- which is what a ConnectX promises under IBV_ATOMIC_HCA (the GPU's own atomics on the word are
+// not coordinated with it).
+bool nic_atomic(uint8_t opcode, uint64_t tgt, MockMr* mr, uint64_t swap_add, uint64_t compare, uint64_t* old) {
+  if (!mr || !mr->cu_ctx) {
+    uint64_t* p = (uint64_t*)tgt;
+    if (opcode == rn::OP_ATOMIC_FA) {
+      *old = __atomic_fetch_add(p, swap_add, __ATOMIC_SEQ_CST);
+    } else {
+      uint64_t expect = compare;
+      __atomic_compare_exchange_n(p, &expect, swap_add, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
+      *old = expect;
+    }
+    return true;
+  }
+  uint64_t v = 0;
+  if (!dma_copy((uint64_t)&v, nullptr, tgt, mr, 8)) return false;
+  *old = v;
+  const uint64_t nv = opcode == rn::OP_ATOMIC_FA ? v + swap_add : (v == compare ? swap_add : v);
+  if (nv == v) return true;
+  return dma_copy(tgt, mr, (uint64_t)&nv, nullptr, 8);
+}
+
 // ------------------------------------------------------------------ CQE writer
 void write_cqe(MockCq* cq, uint8_t opcode, uint8_t wqe_opcode, uint32_t qpn, uint16_t counter, uint32_t bytes, uint32_t imm_be,
                uint8_t syndrome) {
@@ -464,6 +488,18 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         if (syn == rn::SYN_OK) moved = v.bytes;
         break;
       }
+      case rn::OP_ATOMIC_CS: case rn::OP_ATOMIC_FA: {
+        if (v.bytes != 8) { syn = rn::SYN_LOCAL_LENGTH_ERR; break; }
+        uint64_t dst = translate(ldev, v.lkey, v.laddr, 8, IBV_ACCESS_LOCAL_WRITE, false, &syn, &lmr);
+        if (dst && (v.raddr & 7)) { syn = rn::SYN_REMOTE_INVAL_REQ_ERR; break; }
+        uint64_t tgt = dst ? translate(rdev, v.rkey, v.raddr, 8, IBV_ACCESS_REMOTE_ATOMIC, true, &syn, &rmr) : 0;
+        if (syn == rn::SYN_OK && !(peer->access_flags & IBV_ACCESS_REMOTE_ATOMIC)) syn = rn::SYN_REMOTE_ACCESS_ERR;
+        uint64_t old = 0;
+        if (syn == rn::SYN_OK && !nic_atomic(v.opcode, tgt, rmr, v.swap_add, v.compare, &old)) syn = rn::SYN_REMOTE_OP_ERR;
+        if (syn == rn::SYN_OK && !dma_copy(dst, lmr, (uint64_t)&old, nullptr, 8)) syn = rn::SYN_LOCAL_PROT_ERR;
+        if (syn == rn::SYN_OK) moved = 8;
+        break;
+      }
       default: syn = rn::SYN_LOCAL_QP_OP_ERR;
     }
   }
@@ -566,6 +602,8 @@ int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
       case IBV_WR_SEND: opc = rn::OP_SEND; break;
       case IBV_WR_SEND_WITH_IMM: opc = rn::OP_SEND_IMM; break;
       case IBV_WR_RDMA_READ: opc = rn::OP_RDMA_READ; break;
+      case IBV_WR_ATOMIC_CMP_AND_SWP: opc = rn::OP_ATOMIC_CS; break;
+      case IBV_WR_ATOMIC_FETCH_AND_ADD: opc = rn::OP_ATOMIC_FA; break;
       default: opc = 0xff;
     }
     if (opc == 0xff) { if (bad) *bad = wr; errno = EOPNOTSUPP; break; }
@@ -579,6 +617,9 @@ int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
     const uint32_t imm = be32(wr->imm_data);       // imm_data is already big-endian; build_* swaps it back onto the wire
     if (opc == rn::OP_SEND || opc == rn::OP_SEND_IMM)
       rn::build_send_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, len, fm, imm);
+    else if (rn::is_atomic(opc))   // libmlx5: FA carries compare_add as the addend, CS carries swap + compare
+      rn::build_atomic_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, wr->wr.atomic.remote_addr, wr->wr.atomic.rkey,
+                           opc == rn::OP_ATOMIC_FA ? wr->wr.atomic.compare_add : wr->wr.atomic.swap, wr->wr.atomic.compare_add, fm, len);
     else
       rn::build_rdma_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, wr->wr.rdma.remote_addr, wr->wr.rdma.rkey, len, fm, imm);
     memcpy(qp->sq + ((head & (qp->sq_cnt - 1)) << 6), &w, 64);

@@ -310,6 +310,7 @@ RN_API void* rn_verbs_reg_mr(void* dev, uint64_t ptr, uint64_t len, int mode, in
   if (access & 1) acc |= IBV_ACCESS_LOCAL_WRITE;
   if (access & 2) acc |= IBV_ACCESS_REMOTE_WRITE | IBV_ACCESS_LOCAL_WRITE;   // IB: remote write requires local write
   if (access & 4) acc |= IBV_ACCESS_REMOTE_READ;
+  if (access & 8) acc |= IBV_ACCESS_REMOTE_ATOMIC | IBV_ACCESS_LOCAL_WRITE;  // IB: remote atomic requires local write
   ibv_mr* mr = nullptr;
   errno = 0;
   if (mode == 1) {
@@ -381,7 +382,7 @@ RN_API int rn_verbs_connect(void* qp, uint32_t remote_qpn, uint16_t remote_lid, 
   ibv_qp_attr a;
   memset(&a, 0, sizeof a);
   a.qp_state = IBV_QPS_INIT; a.pkey_index = 0; a.port_num = d->port;
-  a.qp_access_flags = IBV_ACCESS_REMOTE_WRITE | IBV_ACCESS_REMOTE_READ | IBV_ACCESS_LOCAL_WRITE;
+  a.qp_access_flags = IBV_ACCESS_REMOTE_WRITE | IBV_ACCESS_REMOTE_READ | IBV_ACCESS_REMOTE_ATOMIC | IBV_ACCESS_LOCAL_WRITE;
   int rc = api().modify_qp(q->qp, &a, IBV_QP_STATE | IBV_QP_PKEY_INDEX | IBV_QP_PORT | IBV_QP_ACCESS_FLAGS);
   if (rc) return why(-rc, "modify_qp(INIT) failed: %d", rc);
   memset(&a, 0, sizeof a);
@@ -432,6 +433,29 @@ RN_API int rn_verbs_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_
   wr.send_flags = signaled ? IBV_SEND_SIGNALED : 0;
   wr.imm_data = __builtin_bswap32(imm);            // host value -> network order
   wr.wr.rdma.remote_addr = raddr; wr.wr.rdma.rkey = rkey;
+  int rc = ibv_post_send(q->qp, &wr, &bad);
+  if (rc) return why(-rc, "ibv_post_send failed: %d (%s)", rc, strerror(rc));
+  if (wr_id_out) *wr_id_out = wr.wr_id;
+  return 0;
+}
+// 8-byte remote atomic (opcode OP_ATOMIC_FA: add = swap_add; OP_ATOMIC_CS: swap = swap_add, compare): the original
+// remote value lands in the 8 local bytes at laddr.
+RN_API int rn_verbs_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
+                                uint64_t swap_add, uint64_t compare, int signaled, uint64_t* wr_id_out) {
+  QpH* q = (QpH*)qp;
+  if (q->raw_owned) return why(-16, "this QP's queues are owned by the GPU poster; host posting would corrupt the producer index");
+  ibv_sge sge = {laddr, 8, lkey};
+  ibv_send_wr wr, *bad = nullptr;
+  memset(&wr, 0, sizeof wr);
+  wr.wr_id = q->next_wr_id++;
+  wr.sg_list = &sge; wr.num_sge = 1;
+  switch (opcode) {
+    case 0x11: wr.opcode = IBV_WR_ATOMIC_CMP_AND_SWP; wr.wr.atomic.compare_add = compare; wr.wr.atomic.swap = swap_add; break;
+    case 0x12: wr.opcode = IBV_WR_ATOMIC_FETCH_AND_ADD; wr.wr.atomic.compare_add = swap_add; break;
+    default: return why(-22, "opcode 0x%x is not an atomic", opcode);
+  }
+  wr.send_flags = signaled ? IBV_SEND_SIGNALED : 0;
+  wr.wr.atomic.remote_addr = raddr; wr.wr.atomic.rkey = rkey;
   int rc = ibv_post_send(q->qp, &wr, &bad);
   if (rc) return why(-rc, "ibv_post_send failed: %d (%s)", rc, strerror(rc));
   if (wr_id_out) *wr_id_out = wr.wr_id;

@@ -221,6 +221,22 @@ RN_HD void build_send_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t q
   encode_data(&w->send.data, laddr, lkey, bytes);
   for (int i = 0; i < 32; ++i) w->send.pad[i] = 0;
 }
+RN_HD void encode_atomic(AtomicSeg* a, uint64_t swap_add, uint64_t compare) {
+  a->swap_add = be64(swap_add);
+  a->compare = be64(compare);
+}
+// 8-byte atomic (ds = 4): ctrl + raddr + atomic + data.  Operand placement as in libmlx5: fetch-and-add
+// carries the addend in swap_add (compare is zero); compare-and-swap carries the swap value in swap_add and
+// the compare value in compare.  The data segment names the local 8 bytes that receive the original remote
+// value.  The remote word and the fetched value are native (little-endian) u64s (DESIGN.md section 3.1).
+RN_HD void build_atomic_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint64_t laddr, uint32_t lkey,
+                            uint64_t raddr, uint32_t rkey, uint64_t swap_add, uint64_t compare, uint8_t fm_ce_se,
+                            uint32_t bytes = 8) {
+  encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, 4, fm_ce_se, 0);
+  encode_raddr(&w->atom.raddr, raddr, rkey);
+  encode_atomic(&w->atom.atomic, swap_add, opcode == OP_ATOMIC_CS ? compare : 0);
+  encode_data(&w->atom.data, laddr, lkey, bytes);
+}
 
 // ---------------------------------------------------------------- decoders
 struct WqeView {
@@ -229,7 +245,9 @@ struct WqeView {
   uint32_t qpn, imm;
   uint64_t raddr, laddr;
   uint32_t rkey, lkey, bytes;
+  uint64_t swap_add, compare;    // atomics only (native byte order)
 };
+RN_HD bool is_atomic(uint8_t opcode) { return opcode == OP_ATOMIC_CS || opcode == OP_ATOMIC_FA; }
 RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
   uint32_t w0 = be32(w->ctrl.opmod_idx_opcode), w1 = be32(w->ctrl.qpn_ds);
   v->opcode = (uint8_t)(w0 & 0xff);
@@ -240,7 +258,18 @@ RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
   v->fm_ce_se = w->ctrl.fm_ce_se;
   v->imm = be32(w->ctrl.imm);
   v->raddr = 0; v->rkey = 0; v->laddr = 0; v->lkey = 0; v->bytes = 0;
+  v->swap_add = 0; v->compare = 0;
   switch (v->opcode) {
+    case OP_ATOMIC_CS: case OP_ATOMIC_FA:
+      if (v->ds != 4) return false;
+      v->raddr = be64(w->atom.raddr.raddr);
+      v->rkey = be32(w->atom.raddr.rkey);
+      v->swap_add = be64(w->atom.atomic.swap_add);
+      v->compare = be64(w->atom.atomic.compare);
+      v->laddr = be64(w->atom.data.addr);
+      v->lkey = be32(w->atom.data.lkey);
+      v->bytes = be32(w->atom.data.byte_count) & 0x7fffffffu;
+      return true;
     case OP_RDMA_WRITE: case OP_RDMA_WRITE_IMM: case OP_RDMA_READ:
       if (v->ds != 3) return false;
       v->raddr = be64(w->rdma.raddr.raddr);

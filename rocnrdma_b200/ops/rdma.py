@@ -171,3 +171,113 @@ def shared_post_stress(qp, src_mr, dst_mr, ctas: int = 64, per_cta: int = 64, ti
     ws.synchronize()
     w = (C.c_int64 * 8).from_buffer(out_view)
     return dict(status=WAIT_STATUS.get(w[0], str(w[0])), device_ns=w[2] - w[1], posted=w[3])
+
+
+# ---------------------------------------------------------------- remote atomics and put-with-signal
+_OP_CS, _OP_FA = 0x11, 0x12
+
+
+def atomic_stream(qps, op: str, target_mr, fetch_mr, iters: int, add: int = 1, compare: int = 0, swap: int = 0,
+                  chain: bool = False, target_stride: int = 0, window: int = 0, burst: int = 1, signal_every: int = 1,
+                  timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = 16384):
+    """Device-posted 8-byte remote atomics: one warp per QP posts ``iters`` FETCH_AND_ADD (``op="fa"``: ``add``) or
+    COMPARE_AND_SWAP (``op="cs"``: ``compare`` / ``swap``) work requests with the same windowed, bursted poster as
+    :func:`rdma_stream`.  QP ``c`` targets the u64 at ``target_mr.addr + c * target_stride`` (``target_stride=0``: every
+    QP on one word); its op ``i`` writes the original value to ``fetch_mr.addr + (c * iters + i) * 8``, so ``fetch_mr``
+    needs ``len(qps) * iters * 8`` bytes.  ``chain=True`` (CS only) posts CS(compare=i, swap=i+1): on a word that
+    starts at 0 every one of them succeeds exactly when the QP executes its atomics in order.  Returns a
+    :class:`StreamResult` (``us_per_msg`` = device time per atomic of one QP)."""
+    if op not in ("fa", "cs"):
+        raise ValueError("op must be 'fa' or 'cs'")
+    lib = N.load()
+    if not isinstance(qps, (list, tuple)):
+        qps = [qps]
+    ctx = qps[0].ctx
+    nq = len(qps)
+    if fetch_mr.length < nq * iters * 8:
+        raise ValueError(f"fetch_mr holds {fetch_mr.length} bytes; {nq} QPs x {iters} atomics need {nq * iters * 8}")
+    ws = work_stream(ctx, stream)
+    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
+    out_addr, out_view = ctx.scratch(nq * 64, offset=scratch_off)
+    m = 0xFFFFFFFFFFFFFFFF
+    rc = lib.rn_k_atomic_stream(_stream_ptr(ws), qp_arr, nq, _OP_FA if op == "fa" else _OP_CS, int(chain), target_mr.addr,
+                                target_mr.rkey, target_stride, fetch_mr.addr, fetch_mr.lkey, add & m, compare & m, swap & m,
+                                iters, window, signal_every, burst, timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"atomic_stream launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_stream_out(out_view, nq, 8)
+
+
+def _fetch_sink(ctx):
+    """An 8-byte-per-slot local buffer for fetched values nobody reads (registered once per context)."""
+    if getattr(ctx, "_atomic_sink", None) is None:
+        t = torch.zeros(4096, dtype=torch.uint8, device=f"cuda:{ctx.device}")
+        ctx._atomic_sink = ctx.reg_mr(t)
+    return ctx._atomic_sink
+
+
+def put_signal(qp, src_mr, dst_mr, nbytes: int, sig_mr, sig_off: int = 0, fetch_mr=None, add: int = 1, iters: int = 1,
+               window: int = 0, slot_stride: int = 0, nslots: int = 1, timeout_ms: int = 2000, stream=None,
+               sync: bool = True, scratch_off: int = 20480):
+    """Device-posted put-with-signal: message ``i`` is an RDMA WRITE of ``nbytes`` from ``src_mr`` to ``dst_mr`` (slot
+    ``i % nslots`` at ``slot_stride``) followed by a FETCH_AND_ADD of ``add`` on the remote u64 at
+    ``sig_mr.addr + sig_off``, both published with one doorbell.  The atomic executes only after the WRITE has landed,
+    so a receiver that sees the signal reach ``k`` (:func:`signal_wait`) may read messages ``0..k-1``.  The fetched
+    values go to ``fetch_mr`` (message ``i`` at ``(i % (fetch_mr.length // 8)) * 8``); by default to a small buffer the
+    context registers the first time it is needed -- pass ``fetch_mr`` when the engine is already running, since a
+    first allocation then waits for it.  ``window`` bounds the messages in flight (0: the send queue does).  Returns a
+    :class:`StreamResult` (``us_per_msg`` = device time per message)."""
+    lib = N.load()
+    ctx = qp.ctx
+    if fetch_mr is None:
+        fetch_mr = _fetch_sink(ctx)
+    ws = work_stream(ctx, stream)
+    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    rc = lib.rn_k_put_signal(_stream_ptr(ws), qp.dev_ptr, src_mr.addr, src_mr.lkey, dst_mr.addr, dst_mr.rkey, nbytes,
+                             slot_stride, nslots, sig_mr.addr + sig_off, sig_mr.rkey, fetch_mr.addr, fetch_mr.lkey,
+                             max(fetch_mr.length // 8, 1), add & 0xFFFFFFFFFFFFFFFF, iters, window, timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"put_signal launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_stream_out(out_view, 1, nbytes)
+
+
+def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, stream=None, sync: bool = True,
+                check=None, scratch_off: int = 20544):
+    """Receiver side of :func:`put_signal`, on the GPU that holds the signal: waits until the u64 at ``signal`` (a
+    tensor, a ``MemoryRegion`` or an ``(address, nbytes)`` pair; the word at its start) reaches each value ``1..until``
+    in turn, with system-scope acquire loads and at most ``timeout_ms`` per arrival.  ``stamps`` (int64 tensor of at
+    least ``until`` entries on that GPU) receives the %globaltimer at which value ``k + 1`` was first seen.
+    ``check=(dst, src, slot_bytes, slot_stride)`` compares slot ``k`` of ``dst`` with ``src`` (``slot_bytes`` a multiple
+    of 16) as soon as the signal covers message ``k``.  Returns ``dict(status, seen, mismatches, device_ns, ...)``."""
+    from ..api import _ptr_len
+    lib = N.load()
+    addr = signal.addr if hasattr(signal, "rkey") else _ptr_len(signal, 8)[0]
+    ws = work_stream(ctx, stream)
+    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    cd = cs = cb = cst = 0
+    if check is not None:
+        d, s, cb, cst = check
+        cd, cs = _ptr_len(d, 1)[0], _ptr_len(s, 1)[0]
+        if cb % 16:
+            raise ValueError("check slot_bytes must be a multiple of 16")
+    rc = lib.rn_k_signal_wait(_stream_ptr(ws), addr, until, stamps.data_ptr() if stamps is not None else 0, out_addr,
+                              timeout_ms, cd, cs, cb, cst)
+    if rc:
+        raise N.NativeError(f"signal_wait launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_signal_wait(out_view)
+
+
+def parse_signal_wait(view) -> dict:
+    """Decode the record :func:`signal_wait` leaves in its scratch slot (for ``sync=False`` callers)."""
+    w = (C.c_int64 * 8).from_buffer(view)
+    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), seen=w[3], mismatches=w[4], device_ns=w[2] - w[1],
+                t_start_ns=w[1], t_end_ns=w[2])

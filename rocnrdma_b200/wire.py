@@ -77,6 +77,20 @@ def send_wqe(opcode, wqe_idx, qpn, laddr, lkey, nbytes, fm_ce_se=CTRL_CQ_UPDATE,
     return b + bytes(WQEBB - len(b))
 
 
+def atomic_seg(swap_add: int, compare: int = 0) -> bytes:
+    """The 16-byte atomic segment: big-endian ``swap_add`` (FA: the addend; CS: the swap value), then ``compare``."""
+    return struct.pack(">QQ", swap_add & 0xFFFFFFFFFFFFFFFF, compare & 0xFFFFFFFFFFFFFFFF)
+
+
+def atomic_wqe(opcode, wqe_idx, qpn, laddr, lkey, raddr, rkey, swap_add, compare=0, fm_ce_se=CTRL_CQ_UPDATE,
+               nbytes=8) -> bytes:
+    """One WQEBB: ctrl + raddr + atomic + data (ds = 4).  FA: ``swap_add`` is the addend and compare is written as 0;
+    CS: ``swap_add`` is the swap value.  The data segment names the local 8 bytes that receive the original value."""
+    cmp = compare if opcode == OP_ATOMIC_CS else 0
+    return (ctrl_seg(opcode, wqe_idx, qpn, 4, fm_ce_se) + raddr_seg(raddr, rkey) + atomic_seg(swap_add, cmp)
+            + data_seg(laddr, lkey, nbytes))
+
+
 @dataclass
 class WqeView:
     opcode: int
@@ -91,6 +105,8 @@ class WqeView:
     laddr: int = 0
     lkey: int = 0
     nbytes: int = 0
+    swap_add: int = 0
+    compare: int = 0
 
 
 def decode_wqe(b: bytes) -> WqeView:
@@ -101,6 +117,11 @@ def decode_wqe(b: bytes) -> WqeView:
     if v.opcode in (OP_RDMA_WRITE, OP_RDMA_WRITE_IMM, OP_RDMA_READ):
         v.raddr, v.rkey, _ = struct.unpack_from(">QII", b, 16)
         n, v.lkey, v.laddr = struct.unpack_from(">IIQ", b, 32)
+        v.nbytes = n & 0x7FFFFFFF
+    elif v.opcode in (OP_ATOMIC_CS, OP_ATOMIC_FA):
+        v.raddr, v.rkey, _ = struct.unpack_from(">QII", b, 16)
+        v.swap_add, v.compare = struct.unpack_from(">QQ", b, 32)
+        n, v.lkey, v.laddr = struct.unpack_from(">IIQ", b, 48)
         v.nbytes = n & 0x7FFFFFFF
     elif v.opcode in (OP_SEND, OP_SEND_IMM):
         n, v.lkey, v.laddr = struct.unpack_from(">IIQ", b, 16)

@@ -1,0 +1,44 @@
+"""The atomic WQE layout against an independent source: DOCA GPUNetIO's definitions in the NCCL wheel
+(tests/native/atomic_crosscheck.cc; every layout assertion is a static_assert, and the program checks the ds the
+encoder writes)."""
+import shutil
+import subprocess
+from pathlib import Path
+
+import pytest
+
+from test_wire_crosscheck import _doca_header
+
+ROOT = Path(__file__).resolve().parent.parent
+SRC = ROOT / "tests" / "native" / "atomic_crosscheck.cc"
+
+
+def _compile(tmp_path, include_dir, hdr):
+    exe = tmp_path / "atomic_crosscheck"
+    cmd = ["g++", "-std=c++17", "-fpermissive", "-w", f"-I{include_dir}", f'-DDOCA_VERBS_DEF_H="{hdr}"', str(SRC), "-o", str(exe)]
+    return exe, subprocess.run(cmd, capture_output=True, text=True, timeout=120)
+
+
+@pytest.mark.skipif(shutil.which("g++") is None, reason="no host compiler")
+def test_atomic_segment_and_segment_count_agree_with_doca_gpunetio(tmp_path):
+    hdr = _doca_header()
+    if hdr is None:
+        pytest.skip("the NCCL wheel in this image does not ship doca_gpunetio_verbs_def.h")
+    exe, r = _compile(tmp_path, ROOT / "rocnrdma_b200" / "csrc", hdr)
+    assert r.returncode == 0, r.stderr[-3000:]
+    assert subprocess.run([str(exe)], timeout=60).returncode == 0
+
+
+def test_the_atomic_crosscheck_can_fail(tmp_path):
+    """Negative control: swap the two fields of our atomic segment and the same translation unit must stop compiling."""
+    hdr = _doca_header()
+    if hdr is None or shutil.which("g++") is None:
+        pytest.skip("no independent header / compiler")
+    src = (ROOT / "rocnrdma_b200" / "csrc" / "wire" / "mlx5_wire.h").read_text()
+    old = "  uint64_t swap_add;             // be64\n  uint64_t compare;              // be64\n"
+    assert old in src
+    broken = src.replace(old, "  uint64_t compare;              // be64\n  uint64_t swap_add;             // be64\n", 1)
+    (tmp_path / "wire").mkdir()
+    (tmp_path / "wire" / "mlx5_wire.h").write_text(broken)
+    _, r = _compile(tmp_path, tmp_path, hdr)
+    assert r.returncode != 0 and "swap_add offset" in r.stderr
