@@ -8,8 +8,9 @@
 //   commit   a short ordered section (parse_seq turn): QP-error flush, receive-WQE
 //            matching for SEND / WRITE_IMM, publish resolved[w], arm the chunk ticket
 //   move     TMA bulk-copy pipeline (cp.async.bulk global->shared->global, one issuing
-//            thread, mbarrier-tracked, no LSU traffic); a multi-chunk WQE is offered to
-//            idle CTAs through a fetch-add ticket, its owner keeps drawing from it too
+//            thread fed by a chunk queue so it streams across chunk boundaries, mbarrier-tracked,
+//            no LSU traffic); a multi-chunk WQE is offered to idle CTAs through a fetch-add
+//            ticket, its owner keeps drawing from it too
 //   retire   strictly in order, warp-collective: one CAS on retire_word = (head << 1) | locked takes the
 //            per-QP lock and proves the turn, lane i publishes the mlx5 CQEs of WQE head + i
 // Large transfers fan out over every engine CTA (HBM / NVLink speed); small messages
@@ -38,7 +39,8 @@ constexpr int kThreads = 128;
 constexpr uint32_t kSub = 16384;        // bytes per TMA bulk transaction
 constexpr int kStages = 12;             // smem ring: 12 x 16 KiB
 // ring split: EngineCtl::stores_in_flight stages (default 4) may hold a TMA store that is still reading smem,
-// the others hold loads in flight (copy_bulk<kSif>)
+// the others hold loads in flight (move_chunks<kSif>)
+constexpr int kMaxSif = 8;             // largest stores_in_flight
 constexpr uint32_t kBulkMin = 4096;     // below this the generic path is as fast
 
 // ------------------------------------------------------------------ PTX helpers
@@ -144,73 +146,157 @@ __device__ __forceinline__ void cqe_tail(uint8_t* cqe, uint32_t log_n, unsigned 
 }
 
 // ------------------------------------------------------------------ chunk copy
+// An engine CTA is split by role.  Warp 0 is control: it finds, claims and parses work, hands bulk chunks to the mover
+// through a small queue and does each chunk's completion accounting.  One lane of warp 1 is the mover: it runs ONE TMA
+// pipeline over that queue, so the ring keeps streaming across chunk boundaries.  Warps 0, 2 and 3 run the generic
+// (unaligned / small) copies.
+constexpr int kQueue = 3;                // chunk descriptors between control and the mover
+constexpr uint32_t kQuitLen = 0xffffffffu;
+constexpr uint32_t kGenericThreads = kThreads - 32;   // warps 0, 2, 3
+
+struct Chunk { uint64_t src, dst; uint32_t len; };   // len == kQuitLen: the mover leaves
+struct Owed { QpDev* qp; unsigned long long w; uint32_t nch; };   // control's record of a queued chunk
+
 struct Smem {
   alignas(128) uint8_t ring[kStages][kSub];
-  alignas(8) uint64_t full[kStages];
-  // work descriptor broadcast from thread 0
-  uint64_t src, dst;
-  uint32_t len, nch;
-  int have_work;
-  uint32_t phase_bits;   // per-stage parity of the next wait
+  alignas(8) uint64_t full[kStages];     // ring stage landed (TMA complete_tx)
+  uint64_t qfull[kQueue];                // control -> mover: entry holds a chunk
+  uint64_t qdone[kQueue];                // mover -> control: that chunk is written and released at gpu scope; entry free
+  Chunk q[kQueue];
+  Owed owed[kQueue];                     // control only
+  uint32_t end[kQueue];                  // mover only: store groups committed up to and including the chunk's last
+  uint64_t gsrc, gdst;                   // generic copy, control -> warps 2, 3
+  uint32_t glen;
+  int gquit;
+  int mover_fatal;
 };
 
-// Bulk path: thread 0 keeps kStages - kSif loads and kSif stores in flight.
-// (With a single store in flight every 16 KiB step exposed the store's smem-read latency,
-// ~0.35 us, which capped a CTA near 45 GB/s.)  Requires 16-byte aligned src, dst and len.
+__device__ __forceinline__ void init_barriers(Smem& s) {
+  for (int i = 0; i < kStages; ++i) mbar_init(&s.full[i], 1);
+  for (int i = 0; i < kQueue; ++i) { mbar_init(&s.qfull[i], 1); mbar_init(&s.qdone[i], 1); }
+  s.gquit = 0;
+  s.mover_fatal = 0;
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+// Non-blocking probe (try_wait may suspend the thread for a while; a probe between other work must not).
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+  return ok != 0;
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {   // release at CTA scope
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void generic_bar() { asm volatile("bar.sync 1, %0;" ::"n"(kGenericThreads) : "memory"); }
+
+// The mover (one thread): kStages - kSif loads and kSif stores in flight, one store group per 16 KiB step.  (With a
+// single store in flight every step exposed the store's smem-read latency, ~0.35 us, which capped a CTA near 45 GB/s.)
+// Loads for the next queued chunk are issued as ring stages free up, while the current chunk's stores are still in
+// flight.  A chunk is written once kSif groups have been committed after its last store: that step waits for the full
+// completion (wait_group kSif) instead of the smem read, then takes the gpu-scope fence and reports the chunk to control
+// (mbarrier arrive: release at CTA scope).  When nothing more is queued the ring drains at once (wait_group 0), so a lone
+// chunk is not held back waiting for work.  Chunks need 16-byte aligned src, dst and len.  Returns false when a load
+// never landed (bad mapping: bounded, the SM is not wedged); true when control queued the quit entry.
 template <int kSif>
-__device__ __forceinline__ bool copy_bulk(Smem& s, uint64_t src, uint64_t dst, uint32_t len) {
-  const uint32_t nsub = (len + kSub - 1) / kSub;
-  uint32_t phase_bits = s.phase_bits;
-  constexpr int P = kStages - kSif;
-  auto sub_len = [&](uint32_t i) { return (i + 1 == nsub) ? (len - i * kSub) : kSub; };
-  uint32_t issued = 0;
-  for (; issued < nsub && issued < (uint32_t)P; ++issued) {
-    int st = issued % kStages;
-    mbar_expect_tx(&s.full[st], sub_len(issued));
-    bulk_g2s(s.ring[st], (const void*)(src + (uint64_t)issued * kSub), sub_len(issued), &s.full[st]);
-  }
-  for (uint32_t i = 0; i < nsub; ++i) {
-    int st = i % kStages;
-    if (!mbar_try_wait(&s.full[st], (phase_bits >> st) & 1u)) {
-      // bounded: a bulk load that never lands (bad mapping) must not wedge the SM
-      unsigned long long t0 = globaltimer_ns();
-      while (!mbar_try_wait(&s.full[st], (phase_bits >> st) & 1u)) {
-        if (globaltimer_ns() - t0 > 1000000000ull) { s.phase_bits = phase_bits; return false; }
+__device__ __noinline__ bool move_chunks(Smem& s) {
+  constexpr uint32_t P = kStages - kSif;
+  uint32_t ring_ph = 0, q_ph = 0;            // parity of the next wait, per ring stage / per queue entry
+  uint32_t n_ld = 0, n_st = 0;               // steps loaded / stored (= store groups committed)
+  uint32_t ld_limit = kStages;               // loads below this index have a free stage
+  int ld_stage = 0, st_stage = 0, e_ld = 0, e_st = 0, e_wr = 0;
+  uint32_t ld_off = 0, st_off = 0, ld_len = 0, st_len = 0;
+  uint64_t ld_src = 0, st_dst = 0;
+  int unwritten = 0;                         // chunks whose stores are all issued, not yet reported
+  bool ld_have = false, quit = false;
+  auto next_stage = [](int i) { return i + 1 == kStages ? 0 : i + 1; };
+  auto next_entry = [](int i) { return i + 1 == kQueue ? 0 : i + 1; };
+  auto report = [&](bool all) {
+    fence_gpu();   // the chunks' bytes (complete for this thread) at gpu scope before control counts them
+    do {
+      mbar_arrive(&s.qdone[e_wr]);
+      e_wr = next_entry(e_wr);
+    } while (--unwritten && (all || n_st - s.end[e_wr] >= (uint32_t)kSif));
+  };
+  for (;;) {
+    if (!ld_have && !quit) {
+      // idle (nothing in the ring, nothing owed): this wait may suspend; otherwise only probe
+      const bool idle = n_st == n_ld && unwritten == 0;
+      const uint32_t par = (q_ph >> e_ld) & 1u;
+      if (idle ? mbar_try_wait(&s.qfull[e_ld], par) : mbar_test_wait(&s.qfull[e_ld], par)) {
+        q_ph ^= 1u << e_ld;
+        ld_len = s.q[e_ld].len;
+        if (ld_len == kQuitLen) quit = true;
+        else { ld_have = true; ld_src = s.q[e_ld].src; ld_off = 0; }
       }
     }
-    phase_bits ^= 1u << st;
-    bulk_s2g((void*)(dst + (uint64_t)i * kSub), s.ring[st], sub_len(i));
-    bulk_commit();
-    if (issued < nsub) {
-      // the stage of load `issued` (= i + P) was last read by store i - kSif:
-      // stores i .. i - kSif + 1 may still be pending
-      bulk_wait_read<kSif>();
-      int ls = issued % kStages;
-      mbar_expect_tx(&s.full[ls], sub_len(issued));
-      bulk_g2s(s.ring[ls], (const void*)(src + (uint64_t)issued * kSub), sub_len(issued), &s.full[ls]);
-      ++issued;
+    while (ld_have && n_ld - n_st < P) {
+      if ((int32_t)(n_ld - ld_limit) >= 0) {
+        // the stage of load n_ld was last read by store n_ld - kStages <= n_st - 1 - kSif
+        bulk_wait_read<kSif>();
+        ld_limit = n_st + P;
+      }
+      const uint32_t len = ld_len - ld_off < kSub ? ld_len - ld_off : kSub;
+      mbar_expect_tx(&s.full[ld_stage], len);
+      bulk_g2s(s.ring[ld_stage], (const void*)(ld_src + ld_off), len, &s.full[ld_stage]);
+      ++n_ld;
+      ld_stage = next_stage(ld_stage);
+      ld_off += len;
+      if (ld_off == ld_len) { ld_have = false; e_ld = next_entry(e_ld); }
+    }
+    if (n_st != n_ld) {
+      const uint32_t par = (ring_ph >> st_stage) & 1u;
+      if (!mbar_try_wait(&s.full[st_stage], par)) {
+        const unsigned long long t0 = globaltimer_ns();
+        while (!mbar_try_wait(&s.full[st_stage], par))
+          if (globaltimer_ns() - t0 > 1000000000ull) return false;
+      }
+      ring_ph ^= 1u << st_stage;
+      if (st_off == 0) { st_dst = s.q[e_st].dst; st_len = s.q[e_st].len; }
+      const uint32_t len = st_len - st_off < kSub ? st_len - st_off : kSub;
+      bulk_s2g((void*)(st_dst + st_off), s.ring[st_stage], len);
+      bulk_commit();
+      ++n_st;
+      st_stage = next_stage(st_stage);
+      st_off += len;
+      if (st_off == st_len) { s.end[e_st] = n_st; e_st = next_entry(e_st); st_off = 0; ++unwritten; }
+      if (unwritten && n_st - s.end[e_wr] >= (uint32_t)kSif) {
+        bulk_wait<kSif>();   // this step only: every group but the last kSif has landed in global memory
+        ld_limit = n_st + P;
+        report(false);
+      }
+    } else if (unwritten && !ld_have) {
+      bulk_wait<0>();        // the queue ran dry: finish now
+      ld_limit = n_st + P;
+      report(true);
+    } else if (quit && !unwritten) {
+      return true;
     }
   }
-  bulk_wait_all();  // writes complete and visible to this thread
-  s.phase_bits = phase_bits;
-  return true;
 }
 
-// Generic path: any alignment, whole CTA.
-__device__ __forceinline__ void copy_generic(uint64_t src, uint64_t dst, uint32_t len) {
+// Generic path: any alignment; thread t of the n threads of warps 0, 2 and 3.
+__device__ __forceinline__ void copy_generic(uint64_t src, uint64_t dst, uint32_t len, uint32_t t, uint32_t n) {
   const uint8_t* s = (const uint8_t*)src;
   uint8_t* d = (uint8_t*)dst;
   if ((((src ^ dst) & 15) == 0) && len >= 64) {
     uint32_t head = (uint32_t)((16 - (src & 15)) & 15);
     if (head > len) head = len;
-    for (uint32_t i = threadIdx.x; i < head; i += kThreads) d[i] = s[i];
+    for (uint32_t i = t; i < head; i += n) d[i] = s[i];
     uint32_t body = (len - head) & ~15u;
     const uint4* s4 = (const uint4*)(s + head);
     uint4* d4 = (uint4*)(d + head);
-    for (uint32_t i = threadIdx.x; i < body / 16; i += kThreads) d4[i] = s4[i];
-    for (uint32_t i = head + body + threadIdx.x; i < len; i += kThreads) d[i] = s[i];
+    for (uint32_t i = t; i < body / 16; i += n) d4[i] = s4[i];
+    for (uint32_t i = head + body + t; i < len; i += n) d[i] = s[i];
   } else {
-    for (uint32_t i = threadIdx.x; i < len; i += kThreads) d[i] = s[i];
+    for (uint32_t i = t; i < len; i += n) d[i] = s[i];
   }
 }
 
@@ -749,21 +835,63 @@ __device__ __forceinline__ void claim_batch(EngineCtl* ctl, QpDev* qp, unsigned 
 }
 
 // ------------------------------------------------------------------ the kernel
+// Control, lane 0: has the mover reported queue entry e written?  With `block` it waits, bounded by the mover, which
+// reports every chunk or sets mover_fatal within its own bound.  1: written, 0: not yet, -1: the mover failed.
+__device__ __forceinline__ int chunk_written(Smem& s, int e, uint32_t& ph, bool block) {
+  for (;;) {
+    if (mbar_test_wait(&s.qdone[e], (ph >> e) & 1u)) { ph ^= 1u << e; return 1; }
+    if (*(volatile int*)&s.mover_fatal) return -1;
+    if (!block) return 0;
+  }
+}
+
+// Control, lane 0: a chunk's bytes are written and released at gpu scope by the threads that wrote them.  Count it;
+// true when that finished its WQE.
+__device__ __forceinline__ bool complete_chunk(QpDev* qp, unsigned long long w, uint32_t nch) {
+  Resolved* r = qp->resolved + (w & ((1u << qp->sq_log) - 1));
+  // This chunk's bytes before the count that may complete the WQE.  gpu scope is enough even
+  // when the CQ or the payload lives in host / peer memory: the retirer's system-scope
+  // fence in write_cqe() is cumulative over everything this chain of gpu-scope releases made
+  // visible to it (a sys fence per chunk cost ~2x on host-resident queues, measured).
+  if (nch > 1) fence_gpu();
+  if (nch == 1 || atomicAdd(&r->done, 1u) + 1 == nch) {
+    trace_stamp(qp, w, TR_COPIED);
+    fence_gpu();  // single chunk: its bytes before "finished"; else observe every other chunk's count -> their bytes precede our CQE
+    *(volatile unsigned long long*)&r->state = (w << 2) | 2ull;
+    __threadfence();  // SC: "finished" store before the retire try-lock (pairs with the unlock / re-check below)
+    return true;
+  }
+  return false;
+}
+
 __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
-  __shared__ Work work, next_work;   // next_work: the following chunk of the same WQE, drawn by a second thread while this one is copied
-  __shared__ int quit, next_valid;
   if (threadIdx.x == 0) {
-    next_valid = 0;
-    for (int i = 0; i < kStages; ++i) mbar_init(&s.full[i], 1);
-    s.phase_bits = 0;
-    quit = 0;
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    init_barriers(s);
     atomicAdd(&ctl->running_ctas, 1u);
     if (blockIdx.x == 0) ctl->t_start = globaltimer_ns();
   }
   __syncthreads();
+  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  if (warp == 1) {
+    if (lane == 0) {
+      const unsigned sif = ctl->stores_in_flight;
+      const bool ok = sif == 8 ? move_chunks<8>(s) : (sif == 6 ? move_chunks<6>(s) : move_chunks<4>(s));
+      if (!ok) { ctl->fatal = 1; *(volatile int*)&s.mover_fatal = 1; }
+    }
+    return;
+  }
+  if (warp != 0) {
+    // warps 2 and 3: the generic copies control hands out, until control leaves
+    for (;;) {
+      generic_bar();
+      if (s.gquit) return;
+      copy_generic(s.gsrc, s.gdst, s.glen, threadIdx.x - 32, kGenericThreads);
+      generic_bar();
+    }
+  }
+  // ---- warp 0: control.  Lane 0 finds the work; the warp parses batches and retires.
   unsigned long long last_activity = globaltimer_ns();
   uint32_t rr = blockIdx.x;
   unsigned spins = 0;
@@ -777,10 +905,40 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
   const bool host_watcher = blockIdx.x == gridDim.x - 1;
   uint32_t n_qps_cached = ctl->n_qps;
   unsigned iter = 0, rot = blockIdx.x;
+  // lane 0's side of the chunk queue: entries e_done .. e_done + outstanding - 1 are with the mover
+  int e_push = 0, e_done = 0, outstanding = 0;
+  uint32_t done_ph = 0;
+  bool fatal = false;
+  // A counted chunk that finished its WQE is retired by the whole warp (lane 0's arguments count).
+  auto finish = [&](QpDev* qp, unsigned long long w, uint32_t nch) {
+    const int fin = lane == 0 ? (int)complete_chunk(qp, w, nch) : 0;
+    if (__shfl_sync(0xffffffffu, fin, 0))
+      retire((QpDev*)__shfl_sync(0xffffffffu, (unsigned long long)qp, 0), lane, __shfl_sync(0xffffffffu, w, 0));
+  };
+  // Count every chunk the mover has written, oldest first; wait while the queue is full, or for all of them.
+  auto reap = [&](bool all) -> bool {   // false: the mover failed
+    for (;;) {
+      int got = 0;
+      if (lane == 0 && outstanding) got = chunk_written(s, e_done, done_ph, all || outstanding == kQueue);
+      got = __shfl_sync(0xffffffffu, got, 0);
+      if (got <= 0) return got == 0;
+      Owed o{};
+      if (lane == 0) {
+        o = s.owed[e_done];
+        e_done = e_done + 1 == kQueue ? 0 : e_done + 1;
+        --outstanding;
+      }
+      finish(o.qp, o.w, o.nch);
+    }
+  };
   for (;;) {
-    int batch_k = 0;
-    if (threadIdx.x == 0) {
-      s.have_work = 0;
+    if (!reap(false)) { fatal = true; break; }
+    int batch_k = 0, act = 0;   // act: -1 leave, 0 nothing, 1 queued for the mover, 2 generic copy, 3 nothing to move,
+                                // 4 queued, small: wait for it
+    Work work;
+    uint32_t nch = 0;
+    if (lane == 0) {
+      bool have = false, quit = false;
       // "everybody leaves" travels with the queue scan (its latency hides behind try_claim's loads); the QP
       // count is re-read every 64 iterations together with the fence that drops stale L1 lines, so host-side
       // updates (new QPs, reconnects) become visible within ~100 us without a dependent load per iteration
@@ -788,14 +946,10 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
       if ((iter++ & 63u) == 0) { fence_gpu(); n_qps_cached = ctl->n_qps; }
       const uint32_t n = n_qps_cached;
       bool pending = false;
-      if (next_valid) {              // drawn (and therefore owed) during the previous chunk's copy
-        work = next_work;
-        next_valid = 0;
-        s.have_work = 1;
-      } else if (sticky_qp) {
+      if (sticky_qp) {
         Resolved* sr = sticky_qp->resolved + (sticky_w & ((1u << sticky_qp->sq_log) - 1));
         // a successful draw is a claim that MUST be executed, whichever generation it names
-        if (draw_chunk(sticky_qp, sr, sticky_w, &work)) s.have_work = 1;
+        if (draw_chunk(sticky_qp, sr, sticky_w, &work)) have = true;
         else sticky_qp = nullptr;
       }
       // Every probe of a QP is at least one L2 round trip, so a CTA does not walk the whole table each
@@ -804,19 +958,21 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
       // still probed by many CTAs per round trip.  The host watcher keeps the full scan: it alone decides
       // "idle" / "drained" and it is the only one that reads host-resident doorbells.
       const uint32_t n_scan = host_watcher ? n : (n < 2 ? n : 2u);
-      for (uint32_t k = 0; k < n_scan && !s.have_work && !batch_k; ++k) {
+      for (uint32_t k = 0; k < n_scan && !have && !batch_k; ++k) {
         const uint32_t qi = (host_watcher || k == 0) ? (rr + k) % n : (rr + 1 + rot % (n - 1)) % n;
         QpDev* qp = *(QpDev* volatile*)&ctl->qps[qi];   // table grows while we run
         if (!qp) continue;
         const int got = try_claim(ctl, qp, &work, &pending, host_watcher);
-        if (got == 1) s.have_work = 1;
+        if (got == 1) have = true;
         else if (got == 2) { batch_k = (int)work.chunk; pending = true; }
         if (got) rr = qi;
       }
       ++rot;
-      if (s.have_work) {
+      if (have) {
+        uint32_t len;
+        uint64_t csrc, cdst;
         if (work.have_desc) {
-          s.len = work.len; s.src = work.src; s.dst = work.dst; s.nch = work.nch;
+          len = work.len; csrc = work.src; cdst = work.dst; nch = work.nch;
         } else {
           Resolved* r = work.qp->resolved + (work.w & ((1u << work.qp->sq_log) - 1));
           const uint4 f = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r) + 16);   // bytes | nchunks | imm | flags
@@ -824,110 +980,98 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
           const uint32_t chunk = *(volatile uint32_t*)&r->chunk;
           const uint64_t off = (uint64_t)work.chunk * chunk;
           const uint32_t bytes = f.x;
-          s.len = bytes == 0 ? 0 : (uint32_t)((bytes - off < chunk) ? (bytes - off) : chunk);
-          s.src = (((uint64_t)a.y << 32) | a.x) + off;
-          s.dst = (((uint64_t)a.w << 32) | a.z) + off;
-          s.nch = f.y;
+          len = bytes == 0 ? 0 : (uint32_t)((bytes - off < chunk) ? (bytes - off) : chunk);
+          csrc = (((uint64_t)a.y << 32) | a.x) + off;
+          cdst = (((uint64_t)a.w << 32) | a.z) + off;
+          nch = f.y;
         }
-        if (s.nch > 1) { sticky_qp = work.qp; sticky_w = work.w; }
+        if (nch > 1) { sticky_qp = work.qp; sticky_w = work.w; }
         last_activity = globaltimer_ns();
         spins = 0;
+        if (len == 0) {
+          act = 3;
+        } else if (len >= kBulkMin && (((csrc | cdst) & 15) == 0) && ((len & 15) == 0)) {
+          // reap() left room: outstanding < kQueue
+          s.q[e_push] = Chunk{csrc, cdst, len};
+          s.owed[e_push] = Owed{work.qp, work.w, nch};
+          mbar_arrive(&s.qfull[e_push]);
+          e_push = e_push + 1 == kQueue ? 0 : e_push + 1;
+          ++outstanding;
+          atomicAdd(&ctl->n_bulk_chunks, 1ull);
+          // A chunk the ring holds at once gains nothing from streaming; finishing it before the next scan keeps
+          // small-message latency what it was (a 4 KiB WQE otherwise waits for the scan to be counted).
+          act = len <= kSub * (kStages - kMaxSif) ? 4 : 1;
+        } else {
+          s.gsrc = csrc; s.gdst = cdst; s.glen = len;
+          act = 2;
+        }
       } else {
         ++spins;
         // The host watcher is the only CTA that sees host-resident doorbells, so it alone may declare
         // the engine idle or drained; everybody else follows quit_all.
         if (pending) last_activity = globaltimer_ns();
-        else if (host_watcher && ctl->oneshot && spins > 4) { quit = 1; ctl->quit_all = 1; }   // drained: every posted WQE has retired
-        if (quit_all_seen) quit = 1;
+        else if (host_watcher && ctl->oneshot && spins > 4) { quit = true; ctl->quit_all = 1; }   // drained: every posted WQE has retired
+        if (quit_all_seen) quit = true;
         if ((spins & 63) == 0) {
-          if (*ctl->stop) quit = 1;   // mapped host word: a PCIe read, hence only every 64 idle spins
-          else if (host_watcher && globaltimer_ns() - last_activity > ctl->idle_timeout_ns) { quit = 1; ctl->exited_idle = 1; ctl->quit_all = 1; }
+          if (*ctl->stop) quit = true;   // mapped host word: a PCIe read, hence only every 64 idle spins
+          else if (host_watcher && globaltimer_ns() - last_activity > ctl->idle_timeout_ns) { quit = true; ctl->exited_idle = 1; ctl->quit_all = 1; }
         }
         if (spins > 256) __nanosleep(200);
+        if (quit) act = -1;
       }
     }
-    if (threadIdx.x < 32) {
-      // a batch claim is parsed by the whole first warp; its chunks are then drawn like anybody else's
-      batch_k = __shfl_sync(0xffffffffu, batch_k, 0);
-      if (batch_k) {
-        // only lane 0 reads the (shared-memory) work record it wrote; the other lanes' operand is ignored by the shuffle
-        unsigned long long wq0 = 0, ww0 = 0;
-        if (threadIdx.x == 0) { wq0 = (unsigned long long)*(QpDev* volatile*)&work.qp; ww0 = *(volatile unsigned long long*)&work.w; }
-        QpDev* bqp = (QpDev*)__shfl_sync(0xffffffffu, wq0, 0);
-        unsigned long long bw = __shfl_sync(0xffffffffu, ww0, 0);
-        claim_batch(ctl, bqp, bw, (uint32_t)batch_k, threadIdx.x);
-      }
+    // a batch claim is parsed by the whole warp; its chunks are then drawn like anybody else's
+    batch_k = __shfl_sync(0xffffffffu, batch_k, 0);
+    if (batch_k) {
+      QpDev* bqp = (QpDev*)__shfl_sync(0xffffffffu, (unsigned long long)work.qp, 0);
+      claim_batch(ctl, bqp, __shfl_sync(0xffffffffu, work.w, 0), (uint32_t)batch_k, lane);
     }
-    __syncthreads();
-    const int q = quit, hw = s.have_work;
-    const uint32_t len = s.len;
-    const uint64_t csrc = s.src, cdst = s.dst;
-    __syncthreads();  // every thread holds the broadcast in registers before thread 0 reuses smem
-    if (q) break;
-    if (!hw) continue;
-    if (len > 0) {
-      const bool bulk = len >= kBulkMin && (((csrc | cdst) & 15) == 0) && ((len & 15) == 0);
-      if (bulk && threadIdx.x == 32 && s.nch > 1) {
-        // While thread 0 runs the copy pipeline, draw the NEXT chunk of the same WQE and fetch its descriptor:
-        // takes the ticket round trips, the fence and the descriptor loads (~2 us) off the per-chunk path.
-        Work nw;
-        if (draw_chunk(work.qp, work.qp->resolved + (work.w & ((1u << work.qp->sq_log) - 1)), work.w, &nw)) {
-          Resolved* r2 = nw.qp->resolved + (nw.w & ((1u << nw.qp->sq_log) - 1));   // the ticket names its own WQE
-          const uint4 f = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r2) + 16);
-          const uint4 a = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r2));
-          const uint32_t chunk = *(volatile uint32_t*)&r2->chunk;
-          const uint64_t off = (uint64_t)nw.chunk * chunk;
-          nw.have_desc = 1;
-          nw.len = f.x == 0 ? 0 : (uint32_t)((f.x - off < chunk) ? (f.x - off) : chunk);
-          nw.src = (((uint64_t)a.y << 32) | a.x) + off;
-          nw.dst = (((uint64_t)a.w << 32) | a.z) + off;
-          nw.nch = f.y;
-          next_work = nw;
-          next_valid = 1;
-        }
-      }
-      if (bulk) {
-        if (threadIdx.x == 0) {
-          const unsigned sif = ctl->stores_in_flight;
-          const bool okc = sif == 8 ? copy_bulk<8>(s, csrc, cdst, len) : (sif == 6 ? copy_bulk<6>(s, csrc, cdst, len) : copy_bulk<4>(s, csrc, cdst, len));
-          if (!okc) { ctl->fatal = 1; quit = 1; }
-          atomicAdd(&ctl->n_bulk_chunks, 1ull);
-        }
-      } else {
-        copy_generic(csrc, cdst, len);
-      }
+    act = __shfl_sync(0xffffffffu, act, 0);
+    if (act < 0) break;
+    if (act == 2) {
+      generic_bar();
+      copy_generic(s.gsrc, s.gdst, s.glen, lane, kGenericThreads);
+      generic_bar();   // every generic thread's stores before lane 0's release in complete_chunk
     }
-    __syncthreads();
-    if (quit) break;   // fatal DMA fault: leave without completing (host sees ctl->fatal)
-    int finished = 0;
-    if (threadIdx.x == 0) {
-      QpDev* qp = work.qp;
-      Resolved* r = qp->resolved + (work.w & ((1u << qp->sq_log) - 1));
-      // This chunk's bytes before the count that may complete the WQE.  gpu scope is enough even
-      // when the CQ or the payload lives in host / peer memory: the retirer's system-scope
-      // fence in write_cqe() is cumulative over everything this chain of gpu-scope releases made
-      // visible to it (a sys fence per chunk cost ~2x on host-resident queues, measured).
-      const uint32_t nch = s.nch;
-      if (nch > 1) fence_gpu();   // this chunk's bytes before the count that may complete the WQE
-      if (nch == 1 || atomicAdd(&r->done, 1u) + 1 == nch) {
-        trace_stamp(qp, work.w, TR_COPIED);
-        fence_gpu();  // single chunk: its bytes before "finished"; else observe every other chunk's count -> their bytes precede our CQE
-        *(volatile unsigned long long*)&r->state = (work.w << 2) | 2ull;
-        __threadfence();  // SC: "finished" store before the retire try-lock (pairs with the unlock / re-check below)
-        finished = 1;
-      }
-    }
-    if (threadIdx.x < 32) {
-      if (__shfl_sync(0xffffffffu, finished, 0)) {
-        unsigned long long wq0 = 0, ww0 = 0;
-        if (threadIdx.x == 0) { wq0 = (unsigned long long)*(QpDev* volatile*)&work.qp; ww0 = *(volatile unsigned long long*)&work.w; }
-        retire((QpDev*)__shfl_sync(0xffffffffu, wq0, 0), threadIdx.x, ww0);
-      }
-    }
+    if (act == 4 && !reap(true)) { fatal = true; break; }
+    if (act == 2 || act == 3) finish(work.qp, work.w, nch);
   }
-  if (threadIdx.x == 0) {
+  // Leaving.  Every chunk handed to the mover is a claim that must be completed; after a mover fault nothing is
+  // completed (the host sees ctl->fatal).
+  if (!fatal && !reap(true)) fatal = true;
+  if (lane == 0) {
+    if (!fatal) {
+      s.q[e_push].len = kQuitLen;
+      mbar_arrive(&s.qfull[e_push]);
+    }
+    s.gquit = 1;
+  }
+  generic_bar();
+  if (lane == 0) {
     if (blockIdx.x == 0) ctl->t_exit = globaltimer_ns();
     atomicSub(&ctl->running_ctas, 1u);
+  }
+}
+
+// ------------------------------------------------------------------ ceiling
+// What the engine's copy loop reaches with nothing around it: CTA b streams span bytes from src + b * span to
+// dst + b * span as ONE queued chunk -- no claims, no chunk boundaries, no completion bookkeeping.  The distance between
+// this and the engine on the same CTA count is what the per-chunk work costs (tools/engine_pipeline.py).
+__global__ void __launch_bounds__(kThreads, 1) engine_ceiling_kernel(uint64_t src, uint64_t dst, uint32_t span, unsigned sif,
+                                                                    unsigned int* fatal) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  Smem& s = *reinterpret_cast<Smem*>(smem_raw);
+  if (threadIdx.x == 0) init_barriers(s);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const uint64_t off = (uint64_t)blockIdx.x * span;
+    s.q[0] = Chunk{src + off, dst + off, span};
+    mbar_arrive(&s.qfull[0]);
+    s.q[1].len = kQuitLen;
+    mbar_arrive(&s.qfull[1]);
+  } else if (threadIdx.x == 32) {
+    const bool ok = sif == 8 ? move_chunks<8>(s) : (sif == 6 ? move_chunks<6>(s) : move_chunks<4>(s));
+    if (!ok && fatal) atomicAdd(fatal, 1u);
   }
 }
 

@@ -159,6 +159,7 @@ void rn_preload_gemm_mx() __attribute__((weak));
 static void preload_all_kernels() {
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, eng::engine_kernel);
+  cudaFuncGetAttributes(&a, eng::engine_ceiling_kernel);
   if (rn_preload_rdma_ops) rn_preload_rdma_ops();
   if (rn_preload_pack) rn_preload_pack();
   if (rn_preload_gemm) rn_preload_gemm();
@@ -1009,6 +1010,22 @@ RN_API int rn_engine_stop(void* hca) {
   *h->h_stop = 0;
   h->engine_launched = false;
   if (e != cudaSuccess) return fail(-5, "engine stop: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+// The engine's copy loop alone on `ctas` CTAs (eng::engine_ceiling_kernel): CTA b copies span bytes at offset b * span.
+// src, dst and span must be 16-byte aligned.  fatal_dev (device u32, may be 0) counts CTAs whose loads never landed.
+RN_API int rn_k_engine_ceiling(uint64_t stream, uint64_t src, uint64_t dst, uint64_t span, int ctas, uint64_t fatal_dev) {
+  if (ctas <= 0 || !span || span > 0xffffffffull || ((src | dst | span) & 15))
+    return fail(-22, "engine_ceiling: need ctas > 0 and a 16-byte aligned span below 4 GiB");
+  const size_t smem = eng::engine_smem_bytes();
+  CU_OK(cudaFuncSetAttribute(eng::engine_ceiling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const char* e = getenv("RN_ENGINE_STORES_IN_FLIGHT");
+  const int v = e ? atoi(e) : 0;
+  const unsigned sif = (v == 4 || v == 6 || v == 8) ? (unsigned)v : 4u;
+  eng::engine_ceiling_kernel<<<ctas, eng::kThreads, smem, (cudaStream_t)stream>>>(src, dst, (uint32_t)span, sif,
+                                                                                  (unsigned int*)fatal_dev);
+  CU_OK(cudaGetLastError());
   return 0;
 }
 
