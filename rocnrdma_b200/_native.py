@@ -95,6 +95,7 @@ _SIGS = {
     "rn_post_send": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, C.POINTER(u64)]),
     "rn_post_recv": (i32, [vp, u64, u32, u32]),
     "rn_post_atomic": (i32, [vp, u32, u64, u32, u64, u32, u64, u64, u32, C.POINTER(u64)]),
+    "rn_post_inline": (i32, [vp, u32, u64, u32, vp, u32, u32, u32, C.POINTER(u64)]),
     "rn_hca_host_native_atomics": (i32, [vp]),
     "rn_host_stream": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, u64, u32, u64, C.POINTER(u64), C.POINTER(u32)]),
     "rn_host_staged_stream": (i32, [vp, u64, u64, u64, u32, u64, u32, u32, u32, u64, u32, u64, C.POINTER(u64)]),
@@ -132,9 +133,13 @@ _SIGS = {
     "rn_wire_decode_cqe": (i32, [C.POINTER(u8), C.POINTER(RnWc)]),
     "rn_wire_build_atomic_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, u64, u32, u64, u64, u32]),
     "rn_wire_decode_wqe": (i32, [C.POINTER(u8), C.POINTER(u64)]),
+    "rn_wire_build_inline_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, C.POINTER(u8), u32, u32, u32]),
+    "rn_wire_decode_wqe_inline": (i32, [C.POINTER(u8), C.POINTER(u64)]),
     "rn_k_atomic_stream": (i32, [u64, C.POINTER(u64), u32, u32, u32, u64, u32, u64, u64, u32, u64, u64, u64, u32, u32, u32, u32, u64, u64]),
     "rn_k_put_signal": (i32, [u64, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32, u32, u64, u64]),
     "rn_k_signal_wait": (i32, [u64, u64, u64, u64, u64, u64, u64, u64, u64, u64]),
+    "rn_k_put_inline": (i32, [u64, C.POINTER(u64), u32, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32,
+                              u32, u32, u32, u64, u64]),
     "rn_gpu_page_size": (u64, []),
     "rn_dmabuf_export": (i32, [u64, u64, C.POINTER(i32)]),
     "rn_dmabuf_close": (i32, [i32]),
@@ -190,6 +195,8 @@ _SIGS = {
     "rn_verbs_post_send": (i32, [vp, u32, u64, u32, u64, u32, u32, i32, u32, C.POINTER(u64)]),
     "rn_verbs_post_recv": (i32, [vp, u64, u32, u32, C.POINTER(u64)]),
     "rn_verbs_post_atomic": (i32, [vp, u32, u64, u32, u64, u32, u64, u64, i32, C.POINTER(u64)]),
+    "rn_verbs_post_inline": (i32, [vp, u32, u64, u32, vp, u32, i32, u32, C.POINTER(u64)]),
+    "rn_verbs_qp_max_inline": (u32, [vp]),
     "rn_verbs_poll": (i32, [vp, i32, C.POINTER(RnVWc)]),
     "rn_verbs_host_stream": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, u64, u32, u64, C.POINTER(u64), C.POINTER(u32)]),
     "rn_verbs_host_staged_stream": (i32, [vp, u64, u64, u64, u32, u64, u32, u32, u32, u64, u32, u64, C.POINTER(u64)]),

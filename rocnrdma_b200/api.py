@@ -66,6 +66,19 @@ def _ptr_len(buf, nbytes=None):
     raise TypeError(f"cannot take the address of {type(buf)!r}")
 
 
+def _inline_bytes(data, limit: int) -> bytes:
+    """The payload of an inline post: ``bytes``-like, or a CPU tensor (its raw bytes); 1..``limit`` bytes."""
+    if hasattr(data, "data_ptr"):
+        import torch
+        if data.device.type != "cpu":
+            raise ValueError("inline data must be host bytes or a CPU tensor (device values: ops.put_inline)")
+        data = data.contiguous().reshape(-1).view(torch.uint8).numpy()
+    b = bytes(memoryview(data).cast("B"))
+    if not 1 <= len(b) <= limit:
+        raise ValueError(f"inline payload of {len(b)} bytes; inline carries 1..{limit}")
+    return b
+
+
 @dataclass
 class WorkCompletion:
     qpn: int
@@ -281,6 +294,32 @@ class QueuePair:
         WQE index."""
         return self._post_atomic(W.OP_ATOMIC_CS, local, remote, swap, compare, local_off, remote_off, signaled)
 
+    @property
+    def max_inline(self) -> int:
+        """Largest payload an inline work request carries: 28 bytes (one 64-byte WQEBB)."""
+        return W.MAX_INLINE
+
+    def _post_inline(self, opcode, raddr, rkey, buf: bytes, signaled, imm) -> int:
+        idx = C.c_uint64()
+        self.ctx.sweep_revoked()
+        N.check(self.ctx._lib.rn_post_inline(self._q, opcode, raddr, rkey, C.create_string_buffer(buf, len(buf)), len(buf),
+                                             W.CTRL_CQ_UPDATE if signaled else 0, imm, C.byref(idx)), "post_inline")
+        return idx.value
+
+    def post_write_inline(self, dst: MemoryRegion, data, dst_off=0, signaled=True, imm=None) -> int:
+        """Inline RDMA WRITE (``imm`` not None: WRITE_WITH_IMM) of ``data`` -- ``bytes``-like or a CPU tensor, 1 to
+        ``max_inline`` bytes -- to ``dst.addr + dst_off``.  The payload is copied into the work request itself: no local
+        memory region, and ``data`` may change as soon as this returns.  Returns the WQE index."""
+        buf = _inline_bytes(data, self.max_inline)
+        op = W.OP_RDMA_WRITE if imm is None else W.OP_RDMA_WRITE_IMM
+        return self._post_inline(op, dst.addr + dst_off, dst.rkey, buf, signaled, imm or 0)
+
+    def post_send_inline(self, data, signaled=True, imm=None) -> int:
+        """Inline SEND (``imm`` not None: SEND_WITH_IMM) of 1 to ``max_inline`` bytes; lands in the responder's next receive
+        buffer.  Returns the WQE index."""
+        buf = _inline_bytes(data, self.max_inline)
+        return self._post_inline(W.OP_SEND if imm is None else W.OP_SEND_IMM, 0, 0, buf, signaled, imm or 0)
+
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
         """Post one receive buffer (consumed in order by SEND / WRITE_WITH_IMM)."""
         n = dst.length - off if nbytes is None else nbytes
@@ -413,6 +452,17 @@ class VerbsQueuePair(QueuePair):
                                                         remote.addr + remote_off, remote.rkey, swap_add & 0xFFFFFFFFFFFFFFFF,
                                                         compare & 0xFFFFFFFFFFFFFFFF, int(bool(signaled)), C.byref(wr)),
                      "post_atomic")
+        return wr.value
+
+    @property
+    def max_inline(self) -> int:
+        """The inline capacity the provider granted, capped at 28 bytes (one WQEBB)."""
+        return min(W.MAX_INLINE, self.ctx._lib.rn_verbs_qp_max_inline(self._vq))
+
+    def _post_inline(self, opcode, raddr, rkey, buf: bytes, signaled, imm) -> int:
+        wr = C.c_uint64()
+        self._vcheck(self.ctx._lib.rn_verbs_post_inline(self._vq, opcode, raddr, rkey, C.create_string_buffer(buf, len(buf)),
+                                                        len(buf), int(bool(signaled)), imm, C.byref(wr)), "post_inline")
         return wr.value
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):

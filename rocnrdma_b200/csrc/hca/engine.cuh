@@ -351,6 +351,13 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
       case OP_NOP: v.bytes = 0; break;
       case OP_RDMA_WRITE:
       case OP_RDMA_WRITE_IMM: {
+        if (v.inl_off) {
+          // Inline: only the remote key is checked, and the source is the payload in this SQ slot.  It is read after
+          // commit (a flushed WQE copies nothing), and the slot is not reused before the WQE retires (DESIGN.md 3.1).
+          p->dst = translate(qp->r.rkeys, qp->r.n_rkeys, v.rkey, v.raddr, v.bytes, ACC_REMOTE_WRITE, true, &p->syn);
+          if (p->dst) p->src = (uint64_t)(slot + v.inl_off);
+          break;
+        }
         const MKeyRaw lk = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey), rk = mkey_load(qp->r.rkeys, qp->r.n_rkeys, v.rkey);
         p->src = mkey_check(lk, v.lkey, v.laddr, v.bytes, 0, false, &p->syn);
         if (p->src) p->dst = mkey_check(rk, v.rkey, v.raddr, v.bytes, ACC_REMOTE_WRITE, true, &p->syn);
@@ -364,7 +371,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
       }
       case OP_SEND:
       case OP_SEND_IMM:
-        p->src = translate(qp->lkeys, qp->n_lkeys, v.lkey, v.laddr, v.bytes, 0, false, &p->syn);
+        p->src = v.inl_off ? (uint64_t)(slot + v.inl_off) : translate(qp->lkeys, qp->n_lkeys, v.lkey, v.laddr, v.bytes, 0, false, &p->syn);
         break;
       case OP_ATOMIC_CS:
       case OP_ATOMIC_FA: parse_atomic(ctl, qp, p); break;

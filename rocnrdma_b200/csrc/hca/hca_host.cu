@@ -906,6 +906,22 @@ RN_API int rn_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lk
   return host_sq_publish(q, w, idx, idx_out);
 }
 
+// Host-posted inline WRITE / WRITE_IMM / SEND / SEND_IMM: the n (1..MAX_INLINE) bytes at `data` (host memory) are copied
+// into the WQE, so the caller may reuse them as soon as this returns.  raddr / rkey are ignored for SEND.
+RN_API int rn_post_inline(void* qp, uint32_t opcode, uint64_t raddr, uint32_t rkey, const void* data, uint32_t n,
+                          uint32_t flags, uint32_t imm, uint64_t* idx_out) {
+  Qp* q = (Qp*)qp;
+  if (opcode != OP_RDMA_WRITE && opcode != OP_RDMA_WRITE_IMM && opcode != OP_SEND && opcode != OP_SEND_IMM)
+    return fail(-22, "post_inline: opcode 0x%x cannot carry inline data", opcode);
+  if (n == 0 || n > MAX_INLINE) return fail(-22, "post_inline: %u bytes (inline carries 1..%u)", n, (unsigned)MAX_INLINE);
+  uint64_t idx = 0;
+  int rc = host_sq_slot(q, "post_inline", &idx);
+  if (rc) return rc;
+  Wqe64 w;
+  build_inline_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, raddr, rkey, data, n, (uint8_t)flags, imm);
+  return host_sq_publish(q, w, idx, idx_out);
+}
+
 RN_API int rn_post_recv(void* qp, uint64_t addr, uint32_t lkey, uint32_t bytes) {
   Qp* q = (Qp*)qp;
   cudaSetDevice(q->hca->dev);
@@ -1071,6 +1087,23 @@ RN_API int rn_wire_decode_wqe(const uint8_t* wqe64, uint64_t* out13) {
   const uint64_t f[13] = {v.opcode, v.wqe_idx, v.qpn, v.ds, v.fm_ce_se, v.imm, v.raddr, v.rkey, v.laddr, v.lkey, v.bytes,
                           v.swap_add, v.compare};
   memcpy(out13, f, sizeof f);
+  return ok ? 1 : 0;
+}
+RN_API void rn_wire_build_inline_wqe(uint8_t* out64, uint32_t opcode, uint32_t idx, uint32_t qpn, uint64_t raddr, uint32_t rkey,
+                                     const uint8_t* data, uint32_t n, uint32_t flags, uint32_t imm) {
+  Wqe64 w;
+  build_inline_wqe(&w, (uint8_t)opcode, (uint16_t)idx, qpn, raddr, rkey, data, n, (uint8_t)flags, imm);
+  memcpy(out64, &w, 64);
+}
+// rn_wire_decode_wqe's 13 fields, then: 1 when the WQE carries its payload inline, and the payload's offset in the WQEBB.
+RN_API int rn_wire_decode_wqe_inline(const uint8_t* wqe64, uint64_t* out15) {
+  Wqe64 w;
+  memcpy(&w, wqe64, 64);
+  WqeView v;
+  const bool ok = decode_wqe(&w, &v);
+  const uint64_t f[15] = {v.opcode, v.wqe_idx, v.qpn, v.ds, v.fm_ce_se, v.imm, v.raddr, v.rkey, v.laddr, v.lkey, v.bytes,
+                          v.swap_add, v.compare, v.inl_off != 0, v.inl_off};
+  memcpy(out15, f, sizeof f);
   return ok ? 1 : 0;
 }
 RN_API int rn_wire_decode_cqe(const uint8_t* cqe64, RnWc* out) {

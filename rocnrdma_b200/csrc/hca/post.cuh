@@ -142,6 +142,56 @@ __device__ __forceinline__ void write_atomic_wqe(QpDev* qp, unsigned long long i
                     swap_add, compare, fm_ce_se);
 }
 
+// Inline payload held in registers: up to MAX_INLINE bytes in memory order (little-endian words), zero past its length.
+struct InlinePayload { uint32_t w[7]; };
+static_assert(sizeof(InlinePayload) == MAX_INLINE, "inline payload");
+
+// Read n (1..MAX_INLINE) bytes at p into registers.  Any address works (the memory need not be registered); word loads
+// when p and n are 4-byte multiples, byte loads otherwise -- nothing past p + n is read.
+__device__ __forceinline__ InlinePayload inline_load(const void* p, uint32_t n) {
+  InlinePayload d;
+  const uint8_t* b = static_cast<const uint8_t*>(p);
+  if ((((uintptr_t)b | n) & 3u) == 0) {
+#pragma unroll
+    for (uint32_t j = 0; j < 7; ++j) d.w[j] = 4 * j < n ? reinterpret_cast<const uint32_t*>(b)[j] : 0u;
+  } else {
+#pragma unroll
+    for (uint32_t j = 0; j < 7; ++j) {
+      uint32_t x = 0;
+#pragma unroll
+      for (uint32_t k = 0; k < 4; ++k)
+        if (4 * j + k < n) x |= (uint32_t)b[4 * j + k] << (8 * k);
+      d.w[j] = x;
+    }
+  }
+  return d;
+}
+
+// Inline WQE (n in 1..MAX_INLINE), the bytes build_inline_wqe writes.  RDMA_WRITE / WRITE_IMM: ctrl | raddr | be32
+// (n | INLINE_SEG) and the payload from byte 36; SEND / SEND_IMM: ctrl | inline header and the payload from byte 20.
+__device__ __forceinline__ void inline_wqe_stores(uint8_t* slot, uint16_t idx, uint32_t qpn, uint8_t opcode, uint64_t raddr,
+                                                  uint32_t rkey, const InlinePayload& d, uint32_t n, uint8_t fm_ce_se,
+                                                  uint32_t imm) {
+  const uint32_t hdr = be32(n | INLINE_SEG);
+  if (opcode == OP_SEND || opcode == OP_SEND_IMM) {
+    st_v4(slot + 0, ctrl_word0(opcode, idx), ctrl_word1(qpn, 1 + inline_segs(n)), (uint32_t)fm_ce_se << 24, be32(imm));
+    st_v4(slot + 16, hdr, d.w[0], d.w[1], d.w[2]);
+    st_v4(slot + 32, d.w[3], d.w[4], d.w[5], d.w[6]);
+    st_v4(slot + 48, 0u, 0u, 0u, 0u);
+  } else {
+    st_v4(slot + 0, ctrl_word0(opcode, idx), ctrl_word1(qpn, 2 + inline_segs(n)), (uint32_t)fm_ce_se << 24, be32(imm));
+    st_v4(slot + 16, be32((uint32_t)(raddr >> 32)), be32((uint32_t)raddr), be32(rkey), 0u);
+    st_v4(slot + 32, hdr, d.w[0], d.w[1], d.w[2]);
+    st_v4(slot + 48, d.w[3], d.w[4], d.w[5], d.w[6]);
+  }
+}
+__device__ __forceinline__ void write_inline_wqe(QpDev* qp, unsigned long long idx, uint8_t opcode, uint64_t raddr,
+                                                 uint32_t rkey, const InlinePayload& d, uint32_t n, uint8_t fm_ce_se,
+                                                 uint32_t imm = 0) {
+  inline_wqe_stores(qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6), (uint16_t)idx, qp->qpn, opcode, raddr, rkey, d, n,
+                    fm_ce_se, imm);
+}
+
 // -------------------------------------------------------------- doorbell
 // Publish WQEs [idx, idx+n): in index order, update the doorbell record, then ring
 // the doorbell register with the first 8 bytes of the last WQE's ctrl segment.
@@ -409,6 +459,11 @@ __device__ __forceinline__ void poster_build_atomic(const Poster& p, unsigned lo
   atomic_wqe_stores(poster_slot(p, idx), ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(p.qpn, 4), opcode, laddr, lkey, raddr,
                     rkey, swap_add, compare, fm_ce_se);
 }
+__device__ __forceinline__ void poster_build_inline(const Poster& p, unsigned long long idx, uint8_t opcode, uint64_t raddr,
+                                                    uint32_t rkey, const InlinePayload& d, uint32_t n, uint8_t fm_ce_se,
+                                                    uint32_t imm = 0) {
+  inline_wqe_stores(poster_slot(p, idx), (uint16_t)idx, p.qpn, opcode, raddr, rkey, d, n, fm_ce_se, imm);
+}
 // Ring ONE doorbell for everything built in [p.head, to): record, release, register.
 __device__ __forceinline__ void poster_ring(Poster& p, unsigned long long to) {
   const unsigned long long last = to - 1;
@@ -469,6 +524,31 @@ __device__ __forceinline__ unsigned long long rdma_cmp_swap(QpDev* qp, uint64_t 
   write_atomic_wqe(qp, idx, OP_ATOMIC_CS, laddr, lkey, raddr, rkey, swap, compare, signaled ? CTRL_CQ_UPDATE : 0);
   if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
   return idx;
+}
+
+// Inline puts through the shared submit: an RDMA WRITE whose 1..MAX_INLINE payload bytes travel in the WQE.  No local
+// buffer and no lkey: `data` may be any memory the calling thread can read (or a register, with rdma_p), and it may be
+// reused as soon as the call returns.  Returns the WQE index, or ~0ull when n is out of range or the queue stayed full.
+__device__ __forceinline__ unsigned long long rdma_put_inline_regs(QpDev* qp, uint64_t raddr, uint32_t rkey,
+                                                                   const InlinePayload& d, uint32_t n, bool signaled) {
+  unsigned long long idx = sq_reserve(qp, 1);
+  if (idx == ~0ull) return idx;
+  write_inline_wqe(qp, idx, OP_RDMA_WRITE, raddr, rkey, d, n, signaled ? CTRL_CQ_UPDATE : 0);
+  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
+  return idx;
+}
+__device__ __forceinline__ unsigned long long rdma_put_inline(QpDev* qp, uint64_t raddr, uint32_t rkey, const void* data,
+                                                              uint32_t n, bool signaled = true) {
+  if (n == 0 || n > MAX_INLINE) return ~0ull;
+  return rdma_put_inline_regs(qp, raddr, rkey, inline_load(data, n), n, signaled);
+}
+// nvshmem_p / doca_gpu_dev_verbs_p: one 1-, 2-, 4- or 8-byte value straight from a register.
+template <typename T>
+__device__ __forceinline__ unsigned long long rdma_p(QpDev* qp, uint64_t raddr, uint32_t rkey, T value, bool signaled = true) {
+  static_assert(sizeof(T) == 1 || sizeof(T) == 2 || sizeof(T) == 4 || sizeof(T) == 8, "rdma_p: 1, 2, 4 or 8 bytes");
+  InlinePayload d = {};
+  memcpy(d.w, &value, sizeof(T));
+  return rdma_put_inline_regs(qp, raddr, rkey, d, (uint32_t)sizeof(T), signaled);
 }
 
 // Post one receive WQE on the QP's own RQ (single poster per RQ).

@@ -404,6 +404,115 @@ RN_API int rn_k_put_signal(uint64_t stream, uint64_t qp_dev, uint64_t src, uint3
   return (int)cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- inline puts (DOCA p / p_signal, nvshmem_p)
+// One warp per QP, windowed and bursted like rdma_stream_kernel.  Message i of CTA c (m = c * iters + i) is an inline
+// RDMA WRITE of nbytes (1..MAX_INLINE) read into registers from row m % rows of `values` -- plain device memory, never
+// registered -- to dst + (m % nslots) * slot_stride.  With a signal word (sig != 0) each message is that WRITE plus a
+// FETCH_AND_ADD of `add` on sig + c * 8, built by two lanes (window and burst then count messages, 2 WQEs each); the
+// engine executes the atomic only after the WRITE has landed, so ops.signal_wait works unchanged on the receiver.
+struct PutInlineArgs {
+  QpDev* qps[kMaxStreamQps];
+  const uint8_t* values;
+  uint64_t row_bytes;
+  uint32_t rows, nbytes;
+  uint64_t dst, slot_stride;
+  uint32_t rkey, nslots;
+  uint64_t sig, fetch, add;           // sig == 0: plain inline puts
+  uint32_t sig_rkey, fetch_lkey, fetch_slots;
+  uint32_t iters, window, signal_every, burst;
+  uint64_t timeout_ns;
+  unsigned long long* out;            // per CTA: [status, t_start, t_end, done, first_idx, last_idx, cons, 0]
+};
+
+__global__ void __launch_bounds__(32, 1) put_inline_kernel(PutInlineArgs a) {
+  const uint32_t lane = threadIdx.x;
+  QpDev* qp = a.qps[blockIdx.x];
+  unsigned long long* out = a.out + (size_t)blockIdx.x * 8;
+  const uint32_t k = a.sig ? 2u : 1u;                 // WQEs per message
+  const uint64_t sig = a.sig + (uint64_t)blockIdx.x * 8;
+  const uint32_t m0 = blockIdx.x * a.iters;
+  int status = WAIT_OK;
+  unsigned long long first = ~0ull, last = 0;
+  uint32_t done = 0;                                  // messages
+  Poster p = poster_open(qp);
+  if (qp->state == QPS_ERR) status = WAIT_QP_ERROR;
+  const unsigned long long t0 = globaltimer_ns();
+  while (done < a.iters && status != WAIT_QP_ERROR) {
+    const uint32_t n = min(a.burst, a.iters - done);
+    unsigned long long idx = 0;
+    int rc = WAIT_OK;
+    if (lane == 0) {
+      // leaves <= window - n messages outstanding: the last WQE of message done + n - window - 1 has completed
+      if (a.window && done + n > a.window) rc = poster_wait(p, last + (unsigned long long)k * n - (unsigned long long)k * a.window, a.timeout_ns);
+      if (rc != WAIT_TIMEOUT) {
+        idx = poster_reserve(p, k * n, a.timeout_ns);
+        if (idx == ~0ull) rc = WAIT_TIMEOUT;
+      }
+    }
+    rc = __shfl_sync(0xffffffffu, rc, 0);
+    idx = __shfl_sync(0xffffffffu, idx, 0);
+    if (rc != WAIT_OK) status = rc;
+    if (rc == WAIT_TIMEOUT) break;
+    if (first == ~0ull) first = idx;
+    if (lane < k * n) {
+      const uint32_t i = done + lane / k, m = m0 + i;
+      const bool sig_msg = (a.signal_every <= 1) || ((i + 1) % a.signal_every == 0) || (i + 1 == a.iters);
+      if (k == 2 && (lane & 1u)) {
+        poster_build_atomic(p, idx + lane, OP_ATOMIC_FA, a.fetch + (uint64_t)(m % a.fetch_slots) * 8, a.fetch_lkey, sig, a.sig_rkey,
+                            a.add, 0, sig_msg ? CTRL_CQ_UPDATE : 0);
+      } else {
+        const InlinePayload d = inline_load(a.values + (uint64_t)(m % a.rows) * a.row_bytes, a.nbytes);
+        poster_build_inline(p, idx + lane, OP_RDMA_WRITE, a.dst + (uint64_t)(m % a.nslots) * a.slot_stride, a.rkey, d, a.nbytes,
+                            (k == 1 && sig_msg) ? CTRL_CQ_UPDATE : 0);
+      }
+    }
+    if (k * n > 1) __syncwarp();
+    if (lane == 0) {
+      const bool outstanding = p.head > p.cons;
+      uint4 tail = make_uint4(0, 0, 0, 0);
+      if (outstanding) tail = poster_peek(p);
+      poster_ring(p, idx + k * n);
+      if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
+    }
+    last = idx + k * n - 1;
+    done += n;
+  }
+  if (lane != 0) return;
+  if (done) {
+    const int rc = poster_wait(p, last, a.timeout_ns);
+    if (rc != WAIT_OK) status = rc;
+  }
+  const unsigned long long t1 = globaltimer_ns();
+  poster_close(p);
+  out[0] = (unsigned long long)(long long)status;
+  out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
+  out[6] = p.cons;
+  out[7] = 0;
+}
+
+RN_API int rn_k_put_inline(uint64_t stream, const uint64_t* qps_host, uint32_t nqp, uint64_t values, uint64_t row_bytes,
+                           uint32_t rows, uint64_t dst, uint32_t rkey, uint32_t nbytes, uint64_t slot_stride, uint32_t nslots,
+                           uint64_t sig, uint32_t sig_rkey, uint64_t fetch, uint32_t fetch_lkey, uint32_t fetch_slots,
+                           uint64_t add, uint32_t iters, uint32_t window, uint32_t signal_every, uint32_t burst,
+                           uint64_t timeout_ms, uint64_t out_dev) {
+  PutInlineArgs a;
+  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps) return -22;
+  if (nbytes == 0 || nbytes > MAX_INLINE || rows == 0 || (uint64_t)nqp * iters > 0xffffffffull) return -22;
+  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
+  a.values = (const uint8_t*)values; a.row_bytes = row_bytes; a.rows = rows; a.nbytes = nbytes;
+  a.dst = dst; a.slot_stride = slot_stride; a.rkey = rkey; a.nslots = nslots ? nslots : 1;
+  a.sig = sig; a.fetch = fetch; a.add = add;
+  a.sig_rkey = sig_rkey; a.fetch_lkey = fetch_lkey; a.fetch_slots = fetch_slots ? fetch_slots : 1;
+  a.iters = iters; a.window = window;
+  if (sig && burst > 16) burst = 16;                  // two WQEs per message, one lane each
+  rn_stream_clamp(window, &burst, &signal_every);
+  a.signal_every = signal_every; a.burst = burst;
+  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.out = (unsigned long long*)out_dev;
+  put_inline_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
 // ---------------------------------------------------------------- signal wait (receiver side)
 // Runs on the GPU that holds the signal word.  Thread 0 polls it with system-scope acquire loads until it reaches
 // `until`; every value 1..until is stamped (%globaltimer) when first seen.  Each wait for the next arrival is bounded
@@ -593,6 +702,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncGetAttributes(&a, shared_post_stress_kernel);
   cudaFuncGetAttributes(&a, atomic_stream_kernel);
   cudaFuncGetAttributes(&a, put_signal_kernel);
+  cudaFuncGetAttributes(&a, put_inline_kernel);
   cudaFuncGetAttributes(&a, signal_wait_kernel);
   cudaFuncGetAttributes(&a, fill_random_kernel);
   cudaFuncGetAttributes(&a, fill_bf16_kernel);

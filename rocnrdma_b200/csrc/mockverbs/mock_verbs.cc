@@ -446,7 +446,9 @@ bool nic_execute(MockQp* qp, uint64_t w) {
             break;
           }
         }
-        uint64_t src = translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
+        // inline: the payload is in the WQE (no local key); else gather it through the lkey
+        uint64_t src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
+                                 : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
         uint64_t dst = src || v.bytes == 0 ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_WRITE, true, &syn, &rmr) : 0;
         if (v.bytes == 0) syn = rn::SYN_OK, src = dst = 1;
         if (syn == rn::SYN_OK && !(peer->access_flags & IBV_ACCESS_REMOTE_WRITE)) syn = rn::SYN_REMOTE_ACCESS_ERR;
@@ -481,7 +483,8 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         const uint32_t rbytes = be32(ds.byte_count) & 0x7fffffffu, rlkey = be32(ds.lkey);
         const uint64_t raddr = be64(ds.addr);
         consumed_rq = true; rq_index = (uint16_t)peer->hw_rq_cons++;
-        uint64_t src = translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
+        uint64_t src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
+                                 : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
         if (src && rbytes < v.bytes) syn = rn::SYN_REMOTE_INVAL_REQ_ERR;
         uint64_t dst = (src && syn == rn::SYN_OK) ? translate(rdev, rlkey, raddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, true, &syn, &rmr) : 0;
         if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, rmr, src, lmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
@@ -615,7 +618,16 @@ int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
     rn::Wqe64 w;
     memset(&w, 0, sizeof w);
     const uint32_t imm = be32(wr->imm_data);       // imm_data is already big-endian; build_* swaps it back onto the wire
-    if (opc == rn::OP_SEND || opc == rn::OP_SEND_IMM)
+    const bool inl = (wr->send_flags & IBV_SEND_INLINE) != 0;
+    if (inl && (opc == rn::OP_RDMA_READ || rn::is_atomic(opc) || len == 0 || len > rn::MAX_INLINE)) {
+      if (bad) *bad = wr;
+      errno = EINVAL;
+      break;
+    }
+    if (inl)   // the payload is copied into the WQE now, from the sge's host address; the lkey is not looked at
+      rn::build_inline_wqe(&w, opc, (uint16_t)head, q->qp_num, wr->wr.rdma.remote_addr, wr->wr.rdma.rkey,
+                           (const void*)(uintptr_t)laddr, len, fm, imm);
+    else if (opc == rn::OP_SEND || opc == rn::OP_SEND_IMM)
       rn::build_send_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, len, fm, imm);
     else if (rn::is_atomic(opc))   // libmlx5: FA carries compare_add as the addend, CS carries swap + compare
       rn::build_atomic_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, wr->wr.atomic.remote_addr, wr->wr.atomic.rkey,
@@ -948,7 +960,8 @@ MOCK_API int ibv_destroy_cq(ibv_cq* c) {
 MOCK_API ibv_qp* ibv_create_qp(ibv_pd* pd, ibv_qp_init_attr* a) {
   if (!pd || !a || !a->send_cq || !a->recv_cq) { errno = EINVAL; return nullptr; }
   if (a->qp_type != IBV_QPT_RC) { errno = EOPNOTSUPP; return nullptr; }
-  if (a->cap.max_send_wr < 1 || a->cap.max_send_wr > 16384 || a->cap.max_recv_wr > 16384 || a->cap.max_send_sge > 1 || a->cap.max_recv_sge > 1) {
+  if (a->cap.max_send_wr < 1 || a->cap.max_send_wr > 16384 || a->cap.max_recv_wr > 16384 || a->cap.max_send_sge > 1 || a->cap.max_recv_sge > 1 ||
+      a->cap.max_inline_data > rn::MAX_INLINE) {
     errno = EINVAL;
     return nullptr;
   }
@@ -976,7 +989,7 @@ MOCK_API ibv_qp* ibv_create_qp(ibv_pd* pd, ibv_qp_init_attr* a) {
   q->v.handle = qpn; q->v.qp_num = qpn; q->v.state = IBV_QPS_RESET; q->v.qp_type = IBV_QPT_RC;
   pthread_mutex_init(&q->v.mutex, nullptr);
   pthread_cond_init(&q->v.cond, nullptr);
-  a->cap.max_send_wr = q->sq_cnt; a->cap.max_recv_wr = q->rq_cnt; a->cap.max_inline_data = 0;
+  a->cap.max_send_wr = q->sq_cnt; a->cap.max_recv_wr = q->rq_cnt; a->cap.max_inline_data = rn::MAX_INLINE;
   a->cap.max_send_sge = 1; a->cap.max_recv_sge = 1;
   dev->qps[qpn] = q;
   return &q->v;

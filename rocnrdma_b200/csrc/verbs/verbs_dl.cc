@@ -38,6 +38,7 @@
 #include <vector>
 
 #include "abi/verbs_abi.h"
+#include "../wire/mlx5_wire.h"
 
 using namespace rnabi;
 
@@ -143,6 +144,7 @@ struct QpH {
   CqH *scq, *rcq;
   ibv_qp* qp;
   uint32_t sq_depth, rq_depth;
+  uint32_t max_inline = 0;    // what the provider granted (asked for: the 28 bytes one WQEBB holds)
   uint64_t next_wr_id = 1;
   bool raw_owned = false;     // queues handed to the GPU: host posting would fight over the producer index
   int proxy_slot = -1;
@@ -358,13 +360,16 @@ RN_API void* rn_verbs_create_qp(void* dev, void* scq, void* rcq, uint32_t sq_dep
   ia.send_cq = ((CqH*)scq)->cq; ia.recv_cq = ((CqH*)(rcq ? rcq : scq))->cq;
   ia.qp_type = IBV_QPT_RC;
   ia.cap.max_send_wr = sq_depth; ia.cap.max_recv_wr = rq_depth; ia.cap.max_send_sge = 1; ia.cap.max_recv_sge = 1;
+  // 28 inline bytes next to ctrl + raddr is still one WQEBB with one SGE, so libmlx5's send WQE size does not grow
+  ia.cap.max_inline_data = rn::MAX_INLINE;
   ibv_qp* qp = api().create_qp(d->pd, &ia);
   if (!qp) { why(0, "ibv_create_qp failed: errno %d", errno); return nullptr; }
   QpH* q = new QpH();
   q->dev = d; q->scq = (CqH*)scq; q->rcq = (CqH*)(rcq ? rcq : scq); q->qp = qp;
-  q->sq_depth = ia.cap.max_send_wr; q->rq_depth = ia.cap.max_recv_wr;
+  q->sq_depth = ia.cap.max_send_wr; q->rq_depth = ia.cap.max_recv_wr; q->max_inline = ia.cap.max_inline_data;
   return q;
 }
+RN_API uint32_t rn_verbs_qp_max_inline(void* qp) { return ((QpH*)qp)->max_inline; }
 RN_API int rn_verbs_destroy_qp(void* qp) {
   QpH* q = (QpH*)qp;
   proxy_detach(q->proxy_slot);
@@ -456,6 +461,34 @@ RN_API int rn_verbs_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint3
   }
   wr.send_flags = signaled ? IBV_SEND_SIGNALED : 0;
   wr.wr.atomic.remote_addr = raddr; wr.wr.atomic.rkey = rkey;
+  int rc = ibv_post_send(q->qp, &wr, &bad);
+  if (rc) return why(-rc, "ibv_post_send failed: %d (%s)", rc, strerror(rc));
+  if (wr_id_out) *wr_id_out = wr.wr_id;
+  return 0;
+}
+// Inline WRITE / WRITE_IMM / SEND / SEND_IMM (opcode as in rn_verbs_post_send): IBV_SEND_INLINE with the sge pointing at
+// the caller's n host bytes; the provider copies them into the WQE, so no lkey is needed and the bytes may be reused at once.
+// The provider is the judge of what may be inline (length, opcode): its error comes back as -errno.
+RN_API int rn_verbs_post_inline(void* qp, uint32_t opcode, uint64_t raddr, uint32_t rkey, const void* data, uint32_t n,
+                                int signaled, uint32_t imm, uint64_t* wr_id_out) {
+  QpH* q = (QpH*)qp;
+  if (q->raw_owned) return why(-16, "this QP's queues are owned by the GPU poster; host posting would corrupt the producer index");
+  ibv_sge sge = {(uint64_t)(uintptr_t)data, n, 0};
+  ibv_send_wr wr, *bad = nullptr;
+  memset(&wr, 0, sizeof wr);
+  wr.wr_id = q->next_wr_id++;
+  wr.sg_list = &sge; wr.num_sge = 1;
+  switch (opcode) {
+    case 0x08: wr.opcode = IBV_WR_RDMA_WRITE; break;
+    case 0x09: wr.opcode = IBV_WR_RDMA_WRITE_WITH_IMM; break;
+    case 0x0a: wr.opcode = IBV_WR_SEND; break;
+    case 0x0b: wr.opcode = IBV_WR_SEND_WITH_IMM; break;
+    case 0x10: wr.opcode = IBV_WR_RDMA_READ; break;
+    default: return why(-22, "unsupported opcode 0x%x for a host post", opcode);
+  }
+  wr.send_flags = IBV_SEND_INLINE | (signaled ? IBV_SEND_SIGNALED : 0);
+  wr.imm_data = __builtin_bswap32(imm);
+  wr.wr.rdma.remote_addr = raddr; wr.wr.rdma.rkey = rkey;
   int rc = ibv_post_send(q->qp, &wr, &bad);
   if (rc) return why(-rc, "ibv_post_send failed: %d (%s)", rc, strerror(rc));
   if (wr_id_out) *wr_id_out = wr.wr_id;

@@ -42,6 +42,8 @@ enum : uint32_t {
   WQEBB = 64,        // basic block of the send queue
   WQE_SEG = 16,      // every segment is 16 bytes; ctrl.ds counts these
   CQE_SIZE = 64,
+  MAX_INLINE = 28,   // largest inline payload: ctrl + raddr + a 4-byte inline header + 28 bytes fill one WQEBB
+  INLINE_SEG = 0x80000000u,   // byte_count flag: the payload follows in the WQE itself
 };
 
 enum Opcode : uint8_t {  // ctrl.opmod_idx_opcode[7:0]
@@ -117,6 +119,9 @@ struct alignas(16) AtomicSeg {   // mlx5_wqe_atomic_seg
   uint64_t swap_add;             // be64
   uint64_t compare;              // be64
 };
+struct InlineSeg {               // mlx5_wqe_inl_data_seg: the payload follows, zero padded to a 16-byte boundary
+  uint32_t byte_count;           // be32 (n | INLINE_SEG)
+};
 // One WQEBB holding ctrl + raddr + one data segment (RDMA write / read), or
 // ctrl + data (send: raddr slot left zero and ds=2 with data in slot 1).
 struct alignas(64) Wqe64 {
@@ -125,12 +130,20 @@ struct alignas(64) Wqe64 {
     struct { RaddrSeg raddr; DataSeg data; uint8_t pad[16]; } rdma;
     struct { DataSeg data; uint8_t pad[32]; } send;
     struct { RaddrSeg raddr; AtomicSeg atomic; DataSeg data; } atom;
+    // inline: the payload travels in the WQE (ds = 2 + ceil((4 + n) / 16) for RDMA, 1 + ... for SEND)
+    struct { RaddrSeg raddr; InlineSeg inl; uint8_t data[MAX_INLINE]; } rdma_inl;
+    struct { InlineSeg inl; uint8_t data[44]; } send_inl;
   };
 };
 static_assert(sizeof(CtrlSeg) == 16, "ctrl seg");
 static_assert(sizeof(RaddrSeg) == 16, "raddr seg");
 static_assert(sizeof(DataSeg) == 16, "data seg");
+static_assert(sizeof(InlineSeg) == 4, "inline seg");
 static_assert(sizeof(Wqe64) == 64, "wqebb");
+// where the inline payload starts within the WQEBB (the engine copies it from there)
+enum : uint32_t { INLINE_OFF_RDMA = 36, INLINE_OFF_SEND = 20 };
+static_assert(__builtin_offsetof(Wqe64, rdma_inl.data) == INLINE_OFF_RDMA, "rdma inline payload");
+static_assert(__builtin_offsetof(Wqe64, send_inl.data) == INLINE_OFF_SEND, "send inline payload");
 
 // Receive WQE: a bare scatter list; we use one data segment per 16-byte stride.
 struct alignas(16) RecvWqe { DataSeg data; };
@@ -237,6 +250,22 @@ RN_HD void build_atomic_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t
   encode_atomic(&w->atom.atomic, swap_add, opcode == OP_ATOMIC_CS ? compare : 0);
   encode_data(&w->atom.data, laddr, lkey, bytes);
 }
+// Segments an inline payload of n bytes takes together with its 4-byte header.
+RN_HD constexpr uint8_t inline_segs(uint32_t n) { return (uint8_t)((4 + n + WQE_SEG - 1) / WQE_SEG); }
+// Inline WQE (1 <= n <= MAX_INLINE; the caller checks): RDMA_WRITE / WRITE_IMM carry ctrl + raddr + the inline segment
+// (ds 3 up to 12 bytes, else 4), SEND / SEND_IMM ctrl + the inline segment (ds 2 up to 12 bytes, else 3).  No lkey, no
+// local address: the n bytes at `data` are copied into the WQE, and the rest of the WQEBB is zero.
+RN_HD void build_inline_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint64_t raddr, uint32_t rkey,
+                            const void* data, uint32_t n, uint8_t fm_ce_se, uint32_t imm) {
+  const bool send = opcode == OP_SEND || opcode == OP_SEND_IMM;
+  uint8_t* b = reinterpret_cast<uint8_t*>(w);
+  for (uint32_t i = WQE_SEG; i < WQEBB; ++i) b[i] = 0;
+  encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, (uint8_t)((send ? 1 : 2) + inline_segs(n)), fm_ce_se, imm);
+  if (!send) encode_raddr(&w->rdma_inl.raddr, raddr, rkey);
+  (send ? w->send_inl.inl : w->rdma_inl.inl).byte_count = be32(n | INLINE_SEG);
+  uint8_t* d = b + (send ? INLINE_OFF_SEND : INLINE_OFF_RDMA);
+  for (uint32_t i = 0; i < n; ++i) d[i] = static_cast<const uint8_t*>(data)[i];
+}
 
 // ---------------------------------------------------------------- decoders
 struct WqeView {
@@ -246,8 +275,13 @@ struct WqeView {
   uint64_t raddr, laddr;
   uint32_t rkey, lkey, bytes;
   uint64_t swap_add, compare;    // atomics only (native byte order)
+  uint8_t inl_off;               // inline WQE: offset of its `bytes` payload bytes in the WQEBB; 0: gather (laddr / lkey)
 };
 RN_HD bool is_atomic(uint8_t opcode) { return opcode == OP_ATOMIC_CS || opcode == OP_ATOMIC_FA; }
+// An inline byte count is well formed when 1 <= n <= MAX_INLINE and ds counts exactly its segments.
+RN_HD bool inline_ok(uint32_t n, uint8_t ds, uint8_t head_segs) {
+  return n >= 1 && n <= MAX_INLINE && ds == head_segs + inline_segs(n);
+}
 RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
   uint32_t w0 = be32(w->ctrl.opmod_idx_opcode), w1 = be32(w->ctrl.qpn_ds);
   v->opcode = (uint8_t)(w0 & 0xff);
@@ -258,32 +292,48 @@ RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
   v->fm_ce_se = w->ctrl.fm_ce_se;
   v->imm = be32(w->ctrl.imm);
   v->raddr = 0; v->rkey = 0; v->laddr = 0; v->lkey = 0; v->bytes = 0;
-  v->swap_add = 0; v->compare = 0;
+  v->swap_add = 0; v->compare = 0; v->inl_off = 0;
   switch (v->opcode) {
     case OP_ATOMIC_CS: case OP_ATOMIC_FA:
-      if (v->ds != 4) return false;
+      if (v->ds != 4 || (be32(w->atom.data.byte_count) & INLINE_SEG)) return false;
       v->raddr = be64(w->atom.raddr.raddr);
       v->rkey = be32(w->atom.raddr.rkey);
       v->swap_add = be64(w->atom.atomic.swap_add);
       v->compare = be64(w->atom.atomic.compare);
       v->laddr = be64(w->atom.data.addr);
       v->lkey = be32(w->atom.data.lkey);
-      v->bytes = be32(w->atom.data.byte_count) & 0x7fffffffu;
+      v->bytes = be32(w->atom.data.byte_count);
       return true;
-    case OP_RDMA_WRITE: case OP_RDMA_WRITE_IMM: case OP_RDMA_READ:
-      if (v->ds != 3) return false;
+    case OP_RDMA_WRITE: case OP_RDMA_WRITE_IMM: case OP_RDMA_READ: {
+      const uint32_t bc = be32(w->rdma.data.byte_count);
+      if (bc & INLINE_SEG) {   // a READ has nothing to carry inline
+        v->bytes = bc & ~INLINE_SEG;
+        if (v->opcode == OP_RDMA_READ || !inline_ok(v->bytes, v->ds, 2)) return false;
+        v->inl_off = INLINE_OFF_RDMA;
+      } else {
+        if (v->ds != 3) return false;
+        v->laddr = be64(w->rdma.data.addr);
+        v->lkey = be32(w->rdma.data.lkey);
+        v->bytes = bc;
+      }
       v->raddr = be64(w->rdma.raddr.raddr);
       v->rkey = be32(w->rdma.raddr.rkey);
-      v->laddr = be64(w->rdma.data.addr);
-      v->lkey = be32(w->rdma.data.lkey);
-      v->bytes = be32(w->rdma.data.byte_count) & 0x7fffffffu;
       return true;
-    case OP_SEND: case OP_SEND_IMM:
+    }
+    case OP_SEND: case OP_SEND_IMM: {
+      const uint32_t bc = be32(w->send.data.byte_count);
+      if (bc & INLINE_SEG) {
+        v->bytes = bc & ~INLINE_SEG;
+        if (!inline_ok(v->bytes, v->ds, 1)) return false;
+        v->inl_off = INLINE_OFF_SEND;
+        return true;
+      }
       if (v->ds != 2) return false;
       v->laddr = be64(w->send.data.addr);
       v->lkey = be32(w->send.data.lkey);
-      v->bytes = be32(w->send.data.byte_count) & 0x7fffffffu;
+      v->bytes = bc;
       return true;
+    }
     case OP_NOP:
       return v->ds == 1;
     default:

@@ -247,6 +247,53 @@ def put_signal(qp, src_mr, dst_mr, nbytes: int, sig_mr, sig_off: int = 0, fetch_
     return parse_stream_out(out_view, 1, nbytes)
 
 
+def put_inline(qps, values, dst_mr, nbytes: int, iters: int = 1, window: int = 0, burst: int = 1, signal_every: int = 1,
+               slot_stride=None, nslots: int = 1, sig_mr=None, sig_off: int = 0, fetch_mr=None, add: int = 1,
+               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = 24576):
+    """Device-posted inline puts (DOCA ``p`` / ``p_signal``, ``nvshmem_p``): one warp per QP posts ``iters`` RDMA WRITEs
+    whose ``nbytes`` (1..28) travel inside the WQE, with the windowed, bursted poster of :func:`rdma_stream`.  Message
+    ``i`` of QP ``c`` (``m = c * iters + i``) reads its bytes into registers from row ``m % rows`` of ``values`` -- a CUDA
+    tensor on the QP's GPU that is never registered (a 2-D tensor: one row per message value; 1-D: rows of ``nbytes``)
+    -- and writes them to ``dst_mr`` slot ``m % nslots`` at ``slot_stride`` (default ``nbytes``).
+    With ``sig_mr`` each message is the inline WRITE plus a FETCH_AND_ADD of ``add`` on the u64 at
+    ``sig_mr.addr + sig_off + c * 8``, built by two lanes and published with one doorbell; the atomic executes after the
+    WRITE has landed, so a receiver may use :func:`signal_wait` unchanged.  Fetched values go to ``fetch_mr`` (default: the
+    context's sink, see :func:`put_signal`).  ``window`` and ``burst`` count messages.  Returns a :class:`StreamResult`."""
+    lib = N.load()
+    if not isinstance(qps, (list, tuple)):
+        qps = [qps]
+    if not 1 <= nbytes <= 28:
+        raise ValueError(f"inline puts carry 1..28 bytes, not {nbytes}")
+    if not values.is_cuda or not values.is_contiguous():
+        raise ValueError("values must be a contiguous CUDA tensor")
+    row_bytes = values.stride(0) * values.element_size() if values.dim() == 2 else nbytes
+    total = values.numel() * values.element_size()
+    if row_bytes < nbytes or total < nbytes:
+        raise ValueError(f"values rows hold {row_bytes} bytes; each message needs {nbytes}")
+    rows = (total - nbytes) // row_bytes + 1
+    ctx = qps[0].ctx
+    nq = len(qps)
+    if slot_stride is None:
+        slot_stride = nbytes
+    if sig_mr is not None and fetch_mr is None:
+        fetch_mr = _fetch_sink(ctx)
+    ws = work_stream(ctx, stream)
+    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
+    out_addr, out_view = ctx.scratch(nq * 64, offset=scratch_off)
+    sig = (sig_mr.addr + sig_off) if sig_mr is not None else 0
+    rc = lib.rn_k_put_inline(_stream_ptr(ws), qp_arr, nq, values.data_ptr(), row_bytes, rows, dst_mr.addr, dst_mr.rkey, nbytes,
+                             slot_stride, nslots, sig, sig_mr.rkey if sig_mr is not None else 0,
+                             fetch_mr.addr if fetch_mr is not None else 0, fetch_mr.lkey if fetch_mr is not None else 0,
+                             max(fetch_mr.length // 8, 1) if fetch_mr is not None else 1, add & 0xFFFFFFFFFFFFFFFF, iters, window,
+                             signal_every, burst, timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"put_inline launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_stream_out(out_view, nq, nbytes)
+
+
 def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, stream=None, sync: bool = True,
                 check=None, scratch_off: int = 20544):
     """Receiver side of :func:`put_signal`, on the GPU that holds the signal: waits until the u64 at ``signal`` (a

@@ -8,9 +8,12 @@ from __future__ import annotations
 
 import struct
 from dataclasses import dataclass
+from typing import Optional
 
 WQEBB = 64
 CQE_SIZE = 64
+MAX_INLINE = 28            # largest inline payload: ctrl + raddr + a 4-byte inline header + 28 bytes fill one WQEBB
+INLINE_SEG = 0x80000000    # byte_count flag of an inline data segment
 
 OP_NOP = 0x00
 OP_SEND_INVAL = 0x01
@@ -91,6 +94,32 @@ def atomic_wqe(opcode, wqe_idx, qpn, laddr, lkey, raddr, rkey, swap_add, compare
             + data_seg(laddr, lkey, nbytes))
 
 
+def inline_seg(data: bytes) -> bytes:
+    """The inline data segment: be32 ``len(data) | INLINE_SEG``, then the payload, zero padded to a 16-byte boundary."""
+    b = struct.pack(">I", len(data) | INLINE_SEG) + bytes(data)
+    return b + bytes(-len(b) % 16)
+
+
+def inline_wqe(opcode, wqe_idx, qpn, data: bytes, raddr=0, rkey=0, fm_ce_se=CTRL_CQ_UPDATE, imm=0) -> bytes:
+    """One WQEBB carrying ``data`` (1..MAX_INLINE bytes) in the WQE itself.  RDMA_WRITE / WRITE_IMM: ctrl + raddr + inline
+    segment (ds 3 up to 12 bytes, else 4); SEND / SEND_IMM: ctrl + inline segment (ds 2 up to 12 bytes, else 3)."""
+    if not 1 <= len(data) <= MAX_INLINE:
+        raise ValueError(f"inline payload of {len(data)} bytes (1..{MAX_INLINE})")
+    seg = inline_seg(data)
+    if opcode in (OP_SEND, OP_SEND_IMM):
+        b = ctrl_seg(opcode, wqe_idx, qpn, 1 + len(seg) // 16, fm_ce_se, imm) + seg
+    else:
+        b = ctrl_seg(opcode, wqe_idx, qpn, 2 + len(seg) // 16, fm_ce_se, imm) + raddr_seg(raddr, rkey) + seg
+    return b + bytes(WQEBB - len(b))
+
+
+def _inline_payload(b: bytes, off: int, ds: int, head_segs: int) -> bytes:
+    n = struct.unpack_from(">I", b, off - 4)[0] & ~INLINE_SEG
+    if not 1 <= n <= MAX_INLINE or ds != head_segs + (4 + n + 15) // 16:
+        raise ValueError(f"malformed inline WQE: {n} bytes with ds = {ds}")
+    return bytes(b[off:off + n])
+
+
 @dataclass
 class WqeView:
     opcode: int
@@ -107,14 +136,26 @@ class WqeView:
     nbytes: int = 0
     swap_add: int = 0
     compare: int = 0
+    inline_data: Optional[bytes] = None    # the payload of an inline WQE (laddr / lkey are then 0)
 
 
 def decode_wqe(b: bytes) -> WqeView:
+    """Decode one WQEBB.  An inline WQE (INLINE_SEG set on a WRITE, WRITE_IMM, SEND or SEND_IMM) fills ``inline_data``;
+    one whose length or ds is out of range raises ``ValueError``, as does the flag on a READ."""
     assert len(b) >= WQEBB
     w0, w1, _sig, _r0, _r1, fm, imm = struct.unpack_from(">IIBBBBI", b, 0)
     v = WqeView(opcode=w0 & 0xFF, opmod=w0 >> 24, wqe_idx=(w0 >> 8) & 0xFFFF, qpn=w1 >> 8, ds=w1 & 0x3F,
                 fm_ce_se=fm, imm=imm)
-    if v.opcode in (OP_RDMA_WRITE, OP_RDMA_WRITE_IMM, OP_RDMA_READ):
+    if v.opcode in (OP_RDMA_WRITE, OP_RDMA_WRITE_IMM, OP_RDMA_READ) and struct.unpack_from(">I", b, 32)[0] & INLINE_SEG:
+        if v.opcode == OP_RDMA_READ:
+            raise ValueError("a READ cannot carry inline data")
+        v.raddr, v.rkey, _ = struct.unpack_from(">QII", b, 16)
+        v.inline_data = _inline_payload(b, 36, v.ds, 2)
+        v.nbytes = len(v.inline_data)
+    elif v.opcode in (OP_SEND, OP_SEND_IMM) and struct.unpack_from(">I", b, 16)[0] & INLINE_SEG:
+        v.inline_data = _inline_payload(b, 20, v.ds, 1)
+        v.nbytes = len(v.inline_data)
+    elif v.opcode in (OP_RDMA_WRITE, OP_RDMA_WRITE_IMM, OP_RDMA_READ):
         v.raddr, v.rkey, _ = struct.unpack_from(">QII", b, 16)
         n, v.lkey, v.laddr = struct.unpack_from(">IIQ", b, 32)
         v.nbytes = n & 0x7FFFFFFF
