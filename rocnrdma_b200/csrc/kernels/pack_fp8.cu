@@ -13,9 +13,14 @@
 //
 // Record layout for a chunk of C elements (C % 8192 == 0):
 //     [ C bytes fp8 e4m3 ][ C/32 bytes UE8M0 scales ][ pad to 64 B ]
-// Quantisation (bit-exact reference in tests/test_pack_fp8.py):
+// Quantisation (bit-exact reference: ops/pack.py, quantize_blocks / ref_pack_fp8 / ref_unpack_fp8):
 //     v = amax * (1/448)  (fp32) ; e = exponent(v) + (mantissa(v) != 0), clamped to [-127, 127]
 //     q = cvt.rn.satfinite.e4m3(x * 2^-e) ; scale byte = e + 127
+// Non-finite input:
+//     NaN   amax is an fmaxf reduction, which drops NaN: a NaN stays in its own element, its neighbours quantise
+//           as if it were absent (an all-NaN block gets scale byte 0 and NaN codes)
+//     +-Inf e clamps to 127 (scale byte 254) and 2^-127 is 0.0 here: the Inf becomes NaN, its neighbours +-0
+// Decode: scale byte 0x00 is 2^-127 (the OCP MX value, fp32 0x00400000), as in the block-scaled GEMM; 0xFF is Inf.
 //
 // No counterpart in the reference (it moves no payload: SURVEY.md section 3.2).
 #include <cuda_bf16.h>
@@ -68,6 +73,8 @@ struct PackArgs {
 };
 
 __device__ __forceinline__ float bf16_bits_to_float(uint32_t hi16) { return __uint_as_float(hi16 << 16); }
+// UE8M0 scale byte -> 2^(e - 127); byte 0 is 2^-127, an fp32 denormal (the same decode as gemm_mxfp8.cu)
+__device__ __forceinline__ float ue8m0(uint32_t e) { return e ? __uint_as_float(e << 23) : __uint_as_float(0x00400000u); }
 
 template <int G>
 __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_tile, uint32_t tiles_per_chunk, uint64_t rec) {
@@ -280,7 +287,7 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
         if (!good) break;
       }
       uint32_t qv[G][8];
-      int e[G];
+      uint32_t e[G];
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         const uint64_t T = T0 + (uint64_t)g * stride;
@@ -288,14 +295,14 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
           const uint32_t chunk = (uint32_t)(T / tiles_per_chunk), t = (uint32_t)(T % tiles_per_chunk);
           const uint8_t* recp = a.staging + (uint64_t)chunk * rec;
           ld256_cs(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems, qv[g]);
-          e[g] = (int)__ldcs(recp + a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x) - 127;
+          e[g] = __ldcs(recp + a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x);
         }
       }
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         const uint64_t T = T0 + (uint64_t)g * stride;
         if (T >= total) break;
-        const float s = __uint_as_float((uint32_t)(e[g] + 127) << 23);
+        const float s = ue8m0(e[g]);
         const uint32_t* q = qv[g];
         uint32_t o[16];
 #pragma unroll

@@ -52,15 +52,13 @@ def panel_record_bytes(N: int) -> int:
 
 def ref_fp8_panels(c_fp32: torch.Tensor) -> torch.Tensor:
     """PyTorch reference of the fp8 epilogue: quantise an fp32 [M, N] result into panel records."""
-    from .pack import _pow2, _scale_exponent
+    from .pack import quantize_blocks
     M0, Nn = c_fp32.shape
     M = -(-M0 // BM) * BM                    # records are whole panels: rows past M quantise zeros
     x = torch.zeros(M, Nn, dtype=torch.float32, device=c_fp32.device)
     x[:M0] = c_fp32.float()
-    x = x.reshape(M, Nn // 32, 32)
-    e = _scale_exponent(x.abs().amax(dim=2))
-    q = (x * _pow2(-e)[..., None]).to(torch.float8_e4m3fn).view(torch.uint8).reshape(M, Nn)
-    sc = (e + 127).to(torch.uint8)
+    q, sc = quantize_blocks(x.reshape(M, Nn // 32, 32))
+    q = q.reshape(M, Nn)
     out = torch.empty(M // BM, panel_record_bytes(Nn), dtype=torch.uint8, device=c_fp32.device)
     out[:, :BM * Nn] = q.reshape(M // BM, BM * Nn)
     out[:, BM * Nn:] = sc.reshape(M // BM, BM * (Nn // 32))
@@ -68,12 +66,12 @@ def ref_fp8_panels(c_fp32: torch.Tensor) -> torch.Tensor:
 
 
 def dequant_fp8_panels(rec: torch.Tensor, M: int, Nn: int) -> torch.Tensor:
-    from .pack import _pow2
+    from .pack import ue8m0
     P = -(-M // BM)
     r = rec[:P * panel_record_bytes(Nn)].reshape(P, panel_record_bytes(Nn))
     q = r[:, :BM * Nn].contiguous().view(torch.float8_e4m3fn).float().reshape(P * BM, Nn // 32, 32)
-    e = r[:, BM * Nn:].to(torch.int32).reshape(P * BM, Nn // 32) - 127
-    return (q * _pow2(e)[..., None]).reshape(P * BM, Nn)[:M]
+    s = ue8m0(r[:, BM * Nn:].reshape(P * BM, Nn // 32))
+    return (q * s[..., None]).reshape(P * BM, Nn)[:M]
 
 
 def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None, qp=None, dst_mr=None,

@@ -8,7 +8,7 @@ from dataclasses import dataclass
 import torch
 
 from .. import _native as N
-from .pack import BLOCK, _pow2, _scale_exponent, record_bytes
+from .pack import BLOCK, quantize_blocks, record_bytes, ue8m0
 from .rdma import WAIT_STATUS, _stream_ptr, work_stream
 
 PANEL_ROWS = 128
@@ -107,13 +107,11 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
 def quantize_mx(x: torch.Tensor):
     """bf16 / fp32 [rows, K] -> (e4m3 bytes [rows, K], UE8M0 scale bytes [rows, K/32]); same rule as the pack kernel."""
     rows, K = x.shape
-    xb = x.float().reshape(rows, K // BLOCK, BLOCK)
-    e = _scale_exponent(xb.abs().amax(dim=2))
-    q = (xb * _pow2(-e)[..., None]).to(torch.float8_e4m3fn).view(torch.uint8).reshape(rows, K)
-    return q.contiguous(), (e + 127).to(torch.uint8).contiguous()
+    q, s = quantize_blocks(x.float().reshape(rows, K // BLOCK, BLOCK))
+    return q.reshape(rows, K).contiguous(), s.contiguous()
 
 
 def dequantize_mx(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
     rows, K = q.shape
     v = q.view(torch.float8_e4m3fn).float().reshape(rows, K // BLOCK, BLOCK)
-    return (v * _pow2(s.to(torch.int32) - 127)[..., None]).reshape(rows, K)
+    return (v * ue8m0(s)[..., None]).reshape(rows, K)

@@ -123,6 +123,12 @@ def parse_unpack(view) -> dict:
 
 
 # ------------------------------------------------------------------ bit-exact references
+# Non-finite rule (the kernels' behaviour, which these references reproduce bit for bit):
+#   * the block amax ignores NaN (the kernels reduce with fmaxf), so a NaN stays in its own element and its
+#     finite neighbours quantise as if it were absent;
+#   * a block holding +-Inf gets exponent 127 (scale byte 254) and multiplier 2^-127 == 0.0, so the Inf becomes
+#     NaN and every finite neighbour becomes +-0;
+#   * decoding, scale byte 0x00 is 2^-127 (the OCP MX value, an fp32 denormal) and 0xFF is 2^128 == Inf.
 def _scale_exponent(amax: torch.Tensor) -> torch.Tensor:
     """e = smallest integer with amax / 2^e <= 448, computed on the fp32 bit pattern exactly
     as the kernel does (no log2 rounding)."""
@@ -133,20 +139,36 @@ def _scale_exponent(amax: torch.Tensor) -> torch.Tensor:
 
 
 def _pow2(e: torch.Tensor) -> torch.Tensor:
+    """2^e for e in [-127, 128] from the biased exponent alone: 2^-127 comes out as 0.0, which is what the
+    quantiser multiplies by (the kernels' ``inv``).  Decoders use ``ue8m0`` instead."""
     return ((e + 127).to(torch.int32) << 23).view(torch.float32)
+
+
+def ue8m0(scale_bytes: torch.Tensor) -> torch.Tensor:
+    """The fp32 value of UE8M0 scale bytes: 2^(byte - 127), with byte 0x00 = 2^-127 (fp32 0x00400000), 0xFF = Inf."""
+    b = scale_bytes.to(torch.int32)
+    return torch.where(b == 0, torch.full_like(b, 0x00400000), b << 23).view(torch.float32)
+
+
+def quantize_blocks(x: torch.Tensor):
+    """Block-scaled e4m3 quantisation of fp32 ``x[..., 32]`` (one block per row of the last dim), the rule every
+    producer kernel applies: returns (e4m3 bytes shaped like ``x``, UE8M0 scale bytes ``x.shape[:-1]``)."""
+    a = x.abs()
+    a = torch.where(torch.isnan(a), torch.zeros_like(a), a)       # fmaxf drops NaN; +Inf stays
+    e = _scale_exponent(a.amax(dim=-1))
+    q = (x * _pow2(-e)[..., None]).to(torch.float8_e4m3fn).view(torch.uint8)
+    return q, (e + 127).to(torch.uint8)
 
 
 def ref_pack_fp8(src: torch.Tensor, chunk_elems: int) -> torch.Tensor:
     """Reference chunk records (uint8) for a bf16 tensor; runs on CPU or GPU."""
-    x = src.float().reshape(-1, BLOCK)
-    e = _scale_exponent(x.abs().amax(dim=1))
-    q = (x * _pow2(-e)[:, None]).to(torch.float8_e4m3fn).view(torch.uint8)
+    q, sc = quantize_blocks(src.float().reshape(-1, BLOCK))
     n = src.numel()
     n_chunks = n // chunk_elems
     rec = record_bytes(chunk_elems)
     out = torch.zeros(n_chunks, rec, dtype=torch.uint8, device=src.device)
     out[:, :chunk_elems] = q.reshape(n_chunks, chunk_elems)
-    out[:, chunk_elems:chunk_elems + chunk_elems // BLOCK] = (e + 127).to(torch.uint8).reshape(n_chunks, -1)
+    out[:, chunk_elems:chunk_elems + chunk_elems // BLOCK] = sc.reshape(n_chunks, -1)
     return out.reshape(-1)
 
 
@@ -155,5 +177,5 @@ def ref_unpack_fp8(records: torch.Tensor, n_elems: int, chunk_elems: int) -> tor
     rec = record_bytes(chunk_elems)
     r = records.reshape(n_chunks, rec)
     q = r[:, :chunk_elems].contiguous().view(torch.float8_e4m3fn).float().reshape(-1, BLOCK)
-    e = r[:, chunk_elems:chunk_elems + chunk_elems // BLOCK].to(torch.int32).reshape(-1) - 127
-    return (q * _pow2(e)[:, None]).to(torch.bfloat16).reshape(-1)
+    s = ue8m0(r[:, chunk_elems:chunk_elems + chunk_elems // BLOCK].reshape(-1))
+    return (q * s[:, None]).to(torch.bfloat16).reshape(-1)
