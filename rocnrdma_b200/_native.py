@@ -105,7 +105,8 @@ _SIGS = {
     "rn_engine_set_oneshot": (i32, [vp, i32]),
     "rn_engine_wait": (i32, [vp]),
     "rn_engine_stats": (i32, [vp, C.POINTER(RnEngineStats)]),
-    "rn_k_engine_ceiling": (i32, [u64, u64, u64, u64, i32, u64]),
+    "rn_engine_mover_profile": (i32, [vp, C.POINTER(u64), i32]),
+    "rn_k_engine_ceiling": (i32, [u64, u64, u64, u64, i32, u64, u64]),
     "rn_hca_scratch": (u64, [vp, C.POINTER(u64)]),
     "rn_set_device": (i32, [i32]),
     "rn_ipc_export": (i32, [u64, C.POINTER(u8), C.POINTER(u64), C.POINTER(u64)]),
@@ -138,6 +139,7 @@ _SIGS = {
     "rn_k_atomic_stream": (i32, [u64, C.POINTER(u64), u32, u32, u32, u64, u32, u64, u64, u32, u64, u64, u64, u32, u32, u32, u32, u64, u64]),
     "rn_k_put_signal": (i32, [u64, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32, u32, u64, u64]),
     "rn_k_signal_wait": (i32, [u64, u64, u64, u64, u64, u64, u64, u64, u64, u64]),
+    "rn_k_cq_watch": (i32, [u64, u64, u32, u64, u64, u64, u32, u64, u64, u64, u64, u64]),
     "rn_k_put_inline": (i32, [u64, C.POINTER(u64), u32, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32,
                               u32, u32, u32, u64, u64]),
     "rn_gpu_page_size": (u64, []),

@@ -40,6 +40,17 @@ _WC_STATUS = {0: "OK", 1: "LOCAL_LENGTH_ERR", 2: "LOCAL_QP_OP_ERR", 4: "LOCAL_PR
               12: "TRANSPORT_RETRY_EXC_ERR", 13: "RNR_RETRY_EXC_ERR", 16: "REMOTE_ABORTED_ERR", 21: "GENERAL_ERR"}
 _IBV_WC_RECV, _IBV_WC_RECV_RDMA_WITH_IMM = 128, 129
 
+# One row of the engine mover's stall profile (enum MoverProf in csrc/hca/hca_types.h): %globaltimer ns per wait, the
+# mover's whole run, and the chunks it reported.
+MOVER_PROFILE_FIELDS = ("wait_read_ns", "full_ns", "chunk_wait_ns", "report_ns", "dry_wait_ns", "qfull_idle_ns", "total_ns",
+                        "chunks")
+
+
+def mover_profile_rows(flat) -> List[dict]:
+    """Split a flat sequence of profile counters into one dict per CTA."""
+    n = len(MOVER_PROFILE_FIELDS)
+    return [dict(zip(MOVER_PROFILE_FIELDS, (int(v) for v in flat[i:i + n]))) for i in range(0, len(flat) - n + 1, n)]
+
 
 def resolve_wire(wire: str = "auto") -> str:
     """'auto' -> 'verbs' when a REAL HCA is usable (libibverbs loads, /dev/infiniband is there, a device
@@ -806,6 +817,18 @@ class Context:
         s = N.RnEngineStats()
         N.check(self._lib.rn_engine_stats(self._h, C.byref(s)), "engine_stats")
         return {k: getattr(s, k) for k, _ in s._fields_}
+
+    def engine_mover_profile(self) -> List[dict]:
+        """Where each engine CTA's mover spent its time in the last engine run started with ``RN_ENGINE_PROFILE=1``: one
+        dict per CTA with the ``MOVER_PROFILE_FIELDS`` (ns blocked per wait, total ns, chunks reported).  Read it after
+        ``engine_stop``; empty when that run was not profiled."""
+        if self.wire == "verbs":
+            return []
+        buf = (C.c_uint64 * (len(MOVER_PROFILE_FIELDS) * 256))()
+        rows = self._lib.rn_engine_mover_profile(self._h, buf, 256)
+        if rows < 0:
+            N.check(rows, "engine_mover_profile")
+        return mover_profile_rows(buf[:rows * len(MOVER_PROFILE_FIELDS)])
 
     @property
     def host_native_atomics(self) -> bool:

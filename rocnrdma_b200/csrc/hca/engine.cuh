@@ -38,9 +38,10 @@ using namespace rn::dev;
 constexpr int kThreads = 128;
 constexpr uint32_t kSub = 16384;        // bytes per TMA bulk transaction
 constexpr int kStages = 12;             // smem ring: 12 x 16 KiB
-// ring split: EngineCtl::stores_in_flight stages (default 4) may hold a TMA store that is still reading smem,
+// ring split: EngineCtl::stores_in_flight stages (default kSifDefault) may hold a TMA store that is still reading smem,
 // the others hold loads in flight (move_chunks<kSif>)
 constexpr int kMaxSif = 8;             // largest stores_in_flight
+constexpr int kSifDefault = 2;         // 10 loads + 2 stores: as fast as 1 or 3 stores, faster than 4 (DESIGN.md 3.1)
 constexpr uint32_t kBulkMin = 4096;     // below this the generic path is as fast
 
 // ------------------------------------------------------------------ PTX helpers
@@ -161,7 +162,7 @@ struct Smem {
   alignas(128) uint8_t ring[kStages][kSub];
   alignas(8) uint64_t full[kStages];     // ring stage landed (TMA complete_tx)
   uint64_t qfull[kQueue];                // control -> mover: entry holds a chunk
-  uint64_t qdone[kQueue];                // mover -> control: that chunk is written and released at gpu scope; entry free
+  uint64_t qdone[kQueue];                // mover -> control: that chunk's bulk stores are complete; entry free
   Chunk q[kQueue];
   Owed owed[kQueue];                     // control only
   uint32_t end[kQueue];                  // mover only: store groups committed up to and including the chunk's last
@@ -201,12 +202,14 @@ __device__ __forceinline__ void generic_bar() { asm volatile("bar.sync 1, %0;" :
 // single store in flight every step exposed the store's smem-read latency, ~0.35 us, which capped a CTA near 45 GB/s.)
 // Loads for the next queued chunk are issued as ring stages free up, while the current chunk's stores are still in
 // flight.  A chunk is written once kSif groups have been committed after its last store: that step waits for the full
-// completion (wait_group kSif) instead of the smem read, then takes the gpu-scope fence and reports the chunk to control
-// (mbarrier arrive: release at CTA scope).  When nothing more is queued the ring drains at once (wait_group 0), so a lone
-// chunk is not held back waiting for work.  Chunks need 16-byte aligned src, dst and len.  Returns false when a load
-// never landed (bad mapping: bounded, the SM is not wedged); true when control queued the quit entry.
-template <int kSif>
-__device__ __noinline__ bool move_chunks(Smem& s) {
+// completion (wait_group kSif) instead of the smem read, then reports the chunk to control (mbarrier arrive: release at
+// CTA scope).  No fence here: control's gpu-scope fence is cumulative over what this hand-off carries (DESIGN.md 3.1).
+// When nothing more is queued the ring drains at once (wait_group 0), so a lone chunk is not held back waiting for work.
+// Chunks need 16-byte aligned src, dst and len.  Returns false when a load never landed (bad mapping: bounded, the SM is
+// not wedged); true when control queued the quit entry.
+// kProf: add %globaltimer ns per wait to prof[MoverProf] (this CTA's row), written once on exit.
+template <int kSif, bool kProf>
+__device__ __noinline__ bool move_chunks(Smem& s, unsigned long long* prof) {
   constexpr uint32_t P = kStages - kSif;
   uint32_t ring_ph = 0, q_ph = 0;            // parity of the next wait, per ring stage / per queue entry
   uint32_t n_ld = 0, n_st = 0;               // steps loaded / stored (= store groups committed)
@@ -216,31 +219,48 @@ __device__ __noinline__ bool move_chunks(Smem& s) {
   uint64_t ld_src = 0, st_dst = 0;
   int unwritten = 0;                         // chunks whose stores are all issued, not yet reported
   bool ld_have = false, quit = false;
+  unsigned long long acc[MOVER_PROF_N] = {}, t_in = 0, t_idle = 0;   // kProf only
+  if constexpr (kProf) t_in = globaltimer_ns();
+  auto stamp = [&]() -> unsigned long long { return kProf ? globaltimer_ns() : 0ull; };
+  auto charge = [&](int b, unsigned long long t0) { if constexpr (kProf) acc[b] += globaltimer_ns() - t0; };
+  auto leave = [&](bool ok) {
+    if constexpr (kProf) {
+      acc[MP_TOTAL] = globaltimer_ns() - t_in;
+      for (int b = 0; b < MOVER_PROF_N; ++b) prof[b] = acc[b];
+    }
+    return ok;
+  };
   auto next_stage = [](int i) { return i + 1 == kStages ? 0 : i + 1; };
   auto next_entry = [](int i) { return i + 1 == kQueue ? 0 : i + 1; };
   auto report = [&](bool all) {
-    fence_gpu();   // the chunks' bytes (complete for this thread) at gpu scope before control counts them
+    const unsigned long long t0 = stamp();
     do {
       mbar_arrive(&s.qdone[e_wr]);
       e_wr = next_entry(e_wr);
+      if constexpr (kProf) ++acc[MP_CHUNKS];
     } while (--unwritten && (all || n_st - s.end[e_wr] >= (uint32_t)kSif));
+    charge(MP_REPORT, t0);
   };
   for (;;) {
     if (!ld_have && !quit) {
       // idle (nothing in the ring, nothing owed): this wait may suspend; otherwise only probe
       const bool idle = n_st == n_ld && unwritten == 0;
       const uint32_t par = (q_ph >> e_ld) & 1u;
+      if constexpr (kProf) if (idle && !t_idle) t_idle = globaltimer_ns();
       if (idle ? mbar_try_wait(&s.qfull[e_ld], par) : mbar_test_wait(&s.qfull[e_ld], par)) {
         q_ph ^= 1u << e_ld;
         ld_len = s.q[e_ld].len;
         if (ld_len == kQuitLen) quit = true;
         else { ld_have = true; ld_src = s.q[e_ld].src; ld_off = 0; }
+        if constexpr (kProf) if (t_idle) { charge(MP_QFULL_IDLE, t_idle); t_idle = 0; }
       }
     }
     while (ld_have && n_ld - n_st < P) {
       if ((int32_t)(n_ld - ld_limit) >= 0) {
         // the stage of load n_ld was last read by store n_ld - kStages <= n_st - 1 - kSif
+        const unsigned long long t0 = stamp();
         bulk_wait_read<kSif>();
+        charge(MP_WAIT_READ, t0);
         ld_limit = n_st + P;
       }
       const uint32_t len = ld_len - ld_off < kSub ? ld_len - ld_off : kSub;
@@ -256,7 +276,8 @@ __device__ __noinline__ bool move_chunks(Smem& s) {
       if (!mbar_try_wait(&s.full[st_stage], par)) {
         const unsigned long long t0 = globaltimer_ns();
         while (!mbar_try_wait(&s.full[st_stage], par))
-          if (globaltimer_ns() - t0 > 1000000000ull) return false;
+          if (globaltimer_ns() - t0 > 1000000000ull) return leave(false);
+        charge(MP_FULL, t0);
       }
       ring_ph ^= 1u << st_stage;
       if (st_off == 0) { st_dst = s.q[e_st].dst; st_len = s.q[e_st].len; }
@@ -268,17 +289,32 @@ __device__ __noinline__ bool move_chunks(Smem& s) {
       st_off += len;
       if (st_off == st_len) { s.end[e_st] = n_st; e_st = next_entry(e_st); st_off = 0; ++unwritten; }
       if (unwritten && n_st - s.end[e_wr] >= (uint32_t)kSif) {
+        const unsigned long long t0 = stamp();
         bulk_wait<kSif>();   // this step only: every group but the last kSif has landed in global memory
+        charge(MP_CHUNK_WAIT, t0);
         ld_limit = n_st + P;
         report(false);
       }
     } else if (unwritten && !ld_have) {
+      const unsigned long long t0 = stamp();
       bulk_wait<0>();        // the queue ran dry: finish now
+      charge(MP_DRY_WAIT, t0);
       ld_limit = n_st + P;
       report(true);
     } else if (quit && !unwritten) {
-      return true;
+      return leave(true);
     }
+  }
+}
+
+// Control's choice of mover: the stores-in-flight split, or the profiled default split when EngineCtl::mover_prof is set.
+__device__ __forceinline__ bool run_mover(Smem& s, unsigned sif, unsigned long long* prof) {
+  if (prof) return move_chunks<kSifDefault, true>(s, prof);
+  switch (sif) {
+    case 8: return move_chunks<8, false>(s, nullptr);
+    case 6: return move_chunks<6, false>(s, nullptr);
+    case 4: return move_chunks<4, false>(s, nullptr);
+    default: return move_chunks<kSifDefault, false>(s, nullptr);
   }
 }
 
@@ -852,11 +888,13 @@ __device__ __forceinline__ int chunk_written(Smem& s, int e, uint32_t& ph, bool 
   }
 }
 
-// Control, lane 0: a chunk's bytes are written and released at gpu scope by the threads that wrote them.  Count it;
-// true when that finished its WQE.
+// Control, lane 0: a chunk's bytes are written, and this thread has observed that through a CTA-scope synchronisation
+// with the threads that wrote them (the mover's qdone arrive, or the generic copy's named barrier).  Count it; true when
+// that finished its WQE.
 __device__ __forceinline__ bool complete_chunk(QpDev* qp, unsigned long long w, uint32_t nch) {
   Resolved* r = qp->resolved + (w & ((1u << qp->sq_log) - 1));
-  // This chunk's bytes before the count that may complete the WQE.  gpu scope is enough even
+  // This chunk's bytes before the count that may complete the WQE: the fence is cumulative over every write this thread
+  // has observed, so it releases the mover's and the generic threads' stores as well as its own.  gpu scope is enough even
   // when the CQ or the payload lives in host / peer memory: the retirer's system-scope
   // fence in write_cqe() is cumulative over everything this chain of gpu-scope releases made
   // visible to it (a sys fence per chunk cost ~2x on host-resident queues, measured).
@@ -883,8 +921,8 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
   const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   if (warp == 1) {
     if (lane == 0) {
-      const unsigned sif = ctl->stores_in_flight;
-      const bool ok = sif == 8 ? move_chunks<8>(s) : (sif == 6 ? move_chunks<6>(s) : move_chunks<4>(s));
+      unsigned long long* prof = ctl->mover_prof;
+      const bool ok = run_mover(s, ctl->stores_in_flight, prof ? prof + (size_t)blockIdx.x * MOVER_PROF_N : nullptr);
       if (!ok) { ctl->fatal = 1; *(volatile int*)&s.mover_fatal = 1; }
     }
     return;
@@ -1064,8 +1102,9 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
 // What the engine's copy loop reaches with nothing around it: CTA b streams span bytes from src + b * span to
 // dst + b * span as ONE queued chunk -- no claims, no chunk boundaries, no completion bookkeeping.  The distance between
 // this and the engine on the same CTA count is what the per-chunk work costs (tools/engine_pipeline.py).
+// prof (may be null): the mover's stall profile, MOVER_PROF_N counters per CTA, as the engine's.
 __global__ void __launch_bounds__(kThreads, 1) engine_ceiling_kernel(uint64_t src, uint64_t dst, uint32_t span, unsigned sif,
-                                                                    unsigned int* fatal) {
+                                                                    unsigned int* fatal, unsigned long long* prof) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
   if (threadIdx.x == 0) init_barriers(s);
@@ -1077,7 +1116,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_ceiling_kernel(uint64_t sr
     s.q[1].len = kQuitLen;
     mbar_arrive(&s.qfull[1]);
   } else if (threadIdx.x == 32) {
-    const bool ok = sif == 8 ? move_chunks<8>(s) : (sif == 6 ? move_chunks<6>(s) : move_chunks<4>(s));
+    const bool ok = run_mover(s, sif, prof ? prof + (size_t)blockIdx.x * MOVER_PROF_N : nullptr);
     if (!ok && fatal) atomicAdd(fatal, 1u);
   }
 }

@@ -86,6 +86,8 @@ struct Hca {
   MKeyEntry* d_mkeys = nullptr;
   std::vector<Mr> mrs;
   EngineCtl* d_ctl = nullptr;
+  unsigned long long* d_prof = nullptr;   // the mover's stall profile: kMaxEngineCtas rows of MOVER_PROF_N
+  bool prof_on = false;                   // the running / last engine was started with RN_ENGINE_PROFILE=1
   volatile uint32_t* h_stop = nullptr;
   uint8_t* scratch = nullptr;          // mapped pinned result area (kernels write, host reads)
   size_t scratch_size = 0;
@@ -211,6 +213,7 @@ RN_API int rn_hca_open(int dev, uint32_t max_mkeys, uint32_t max_qps, uint64_t a
   h->d_mkeys = (MKeyEntry*)arena_alloc(h, sizeof(MKeyEntry) * h->max_mkeys, false);
   h->d_ctl = (EngineCtl*)arena_alloc(h, sizeof(EngineCtl), false);
   h->d_qptab = (QpDev**)arena_alloc(h, sizeof(QpDev*) * h->max_qps, false);
+  h->d_prof = (unsigned long long*)arena_alloc(h, sizeof(unsigned long long) * MOVER_PROF_N * kMaxEngineCtas, false);
   h->h_stop = (volatile uint32_t*)arena_alloc(h, 64, true);
   h->scratch_size = 256 << 10;
   h->scratch = (uint8_t*)arena_alloc(h, h->scratch_size, true);
@@ -1003,7 +1006,16 @@ RN_API int rn_engine_start(void* hca, int n_ctas, uint64_t idle_timeout_ms, uint
   {
     const char* e = getenv("RN_ENGINE_STORES_IN_FLIGHT");
     int v = e ? atoi(e) : 0;
-    c.stores_in_flight = (v == 4 || v == 6 || v == 8) ? (unsigned)v : 4u;
+    c.stores_in_flight = (v == 2 || v == 4 || v == 6 || v == 8) ? (unsigned)v : (unsigned)eng::kSifDefault;
+  }
+  {
+    // The mover's stall profile (rn_engine_mover_profile); off, the engine runs the unprofiled movers.
+    const char* e = getenv("RN_ENGINE_PROFILE");
+    h->prof_on = e && atoi(e) == 1;
+    if (h->prof_on) {
+      CU_OK(cudaMemsetAsync(h->d_prof, 0, sizeof(unsigned long long) * MOVER_PROF_N * n_ctas, h->ctl));
+      c.mover_prof = h->d_prof;
+    }
   }
   int rc = push(h, h->d_ctl, &c, sizeof c);
   if (rc) return rc;
@@ -1031,16 +1043,19 @@ RN_API int rn_engine_stop(void* hca) {
 
 // The engine's copy loop alone on `ctas` CTAs (eng::engine_ceiling_kernel): CTA b copies span bytes at offset b * span.
 // src, dst and span must be 16-byte aligned.  fatal_dev (device u32, may be 0) counts CTAs whose loads never landed.
-RN_API int rn_k_engine_ceiling(uint64_t stream, uint64_t src, uint64_t dst, uint64_t span, int ctas, uint64_t fatal_dev) {
+// prof_dev (device u64[ctas * MOVER_PROF_N], zeroed by the caller, may be 0) receives the mover's stall profile.
+RN_API int rn_k_engine_ceiling(uint64_t stream, uint64_t src, uint64_t dst, uint64_t span, int ctas, uint64_t fatal_dev,
+                               uint64_t prof_dev) {
   if (ctas <= 0 || !span || span > 0xffffffffull || ((src | dst | span) & 15))
     return fail(-22, "engine_ceiling: need ctas > 0 and a 16-byte aligned span below 4 GiB");
   const size_t smem = eng::engine_smem_bytes();
   CU_OK(cudaFuncSetAttribute(eng::engine_ceiling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const char* e = getenv("RN_ENGINE_STORES_IN_FLIGHT");
   const int v = e ? atoi(e) : 0;
-  const unsigned sif = (v == 4 || v == 6 || v == 8) ? (unsigned)v : 4u;
+  const unsigned sif = (v == 2 || v == 4 || v == 6 || v == 8) ? (unsigned)v : (unsigned)eng::kSifDefault;
   eng::engine_ceiling_kernel<<<ctas, eng::kThreads, smem, (cudaStream_t)stream>>>(src, dst, (uint32_t)span, sif,
-                                                                                  (unsigned int*)fatal_dev);
+                                                                                  (unsigned int*)fatal_dev,
+                                                                                  (unsigned long long*)prof_dev);
   CU_OK(cudaGetLastError());
   return 0;
 }
@@ -1056,6 +1071,20 @@ RN_API int rn_engine_stats(void* hca, RnEngineStats* out) {
   out->running_ctas = c.running_ctas; out->exited_idle = c.exited_idle; out->n_qps = c.n_qps;
   out->ctas = (uint32_t)h->engine_ctas;
   return 0;
+}
+
+// The mover's stall profile of the last engine run started with RN_ENGINE_PROFILE=1 (rows are written as each mover
+// leaves, so read it after the engine stopped): copies min(engine CTAs, max_rows) rows of MOVER_PROF_N u64 (MoverProf
+// order) to out and returns the number of rows; 0 when that run was not profiled.
+RN_API int rn_engine_mover_profile(void* hca, uint64_t* out, int max_rows) {
+  Hca* h = (Hca*)hca;
+  if (!h->prof_on) return 0;
+  if (rn_engine_running(h)) return fail(-16, "engine_mover_profile: the engine is still running");
+  const int rows = h->engine_ctas < max_rows ? h->engine_ctas : max_rows;
+  if (rows <= 0) return 0;
+  CU_OK(cudaSetDevice(h->dev));
+  const int rc = pull(h, out, h->d_prof, sizeof(unsigned long long) * MOVER_PROF_N * rows);
+  return rc ? rc : rows;
 }
 
 // ------------------------------------------------------------------ test hooks (tier-0, no GPU)

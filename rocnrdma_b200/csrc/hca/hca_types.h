@@ -152,12 +152,28 @@ struct EngineCtl {
   unsigned int exited_idle;        // set when the watchdog ended the engine
   unsigned int fatal;              // a DMA never completed; engine bailed out
   unsigned int quit_all;           // the host-doorbell watcher found the engine idle / drained: everybody leaves
-  unsigned int stores_in_flight;   // smem ring split: this many TMA stores may still be reading smem, the rest of the ring holds loads (4, 6 or 8)
+  unsigned int stores_in_flight;   // smem ring split: this many TMA stores may still be reading smem, the rest of the ring holds loads (2, 4, 6 or 8)
   unsigned int oneshot;            // exit as soon as every queue is drained (profiling under ncu: kernels are serialised there)
   unsigned int host_native_atomics;  // cudaDevAttrHostNativeAtomicSupported: a GPU atomic on pinned host memory is atomic there
   unsigned long long n_bulk_chunks;     // chunks moved through the TMA bulk path
   unsigned long long t_start, t_exit;   // %globaltimer of engine start / exit (CTA 0)
+  unsigned long long* mover_prof;       // RN_ENGINE_PROFILE=1: MOVER_PROF_N counters per CTA (eng::move_chunks), else null
 };
+
+// The mover's stall profile, one row of MOVER_PROF_N u64 per CTA: %globaltimer ns spent in each wait, the mover's whole
+// run, and the chunks it reported.  Order shared with api.MOVER_PROFILE_FIELDS.
+enum MoverProf : int {
+  MP_WAIT_READ = 0,   // bulk_wait_read: no free ring stage for the next load
+  MP_FULL,            // full[] mbarrier: the next stage's load has not landed
+  MP_CHUNK_WAIT,      // bulk_wait<kSif>: a chunk's stores completing before it is reported
+  MP_REPORT,          // reporting written chunks to control (qdone arrive)
+  MP_DRY_WAIT,        // bulk_wait<0>: the queue ran dry, the ring drains
+  MP_QFULL_IDLE,      // ring empty, nothing owed: waiting for control to queue a chunk
+  MP_TOTAL,           // entry to exit
+  MP_CHUNKS,          // chunks reported
+  MOVER_PROF_N
+};
+constexpr int kMaxEngineCtas = 256;     // rows of the profile array
 
 // Status codes returned by device-side waits (never spin forever: SURVEY.md section 5).
 enum WaitStatus : int { WAIT_OK = 0, WAIT_TIMEOUT = -1, WAIT_CQE_ERROR = -2, WAIT_QP_ERROR = -3 };

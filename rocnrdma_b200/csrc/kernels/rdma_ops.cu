@@ -586,6 +586,75 @@ RN_API int rn_k_signal_wait(uint64_t stream, uint64_t signal, uint64_t until, ui
   return (int)cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- CQ watch (receiver-side payload check)
+// Watches a send CQ without consuming it (the poster that owns the CQ keeps reaping it; the ring must hold all n CQEs, so
+// no slot is reused while this runs).  Thread 0 waits for CQE k (k = 0 .. n-1) with a relaxed load of its owner byte and
+// a system-scope fence (acquire); then the whole CTA compares, at once, the message the CQE names (wqe_counter c: bytes
+// at (c % nslots) * stride of dst and src).  Of each `piece` bytes of a message only the last `tail` are compared --
+// what a chunk of `piece` bytes stores last -- so the check keeps up with a full-rate stream.  Each wait is bounded by
+// timeout_ns.  out: [status, t_start, t_end, CQEs seen, mismatching 16-byte words, error CQEs, 0, 0]
+constexpr int kCqWatchThreads = 1024;
+__global__ void __launch_bounds__(kCqWatchThreads, 1) cq_watch_kernel(const CqDev* cq, uint32_t n, const uint8_t* dst,
+                                                                      const uint8_t* src, uint64_t stride, uint32_t nslots,
+                                                                      uint64_t msg_bytes, uint64_t piece, uint64_t tail,
+                                                                      unsigned long long timeout_ns, unsigned long long* out) {
+  __shared__ unsigned long long s_bad;
+  __shared__ uint32_t s_counter, s_errs;
+  __shared__ int s_status;
+  const unsigned long long t0 = globaltimer_ns();
+  const uint8_t* buf = cq->buf;
+  const uint32_t log_n = cq->log_n;
+  unsigned long long bad = 0;
+  if (threadIdx.x == 0) { s_bad = 0; s_errs = 0; s_status = WAIT_OK; }
+  __syncthreads();
+  uint32_t k = 0;
+  for (; k < n; ++k) {
+    if (threadIdx.x == 0) {
+      const uint8_t* cqe = buf + ((size_t)(k & ((1u << log_n) - 1)) << 6);
+      const unsigned long long tw = globaltimer_ns();
+      uint4 t = ld_v4_volatile(cqe + 48);
+      while (!cqe_valid((uint8_t)(t.w >> 24), k, log_n)) {
+        if (globaltimer_ns() - tw > timeout_ns) { s_status = WAIT_TIMEOUT; break; }
+        t = ld_v4_volatile(cqe + 48);
+      }
+      fence_sys();   // acquire: the payload the CQE announces
+      s_counter = be16((uint16_t)(t.w & 0xffff));
+      if (cqe_opcode((uint8_t)(t.w >> 24)) == CQE_REQ_ERR) ++s_errs;
+    }
+    __syncthreads();   // thread 0's acquire, then the barrier: every thread's loads below see the message
+    if (s_status != WAIT_OK) break;
+    const uint64_t base = (uint64_t)(s_counter % nslots) * stride;
+    for (uint64_t p = 0; p < msg_bytes; p += piece) {
+      const uint64_t end = p + piece < msg_bytes ? p + piece : msg_bytes;
+      const uint64_t beg = end - (end - p < tail ? end - p : tail);
+      for (uint64_t o = beg + (uint64_t)threadIdx.x * 16; o + 16 <= end; o += (uint64_t)kCqWatchThreads * 16) {
+        const uint4 x = ld_v4_volatile(dst + base + o), y = ld_v4_volatile(src + base + o);
+        if (x.x != y.x || x.y != y.y || x.z != y.z || x.w != y.w) ++bad;
+      }
+    }
+    __syncthreads();   // s_counter is rewritten next round
+  }
+  for (int o = 16; o; o >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, o);
+  if ((threadIdx.x & 31) == 0 && bad) atomicAdd(&s_bad, bad);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    out[0] = (unsigned long long)(long long)s_status;
+    out[1] = t0; out[2] = globaltimer_ns(); out[3] = k; out[4] = s_bad; out[5] = s_errs;
+  }
+}
+
+RN_API int rn_k_cq_watch(uint64_t stream, uint64_t cq_dev, uint32_t n, uint64_t dst, uint64_t src, uint64_t stride,
+                         uint32_t nslots, uint64_t msg_bytes, uint64_t piece, uint64_t tail, uint64_t timeout_ms,
+                         uint64_t out_dev) {
+  if (!nslots || !piece || !tail || ((dst | src | stride | piece | tail) & 15)) return -22;
+  unsigned long long* o = (unsigned long long*)out_dev;
+  for (int i = 0; i < 8; ++i) o[i] = 0;
+  cq_watch_kernel<<<1, kCqWatchThreads, 0, (cudaStream_t)stream>>>(
+      (const CqDev*)cq_dev, n, (const uint8_t*)dst, (const uint8_t*)src, stride, nslots, msg_bytes, piece, tail,
+      (timeout_ms ? timeout_ms : 2000) * 1000000ull, o);
+  return (int)cudaGetLastError();
+}
+
 // ---------------------------------------------------------------- K6: verification
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x += 0x9e3779b97f4a7c15ull;
@@ -704,6 +773,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncGetAttributes(&a, put_signal_kernel);
   cudaFuncGetAttributes(&a, put_inline_kernel);
   cudaFuncGetAttributes(&a, signal_wait_kernel);
+  cudaFuncGetAttributes(&a, cq_watch_kernel);
   cudaFuncGetAttributes(&a, fill_random_kernel);
   cudaFuncGetAttributes(&a, fill_bf16_kernel);
   cudaFuncGetAttributes(&a, checksum_kernel);

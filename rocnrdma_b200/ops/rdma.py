@@ -323,6 +323,33 @@ def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, st
     return parse_signal_wait(out_view)
 
 
+def cq_watch(cq, n: int, dst, src, slot_stride: int, nslots: int, msg_bytes: int, piece: int, tail: int = 16384,
+             timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = 30720):
+    """Receiver-side check of a device send CQ that another kernel (the poster) consumes: waits for each of its first
+    ``n`` CQEs in turn without consuming them (the CQ must hold ``n``), and the moment CQE ``k`` is visible compares the
+    message it names -- slot ``wqe_counter % nslots`` of ``dst`` and ``src`` (tensors or ``(address, nbytes)`` pairs) at
+    ``slot_stride`` -- with every ``piece`` bytes checked on their last ``tail`` bytes.  Returns
+    ``dict(status, seen, mismatches, error_cqes, device_ns)``."""
+    from ..api import _ptr_len
+    ctx = cq.ctx
+    ws = work_stream(ctx, stream)
+    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    rc = N.load().rn_k_cq_watch(_stream_ptr(ws), cq.dev_ptr, n, _ptr_len(dst, 1)[0], _ptr_len(src, 1)[0], slot_stride, nslots,
+                                msg_bytes, piece, tail, timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"cq_watch launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_cq_watch(out_view)
+
+
+def parse_cq_watch(view) -> dict:
+    """Decode the record :func:`cq_watch` leaves in its scratch slot (for ``sync=False`` callers)."""
+    w = (C.c_int64 * 8).from_buffer(view)
+    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), seen=w[3], mismatches=w[4], error_cqes=w[5], device_ns=w[2] - w[1])
+
+
 def parse_signal_wait(view) -> dict:
     """Decode the record :func:`signal_wait` leaves in its scratch slot (for ``sync=False`` callers)."""
     w = (C.c_int64 * 8).from_buffer(view)

@@ -10,7 +10,12 @@ derived from (a) and (b): the engine cuts a 256 MiB WQE into granules of max(chu
 CTA moves one granule in granule / (rate / CTAs); the dead time is the engine's time per granule minus the ceiling's.
 The card name, power limit and max SM clock are read (nvidia-smi --query-gpu, read-only) in the same run.
 
-    python tools/engine_pipeline.py [--ctas 8,16,32,64] [--reps 3] [--out results.json]
+--profile adds, once per CTA count after the timed runs, one profiled run of each (the engine under RN_ENGINE_PROFILE=1,
+the ceiling kernel with a profile buffer): where the mover's time went, as µs per granule summed over the CTAs' movers
+and divided by the granules moved (Context.engine_mover_profile; bucket names in api.MOVER_PROFILE_FIELDS).  "issue" is
+what is left of the mover's total after every wait: issuing loads and stores, polling, bookkeeping.
+
+    python tools/engine_pipeline.py [--ctas 8,16,32,64] [--reps 3] [--profile] [--out results.json]
 
 The result is printed as JSON; --out also writes it to a file.
 """
@@ -58,6 +63,7 @@ def main():
     ap.add_argument("--ctas", default="8,16,32,64")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--seconds", type=float, default=0.4, help="approximate length of each timed window")
+    ap.add_argument("--profile", action="store_true", help="also profile where the mover's time goes (engine and ceiling)")
     ap.add_argument("--out", default="", help="also write the JSON result to this file")
     args = ap.parse_args()
 
@@ -80,10 +86,14 @@ def main():
     total = MSG * NSLOTS
     torch.cuda.synchronize()
 
-    def ceiling(n: int) -> float:
+    nf = len(rn.api.MOVER_PROFILE_FIELDS)
+    prof = torch.zeros(max(ctas_list) * nf, dtype=torch.int64, device=dev)
+
+    def ceiling(n: int, profile: bool = False) -> float:
         span = total // n // KSUB * KSUB
+        pp = prof.data_ptr() if profile else 0
         launch = lambda: N.check(lib.rn_k_engine_ceiling(stream.cuda_stream, src.data_ptr(), dst.data_ptr(), span, n,
-                                                         fatal.data_ptr()), "engine_ceiling")
+                                                         fatal.data_ptr(), pp), "engine_ceiling")
         launch()
         launch()
         stream.synchronize()
@@ -96,7 +106,8 @@ def main():
         assert int(fatal.item()) == 0, "ceiling kernel: a bulk load never landed"
         return iters * span * n / (ev0.elapsed_time(ev1) * 1e-3) / 1e9
 
-    def engine(n: int) -> float:
+    def engine(n: int, profile: bool = False) -> float:
+        os.environ["RN_ENGINE_PROFILE"] = "1" if profile else "0"
         ctx.engine_start(ctas=n, idle_timeout_ms=20000)
         kw = dict(window=8, slot_stride=MSG, nslots=NSLOTS, stream=stream, timeout_ms=20000)
         r = ops.rdma_stream(qp, W.OP_RDMA_WRITE, ms, md, MSG, iters=8, **kw)
@@ -107,6 +118,30 @@ def main():
         st = ctx.engine_stats()
         assert r.ok and st["fatal"] == 0, (r.status, st)
         return r.gbps
+
+    def per_granule(rows, n_granules: float) -> dict:
+        """Bucket ns summed over the movers, as µs per granule moved."""
+        tot = {k: sum(r[k] for r in rows) for k in rn.api.MOVER_PROFILE_FIELDS}
+        out = {k[:-3]: round(tot[k] / n_granules / 1e3, 3) for k in rn.api.MOVER_PROFILE_FIELDS if k.endswith("_ns")}
+        waits = sum(v for k, v in out.items() if k != "total")
+        out["issue"] = round(out["total"] - waits, 3)
+        out["chunks"] = tot["chunks"]
+        return out
+
+    def profile(n: int) -> dict:
+        g = granule(MSG, n)
+        prof.zero_()
+        gb_c = ceiling(n, profile=True)         # rows are those of the last launch: n spans
+        span = total // n // KSUB * KSUB
+        ceil_rows = rn.api.mover_profile_rows(prof[:n * nf].cpu().tolist())
+        gb_e = engine(n, profile=True)
+        eng_rows = ctx.engine_mover_profile()
+        os.environ.pop("RN_ENGINE_PROFILE", None)
+        n_chunks = sum(r["chunks"] for r in eng_rows)
+        assert n_chunks == ctx.engine_stats()["n_bulk_chunks"], (n_chunks, ctx.engine_stats())
+        return {"ctas": n, "granule_bytes": g,
+                "ceiling": {"gbps": round(gb_c, 1), "us_per_granule": per_granule(ceil_rows, n * span / g)},
+                "engine": {"gbps": round(gb_e, 1), "us_per_granule": per_granule(eng_rows, n_chunks)}}
 
     def memcpy() -> float:
         with torch.cuda.stream(stream):
@@ -133,6 +168,14 @@ def main():
         runs[("memcpy", 0)].append(memcpy())
         print(f"rep {rep}: memcpy d2d {runs[('memcpy', 0)][-1]:.1f} GB/s", flush=True)
 
+    profiles = []
+    if args.profile:
+        for n in ctas_list:
+            profiles.append(profile(n))
+            p = profiles[-1]
+            print(f"profile ctas {n}: ceiling {p['ceiling']['us_per_granule']}", flush=True)
+            print(f"profile ctas {n}: engine  {p['engine']['us_per_granule']}", flush=True)
+
     rows = []
     for n in ctas_list:
         a, b = summary(runs[("ceiling", n)]), summary(runs[("engine", n)])
@@ -144,8 +187,10 @@ def main():
                      "us_per_granule_ceiling": round(t_a, 2), "us_per_granule_engine": round(t_b, 2),
                      "dead_us_per_chunk": round(t_b - t_a, 2)})
     out = {"card": card(), "msg_bytes": MSG, "window": 8, "nslots": NSLOTS, "reps": args.reps,
-           "stores_in_flight": int(os.environ.get("RN_ENGINE_STORES_IN_FLIGHT", "4") or 4),
+           "stores_in_flight": int(os.environ.get("RN_ENGINE_STORES_IN_FLIGHT", "2") or 2),
            "memcpy_d2d_gbps": summary(runs[("memcpy", 0)]), "rows": rows}
+    if profiles:
+        out["mover_profile"] = profiles
     ctx.close()
     print(json.dumps(out, indent=1))
     if args.out:
