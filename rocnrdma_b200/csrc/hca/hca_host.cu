@@ -610,7 +610,7 @@ RN_API int rn_create_qp(void* hca, void* scq, void* rcq, uint32_t nsq, uint32_t 
   q->h.sq_in_device = host ? 0 : 1;
   q->h.sys_scope = (host || q->scq->mem == MEM_HOST_PINNED || q->rcq->mem == MEM_HOST_PINNED) ? 1 : 0;
   // doorbell register idle value: "last posted index = 0xffff" <=> nothing posted
-  unsigned long long bf0 = (unsigned long long)ctrl_word0(OP_NOP, 0xffff) | ((unsigned long long)ctrl_word1(q->h.qpn, 0) << 32);
+  unsigned long long bf0 = doorbell_word(q->h.qpn, 0xffff);
   int rc = 0;
   if (host) *bf = bf0; else rc = push(h, bf, &bf0, 8);
   if (!rc) rc = push(h, q->d, &q->h, sizeof(QpDev));
@@ -693,7 +693,7 @@ RN_API int rn_modify_qp(void* qp, uint32_t new_state) {
     fresh.state = QPS_RESET;
     q->h = fresh;
     q->h_sq_pi = q->h_rq_pi = 0;
-    unsigned long long bf0 = (unsigned long long)ctrl_word0(OP_NOP, 0xffff) | ((unsigned long long)ctrl_word1(q->h.qpn, 0) << 32);
+    unsigned long long bf0 = doorbell_word(q->h.qpn, 0xffff);
     int rc = push(h, q->h.bf, &bf0, 8);
     uint32_t z[2] = {0, 0};
     if (!rc) rc = push(h, q->h.dbr, z, 8);
@@ -858,7 +858,7 @@ static int host_sq_publish(Qp* q, const Wqe64& w, uint64_t idx, uint64_t* idx_ou
   rc = host_store(q, &q->h.dbr[DBR_SND], &rec, 4);
   if (rc) return rc;
   __sync_synchronize();
-  unsigned long long db = (unsigned long long)ctrl_word0(OP_NOP, (uint16_t)idx) | ((unsigned long long)ctrl_word1(q->h.qpn, 0) << 32);
+  unsigned long long db = doorbell_word(q->h.qpn, (uint16_t)idx);
   rc = host_store(q, q->h.bf, &db, 8);
   if (rc) return rc;
   q->h_sq_pi = idx + 1;
@@ -886,7 +886,7 @@ RN_API int rn_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey
       build_atomic_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, laddr, lkey, raddr, rkey, 0, 0, (uint8_t)flags, bytes);
       break;
     case OP_NOP:
-      encode_ctrl(&w.ctrl, OP_NOP, (uint16_t)idx, q->h.qpn, 1, (uint8_t)flags, 0);
+      build_nop_wqe(&w, (uint16_t)idx, q->h.qpn, (uint8_t)flags);
       break;
     default:
       // deliberately still posted: lets tests drive the engine's bad-opcode path

@@ -96,55 +96,16 @@ __device__ __forceinline__ unsigned long long sq_reserve(QpDev* qp, uint32_t n,
   return idx;
 }
 
-// -------------------------------------------------------------- WQE writers
-// Four 16-byte stores = one WQEBB.  Fields are big-endian on the wire.
-__device__ __forceinline__ void write_rdma_wqe(QpDev* qp, unsigned long long idx, uint8_t opcode,
-                                               uint64_t laddr, uint32_t lkey, uint64_t raddr,
-                                               uint32_t rkey, uint32_t bytes, uint8_t fm_ce_se,
-                                               uint32_t imm = 0) {
-  uint8_t* slot = qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6);
-  // ctrl: opmod_idx_opcode | qpn_ds | sig,rsvd,fm_ce_se | imm
-  st_v4(slot + 0, ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(qp->qpn, 3), (uint32_t)fm_ce_se << 24,
-        be32(imm));
-  // raddr: be64 raddr | be32 rkey | 0      (be64 in memory = be32(hi), be32(lo))
-  st_v4(slot + 16, be32((uint32_t)(raddr >> 32)), be32((uint32_t)raddr), be32(rkey), 0u);
-  // data: be32 byte_count | be32 lkey | be64 addr
-  st_v4(slot + 32, be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(laddr >> 32)), be32((uint32_t)laddr));
-  st_v4(slot + 48, 0u, 0u, 0u, 0u);
+// -------------------------------------------------------------- WQE store
+__device__ __forceinline__ uint8_t* sq_slot(const QpDev* qp, unsigned long long idx) {
+  return qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6);
 }
-__device__ __forceinline__ void write_send_wqe(QpDev* qp, unsigned long long idx, uint8_t opcode,
-                                               uint64_t laddr, uint32_t lkey, uint32_t bytes,
-                                               uint8_t fm_ce_se, uint32_t imm = 0) {
-  uint8_t* slot = qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6);
-  st_v4(slot + 0, ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(qp->qpn, 2), (uint32_t)fm_ce_se << 24,
-        be32(imm));
-  st_v4(slot + 16, be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(laddr >> 32)), be32((uint32_t)laddr));
-  st_v4(slot + 32, 0u, 0u, 0u, 0u);
-  st_v4(slot + 48, 0u, 0u, 0u, 0u);
+// One WQEBB as four 16-byte stores.  The bytes come from the mlx5_wire.h builders, built into a local Wqe64.
+__device__ __forceinline__ void store_wqe(uint8_t* dst, const Wqe64& w) {
+  const uint4* v = reinterpret_cast<const uint4*>(&w);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) st_v4(dst + 16 * i, v[i].x, v[i].y, v[i].z, v[i].w);
 }
-
-// 8-byte atomic (ds = 4): ctrl | raddr | atomic (swap_add, compare) | data (the local 8 bytes that receive the
-// original remote value).  FA: swap_add = addend, compare unused (0); CS: swap_add = swap, compare = compare.
-__device__ __forceinline__ void atomic_wqe_stores(uint8_t* slot, uint32_t w0, uint32_t w1, uint8_t opcode, uint64_t laddr,
-                                                  uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add,
-                                                  uint64_t compare, uint8_t fm_ce_se) {
-  if (opcode != OP_ATOMIC_CS) compare = 0;
-  st_v4(slot + 0, w0, w1, (uint32_t)fm_ce_se << 24, 0u);
-  st_v4(slot + 16, be32((uint32_t)(raddr >> 32)), be32((uint32_t)raddr), be32(rkey), 0u);
-  st_v4(slot + 32, be32((uint32_t)(swap_add >> 32)), be32((uint32_t)swap_add), be32((uint32_t)(compare >> 32)), be32((uint32_t)compare));
-  st_v4(slot + 48, be32(8u), be32(lkey), be32((uint32_t)(laddr >> 32)), be32((uint32_t)laddr));
-}
-__device__ __forceinline__ void write_atomic_wqe(QpDev* qp, unsigned long long idx, uint8_t opcode, uint64_t laddr,
-                                                 uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add,
-                                                 uint64_t compare, uint8_t fm_ce_se) {
-  uint8_t* slot = qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6);
-  atomic_wqe_stores(slot, ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(qp->qpn, 4), opcode, laddr, lkey, raddr, rkey,
-                    swap_add, compare, fm_ce_se);
-}
-
-// Inline payload held in registers: up to MAX_INLINE bytes in memory order (little-endian words), zero past its length.
-struct InlinePayload { uint32_t w[7]; };
-static_assert(sizeof(InlinePayload) == MAX_INLINE, "inline payload");
 
 // Read n (1..MAX_INLINE) bytes at p into registers.  Any address works (the memory need not be registered); word loads
 // when p and n are 4-byte multiples, byte loads otherwise -- nothing past p + n is read.
@@ -167,31 +128,6 @@ __device__ __forceinline__ InlinePayload inline_load(const void* p, uint32_t n) 
   return d;
 }
 
-// Inline WQE (n in 1..MAX_INLINE), the bytes build_inline_wqe writes.  RDMA_WRITE / WRITE_IMM: ctrl | raddr | be32
-// (n | INLINE_SEG) and the payload from byte 36; SEND / SEND_IMM: ctrl | inline header and the payload from byte 20.
-__device__ __forceinline__ void inline_wqe_stores(uint8_t* slot, uint16_t idx, uint32_t qpn, uint8_t opcode, uint64_t raddr,
-                                                  uint32_t rkey, const InlinePayload& d, uint32_t n, uint8_t fm_ce_se,
-                                                  uint32_t imm) {
-  const uint32_t hdr = be32(n | INLINE_SEG);
-  if (opcode == OP_SEND || opcode == OP_SEND_IMM) {
-    st_v4(slot + 0, ctrl_word0(opcode, idx), ctrl_word1(qpn, 1 + inline_segs(n)), (uint32_t)fm_ce_se << 24, be32(imm));
-    st_v4(slot + 16, hdr, d.w[0], d.w[1], d.w[2]);
-    st_v4(slot + 32, d.w[3], d.w[4], d.w[5], d.w[6]);
-    st_v4(slot + 48, 0u, 0u, 0u, 0u);
-  } else {
-    st_v4(slot + 0, ctrl_word0(opcode, idx), ctrl_word1(qpn, 2 + inline_segs(n)), (uint32_t)fm_ce_se << 24, be32(imm));
-    st_v4(slot + 16, be32((uint32_t)(raddr >> 32)), be32((uint32_t)raddr), be32(rkey), 0u);
-    st_v4(slot + 32, hdr, d.w[0], d.w[1], d.w[2]);
-    st_v4(slot + 48, d.w[3], d.w[4], d.w[5], d.w[6]);
-  }
-}
-__device__ __forceinline__ void write_inline_wqe(QpDev* qp, unsigned long long idx, uint8_t opcode, uint64_t raddr,
-                                                 uint32_t rkey, const InlinePayload& d, uint32_t n, uint8_t fm_ce_se,
-                                                 uint32_t imm = 0) {
-  inline_wqe_stores(qp->sq + ((idx & ((1ull << qp->sq_log) - 1)) << 6), (uint16_t)idx, qp->qpn, opcode, raddr, rkey, d, n,
-                    fm_ce_se, imm);
-}
-
 // -------------------------------------------------------------- doorbell
 // Publish WQEs [idx, idx+n): in index order, update the doorbell record, then ring
 // the doorbell register with the first 8 bytes of the last WQE's ctrl segment.
@@ -201,16 +137,14 @@ __device__ __forceinline__ void st_u64_release_scope(void* p, unsigned long long
   if (sys) asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
   else asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
-// Ring the doorbell for WQEs [from, to): record, then register (a release store), then ready_head.
-__device__ __forceinline__ void ring_doorbell(QpDev* qp, unsigned long long to, bool sys) {
-  const unsigned long long last = to - 1;
-  st_u32_volatile(&qp->dbr[DBR_SND], be32((uint32_t)(to & 0xffff)));
-  unsigned long long db = (unsigned long long)ctrl_word0(OP_NOP, (uint16_t)last) |
-                          ((unsigned long long)ctrl_word1(qp->qpn, 0) << 32);
+// Ring the doorbell for every WQE below `to`: record, then register.
+__device__ __forceinline__ void ring_doorbell(uint32_t* dbr, unsigned long long* bf, uint32_t qpn, unsigned long long to,
+                                              bool sys) {
+  st_u32_volatile(&dbr[DBR_SND], be32((uint32_t)(to & 0xffff)));
   // The doorbell register store is a RELEASE: WQE bytes and the doorbell record are visible before
   // it (what the engine audits, and what a ConnectX requires: it may fetch the record and the WQE as
   // soon as the MMIO write lands).
-  st_u64_release_scope(qp->bf, db, sys);
+  st_u64_release_scope(bf, doorbell_word(qpn, (uint16_t)(to - 1)), sys);
 }
 
 // Single-poster submit: the calling thread is the only one posting to this QP.
@@ -222,8 +156,7 @@ __device__ __forceinline__ void ring_doorbell(QpDev* qp, unsigned long long to, 
 __device__ __forceinline__ bool poster_sys(const QpDev* qp) { return qp->sq_in_device == 0; }
 
 __device__ __forceinline__ int sq_submit_exclusive(QpDev* qp, unsigned long long idx, uint32_t n) {
-  const bool sys = poster_sys(qp);
-  ring_doorbell(qp, idx + n, sys);
+  ring_doorbell(qp->dbr, qp->bf, qp->qpn, idx + n, poster_sys(qp));
   trace_stamp(qp, idx, TR_POST);
   st_u64_relaxed(&qp->ready_head, idx + n);
   return WAIT_OK;
@@ -253,7 +186,7 @@ __device__ __forceinline__ int sq_submit_shared(QpDev* qp, unsigned long long id
     while (to - h <= mask && ld_u32_volatile(&qp->ready_flags[to & mask]) == (uint32_t)(to + 1)) ++to;
     if (to > h) {
       if (sys) __threadfence_system(); else __threadfence();      // other posters' WQE bytes (seen via their flags) before the doorbell
-      ring_doorbell(qp, to, sys);
+      ring_doorbell(qp->dbr, qp->bf, qp->qpn, to, sys);
       st_u64_relaxed(&qp->ready_head, to);
     }
     __threadfence();
@@ -263,35 +196,42 @@ __device__ __forceinline__ int sq_submit_shared(QpDev* qp, unsigned long long id
   }
 }
 
-__device__ __forceinline__ int sq_submit(QpDev* qp, unsigned long long idx, uint32_t n,
-                                         unsigned long long timeout_ns = 2000000000ull, bool shared = true) {
-  (void)timeout_ns;
+__device__ __forceinline__ int sq_submit(QpDev* qp, unsigned long long idx, uint32_t n, bool shared = true) {
   return shared ? sq_submit_shared(qp, idx, n) : sq_submit_exclusive(qp, idx, n);
 }
 
 // -------------------------------------------------------------- completion queue
+// Every send-CQ consumer reads a CQE's last 16 bytes (timestamp_l | sop_drop_qpn | wqe_counter,sig,op_own) and, once
+// cqe_valid holds, asks whether it is a requester completion of its QP; a failed one also sets rc = WAIT_CQE_ERROR.
+// A CQ may be shared (send + receive side of a loopback QP, or several QPs): a responder completion, or a
+// requester completion of another QP, is NOT ours -- its wqe_counter is an index into another queue, so crediting it to
+// sq_cons would hand out SQ slots that have not executed yet.  Leave it at the head for its own consumer (recv_wait /
+// the other QP's poller).
+__device__ __forceinline__ uint8_t cqe_tail_op_own(const uint4& tail) { return (uint8_t)(tail.w >> 24); }
+__device__ __forceinline__ bool req_cqe(const uint4& tail, uint32_t qpn, int& rc) {
+  const uint8_t opc = cqe_opcode(cqe_tail_op_own(tail));
+  if ((opc != CQE_REQ && opc != CQE_REQ_ERR) || (be32(tail.z) & 0xffffffu) != qpn) return false;
+  if (opc == CQE_REQ_ERR) rc = WAIT_CQE_ERROR;
+  return true;
+}
+// The completed index after an accepted CQE: its 16-bit wqe_counter expanded against the consumer position `cons`.
+__device__ __forceinline__ unsigned long long req_cqe_done(const uint4& tail, unsigned long long cons) {
+  const uint16_t wqe_counter = be16((uint16_t)(tail.w & 0xffff));
+  return cons + (unsigned long long)((uint16_t)(wqe_counter + 1 - (uint16_t)cons));
+}
+
 // Consume at most one CQE of the QP's send CQ.  Returns 1 if one was consumed, 0 if
 // none was ready, <0 on an error CQE (which also moves the QP to ERR).
 __device__ __forceinline__ int cq_poll_once(QpDev* qp) {
   CqDev* cq = qp->scq;
   unsigned int ci = *(volatile unsigned int*)&cq->ci;
   const uint8_t* cqe = cq->buf + ((size_t)(ci & ((1u << cq->log_n) - 1)) << 6);
-  uint4 tail = ld_v4_volatile(cqe + 48);  // timestamp_l | sop_drop_qpn | wqe_counter,sig,op_own
-  uint8_t op_own = (uint8_t)(tail.w >> 24);
-  if (!cqe_valid(op_own, ci, cq->log_n)) return 0;
+  const uint4 tail = ld_v4_volatile(cqe + 48);
+  if (!cqe_valid(cqe_tail_op_own(tail), ci, cq->log_n)) return 0;
   __threadfence();  // acquire: payload and the rest of the CQE are visible past this point
-  uint16_t wqe_counter = be16((uint16_t)(tail.w & 0xffff));
   int rc = 1;
-  uint8_t opc = cqe_opcode(op_own);
-  // A CQ may be shared (send + receive side of a loopback QP, or several QPs): a responder completion,
-  // or a requester completion of another QP, is NOT ours -- its wqe_counter is an index into another
-  // queue, so crediting it to sq_cons would hand out SQ slots that have not executed yet.  Leave it at
-  // the head for its own consumer (recv_wait / the other QP's poller).
-  if ((opc != CQE_REQ && opc != CQE_REQ_ERR) || (be32(tail.z) & 0xffffffu) != qp->qpn) return 0;
-  if (opc == CQE_REQ_ERR) rc = WAIT_CQE_ERROR;
-  // Expand the 16-bit counter against the current consumer position.
-  unsigned long long cons = ld_u64_volatile(&qp->sq_cons);
-  unsigned long long done = cons + (unsigned long long)((uint16_t)(wqe_counter + 1 - (uint16_t)cons));
+  if (!req_cqe(tail, qp->qpn, rc)) return 0;
+  unsigned long long done = req_cqe_done(tail, ld_u64_volatile(&qp->sq_cons));
   if (atomicCAS(&cq->ci, ci, ci + 1) == ci) {
     trace_stamp(qp, done - 1, TR_SEEN);
     atomicMax(&qp->sq_cons, done);
@@ -310,9 +250,6 @@ __device__ __forceinline__ int sq_wait(QpDev* qp, unsigned long long idx,
     int rc = cq_poll_once(qp);
     if (rc < 0) err = rc;
     if (rc == 0) {
-      if (qp->state == QPS_ERR && ld_u64_volatile(&qp->sq_cons) <= idx && it > 64) {
-        // keep draining: flushed WQEs still produce error CQEs
-      }
       if (t0 == 0) t0 = globaltimer_ns();
       else if ((it & 15) == 0 && globaltimer_ns() - t0 > timeout_ns) return WAIT_TIMEOUT;
     }
@@ -369,13 +306,9 @@ __device__ __forceinline__ int poster_poll(Poster& p, int max_cqes = 8) {
   while (n < max_cqes) {
     const uint8_t* cqe = p.cq_buf + ((size_t)(p.ci & ((1u << p.cq_log) - 1)) << 6);
     const uint4 tail = ld_v4_volatile(cqe + 48);
-    const uint8_t op_own = (uint8_t)(tail.w >> 24);
-    if (!cqe_valid(op_own, p.ci, p.cq_log)) break;
-    const uint8_t opc = cqe_opcode(op_own);
-    if ((opc != CQE_REQ && opc != CQE_REQ_ERR) || (be32(tail.z) & 0xffffffu) != p.qpn) break;
-    if (opc == CQE_REQ_ERR) rc = WAIT_CQE_ERROR;
-    const uint16_t wqe_counter = be16((uint16_t)(tail.w & 0xffff));
-    p.cons += (unsigned long long)((uint16_t)(wqe_counter + 1 - (uint16_t)p.cons));
+    if (!cqe_valid(cqe_tail_op_own(tail), p.ci, p.cq_log)) break;
+    if (!req_cqe(tail, p.qpn, rc)) break;
+    p.cons = req_cqe_done(tail, p.cons);
     if (p.trace) trace_stamp(p.qp, p.cons - 1, TR_SEEN);
     ++p.ci;
     ++n;
@@ -396,17 +329,15 @@ __device__ __forceinline__ uint4 poster_peek(const Poster& p) {
 }
 // Consume the CQE whose tail was loaded by poster_peek, if it was ready and ours.  Returns 1 / 0 / WAIT_CQE_ERROR.
 __device__ __forceinline__ int poster_take(Poster& p, const uint4 tail) {
-  const uint8_t op_own = (uint8_t)(tail.w >> 24);
-  if (!cqe_valid(op_own, p.ci, p.cq_log)) return 0;
-  const uint8_t opc = cqe_opcode(op_own);
-  if ((opc != CQE_REQ && opc != CQE_REQ_ERR) || (be32(tail.z) & 0xffffffu) != p.qpn) return 0;
-  const uint16_t wqe_counter = be16((uint16_t)(tail.w & 0xffff));
-  p.cons += (unsigned long long)((uint16_t)(wqe_counter + 1 - (uint16_t)p.cons));
+  if (!cqe_valid(cqe_tail_op_own(tail), p.ci, p.cq_log)) return 0;
+  int rc = 1;
+  if (!req_cqe(tail, p.qpn, rc)) return 0;
+  p.cons = req_cqe_done(tail, p.cons);
   if (p.trace) trace_stamp(p.qp, p.cons - 1, TR_SEEN);
   ++p.ci;
   __threadfence();                                                // acquire: payload behind the CQE
   st_u32_volatile(&p.cq->dbrec[0], be32(p.ci & 0xffffff));
-  return opc == CQE_REQ_ERR ? WAIT_CQE_ERROR : 1;
+  return rc;
 }
 
 // Block until WQE `idx` completed (or timeout / error).
@@ -436,73 +367,50 @@ __device__ __forceinline__ unsigned long long poster_reserve(Poster& p, uint32_t
 __device__ __forceinline__ uint8_t* poster_slot(const Poster& p, unsigned long long idx) {
   return p.sq + ((idx & p.sq_mask) << 6);
 }
-__device__ __forceinline__ void poster_build_rdma(const Poster& p, unsigned long long idx, uint8_t opcode, uint64_t laddr,
-                                                  uint32_t lkey, uint64_t raddr, uint32_t rkey, uint32_t bytes,
-                                                  uint8_t fm_ce_se, uint32_t imm = 0) {
-  uint8_t* slot = poster_slot(p, idx);
-  st_v4(slot + 0, ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(p.qpn, 3), (uint32_t)fm_ce_se << 24, be32(imm));
-  st_v4(slot + 16, be32((uint32_t)(raddr >> 32)), be32((uint32_t)raddr), be32(rkey), 0u);
-  st_v4(slot + 32, be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(laddr >> 32)), be32((uint32_t)laddr));
-  st_v4(slot + 48, 0u, 0u, 0u, 0u);
-}
-__device__ __forceinline__ void poster_build_send(const Poster& p, unsigned long long idx, uint8_t opcode, uint64_t laddr,
-                                                  uint32_t lkey, uint32_t bytes, uint8_t fm_ce_se, uint32_t imm = 0) {
-  uint8_t* slot = poster_slot(p, idx);
-  st_v4(slot + 0, ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(p.qpn, 2), (uint32_t)fm_ce_se << 24, be32(imm));
-  st_v4(slot + 16, be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(laddr >> 32)), be32((uint32_t)laddr));
-  st_v4(slot + 32, 0u, 0u, 0u, 0u);
-  st_v4(slot + 48, 0u, 0u, 0u, 0u);
-}
-__device__ __forceinline__ void poster_build_atomic(const Poster& p, unsigned long long idx, uint8_t opcode, uint64_t laddr,
-                                                    uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t swap_add,
-                                                    uint64_t compare, uint8_t fm_ce_se) {
-  atomic_wqe_stores(poster_slot(p, idx), ctrl_word0(opcode, (uint16_t)idx), ctrl_word1(p.qpn, 4), opcode, laddr, lkey, raddr,
-                    rkey, swap_add, compare, fm_ce_se);
-}
-__device__ __forceinline__ void poster_build_inline(const Poster& p, unsigned long long idx, uint8_t opcode, uint64_t raddr,
-                                                    uint32_t rkey, const InlinePayload& d, uint32_t n, uint8_t fm_ce_se,
-                                                    uint32_t imm = 0) {
-  inline_wqe_stores(poster_slot(p, idx), (uint16_t)idx, p.qpn, opcode, raddr, rkey, d, n, fm_ce_se, imm);
-}
-// Ring ONE doorbell for everything built in [p.head, to): record, release, register.
+// Ring ONE doorbell for everything built in [p.head, to).
 __device__ __forceinline__ void poster_ring(Poster& p, unsigned long long to) {
-  const unsigned long long last = to - 1;
-  st_u32_volatile(&p.dbr[DBR_SND], be32((uint32_t)(to & 0xffff)));
-  const unsigned long long db = (unsigned long long)ctrl_word0(OP_NOP, (uint16_t)last) |
-                                ((unsigned long long)ctrl_word1(p.qpn, 0) << 32);
-  st_u64_release_scope(p.bf, db, p.sys);
+  ring_doorbell(p.dbr, p.bf, p.qpn, to, p.sys);
   if (p.trace) for (unsigned long long i = p.head; i < to; ++i) trace_stamp(p.qp, i, TR_POST);
   p.head = to;
+}
+
+// -------------------------------------------------------------- one WQE through the shared submit
+// Reserve a slot, let build(Wqe64*, idx) encode WQE idx (an mlx5_wire.h builder), store it, submit.  Returns the WQE
+// index, or ~0ull when the queue stayed full or the QP is in ERR.
+template <typename Build>
+__device__ __forceinline__ unsigned long long post_one(QpDev* qp, Build build,
+                                                       unsigned long long timeout_ns = 2000000000ull) {
+  const unsigned long long idx = sq_reserve(qp, 1, timeout_ns);
+  if (idx == ~0ull) return idx;
+  Wqe64 w;
+  build(&w, idx);
+  store_wqe(sq_slot(qp, idx), w);
+  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
+  return idx;
 }
 
 // -------------------------------------------------------------- one-call verbs
 __device__ __forceinline__ unsigned long long rdma_write(QpDev* qp, uint64_t laddr, uint32_t lkey,
                                                          uint64_t raddr, uint32_t rkey, uint32_t bytes,
                                                          bool signaled = true) {
-  unsigned long long idx = sq_reserve(qp, 1);
-  if (idx == ~0ull) return idx;
-  write_rdma_wqe(qp, idx, OP_RDMA_WRITE, laddr, lkey, raddr, rkey, bytes, signaled ? CTRL_CQ_UPDATE : 0);
-  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
-  return idx;
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_rdma_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, bytes, signaled ? CTRL_CQ_UPDATE : 0, 0);
+  });
 }
 __device__ __forceinline__ unsigned long long rdma_read(QpDev* qp, uint64_t laddr, uint32_t lkey,
                                                         uint64_t raddr, uint32_t rkey, uint32_t bytes,
                                                         bool signaled = true) {
-  unsigned long long idx = sq_reserve(qp, 1);
-  if (idx == ~0ull) return idx;
-  write_rdma_wqe(qp, idx, OP_RDMA_READ, laddr, lkey, raddr, rkey, bytes, signaled ? CTRL_CQ_UPDATE : 0);
-  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
-  return idx;
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_rdma_wqe(w, OP_RDMA_READ, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, bytes, signaled ? CTRL_CQ_UPDATE : 0, 0);
+  });
 }
 __device__ __forceinline__ unsigned long long rdma_send(QpDev* qp, uint64_t laddr, uint32_t lkey,
                                                         uint32_t bytes, bool signaled = true,
                                                         uint32_t imm = 0, bool with_imm = false) {
-  unsigned long long idx = sq_reserve(qp, 1);
-  if (idx == ~0ull) return idx;
-  write_send_wqe(qp, idx, with_imm ? OP_SEND_IMM : OP_SEND, laddr, lkey, bytes,
-                 signaled ? CTRL_CQ_UPDATE : 0, imm);
-  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
-  return idx;
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_send_wqe(w, with_imm ? OP_SEND_IMM : OP_SEND, (uint16_t)idx, qp->qpn, laddr, lkey, bytes,
+                   signaled ? CTRL_CQ_UPDATE : 0, imm);
+  });
 }
 
 // Remote 8-byte atomics through the shared submit: any thread of any kernel may call them (a producer signalling
@@ -510,37 +418,29 @@ __device__ __forceinline__ unsigned long long rdma_send(QpDev* qp, uint64_t ladd
 // The original remote value lands in the 8 local bytes at laddr.
 __device__ __forceinline__ unsigned long long rdma_fetch_add(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr,
                                                              uint32_t rkey, uint64_t add, bool signaled = true) {
-  unsigned long long idx = sq_reserve(qp, 1);
-  if (idx == ~0ull) return idx;
-  write_atomic_wqe(qp, idx, OP_ATOMIC_FA, laddr, lkey, raddr, rkey, add, 0, signaled ? CTRL_CQ_UPDATE : 0);
-  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
-  return idx;
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_atomic_wqe(w, OP_ATOMIC_FA, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, add, 0, signaled ? CTRL_CQ_UPDATE : 0);
+  });
 }
 __device__ __forceinline__ unsigned long long rdma_cmp_swap(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr,
                                                             uint32_t rkey, uint64_t compare, uint64_t swap,
                                                             bool signaled = true) {
-  unsigned long long idx = sq_reserve(qp, 1);
-  if (idx == ~0ull) return idx;
-  write_atomic_wqe(qp, idx, OP_ATOMIC_CS, laddr, lkey, raddr, rkey, swap, compare, signaled ? CTRL_CQ_UPDATE : 0);
-  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
-  return idx;
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_atomic_wqe(w, OP_ATOMIC_CS, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, swap, compare,
+                     signaled ? CTRL_CQ_UPDATE : 0);
+  });
 }
 
 // Inline puts through the shared submit: an RDMA WRITE whose 1..MAX_INLINE payload bytes travel in the WQE.  No local
 // buffer and no lkey: `data` may be any memory the calling thread can read (or a register, with rdma_p), and it may be
 // reused as soon as the call returns.  Returns the WQE index, or ~0ull when n is out of range or the queue stayed full.
-__device__ __forceinline__ unsigned long long rdma_put_inline_regs(QpDev* qp, uint64_t raddr, uint32_t rkey,
-                                                                   const InlinePayload& d, uint32_t n, bool signaled) {
-  unsigned long long idx = sq_reserve(qp, 1);
-  if (idx == ~0ull) return idx;
-  write_inline_wqe(qp, idx, OP_RDMA_WRITE, raddr, rkey, d, n, signaled ? CTRL_CQ_UPDATE : 0);
-  if (sq_submit(qp, idx, 1) != WAIT_OK) return ~0ull;
-  return idx;
-}
 __device__ __forceinline__ unsigned long long rdma_put_inline(QpDev* qp, uint64_t raddr, uint32_t rkey, const void* data,
                                                               uint32_t n, bool signaled = true) {
   if (n == 0 || n > MAX_INLINE) return ~0ull;
-  return rdma_put_inline_regs(qp, raddr, rkey, inline_load(data, n), n, signaled);
+  const InlinePayload d = inline_load(data, n);
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_inline_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, raddr, rkey, d, n, signaled ? CTRL_CQ_UPDATE : 0, 0);
+  });
 }
 // nvshmem_p / doca_gpu_dev_verbs_p: one 1-, 2-, 4- or 8-byte value straight from a register.
 template <typename T>
@@ -548,7 +448,41 @@ __device__ __forceinline__ unsigned long long rdma_p(QpDev* qp, uint64_t raddr, 
   static_assert(sizeof(T) == 1 || sizeof(T) == 2 || sizeof(T) == 4 || sizeof(T) == 8, "rdma_p: 1, 2, 4 or 8 bytes");
   InlinePayload d = {};
   memcpy(d.w, &value, sizeof(T));
-  return rdma_put_inline_regs(qp, raddr, rkey, d, (uint32_t)sizeof(T), signaled);
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_inline_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, raddr, rkey, d, (uint32_t)sizeof(T),
+                     signaled ? CTRL_CQ_UPDATE : 0, 0);
+  });
+}
+
+// -------------------------------------------------------------- fused kernels' posts
+// One record WRITE (or WRITE_IMM, carrying `imm`), posted by whichever CTA finishes the record.  Records go out in
+// completion order, not record order, so they are signaled by WQE index (every signal_every-th slot): the CQ keeps
+// freeing the send queue.  A posted record is counted in acc = [highest index + 1, records posted, ~earliest post time];
+// a failed post sets out[0] = WAIT_TIMEOUT.
+__device__ __forceinline__ void post_record(QpDev* qp, uint8_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr,
+                                            uint32_t rkey, uint32_t bytes, uint32_t imm, uint32_t signal_every,
+                                            unsigned long long* acc, unsigned long long* out,
+                                            unsigned long long timeout_ns) {
+  const unsigned long long idx = post_one(qp, [&](Wqe64* w, unsigned long long i) {
+    const bool sig = signal_every <= 1 || ((i + 1) % signal_every == 0);
+    build_rdma_wqe(w, opcode, (uint16_t)i, qp->qpn, laddr, lkey, raddr, rkey, bytes, sig ? CTRL_CQ_UPDATE : 0, imm);
+  }, timeout_ns);
+  if (idx == ~0ull) {
+    out[0] = (unsigned long long)(long long)WAIT_TIMEOUT;
+    return;
+  }
+  atomicMax(&acc[0], idx + 1);
+  atomicAdd(&acc[1], 1ull);
+  atomicMax(&acc[2], ~globaltimer_ns());
+}
+// Flush: one signaled NOP behind everything posted so far.  RC completes in order, so its CQE shows that every earlier
+// WQE of the QP has completed.  Waits for it unless post_only (then the caller reaps it).  Returns a WAIT_* status.
+__device__ __forceinline__ int post_flush(QpDev* qp, bool post_only, unsigned long long timeout_ns) {
+  const unsigned long long idx = post_one(qp, [&](Wqe64* w, unsigned long long i) {
+    build_nop_wqe(w, (uint16_t)i, qp->qpn, CTRL_CQ_UPDATE);
+  }, timeout_ns);
+  if (idx == ~0ull) return WAIT_TIMEOUT;
+  return post_only ? WAIT_OK : sq_wait(qp, idx, timeout_ns);
 }
 
 // Post one receive WQE on the QP's own RQ (single poster per RQ).

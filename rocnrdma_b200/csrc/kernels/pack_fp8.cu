@@ -146,24 +146,9 @@ __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a
         // acquire every other group's bytes; fences are cumulative, so on a NIC-facing QP one
         // system-scope fence here covers the whole record without a sys fence per group
         fence_scope(sys || a.direct);
-        unsigned long long idx = sq_reserve(a.qp, 1, a.timeout_ns);
-        // Chunks are posted by whichever CTA finishes them, so WQE order != chunk order:
-        // signal by WQE index (every k-th slot) so the CQ keeps freeing the send queue.
-        const bool sig = a.signal_every <= 1 || ((idx + 1) % a.signal_every == 0);
-        if (idx != ~0ull) {
-          write_rdma_wqe(a.qp, idx, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.staging_va + (uint64_t)chunk * rec,
-                         a.lkey, a.remote_va + (uint64_t)chunk * rec, a.rkey, a.direct ? 0u : (uint32_t)rec,
-                         sig ? CTRL_CQ_UPDATE : 0, chunk);
-          if (sq_submit(a.qp, idx, 1, a.timeout_ns, /*shared=*/true) == WAIT_OK) {
-            atomicMax(&a.acc[0], idx + 1);
-            atomicAdd(&a.acc[1], 1ull);
-            atomicMax(&a.acc[2], ~globaltimer_ns());
-          } else {
-            a.out[0] = (unsigned long long)(long long)WAIT_TIMEOUT;
-          }
-        } else {
-          a.out[0] = (unsigned long long)(long long)WAIT_TIMEOUT;
-        }
+        post_record(a.qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.staging_va + (uint64_t)chunk * rec, a.lkey,
+                    a.remote_va + (uint64_t)chunk * rec, a.rkey, a.direct ? 0u : (uint32_t)rec, chunk, a.signal_every, a.acc,
+                    a.out, a.timeout_ns);
         a.counters[chunk] = 0;   // self-clean for the next launch
       }
     }
@@ -178,18 +163,8 @@ __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a
       const unsigned long long t_pack_end = globaltimer_ns();
       fence_gpu();
       unsigned long long posted = ld_u64_volatile(&a.acc[1]);
-      // Flush: one signaled zero-length NOP behind everything this launch posted.  RC
-      // completes in order, so its CQE proves every record has landed.
-      int rc = WAIT_TIMEOUT;
-      unsigned long long fidx = sq_reserve(a.qp, 1, a.timeout_ns);
-      if (fidx != ~0ull) {
-        uint8_t* slot = a.qp->sq + ((fidx & ((1ull << a.qp->sq_log) - 1)) << 6);
-        st_v4(slot + 0, ctrl_word0(OP_NOP, (uint16_t)fidx), ctrl_word1(a.qp->qpn, 1), (uint32_t)CTRL_CQ_UPDATE << 24, 0u);
-        st_v4(slot + 16, 0u, 0u, 0u, 0u);
-        st_v4(slot + 32, 0u, 0u, 0u, 0u);
-        st_v4(slot + 48, 0u, 0u, 0u, 0u);
-        if (sq_submit(a.qp, fidx, 1, a.timeout_ns, /*shared=*/true) == WAIT_OK) rc = a.post_only ? WAIT_OK : sq_wait(a.qp, fidx, a.timeout_ns);
-      }
+      // the flush's CQE proves every record this launch posted has landed
+      int rc = post_flush(a.qp, a.post_only, a.timeout_ns);
       if (posted != a.n_chunks && rc == WAIT_OK) rc = WAIT_TIMEOUT;
       if (rc != WAIT_OK) a.out[0] = (unsigned long long)(long long)rc;
       a.out[1] = t_start;                 // this CTA's start: within a launch skew of the grid's

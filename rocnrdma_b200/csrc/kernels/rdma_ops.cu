@@ -38,33 +38,42 @@ struct StreamArgs {
   unsigned long long* out; // per CTA: [status, t_start, t_end, done, first_idx, last_idx, 0, 0]
 };
 
-// One warp per QP.  Work requests go out in bursts (perftest's --post_list): lane 0 reserves `burst`
-// slots with ONE atomic, lanes 0..n-1 each build one 64-byte WQE, lane 0 publishes the burst with ONE
-// doorbell and, when the window is full, polls the CQ for the oldest burst.  With burst = 1 this is the
-// plain post-one / poll-one loop (5-6 dependent L2 round trips per message, ~3.7 us measured); bursts
-// amortise the reservation, the fences, the doorbell and -- with signal_every (perftest's --cq-mod) --
-// the completion polling over up to 32 messages.
-__global__ void __launch_bounds__(32, 1) rdma_stream_kernel(StreamArgs a) {
+// The streaming kernels' windowed burst loop.  One warp per QP: the warp owns the QP and its send CQ for the whole
+// kernel, so queue state lives in lane 0's registers (dev::Poster), no atomics, and the CQ is only read when the window
+// is full.  Messages of k WQEs each (k = 1, or 2: a WRITE and its signal) go out in bursts of n (perftest's --post_list):
+// lane 0 reserves the burst's k * n slots at once, lane j builds WQE j of the burst, lane 0 publishes it with ONE
+// doorbell and, when the window (counted in messages) is full, polls the CQ for the oldest burst.  With burst = 1 this is
+// the plain post-one / poll-one loop (5-6 dependent L2 round trips per message, ~3.7 us measured); bursts amortise the
+// reservation, the fences, the doorbell and -- with signal_every (perftest's --cq-mod) -- the completion polling over up
+// to 32 WQEs.  A message's last WQE is signaled when the message is (every signal_every-th message, and the last one);
+// its other WQEs never are.
+//   build(uint8_t* slot, uint16_t wqe_idx, uint32_t qpn, uint32_t i, uint32_t part, uint8_t fm_ce_se): builds WQE `part` of
+//   message i with an mlx5_wire.h builder and stores it to its SQ slot (store_wqe)
+//   out: [status, t_start, t_end, messages done, first_idx, last_idx, cons, 0]
+template <typename Build>
+__device__ __forceinline__ void stream_post(QpDev* qp, uint32_t k, uint32_t iters, uint32_t window, uint32_t burst,
+                                            uint32_t signal_every, bool post_only, unsigned long long timeout_ns,
+                                            unsigned long long* out, Build build) {
   const uint32_t lane = threadIdx.x;
-  QpDev* qp = a.qps[blockIdx.x];
-  unsigned long long* out = a.out + (size_t)blockIdx.x * 8;
-  const uint64_t lbase = a.laddr + blockIdx.x * a.stride, rbase = a.raddr + blockIdx.x * a.stride;
   int status = WAIT_OK;
   unsigned long long first = ~0ull, last = 0;
-  uint32_t done = 0;
-  // The warp owns this QP and its send CQ for the whole kernel: queue state lives in lane 0's registers
-  // (dev::Poster), no atomics, the CQ is only read when the window is full.
+  uint32_t done = 0;                                  // messages
   Poster p = poster_open(qp);
   if (qp->state == QPS_ERR) status = WAIT_QP_ERROR;
   const unsigned long long t0 = globaltimer_ns();
-  while (done < a.iters && status != WAIT_QP_ERROR) {
-    const uint32_t n = min(a.burst, a.iters - done);
+  while (done < iters && status != WAIT_QP_ERROR) {
+    const uint32_t n = min(burst, iters - done);
+    // this lane's WQE of the burst, worked out before the window wait so that it stays off the path from a completion
+    // to the next doorbell
+    const uint32_t i = done + lane / k, part = lane % k;
+    const bool sig = part == k - 1 && ((signal_every <= 1) || ((i + 1) % signal_every == 0) || (i + 1 == iters));
     unsigned long long idx = 0;
     int rc = WAIT_OK;
     if (lane == 0) {
-      if (a.window && done + n > a.window) rc = poster_wait(p, last + n - a.window, a.timeout_ns);   // leaves <= window - n outstanding
+      // leaves <= window - n messages outstanding: the last WQE of message done + n - window - 1 has completed
+      if (window && done + n > window) rc = poster_wait(p, last + (unsigned long long)k * n - (unsigned long long)k * window, timeout_ns);
       if (rc != WAIT_TIMEOUT) {
-        idx = poster_reserve(p, n, a.timeout_ns);
+        idx = poster_reserve(p, k * n, timeout_ns);
         if (idx == ~0ull) rc = WAIT_TIMEOUT;
       }
     }
@@ -73,32 +82,23 @@ __global__ void __launch_bounds__(32, 1) rdma_stream_kernel(StreamArgs a) {
     if (rc != WAIT_OK) status = rc;
     if (rc == WAIT_TIMEOUT) break;
     if (first == ~0ull) first = idx;
-    if (lane < n) {
-      const uint32_t i = done + lane;
-      const uint64_t off = (uint64_t)(i % a.nslots) * a.slot_stride;
-      const bool sig = (a.signal_every <= 1) || ((i + 1) % a.signal_every == 0) || (i + 1 == a.iters);
-      const uint8_t flags = sig ? CTRL_CQ_UPDATE : 0;
-      if (a.opcode == OP_SEND)
-        poster_build_send(p, idx + lane, OP_SEND, lbase + off, a.lkey, a.bytes, flags);
-      else
-        poster_build_rdma(p, idx + lane, (uint8_t)a.opcode, lbase + off, a.lkey, rbase + off, a.rkey, a.bytes, flags);
-    }
-    if (n > 1) __syncwarp();                         // the burst's WQE bytes happen-before lane 0's release
+    if (lane < k * n) build(poster_slot(p, idx + lane), (uint16_t)(idx + lane), p.qpn, i, part, sig ? CTRL_CQ_UPDATE : 0);
+    if (k * n > 1) __syncwarp();                     // the burst's WQE bytes happen-before lane 0's release
     if (lane == 0) {
       // overlap the completion poll with the doorbell release: the CQE load is in flight while the fence in
       // front of the doorbell waits for the WQE stores (one exposed round trip per post instead of two)
       const bool outstanding = p.head > p.cons;
       uint4 tail = make_uint4(0, 0, 0, 0);
       if (outstanding) tail = poster_peek(p);
-      poster_ring(p, idx + n);
+      poster_ring(p, idx + k * n);
       if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
     }
-    last = idx + n - 1;
+    last = idx + k * n - 1;
     done += n;
   }
   if (lane != 0) return;
-  if (done && !a.post_only) {
-    int rc = poster_wait(p, last, a.timeout_ns);
+  if (done && !post_only) {
+    const int rc = poster_wait(p, last, timeout_ns);
     if (rc != WAIT_OK) status = rc;
   }
   const unsigned long long t1 = globaltimer_ns();
@@ -107,6 +107,23 @@ __global__ void __launch_bounds__(32, 1) rdma_stream_kernel(StreamArgs a) {
   out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
   out[6] = p.cons;
   out[7] = 0;
+}
+
+__global__ void __launch_bounds__(32, 1) rdma_stream_kernel(StreamArgs a) {
+  const uint64_t lbase = a.laddr + blockIdx.x * a.stride, rbase = a.raddr + blockIdx.x * a.stride;
+  stream_post(a.qps[blockIdx.x], 1, a.iters, a.window, a.burst, a.signal_every, a.post_only, a.timeout_ns,
+              a.out + (size_t)blockIdx.x * 8,
+              [&](uint8_t* slot, uint16_t idx, uint32_t qpn, uint32_t i, uint32_t, uint8_t flags) {
+                const uint64_t off = (uint64_t)(i % a.nslots) * a.slot_stride;
+                Wqe64 w;
+                if (a.opcode == OP_SEND) {
+                  build_send_wqe(&w, OP_SEND, idx, qpn, lbase + off, a.lkey, a.bytes, flags, 0);
+                  store_wqe(slot, w);
+                } else {
+                  build_rdma_wqe(&w, (uint8_t)a.opcode, idx, qpn, lbase + off, a.lkey, rbase + off, a.rkey, a.bytes, flags, 0);
+                  store_wqe(slot, w);
+                }
+              });
 }
 
 // Posting parameters that can always make progress (pure host function, unit-tested on the CPU):
@@ -152,23 +169,16 @@ __global__ void __launch_bounds__(32) shared_post_stress_kernel(QpDev* qp, uint6
   int status = WAIT_OK;
   for (uint32_t i = 0; i < per_cta; ++i) {
     const uint64_t cell = ((uint64_t)blockIdx.x * per_cta + i) * 64;
-    unsigned long long idx = sq_reserve(qp, 1, timeout_ns);
+    const unsigned long long idx = post_one(qp, [&](Wqe64* w, unsigned long long j) {
+      build_rdma_wqe(w, OP_RDMA_WRITE, (uint16_t)j, qp->qpn, laddr + cell, lkey, raddr + cell, rkey, 64,
+                     ((j & 7) == 7) ? CTRL_CQ_UPDATE : 0, 0);
+    }, timeout_ns);
     if (idx == ~0ull) { status = WAIT_TIMEOUT; break; }
-    write_rdma_wqe(qp, idx, OP_RDMA_WRITE, laddr + cell, lkey, raddr + cell, rkey, 64, ((idx & 7) == 7) ? CTRL_CQ_UPDATE : 0);
-    sq_submit_shared(qp, idx, 1);
   }
   if (status != WAIT_OK) out[0] = (unsigned long long)(long long)status;
   fence_gpu();
   if (atomicAdd(done_ctas, 1u) + 1 == gridDim.x) {
-    unsigned long long fidx = sq_reserve(qp, 1, timeout_ns);
-    int rc = WAIT_TIMEOUT;
-    if (fidx != ~0ull) {
-      uint8_t* slot = qp->sq + ((fidx & ((1ull << qp->sq_log) - 1)) << 6);
-      st_v4(slot + 0, ctrl_word0(OP_NOP, (uint16_t)fidx), ctrl_word1(qp->qpn, 1), (uint32_t)CTRL_CQ_UPDATE << 24, 0u);
-      st_v4(slot + 16, 0u, 0u, 0u, 0u); st_v4(slot + 32, 0u, 0u, 0u, 0u); st_v4(slot + 48, 0u, 0u, 0u, 0u);
-      sq_submit_shared(qp, fidx, 1);
-      rc = sq_wait(qp, fidx, timeout_ns);
-    }
+    const int rc = post_flush(qp, false, timeout_ns);
     if (rc != WAIT_OK) out[0] = (unsigned long long)(long long)rc;
     out[1] = t0; out[2] = globaltimer_ns(); out[3] = (unsigned long long)gridDim.x * per_cta;
     *done_ctas = 0;
@@ -238,62 +248,17 @@ struct AtomicArgs {
 };
 
 __global__ void __launch_bounds__(32, 1) atomic_stream_kernel(AtomicArgs a) {
-  const uint32_t lane = threadIdx.x;
-  QpDev* qp = a.qps[blockIdx.x];
-  unsigned long long* out = a.out + (size_t)blockIdx.x * 8;
   const uint64_t tgt = a.target + blockIdx.x * a.target_stride;
   const uint64_t fbase = a.fetch + (uint64_t)blockIdx.x * a.iters * 8;
-  int status = WAIT_OK;
-  unsigned long long first = ~0ull, last = 0;
-  uint32_t done = 0;
-  Poster p = poster_open(qp);
-  if (qp->state == QPS_ERR) status = WAIT_QP_ERROR;
-  const unsigned long long t0 = globaltimer_ns();
-  while (done < a.iters && status != WAIT_QP_ERROR) {
-    const uint32_t n = min(a.burst, a.iters - done);
-    unsigned long long idx = 0;
-    int rc = WAIT_OK;
-    if (lane == 0) {
-      if (a.window && done + n > a.window) rc = poster_wait(p, last + n - a.window, a.timeout_ns);
-      if (rc != WAIT_TIMEOUT) {
-        idx = poster_reserve(p, n, a.timeout_ns);
-        if (idx == ~0ull) rc = WAIT_TIMEOUT;
-      }
-    }
-    rc = __shfl_sync(0xffffffffu, rc, 0);
-    idx = __shfl_sync(0xffffffffu, idx, 0);
-    if (rc != WAIT_OK) status = rc;
-    if (rc == WAIT_TIMEOUT) break;
-    if (first == ~0ull) first = idx;
-    if (lane < n) {
-      const uint32_t i = done + lane;
-      const bool sig = (a.signal_every <= 1) || ((i + 1) % a.signal_every == 0) || (i + 1 == a.iters);
-      const uint64_t cmp = a.chain ? (uint64_t)i : a.compare, swp = a.chain ? (uint64_t)i + 1 : a.swap;
-      poster_build_atomic(p, idx + lane, (uint8_t)a.opcode, fbase + (uint64_t)i * 8, a.lkey, tgt, a.rkey,
-                          a.opcode == OP_ATOMIC_FA ? a.add : swp, cmp, sig ? CTRL_CQ_UPDATE : 0);
-    }
-    if (n > 1) __syncwarp();
-    if (lane == 0) {
-      const bool outstanding = p.head > p.cons;
-      uint4 tail = make_uint4(0, 0, 0, 0);
-      if (outstanding) tail = poster_peek(p);
-      poster_ring(p, idx + n);
-      if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
-    }
-    last = idx + n - 1;
-    done += n;
-  }
-  if (lane != 0) return;
-  if (done) {
-    const int rc = poster_wait(p, last, a.timeout_ns);
-    if (rc != WAIT_OK) status = rc;
-  }
-  const unsigned long long t1 = globaltimer_ns();
-  poster_close(p);
-  out[0] = (unsigned long long)(long long)status;
-  out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
-  out[6] = p.cons;
-  out[7] = 0;
+  stream_post(a.qps[blockIdx.x], 1, a.iters, a.window, a.burst, a.signal_every, false, a.timeout_ns,
+              a.out + (size_t)blockIdx.x * 8,
+              [&](uint8_t* slot, uint16_t idx, uint32_t qpn, uint32_t i, uint32_t, uint8_t flags) {
+                const uint64_t cmp = a.chain ? (uint64_t)i : a.compare, swp = a.chain ? (uint64_t)i + 1 : a.swap;
+                Wqe64 w;
+                build_atomic_wqe(&w, (uint8_t)a.opcode, idx, qpn, fbase + (uint64_t)i * 8, a.lkey, tgt, a.rkey,
+                                 a.opcode == OP_ATOMIC_FA ? a.add : swp, cmp, flags);
+                store_wqe(slot, w);
+              });
 }
 
 RN_API int rn_k_atomic_stream(uint64_t stream, const uint64_t* qps_host, uint32_t nqp, uint32_t opcode, uint32_t chain,
@@ -336,56 +301,19 @@ struct PutSignalArgs {
 };
 
 __global__ void __launch_bounds__(32, 1) put_signal_kernel(PutSignalArgs a) {
-  const uint32_t lane = threadIdx.x;
-  int status = WAIT_OK;
-  unsigned long long first = ~0ull, last = 0;
-  uint32_t done = 0;
-  Poster p = poster_open(a.qp);
-  if (a.qp->state == QPS_ERR) status = WAIT_QP_ERROR;
-  const unsigned long long t0 = globaltimer_ns();
-  for (; done < a.iters && status != WAIT_QP_ERROR; ++done) {
-    unsigned long long idx = 0;
-    int rc = WAIT_OK;
-    if (lane == 0) {
-      // window counts messages: the FA of message done - window (2 WQEs per message) must have completed
-      if (a.window && done >= a.window) rc = poster_wait(p, first + 2ull * (done - a.window) + 1, a.timeout_ns);
-      if (rc != WAIT_TIMEOUT) {
-        idx = poster_reserve(p, 2, a.timeout_ns);
-        if (idx == ~0ull) rc = WAIT_TIMEOUT;
-      }
-    }
-    rc = __shfl_sync(0xffffffffu, rc, 0);
-    idx = __shfl_sync(0xffffffffu, idx, 0);
-    if (rc != WAIT_OK) status = rc;
-    if (rc == WAIT_TIMEOUT) break;
-    if (first == ~0ull) first = idx;
-    const uint64_t off = (uint64_t)(done % a.nslots) * a.slot_stride;
-    if (lane == 0) poster_build_rdma(p, idx, OP_RDMA_WRITE, a.src + off, a.lkey, a.dst + off, a.rkey, a.nbytes, 0);
-    if (lane == 1)
-      poster_build_atomic(p, idx + 1, OP_ATOMIC_FA, a.fetch + (uint64_t)(done % a.fetch_slots) * 8, a.fetch_lkey, a.sig,
-                          a.sig_rkey, a.add, 0, CTRL_CQ_UPDATE);
-    __syncwarp();
-    if (lane == 0) {
-      const bool outstanding = p.head > p.cons;
-      uint4 tail = make_uint4(0, 0, 0, 0);
-      if (outstanding) tail = poster_peek(p);
-      poster_ring(p, idx + 2);
-      if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
-    }
-    last = idx + 1;
-  }
-  if (lane != 0) return;
-  if (done) {
-    const int rc = poster_wait(p, last, a.timeout_ns);
-    if (rc != WAIT_OK) status = rc;
-  }
-  const unsigned long long t1 = globaltimer_ns();
-  poster_close(p);
-  unsigned long long* out = a.out;
-  out[0] = (unsigned long long)(long long)status;
-  out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
-  out[6] = p.cons;
-  out[7] = 0;
+  stream_post(a.qp, 2, a.iters, a.window, 1, 1, false, a.timeout_ns, a.out,
+              [&](uint8_t* slot, uint16_t idx, uint32_t qpn, uint32_t i, uint32_t part, uint8_t flags) {
+                Wqe64 w;
+                if (part == 0) {
+                  const uint64_t off = (uint64_t)(i % a.nslots) * a.slot_stride;
+                  build_rdma_wqe(&w, OP_RDMA_WRITE, idx, qpn, a.src + off, a.lkey, a.dst + off, a.rkey, a.nbytes, flags, 0);
+                  store_wqe(slot, w);
+                } else {
+                  build_atomic_wqe(&w, OP_ATOMIC_FA, idx, qpn, a.fetch + (uint64_t)(i % a.fetch_slots) * 8, a.fetch_lkey, a.sig,
+                                   a.sig_rkey, a.add, 0, flags);
+                  store_wqe(slot, w);
+                }
+              });
 }
 
 RN_API int rn_k_put_signal(uint64_t stream, uint64_t qp_dev, uint64_t src, uint32_t lkey, uint64_t dst, uint32_t rkey,
@@ -425,69 +353,24 @@ struct PutInlineArgs {
 };
 
 __global__ void __launch_bounds__(32, 1) put_inline_kernel(PutInlineArgs a) {
-  const uint32_t lane = threadIdx.x;
-  QpDev* qp = a.qps[blockIdx.x];
-  unsigned long long* out = a.out + (size_t)blockIdx.x * 8;
-  const uint32_t k = a.sig ? 2u : 1u;                 // WQEs per message
   const uint64_t sig = a.sig + (uint64_t)blockIdx.x * 8;
   const uint32_t m0 = blockIdx.x * a.iters;
-  int status = WAIT_OK;
-  unsigned long long first = ~0ull, last = 0;
-  uint32_t done = 0;                                  // messages
-  Poster p = poster_open(qp);
-  if (qp->state == QPS_ERR) status = WAIT_QP_ERROR;
-  const unsigned long long t0 = globaltimer_ns();
-  while (done < a.iters && status != WAIT_QP_ERROR) {
-    const uint32_t n = min(a.burst, a.iters - done);
-    unsigned long long idx = 0;
-    int rc = WAIT_OK;
-    if (lane == 0) {
-      // leaves <= window - n messages outstanding: the last WQE of message done + n - window - 1 has completed
-      if (a.window && done + n > a.window) rc = poster_wait(p, last + (unsigned long long)k * n - (unsigned long long)k * a.window, a.timeout_ns);
-      if (rc != WAIT_TIMEOUT) {
-        idx = poster_reserve(p, k * n, a.timeout_ns);
-        if (idx == ~0ull) rc = WAIT_TIMEOUT;
-      }
-    }
-    rc = __shfl_sync(0xffffffffu, rc, 0);
-    idx = __shfl_sync(0xffffffffu, idx, 0);
-    if (rc != WAIT_OK) status = rc;
-    if (rc == WAIT_TIMEOUT) break;
-    if (first == ~0ull) first = idx;
-    if (lane < k * n) {
-      const uint32_t i = done + lane / k, m = m0 + i;
-      const bool sig_msg = (a.signal_every <= 1) || ((i + 1) % a.signal_every == 0) || (i + 1 == a.iters);
-      if (k == 2 && (lane & 1u)) {
-        poster_build_atomic(p, idx + lane, OP_ATOMIC_FA, a.fetch + (uint64_t)(m % a.fetch_slots) * 8, a.fetch_lkey, sig, a.sig_rkey,
-                            a.add, 0, sig_msg ? CTRL_CQ_UPDATE : 0);
-      } else {
-        const InlinePayload d = inline_load(a.values + (uint64_t)(m % a.rows) * a.row_bytes, a.nbytes);
-        poster_build_inline(p, idx + lane, OP_RDMA_WRITE, a.dst + (uint64_t)(m % a.nslots) * a.slot_stride, a.rkey, d, a.nbytes,
-                            (k == 1 && sig_msg) ? CTRL_CQ_UPDATE : 0);
-      }
-    }
-    if (k * n > 1) __syncwarp();
-    if (lane == 0) {
-      const bool outstanding = p.head > p.cons;
-      uint4 tail = make_uint4(0, 0, 0, 0);
-      if (outstanding) tail = poster_peek(p);
-      poster_ring(p, idx + k * n);
-      if (outstanding && poster_take(p, tail) < 0) status = WAIT_CQE_ERROR;
-    }
-    last = idx + k * n - 1;
-    done += n;
-  }
-  if (lane != 0) return;
-  if (done) {
-    const int rc = poster_wait(p, last, a.timeout_ns);
-    if (rc != WAIT_OK) status = rc;
-  }
-  const unsigned long long t1 = globaltimer_ns();
-  poster_close(p);
-  out[0] = (unsigned long long)(long long)status;
-  out[1] = t0; out[2] = t1; out[3] = done; out[4] = first; out[5] = last;
-  out[6] = p.cons;
-  out[7] = 0;
+  stream_post(a.qps[blockIdx.x], a.sig ? 2u : 1u, a.iters, a.window, a.burst, a.signal_every, false, a.timeout_ns,
+              a.out + (size_t)blockIdx.x * 8,
+              [&](uint8_t* slot, uint16_t idx, uint32_t qpn, uint32_t i, uint32_t part, uint8_t flags) {
+                const uint32_t m = m0 + i;
+                Wqe64 w;
+                if (part == 1) {
+                  build_atomic_wqe(&w, OP_ATOMIC_FA, idx, qpn, a.fetch + (uint64_t)(m % a.fetch_slots) * 8, a.fetch_lkey, sig,
+                                   a.sig_rkey, a.add, 0, flags);
+                  store_wqe(slot, w);
+                } else {
+                  const InlinePayload d = inline_load(a.values + (uint64_t)(m % a.rows) * a.row_bytes, a.nbytes);
+                  build_inline_wqe(&w, OP_RDMA_WRITE, idx, qpn, a.dst + (uint64_t)(m % a.nslots) * a.slot_stride, a.rkey, d,
+                                   a.nbytes, flags, 0);
+                  store_wqe(slot, w);
+                }
+              });
 }
 
 RN_API int rn_k_put_inline(uint64_t stream, const uint64_t* qps_host, uint32_t nqp, uint64_t values, uint64_t row_bytes,

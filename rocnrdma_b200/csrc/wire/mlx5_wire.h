@@ -122,6 +122,9 @@ struct alignas(16) AtomicSeg {   // mlx5_wqe_atomic_seg
 struct InlineSeg {               // mlx5_wqe_inl_data_seg: the payload follows, zero padded to a 16-byte boundary
   uint32_t byte_count;           // be32 (n | INLINE_SEG)
 };
+// An inline payload: up to MAX_INLINE bytes in memory order (little-endian words), zero past its length.  Whole words,
+// so device code can keep it in registers.
+struct InlinePayload { uint32_t w[7]; };
 // One WQEBB holding ctrl + raddr + one data segment (RDMA write / read), or
 // ctrl + data (send: raddr slot left zero and ds=2 with data in slot 1).
 struct alignas(64) Wqe64 {
@@ -131,14 +134,16 @@ struct alignas(64) Wqe64 {
     struct { DataSeg data; uint8_t pad[32]; } send;
     struct { RaddrSeg raddr; AtomicSeg atomic; DataSeg data; } atom;
     // inline: the payload travels in the WQE (ds = 2 + ceil((4 + n) / 16) for RDMA, 1 + ... for SEND)
-    struct { RaddrSeg raddr; InlineSeg inl; uint8_t data[MAX_INLINE]; } rdma_inl;
-    struct { InlineSeg inl; uint8_t data[44]; } send_inl;
+    struct { RaddrSeg raddr; InlineSeg inl; InlinePayload data; } rdma_inl;
+    struct { InlineSeg inl; InlinePayload data; uint32_t pad[4]; } send_inl;
+    struct { uint32_t pad[12]; } nop;
   };
 };
 static_assert(sizeof(CtrlSeg) == 16, "ctrl seg");
 static_assert(sizeof(RaddrSeg) == 16, "raddr seg");
 static_assert(sizeof(DataSeg) == 16, "data seg");
 static_assert(sizeof(InlineSeg) == 4, "inline seg");
+static_assert(sizeof(InlinePayload) == MAX_INLINE, "inline payload");
 static_assert(sizeof(Wqe64) == 64, "wqebb");
 // where the inline payload starts within the WQEBB (the engine copies it from there)
 enum : uint32_t { INLINE_OFF_RDMA = 36, INLINE_OFF_SEND = 20 };
@@ -197,6 +202,10 @@ RN_HD uint32_t ctrl_word0(uint8_t opcode, uint16_t wqe_idx, uint8_t opmod = 0) {
   return be32(((uint32_t)opmod << 24) | ((uint32_t)wqe_idx << 8) | opcode);
 }
 RN_HD uint32_t ctrl_word1(uint32_t qpn, uint8_t ds) { return be32((qpn << 8) | (ds & 0x3f)); }
+// The doorbell register word: the first 8 bytes of a ctrl segment naming the QP and the last WQE posted (opcode NOP, ds 0).
+RN_HD uint64_t doorbell_word(uint32_t qpn, uint16_t last) {
+  return (uint64_t)ctrl_word0(OP_NOP, last) | ((uint64_t)ctrl_word1(qpn, 0) << 32);
+}
 
 RN_HD void encode_ctrl(CtrlSeg* c, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint8_t ds,
                        uint8_t fm_ce_se, uint32_t imm) {
@@ -218,8 +227,8 @@ RN_HD void encode_data(DataSeg* d, uint64_t addr, uint32_t lkey, uint32_t bytes)
   d->addr = be64(addr);
 }
 
-// Full WQE builders (host and slow-path device use; the fast device path in
-// hca/post.cuh emits the same bytes with four 16-byte vector stores).
+// Full WQE builders, each writing all 64 bytes.  Device code builds into a local Wqe64 (registers) and stores it
+// with four 16-byte vector stores (dev::store_wqe in hca/post.cuh).
 RN_HD void build_rdma_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint64_t laddr,
                           uint32_t lkey, uint64_t raddr, uint32_t rkey, uint32_t bytes,
                           uint8_t fm_ce_se, uint32_t imm) {
@@ -254,17 +263,33 @@ RN_HD void build_atomic_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t
 RN_HD constexpr uint8_t inline_segs(uint32_t n) { return (uint8_t)((4 + n + WQE_SEG - 1) / WQE_SEG); }
 // Inline WQE (1 <= n <= MAX_INLINE; the caller checks): RDMA_WRITE / WRITE_IMM carry ctrl + raddr + the inline segment
 // (ds 3 up to 12 bytes, else 4), SEND / SEND_IMM ctrl + the inline segment (ds 2 up to 12 bytes, else 3).  No lkey, no
-// local address: the n bytes at `data` are copied into the WQE, and the rest of the WQEBB is zero.
+// local address: the payload's n bytes travel in the WQE, and the rest of the WQEBB is zero.
+RN_HD void build_inline_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint64_t raddr, uint32_t rkey,
+                            const InlinePayload& d, uint32_t n, uint8_t fm_ce_se, uint32_t imm) {
+  if (opcode == OP_SEND || opcode == OP_SEND_IMM) {
+    encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, (uint8_t)(1 + inline_segs(n)), fm_ce_se, imm);
+    w->send_inl.inl.byte_count = be32(n | INLINE_SEG);
+    w->send_inl.data = d;
+    for (int i = 0; i < 4; ++i) w->send_inl.pad[i] = 0;
+  } else {
+    encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, (uint8_t)(2 + inline_segs(n)), fm_ce_se, imm);
+    encode_raddr(&w->rdma_inl.raddr, raddr, rkey);
+    w->rdma_inl.inl.byte_count = be32(n | INLINE_SEG);
+    w->rdma_inl.data = d;
+  }
+}
+// The same WQE with its payload taken from the n bytes at `data` (host callers; device code loads the payload into
+// registers with dev::inline_load).
 RN_HD void build_inline_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint64_t raddr, uint32_t rkey,
                             const void* data, uint32_t n, uint8_t fm_ce_se, uint32_t imm) {
-  const bool send = opcode == OP_SEND || opcode == OP_SEND_IMM;
-  uint8_t* b = reinterpret_cast<uint8_t*>(w);
-  for (uint32_t i = WQE_SEG; i < WQEBB; ++i) b[i] = 0;
-  encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, (uint8_t)((send ? 1 : 2) + inline_segs(n)), fm_ce_se, imm);
-  if (!send) encode_raddr(&w->rdma_inl.raddr, raddr, rkey);
-  (send ? w->send_inl.inl : w->rdma_inl.inl).byte_count = be32(n | INLINE_SEG);
-  uint8_t* d = b + (send ? INLINE_OFF_SEND : INLINE_OFF_RDMA);
-  for (uint32_t i = 0; i < n; ++i) d[i] = static_cast<const uint8_t*>(data)[i];
+  InlinePayload d = {};
+  for (uint32_t i = 0; i < n; ++i) d.w[i / 4] |= (uint32_t)static_cast<const uint8_t*>(data)[i] << (8 * (i % 4));
+  build_inline_wqe(w, opcode, wqe_idx, qpn, raddr, rkey, d, n, fm_ce_se, imm);
+}
+// NOP (ds = 1): a ctrl segment and nothing else.  Signaled, its CQE shows that every earlier WQE of the QP completed.
+RN_HD void build_nop_wqe(Wqe64* w, uint16_t wqe_idx, uint32_t qpn, uint8_t fm_ce_se) {
+  encode_ctrl(&w->ctrl, OP_NOP, wqe_idx, qpn, 1, fm_ce_se, 0);
+  for (int i = 0; i < 12; ++i) w->nop.pad[i] = 0;
 }
 
 // ---------------------------------------------------------------- decoders
