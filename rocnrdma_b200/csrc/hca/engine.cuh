@@ -387,6 +387,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
       case OP_NOP: v.bytes = 0; break;
       case OP_RDMA_WRITE:
       case OP_RDMA_WRITE_IMM: {
+        if (v.bytes == 0) { p->src = p->dst = 1; break; }   // zero length: no key is looked at, nothing moves (DESIGN.md 3.1)
         if (v.inl_off) {
           // Inline: only the remote key is checked, and the source is the payload in this SQ slot.  It is read after
           // commit (a flushed WQE copies nothing), and the slot is not reused before the WQE retires (DESIGN.md 3.1).
@@ -400,6 +401,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
         break;
       }
       case OP_RDMA_READ: {
+        if (v.bytes == 0) { p->src = p->dst = 1; break; }
         const MKeyRaw lk = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey), rk = mkey_load(qp->r.rkeys, qp->r.n_rkeys, v.rkey);
         p->dst = mkey_check(lk, v.lkey, v.laddr, v.bytes, ACC_LOCAL_WRITE, false, &p->syn);
         if (p->dst) p->src = mkey_check(rk, v.rkey, v.raddr, v.bytes, ACC_REMOTE_READ, true, &p->syn);

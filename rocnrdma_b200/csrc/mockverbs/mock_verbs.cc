@@ -404,6 +404,17 @@ void write_cqe(MockCq* cq, uint8_t opcode, uint8_t wqe_opcode, uint32_t qpn, uin
   cq->pi.store(slot + 1, std::memory_order_release);
 }
 
+// A receive-consuming request (SEND, SEND_IMM, WRITE_IMM) that passed its own checks waits for the responder to post a
+// receive, up to the RNR timeout.  Returns 1 when a receive is there, 0 while the WQE must be retried later, -1 once the
+// timeout has passed.
+int recv_wait(MockQp* qp, MockQp* peer) {
+  const uint16_t rpi = (uint16_t)be32(*(volatile uint32_t*)&peer->dbrec[rn::DBR_RCV]);
+  if ((uint16_t)(rpi - (uint16_t)peer->hw_rq_cons) != 0) return 1;
+  const uint64_t t = now_ns();
+  if (!qp->rnr_since_ns) { qp->rnr_since_ns = t; qp->n_rnr++; }
+  return t - qp->rnr_since_ns < g_rnr_timeout_ns.load() ? 0 : -1;
+}
+
 MockQp* find_qp(uint16_t lid, uint32_t qpn) {
   if (lid < 1 || lid > g_ndev) return nullptr;
   MockDev& d = g_devs[lid - 1];
@@ -436,22 +447,21 @@ bool nic_execute(MockQp* qp, uint64_t w) {
     MockMr *lmr = nullptr, *rmr = nullptr;
     switch (v.opcode) {
       case rn::OP_RDMA_WRITE: case rn::OP_RDMA_WRITE_IMM: {
-        if (v.opcode == rn::OP_RDMA_WRITE_IMM) {
-          const uint16_t rpi = (uint16_t)be32(*(volatile uint32_t*)&peer->dbrec[rn::DBR_RCV]);
-          if ((uint16_t)(rpi - (uint16_t)peer->hw_rq_cons) == 0) {
-            const uint64_t t = now_ns();
-            if (!qp->rnr_since_ns) { qp->rnr_since_ns = t; qp->n_rnr++; }
-            if (t - qp->rnr_since_ns < g_rnr_timeout_ns.load()) return false;
-            syn = rn::SYN_RNR_RETRY_EXC_ERR;
-            break;
-          }
+        // Zero length: no key is looked at and nothing moves (DESIGN.md 3.1).  Otherwise the keys are checked before the
+        // receive wait, so a WRITE_IMM that fails them never takes a receive.  Inline: the payload is in the WQE (no
+        // local key); else it is gathered through the lkey.
+        uint64_t src = 0, dst = 0;
+        if (v.bytes) {
+          src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
+                          : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
+          dst = src ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_WRITE, true, &syn, &rmr) : 0;
         }
-        // inline: the payload is in the WQE (no local key); else gather it through the lkey
-        uint64_t src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
-                                 : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
-        uint64_t dst = src || v.bytes == 0 ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_WRITE, true, &syn, &rmr) : 0;
-        if (v.bytes == 0) syn = rn::SYN_OK, src = dst = 1;
         if (syn == rn::SYN_OK && !(peer->access_flags & IBV_ACCESS_REMOTE_WRITE)) syn = rn::SYN_REMOTE_ACCESS_ERR;
+        if (syn == rn::SYN_OK && v.opcode == rn::OP_RDMA_WRITE_IMM) {
+          const int r = recv_wait(qp, peer);
+          if (r == 0) return false;
+          if (r < 0) { syn = rn::SYN_RNR_RETRY_EXC_ERR; break; }
+        }
         if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, rmr, src, lmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) {
           moved = v.bytes;
@@ -460,22 +470,25 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         break;
       }
       case rn::OP_RDMA_READ: {
-        uint64_t dst = translate(ldev, v.lkey, v.laddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, false, &syn, &lmr);
-        uint64_t src = dst ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_READ, true, &syn, &rmr) : 0;
+        uint64_t dst = 0, src = 0;
+        if (v.bytes) {   // zero length: no key is looked at, as for WRITE
+          dst = translate(ldev, v.lkey, v.laddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, false, &syn, &lmr);
+          src = dst ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_READ, true, &syn, &rmr) : 0;
+        }
         if (syn == rn::SYN_OK && !(peer->access_flags & IBV_ACCESS_REMOTE_READ)) syn = rn::SYN_REMOTE_ACCESS_ERR;
         if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, lmr, src, rmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) moved = v.bytes;
         break;
       }
       case rn::OP_SEND: case rn::OP_SEND_IMM: {
-        const uint16_t rpi = (uint16_t)be32(*(volatile uint32_t*)&peer->dbrec[rn::DBR_RCV]);
-        if ((uint16_t)(rpi - (uint16_t)peer->hw_rq_cons) == 0) {
-          const uint64_t t = now_ns();
-          if (!qp->rnr_since_ns) { qp->rnr_since_ns = t; qp->n_rnr++; }
-          if (t - qp->rnr_since_ns < g_rnr_timeout_ns.load()) return false;
-          syn = rn::SYN_RNR_RETRY_EXC_ERR;
-          break;
-        }
+        // The requester's own check comes first: a SEND whose lkey fails never reaches the responder, so it neither
+        // waits for nor consumes a receive.
+        uint64_t src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
+                                 : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
+        if (syn != rn::SYN_OK) break;
+        const int r = recv_wait(qp, peer);
+        if (r == 0) return false;
+        if (r < 0) { syn = rn::SYN_RNR_RETRY_EXC_ERR; break; }
         std::atomic_thread_fence(std::memory_order_acquire);
         const uint8_t* rs = peer->rq + ((peer->hw_rq_cons & (peer->rq_cnt - 1)) << 4);
         rn::DataSeg ds;
@@ -483,10 +496,8 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         const uint32_t rbytes = be32(ds.byte_count) & 0x7fffffffu, rlkey = be32(ds.lkey);
         const uint64_t raddr = be64(ds.addr);
         consumed_rq = true; rq_index = (uint16_t)peer->hw_rq_cons++;
-        uint64_t src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
-                                 : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
-        if (src && rbytes < v.bytes) syn = rn::SYN_REMOTE_INVAL_REQ_ERR;
-        uint64_t dst = (src && syn == rn::SYN_OK) ? translate(rdev, rlkey, raddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, true, &syn, &rmr) : 0;
+        if (rbytes < v.bytes) syn = rn::SYN_REMOTE_INVAL_REQ_ERR;
+        uint64_t dst = syn == rn::SYN_OK ? translate(rdev, rlkey, raddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, true, &syn, &rmr) : 0;
         if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, rmr, src, lmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) moved = v.bytes;
         break;

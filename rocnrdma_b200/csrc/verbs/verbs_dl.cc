@@ -148,6 +148,7 @@ struct QpH {
   uint64_t next_wr_id = 1;
   bool raw_owned = false;     // queues handed to the GPU: host posting would fight over the producer index
   int proxy_slot = -1;
+  std::vector<uint64_t> host_regs;   // pages of the g_host_regs ranges this QP's GPU mapping holds a reference on
 };
 struct MrH { Dev* dev; ibv_mr* mr; int mode; };
 
@@ -370,9 +371,46 @@ RN_API void* rn_verbs_create_qp(void* dev, void* scq, void* rcq, uint32_t sq_dep
   return q;
 }
 RN_API uint32_t rn_verbs_qp_max_inline(void* qp) { return ((QpH*)qp)->max_inline; }
+// Host ranges rn_verbs_map_qp_to_gpu registered with CUDA, reference-counted: a CQ shared by two QPs is registered
+// once and stays mapped until the last QP that mapped it is destroyed.  Each range is unregistered before the provider
+// frees its memory.  A registration left behind on freed memory would make a later queue that lands on overlapping
+// pages fail to map (cudaHostRegister: already registered; cudaHostGetDevicePointer: fails outside the old range).
+namespace {
+struct HostReg { uint64_t page; size_t len; int refs; };
+std::mutex g_host_regs_mu;
+std::vector<HostReg> g_host_regs;
+
+void host_reg_track(QpH* q, uint64_t page, size_t len, bool registered_now) {
+  std::lock_guard<std::mutex> g(g_host_regs_mu);
+  if (registered_now) {
+    g_host_regs.push_back({page, len, 1});
+    q->host_regs.push_back(page);
+    return;
+  }
+  for (auto& r : g_host_regs)   // already registered: take a reference if the range is one of ours
+    if (page >= r.page && page + len <= r.page + r.len) { r.refs++; q->host_regs.push_back(r.page); return; }
+}
+
+void host_reg_release(QpH* q) {
+  std::lock_guard<std::mutex> g(g_host_regs_mu);
+  for (uint64_t page : q->host_regs)
+    for (size_t i = 0; i < g_host_regs.size(); ++i)
+      if (g_host_regs[i].page == page) {
+        if (--g_host_regs[i].refs == 0) {
+          cudaHostUnregister((void*)page);
+          cudaGetLastError();
+          g_host_regs.erase(g_host_regs.begin() + (long)i);
+        }
+        break;
+      }
+  q->host_regs.clear();
+}
+}  // namespace
+
 RN_API int rn_verbs_destroy_qp(void* qp) {
   QpH* q = (QpH*)qp;
   proxy_detach(q->proxy_slot);
+  host_reg_release(q);      // before the provider frees the queue memory
   int rc = api().destroy_qp(q->qp);
   delete q;
   return rc ? -rc : 0;
@@ -668,6 +706,7 @@ RN_API int rn_verbs_map_qp_to_gpu(void* qp, RnGpuQp* out) {
       return -5;
     }
     cudaGetLastError();
+    host_reg_track(q, page, len, e == cudaSuccess);
     void* d = nullptr;
     if (cudaHostGetDevicePointer(&d, (void*)page, 0) != cudaSuccess) { cudaGetLastError(); if (!quiet) why(-5, "cudaHostGetDevicePointer failed"); return -5; }
     *dev = (uint64_t)d + (host - page);

@@ -6,17 +6,9 @@ import torch
 
 import rocnrdma_b200 as rn
 from rocnrdma_b200 import ops, wire as W
+from rc_model import BULK_MIN, _chunks
 
 pytestmark = pytest.mark.gpu
-
-KSUB, BULK_MIN = 16384, 4096
-
-
-def _chunks(nbytes, ctas, chunk_bytes):
-    """The chunk lengths the engine cuts a WQE into (write_resolved's granule policy)."""
-    want = -(-nbytes // (8 * ctas))
-    g = max(chunk_bytes, -(-want // KSUB) * KSUB)
-    return [min(g, nbytes - off) for off in range(0, nbytes, g)]
 
 
 def _left_cleanly(ctx):

@@ -129,6 +129,24 @@ def test_doorbell_through_the_cpu_proxy(monkeypatch):
         c.close()
 
 
+def test_destroying_a_gpu_mapped_qp_unregisters_its_queues():
+    """to_gpu() registers the QP's rings, doorbell records and CQs with CUDA.  Destroying the QP must unregister them
+    before the provider frees that memory: a registration left on freed pages makes a later QP whose queues land on
+    overlapping pages fail to map (cudaHostGetDevicePointer fails outside the stale range)."""
+    lib = N.load()
+    pinned = lambda p: lib.rn_classify_ptr(p, None) == 2      # cudaMemoryTypeHost: registered host memory
+    c = rn.Context(device=0, wire="verbs", nic=0)
+    try:
+        qp = c.loopback_qp(depth=64)                             # MEM_DEVICE: the queues are handed to the GPU
+        assert qp.on_gpu
+        raw = qp.raw_queues()
+        pages = {k: raw[k] for k in ("sq_buf", "dbrec", "cq_buf", "cq_dbrec", "rcq_buf", "rcq_dbrec")}
+        assert all(pinned(p) for p in pages.values()), pages
+    finally:
+        c.close()
+    assert not [k for k, p in pages.items() if pinned(p)], "still registered after the QP was destroyed"
+
+
 @pytest.mark.parametrize("with_imm", [False, True])
 def test_fused_pack_posts_to_the_nic(vctx, with_imm):
     """K3 on the verbs wire: every CTA that completes a record posts its own WQE into the shared mlx5 send queue."""
