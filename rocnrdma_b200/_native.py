@@ -34,7 +34,8 @@ class RnRemote(C.Structure):
 class RnQpCounters(C.Structure):
     _fields_ = [("n_wqe", u64), ("n_cqe", u64), ("n_err", u64), ("n_db_order_violations", u64),
                 ("n_bytes", u64), ("n_rnr", u64), ("resv_head", u64), ("ready_head", u64),
-                ("sq_cons", u64), ("cursor", u64), ("retire_head", u64), ("state", u32), ("pad", u32)]
+                ("sq_cons", u64), ("cursor", u64), ("retire_head", u64), ("state", u32), ("pad", u32),
+                ("n_fence_waits", u64)]
 
 
 class RnVWc(C.Structure):
@@ -128,7 +129,8 @@ _SIGS = {
     "rn_k_recv_consume": (i32, [u64, u64, u32, u32, u64, u64, u64, u64, u32, u32]),
     "rn_hca_enable_peer": (i32, [vp, i32]),
     "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64]),
-    "rn_k_rdma_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u32, u32, u32, u32, u64, u32, u64, u64]),
+    "rn_k_rdma_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u32, u32, u32, u32, u64, u32, u64, u64, u32]),
+    "rn_k_write_read": (i32, [u64, u64, u64, u32, u64, u32, u64, u32, u32, u32, u32, u64, u64]),
     "rn_stream_clamp": (None, [u32, C.POINTER(u32), C.POINTER(u32)]),
     "rn_wire_build_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, u64, u32, u32, u32, u32]),
     "rn_wire_decode_cqe": (i32, [C.POINTER(u8), C.POINTER(RnWc)]),

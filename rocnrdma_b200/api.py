@@ -90,6 +90,16 @@ def _inline_bytes(data, limit: int) -> bytes:
     return b
 
 
+def _ctrl_flags(signaled: bool, fence: bool) -> int:
+    """The WQE ctrl segment's fm_ce_se byte of a host post (softhca wire)."""
+    return (W.CTRL_CQ_UPDATE if signaled else 0) | (W.CTRL_FENCE if fence else 0)
+
+
+def _verbs_flags(signaled: bool, fence: bool) -> int:
+    """The flags word of rn_verbs_post_*: bit 0 signaled (IBV_SEND_SIGNALED), bit 1 fence (IBV_SEND_FENCE)."""
+    return (1 if signaled else 0) | (2 if fence else 0)
+
+
 @dataclass
 class WorkCompletion:
     qpn: int
@@ -251,85 +261,91 @@ class QueuePair:
         return self
 
     # ---- host-posted verbs (the "ibv_post_send" baseline path)
-    def _post(self, opcode, laddr, lkey, raddr, rkey, nbytes, signaled=True, imm=0) -> int:
+    def _post(self, opcode, laddr, lkey, raddr, rkey, nbytes, signaled=True, imm=0, fence=False) -> int:
         idx = C.c_uint64()
-        flags = W.CTRL_CQ_UPDATE if signaled else 0
+        flags = _ctrl_flags(signaled, fence)
         self.ctx.sweep_revoked()          # a freed allocation must not be reachable through a stale key
         N.check(self.ctx._lib.rn_post_send(self._q, opcode, laddr, lkey, raddr, rkey, nbytes, flags, imm,
                                            C.byref(idx)), "post_send")
         return idx.value
 
     def post_write(self, src: MemoryRegion, dst: MemoryRegion, nbytes=None, src_off=0, dst_off=0, signaled=True,
-                   imm=None) -> int:
-        """Host-posted RDMA WRITE (``imm`` not None: WRITE_WITH_IMM, consumes a receive WQE at the responder).  Returns the WQE index."""
+                   imm=None, fence=False) -> int:
+        """Host-posted RDMA WRITE (``imm`` not None: WRITE_WITH_IMM, consumes a receive WQE at the responder).
+        ``fence=True`` (``IBV_SEND_FENCE``): it moves no byte before every earlier work request of this QP has finished,
+        so it may overwrite what an earlier WRITE wrote, or send what an earlier READ fetched.  Returns the WQE index."""
         n = src.length - src_off if nbytes is None else nbytes
         op = W.OP_RDMA_WRITE if imm is None else W.OP_RDMA_WRITE_IMM
-        return self._post(op, src.addr + src_off, src.lkey, dst.addr + dst_off, dst.rkey, n, signaled, imm or 0)
+        return self._post(op, src.addr + src_off, src.lkey, dst.addr + dst_off, dst.rkey, n, signaled, imm or 0, fence)
 
     def post_read(self, dst_local: MemoryRegion, src_remote: MemoryRegion, nbytes=None, local_off=0, remote_off=0,
-                  signaled=True) -> int:
-        """Host-posted RDMA READ into ``dst_local``.  Returns the WQE index."""
+                  signaled=True, fence=False) -> int:
+        """Host-posted RDMA READ into ``dst_local``.  ``fence=True``: it reads nothing before every earlier work request
+        of this QP has finished (a READ of bytes an earlier WRITE wrote returns the written bytes).  Returns the WQE index."""
         n = dst_local.length - local_off if nbytes is None else nbytes
         return self._post(W.OP_RDMA_READ, dst_local.addr + local_off, dst_local.lkey, src_remote.addr + remote_off,
-                          src_remote.rkey, n, signaled)
+                          src_remote.rkey, n, signaled, 0, fence)
 
-    def post_send(self, src: MemoryRegion, nbytes=None, src_off=0, signaled=True, imm=None) -> int:
-        """Host-posted SEND (``imm`` not None: SEND_WITH_IMM); lands in the responder's next receive buffer."""
+    def post_send(self, src: MemoryRegion, nbytes=None, src_off=0, signaled=True, imm=None, fence=False) -> int:
+        """Host-posted SEND (``imm`` not None: SEND_WITH_IMM); lands in the responder's next receive buffer.
+        ``fence=True``: its payload is read only after every earlier work request of this QP has finished (the receive
+        is still matched in posting order)."""
         n = src.length - src_off if nbytes is None else nbytes
         op = W.OP_SEND if imm is None else W.OP_SEND_IMM
-        return self._post(op, src.addr + src_off, src.lkey, 0, 0, n, signaled, imm or 0)
+        return self._post(op, src.addr + src_off, src.lkey, 0, 0, n, signaled, imm or 0, fence)
 
-    def post_raw(self, opcode, laddr=0, lkey=0, raddr=0, rkey=0, nbytes=0, signaled=True, imm=0) -> int:
+    def post_raw(self, opcode, laddr=0, lkey=0, raddr=0, rkey=0, nbytes=0, signaled=True, imm=0, fence=False) -> int:
         """Post a WQE with arbitrary fields (error-path tests: bad keys, bad opcodes, NOP)."""
-        return self._post(opcode, laddr, lkey, raddr, rkey, nbytes, signaled, imm)
+        return self._post(opcode, laddr, lkey, raddr, rkey, nbytes, signaled, imm, fence)
 
-    def _post_atomic(self, opcode, local, remote, swap_add, compare, local_off, remote_off, signaled) -> int:
+    def _post_atomic(self, opcode, local, remote, swap_add, compare, local_off, remote_off, signaled, fence=False) -> int:
         idx = C.c_uint64()
         self.ctx.sweep_revoked()
         N.check(self.ctx._lib.rn_post_atomic(self._q, opcode, local.addr + local_off, local.lkey, remote.addr + remote_off,
                                              remote.rkey, swap_add & 0xFFFFFFFFFFFFFFFF, compare & 0xFFFFFFFFFFFFFFFF,
-                                             W.CTRL_CQ_UPDATE if signaled else 0, C.byref(idx)), "post_atomic")
+                                             _ctrl_flags(signaled, fence), C.byref(idx)), "post_atomic")
         return idx.value
 
     def post_fetch_add(self, local: MemoryRegion, remote: MemoryRegion, add: int, local_off=0, remote_off=0,
-                       signaled=True) -> int:
+                       signaled=True, fence=False) -> int:
         """Host-posted 8-byte FETCH_AND_ADD: adds ``add`` to the u64 at ``remote.addr + remote_off`` (8-byte aligned,
         registered with ``ACC_REMOTE_ATOMIC``) and writes its original value to the 8 bytes at ``local.addr + local_off``.
-        Executes after every earlier work request of this QP.  Returns the WQE index."""
-        return self._post_atomic(W.OP_ATOMIC_FA, local, remote, add, 0, local_off, remote_off, signaled)
+        Executes after every earlier work request of this QP, ``fence`` or not.  Returns the WQE index."""
+        return self._post_atomic(W.OP_ATOMIC_FA, local, remote, add, 0, local_off, remote_off, signaled, fence)
 
     def post_cmp_swap(self, local: MemoryRegion, remote: MemoryRegion, compare: int, swap: int, local_off=0, remote_off=0,
-                      signaled=True) -> int:
+                      signaled=True, fence=False) -> int:
         """Host-posted 8-byte COMPARE_AND_SWAP: the remote u64 becomes ``swap`` if it equals ``compare``; its original
         value lands in the local 8 bytes either way (equal to ``compare`` exactly when the swap happened).  Returns the
         WQE index."""
-        return self._post_atomic(W.OP_ATOMIC_CS, local, remote, swap, compare, local_off, remote_off, signaled)
+        return self._post_atomic(W.OP_ATOMIC_CS, local, remote, swap, compare, local_off, remote_off, signaled, fence)
 
     @property
     def max_inline(self) -> int:
         """Largest payload an inline work request carries: 28 bytes (one 64-byte WQEBB)."""
         return W.MAX_INLINE
 
-    def _post_inline(self, opcode, raddr, rkey, buf: bytes, signaled, imm) -> int:
+    def _post_inline(self, opcode, raddr, rkey, buf: bytes, signaled, imm, fence=False) -> int:
         idx = C.c_uint64()
         self.ctx.sweep_revoked()
         N.check(self.ctx._lib.rn_post_inline(self._q, opcode, raddr, rkey, C.create_string_buffer(buf, len(buf)), len(buf),
-                                             W.CTRL_CQ_UPDATE if signaled else 0, imm, C.byref(idx)), "post_inline")
+                                             _ctrl_flags(signaled, fence), imm, C.byref(idx)), "post_inline")
         return idx.value
 
-    def post_write_inline(self, dst: MemoryRegion, data, dst_off=0, signaled=True, imm=None) -> int:
+    def post_write_inline(self, dst: MemoryRegion, data, dst_off=0, signaled=True, imm=None, fence=False) -> int:
         """Inline RDMA WRITE (``imm`` not None: WRITE_WITH_IMM) of ``data`` -- ``bytes``-like or a CPU tensor, 1 to
         ``max_inline`` bytes -- to ``dst.addr + dst_off``.  The payload is copied into the work request itself: no local
-        memory region, and ``data`` may change as soon as this returns.  Returns the WQE index."""
+        memory region, and ``data`` may change as soon as this returns.  ``fence`` as in :meth:`post_write`.  Returns the
+        WQE index."""
         buf = _inline_bytes(data, self.max_inline)
         op = W.OP_RDMA_WRITE if imm is None else W.OP_RDMA_WRITE_IMM
-        return self._post_inline(op, dst.addr + dst_off, dst.rkey, buf, signaled, imm or 0)
+        return self._post_inline(op, dst.addr + dst_off, dst.rkey, buf, signaled, imm or 0, fence)
 
-    def post_send_inline(self, data, signaled=True, imm=None) -> int:
+    def post_send_inline(self, data, signaled=True, imm=None, fence=False) -> int:
         """Inline SEND (``imm`` not None: SEND_WITH_IMM) of 1 to ``max_inline`` bytes; lands in the responder's next receive
-        buffer.  Returns the WQE index."""
+        buffer.  ``fence`` as in :meth:`post_send`.  Returns the WQE index."""
         buf = _inline_bytes(data, self.max_inline)
-        return self._post_inline(W.OP_SEND if imm is None else W.OP_SEND_IMM, 0, 0, buf, signaled, imm or 0)
+        return self._post_inline(W.OP_SEND if imm is None else W.OP_SEND_IMM, 0, 0, buf, signaled, imm or 0, fence)
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
         """Post one receive buffer (consumed in order by SEND / WRITE_WITH_IMM)."""
@@ -351,7 +367,8 @@ class QueuePair:
         return [{k: buf[i * 8 + j] for j, k in enumerate(names)} for i in range(n)]
 
     def counters(self) -> dict:
-        """Engine-side counters of this QP (WQEs, CQEs, errors, bytes, RNR waits, doorbell-order violations) and its queue indices."""
+        """Engine-side counters of this QP (WQEs, CQEs, errors, bytes, RNR waits, doorbell-order violations, fenced WQEs
+        that found their gate closed: ``n_fence_waits``) and its queue indices."""
         c = N.RnQpCounters()
         N.check(self.ctx._lib.rn_qp_query(self._q, C.byref(c)), "qp_query")
         d = {k: getattr(c, k) for k, _ in c._fields_ if k != "pad"}
@@ -451,17 +468,17 @@ class VerbsQueuePair(QueuePair):
         self._vcheck(self.ctx._lib.rn_verbs_raw_qp(self._vq, C.byref(r)), "raw_qp")
         return {k: getattr(r, k) for k, _ in r._fields_ if not k.startswith("pad")}
 
-    def _post(self, opcode, laddr, lkey, raddr, rkey, nbytes, signaled=True, imm=0) -> int:
+    def _post(self, opcode, laddr, lkey, raddr, rkey, nbytes, signaled=True, imm=0, fence=False) -> int:
         wr = C.c_uint64()
-        self._vcheck(self.ctx._lib.rn_verbs_post_send(self._vq, opcode, laddr, lkey, raddr, rkey, nbytes, int(bool(signaled)), imm,
-                                                      C.byref(wr)), "post_send")
+        self._vcheck(self.ctx._lib.rn_verbs_post_send(self._vq, opcode, laddr, lkey, raddr, rkey, nbytes, _verbs_flags(signaled, fence),
+                                                      imm, C.byref(wr)), "post_send")
         return wr.value
 
-    def _post_atomic(self, opcode, local, remote, swap_add, compare, local_off, remote_off, signaled) -> int:
+    def _post_atomic(self, opcode, local, remote, swap_add, compare, local_off, remote_off, signaled, fence=False) -> int:
         wr = C.c_uint64()
         self._vcheck(self.ctx._lib.rn_verbs_post_atomic(self._vq, opcode, local.addr + local_off, local.lkey,
                                                         remote.addr + remote_off, remote.rkey, swap_add & 0xFFFFFFFFFFFFFFFF,
-                                                        compare & 0xFFFFFFFFFFFFFFFF, int(bool(signaled)), C.byref(wr)),
+                                                        compare & 0xFFFFFFFFFFFFFFFF, _verbs_flags(signaled, fence), C.byref(wr)),
                      "post_atomic")
         return wr.value
 
@@ -470,10 +487,10 @@ class VerbsQueuePair(QueuePair):
         """The inline capacity the provider granted, capped at 28 bytes (one WQEBB)."""
         return min(W.MAX_INLINE, self.ctx._lib.rn_verbs_qp_max_inline(self._vq))
 
-    def _post_inline(self, opcode, raddr, rkey, buf: bytes, signaled, imm) -> int:
+    def _post_inline(self, opcode, raddr, rkey, buf: bytes, signaled, imm, fence=False) -> int:
         wr = C.c_uint64()
         self._vcheck(self.ctx._lib.rn_verbs_post_inline(self._vq, opcode, raddr, rkey, C.create_string_buffer(buf, len(buf)),
-                                                        len(buf), int(bool(signaled)), imm, C.byref(wr)), "post_inline")
+                                                        len(buf), _verbs_flags(signaled, fence), imm, C.byref(wr)), "post_inline")
         return wr.value
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):

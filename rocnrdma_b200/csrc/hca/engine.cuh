@@ -670,13 +670,34 @@ __device__ __forceinline__ void retire(QpDev* qp, uint32_t lane, unsigned long l
   }
 }
 
+// ------------------------------------------------------------------ fence gate
+// A WQE posted with CTRL_FENCE (fm = 4; the other fm values gate nothing) moves no byte before every earlier WQE of its
+// QP has finished (DESIGN.md 3.1).  Only a clean WQE that moves bytes is gated: an atomic executes at retirement, which
+// is in order already, and a flushed or zero-length WQE has nothing to hold back.  Tested on the decoded WQE, so an
+// unfenced one pays a bit test.
+__device__ __forceinline__ bool fence_gated(const WqeView& v, uint8_t syn) {
+  return (v.fm_ce_se & 0xe0u) == CTRL_FENCE && syn == SYN_OK && v.bytes != 0;
+}
+// Has every WQE before w finished?  Retirement is in order and a WQE retires only once its chunks are written and its
+// atomic executed, so "the retirer has reached w" is exactly that.  It is read from retire_word, not retire_head: the
+// retirer unlocks with (w << 1) behind its release fence, and nobody can lock at head w before w itself finished, so the
+// word reads exactly (w << 1) from then until w retires.  On true, the fence acquires every earlier WQE's bytes for the
+// loads of w's chunks (and releases the ticket the caller arms or opens next).
+__device__ __forceinline__ bool gate_open(QpDev* qp, unsigned long long w) {
+  if (ld_u64_volatile(&qp->retire_word) != (w << 1)) return false;
+  fence_gpu();
+  return true;
+}
+// Generic-proxy writes (and what the acquire above carried) before this CTA's later TMA loads (the async proxy).
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
 // ------------------------------------------------------------------ claim
 struct Work {
   QpDev* qp;
   unsigned long long w;
   uint32_t chunk;
   // filled by a direct (single-WQE) claim, which has just computed them: saves re-reading resolved[w]
-  uint32_t have_desc, len, nch;
+  uint32_t have_desc, len, nch, fenced;
   uint64_t src, dst;
 };
 
@@ -767,20 +788,29 @@ __device__ __forceinline__ int try_claim(EngineCtl* ctl, QpDev* qp, Work* out, b
         fence_gpu();  // release rq_head
       }
       if (syn != SYN_OK && !err) { qp->state = QPS_ERR; err = true; }
+      // A fenced WQE whose gate is still closed is not moved by its claimer: even with one chunk it gets a gated ticket,
+      // which the helpers' offer scan stops at and opens once the retirer reaches it.
+      const bool fenced = fence_gated(p.v, syn);
+      const bool closed = fenced && !gate_open(qp, w);
       Resolved* res = qp->resolved + (w & mask);
       const unsigned long long next = (w + 1) | (err ? (unsigned long long)PARSE_ERR_BIT : 0ull);
-      if (n > 1) {
+      if (n > 1 || closed) {
         fence_gpu();  // release resolved[w] before the ticket that lets helpers read it
-        st_u64_relaxed(&res->ticket, TICKET_ONE | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | n);
+        st_u64_relaxed(&res->ticket, (closed ? TICKET_GATED : TICKET_ONE) | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | n);
         st_u64_release_scope(&qp->parse_seq, next, false);   // helpers trust: committed => ticket armed
       } else {
         st_u64_relaxed(&qp->parse_seq, next);
       }
       trace_stamp(qp, w, TR_PARSED);
+      if (closed) {
+        atomicAdd(&qp->n_fence_waits, 1ull);
+        *saw_pending = true;
+        return 0;
+      }
       out->qp = qp; out->w = w; out->chunk = 0;
       {
         const uint32_t bytes = syn == SYN_OK ? p.v.bytes : 0;
-        out->have_desc = 1; out->nch = n; out->src = fsrc; out->dst = fdst;
+        out->have_desc = 1; out->nch = n; out->src = fsrc; out->dst = fdst; out->fenced = fenced;
         out->len = bytes < chunk_sz ? bytes : chunk_sz;     // chunk 0
       }
       return 1;
@@ -795,17 +825,33 @@ __device__ __forceinline__ int try_claim(EngineCtl* ctl, QpDev* qp, Work* out, b
     unsigned long long t[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) t[k] = (uint32_t)k < cnt ? ld_u64_volatile(&(qp->resolved + ((off + k) & mask))->ticket) : 0ull;
-    uint32_t avail[8], total = 0, lead = 0;
+    uint32_t avail[8], total = 0, lead = 0, gk = 8;
+    unsigned long long gt = 0;
     bool leading = true;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const bool mine = (uint32_t)((t[k] >> TICKET_GEN_SHIFT) & TICKET_FIELD_MASK) == (uint32_t)((off + k) & TICKET_FIELD_MASK);
       const uint32_t cc = (uint32_t)(t[k] >> 40), nn = (uint32_t)(t[k] & TICKET_FIELD_MASK);
+      // gated (a fenced WQE waiting for its gate): nothing to draw yet, but the offer must not pass it
+      const bool gated = (uint32_t)k < cnt && mine && (t[k] & TICKET_GATED);
+      if (gated && gk == 8) { gk = k; gt = t[k]; }
       avail[k] = ((uint32_t)k < cnt && mine && cc < nn) ? nn - cc : 0u;   // single-chunk WQE taken by its claimer, or fully drawn: 0
       total += avail[k];
-      if (leading && (uint32_t)k < cnt && avail[k] == 0) ++lead; else leading = false;
+      if (leading && (uint32_t)k < cnt && avail[k] == 0 && !gated) ++lead; else leading = false;
     }
     if (lead) atomicMax(&qp->offer, off + lead);
+    // The gate is polled here: every CTA that scans the QP re-checks it, so it cannot be missed and nobody blocks on it.
+    // Only the oldest gated WQE can be at the retire head.  Opening resets the chunk counter (one CAS: a second opener, or
+    // a stray draw that bumped the gated counter, makes it fail and the next scan looks again).
+    if (gk < 8) {
+      *saw_pending = true;
+      const unsigned long long gw = off + gk;
+      Resolved* gr = qp->resolved + (gw & mask);
+      if (gate_open(qp, gw)) {
+        atomicCAS(&gr->ticket, gt, gt & TICKET_LOW_MASK);
+        if (draw_chunk(qp, gr, gw, out)) return 1;
+      }
+    }
     if (total) {
       *saw_pending = true;
       uint32_t pick = blockIdx.x % (total < gridDim.x ? total : gridDim.x), sel = 0;
@@ -867,7 +913,10 @@ __device__ __forceinline__ void claim_batch(EngineCtl* ctl, QpDev* qp, unsigned 
       }
       if (syn != SYN_OK && !err) { qp->state = QPS_ERR; err = 1; }
       Resolved* res = qp->resolved + (w & mask);
-      st_u64_relaxed(&res->ticket, ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | n);    // chunk counter starts at 0
+      // a fenced WQE is armed gated unless its gate is already open (gate_open's fence then orders it before the ticket)
+      const bool closed = fence_gated(p.v, syn) && !gate_open(qp, w);
+      if (closed) atomicAdd(&qp->n_fence_waits, 1ull);
+      st_u64_relaxed(&res->ticket, (closed ? TICKET_GATED : 0ull) | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | n);    // chunk counter starts at 0
       trace_stamp(qp, w, TR_PARSED);
     }
     __syncwarp();
@@ -1018,8 +1067,9 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
       if (have) {
         uint32_t len;
         uint64_t csrc, cdst;
+        bool fenced;
         if (work.have_desc) {
-          len = work.len; csrc = work.src; cdst = work.dst; nch = work.nch;
+          len = work.len; csrc = work.src; cdst = work.dst; nch = work.nch; fenced = work.fenced != 0;
         } else {
           Resolved* r = work.qp->resolved + (work.w & ((1u << work.qp->sq_log) - 1));
           const uint4 f = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r) + 16);   // bytes | nchunks | imm | flags
@@ -1031,6 +1081,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
           csrc = (((uint64_t)a.y << 32) | a.x) + off;
           cdst = (((uint64_t)a.w << 32) | a.z) + off;
           nch = f.y;
+          fenced = ((f.w >> 8) & 0xe0u) == CTRL_FENCE;
         }
         if (nch > 1) { sticky_qp = work.qp; sticky_w = work.w; }
         last_activity = globaltimer_ns();
@@ -1039,6 +1090,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
           act = 3;
         } else if (len >= kBulkMin && (((csrc | cdst) & 15) == 0) && ((len & 15) == 0)) {
           // reap() left room: outstanding < kQueue
+          if (fenced) fence_proxy_async_global();   // the mover's TMA loads see what the gate's acquire made visible
           s.q[e_push] = Chunk{csrc, cdst, len};
           s.owed[e_push] = Owed{work.qp, work.w, nch};
           mbar_arrive(&s.qfull[e_push]);

@@ -746,6 +746,7 @@ struct RnQpCounters {
   uint64_t n_wqe, n_cqe, n_err, n_db_order_violations, n_bytes, n_rnr;
   uint64_t resv_head, ready_head, sq_cons, cursor, retire_head;
   uint32_t state, pad;
+  uint64_t n_fence_waits;
 };
 RN_API int rn_qp_query(void* qp, RnQpCounters* out) {
   Qp* q = (Qp*)qp;
@@ -758,6 +759,7 @@ RN_API int rn_qp_query(void* qp, RnQpCounters* out) {
   out->resv_head = d.resv_head; out->ready_head = d.ready_head; out->sq_cons = d.sq_cons;
   out->cursor = d.cursor; out->retire_head = d.retire_head;  // cursor = claim head
   out->state = d.state; out->pad = 0;
+  out->n_fence_waits = d.n_fence_waits;
   return 0;
 }
 

@@ -135,11 +135,16 @@ struct QpDev {
   unsigned long long rq_cached_pi; // responder receive-producer count as last read (a remote read: refreshed only when exhausted)
   // ---- counters (readable from the host; SURVEY.md section 5 "metrics")
   unsigned long long n_wqe, n_cqe, n_err, n_db_order_violations, n_bytes, n_rnr;
+  unsigned long long n_fence_waits;  // fenced WQEs whose gate was still closed when they committed
 };
 
 // Chunk tickets: one atomicAdd(TICKET_ONE) hands out a self-describing claim.
 enum : unsigned long long { PARSE_ERR_BIT = 1ull << 63 };
 enum : unsigned long long { TICKET_ONE = 1ull << 40, TICKET_GEN_SHIFT = 20, TICKET_FIELD_MASK = 0xfffffull };
+// A fenced WQE's ticket before its gate opens: the top bit of the chunk counter.  The counter then reads >= 2^23, above
+// any chunk count, so every existing "next chunk < nchunks" test sees nothing to draw (a stray draw only bumps it).  The
+// gate is opened by resetting the counter to 0 (eng::try_claim), which also drops this bit.
+enum : unsigned long long { TICKET_GATED = 1ull << 63, TICKET_LOW_MASK = TICKET_ONE - 1 };
 
 struct EngineCtl {
   volatile uint32_t* stop;         // mapped pinned host word: nonzero = exit

@@ -390,26 +390,31 @@ __device__ __forceinline__ unsigned long long post_one(QpDev* qp, Build build,
 }
 
 // -------------------------------------------------------------- one-call verbs
+// Every one-call verb takes `signaled` (a CQE on success) and, last, `fence` (IBV_SEND_FENCE: the WR moves no byte, and
+// its atomic does not execute, before every earlier WR of the QP has finished -- DESIGN.md 3.1).
+__device__ __forceinline__ uint8_t wr_flags(bool signaled, bool fence) {
+  return (uint8_t)((signaled ? CTRL_CQ_UPDATE : 0) | (fence ? CTRL_FENCE : 0));
+}
 __device__ __forceinline__ unsigned long long rdma_write(QpDev* qp, uint64_t laddr, uint32_t lkey,
                                                          uint64_t raddr, uint32_t rkey, uint32_t bytes,
-                                                         bool signaled = true) {
+                                                         bool signaled = true, bool fence = false) {
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
-    build_rdma_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, bytes, signaled ? CTRL_CQ_UPDATE : 0, 0);
+    build_rdma_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, bytes, wr_flags(signaled, fence), 0);
   });
 }
 __device__ __forceinline__ unsigned long long rdma_read(QpDev* qp, uint64_t laddr, uint32_t lkey,
                                                         uint64_t raddr, uint32_t rkey, uint32_t bytes,
-                                                        bool signaled = true) {
+                                                        bool signaled = true, bool fence = false) {
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
-    build_rdma_wqe(w, OP_RDMA_READ, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, bytes, signaled ? CTRL_CQ_UPDATE : 0, 0);
+    build_rdma_wqe(w, OP_RDMA_READ, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, bytes, wr_flags(signaled, fence), 0);
   });
 }
 __device__ __forceinline__ unsigned long long rdma_send(QpDev* qp, uint64_t laddr, uint32_t lkey,
                                                         uint32_t bytes, bool signaled = true,
-                                                        uint32_t imm = 0, bool with_imm = false) {
+                                                        uint32_t imm = 0, bool with_imm = false, bool fence = false) {
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
     build_send_wqe(w, with_imm ? OP_SEND_IMM : OP_SEND, (uint16_t)idx, qp->qpn, laddr, lkey, bytes,
-                   signaled ? CTRL_CQ_UPDATE : 0, imm);
+                   wr_flags(signaled, fence), imm);
   });
 }
 
@@ -417,17 +422,18 @@ __device__ __forceinline__ unsigned long long rdma_send(QpDev* qp, uint64_t ladd
 // "data landed" after its RDMA WRITEs: the engine executes the atomic only after every earlier WQE of the QP).
 // The original remote value lands in the 8 local bytes at laddr.
 __device__ __forceinline__ unsigned long long rdma_fetch_add(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr,
-                                                             uint32_t rkey, uint64_t add, bool signaled = true) {
+                                                             uint32_t rkey, uint64_t add, bool signaled = true,
+                                                             bool fence = false) {
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
-    build_atomic_wqe(w, OP_ATOMIC_FA, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, add, 0, signaled ? CTRL_CQ_UPDATE : 0);
+    build_atomic_wqe(w, OP_ATOMIC_FA, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, add, 0, wr_flags(signaled, fence));
   });
 }
 __device__ __forceinline__ unsigned long long rdma_cmp_swap(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr,
                                                             uint32_t rkey, uint64_t compare, uint64_t swap,
-                                                            bool signaled = true) {
+                                                            bool signaled = true, bool fence = false) {
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
     build_atomic_wqe(w, OP_ATOMIC_CS, (uint16_t)idx, qp->qpn, laddr, lkey, raddr, rkey, swap, compare,
-                     signaled ? CTRL_CQ_UPDATE : 0);
+                     wr_flags(signaled, fence));
   });
 }
 
@@ -435,22 +441,23 @@ __device__ __forceinline__ unsigned long long rdma_cmp_swap(QpDev* qp, uint64_t 
 // buffer and no lkey: `data` may be any memory the calling thread can read (or a register, with rdma_p), and it may be
 // reused as soon as the call returns.  Returns the WQE index, or ~0ull when n is out of range or the queue stayed full.
 __device__ __forceinline__ unsigned long long rdma_put_inline(QpDev* qp, uint64_t raddr, uint32_t rkey, const void* data,
-                                                              uint32_t n, bool signaled = true) {
+                                                              uint32_t n, bool signaled = true, bool fence = false) {
   if (n == 0 || n > MAX_INLINE) return ~0ull;
   const InlinePayload d = inline_load(data, n);
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
-    build_inline_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, raddr, rkey, d, n, signaled ? CTRL_CQ_UPDATE : 0, 0);
+    build_inline_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, raddr, rkey, d, n, wr_flags(signaled, fence), 0);
   });
 }
 // nvshmem_p / doca_gpu_dev_verbs_p: one 1-, 2-, 4- or 8-byte value straight from a register.
 template <typename T>
-__device__ __forceinline__ unsigned long long rdma_p(QpDev* qp, uint64_t raddr, uint32_t rkey, T value, bool signaled = true) {
+__device__ __forceinline__ unsigned long long rdma_p(QpDev* qp, uint64_t raddr, uint32_t rkey, T value, bool signaled = true,
+                                                     bool fence = false) {
   static_assert(sizeof(T) == 1 || sizeof(T) == 2 || sizeof(T) == 4 || sizeof(T) == 8, "rdma_p: 1, 2, 4 or 8 bytes");
   InlinePayload d = {};
   memcpy(d.w, &value, sizeof(T));
   return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
     build_inline_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, raddr, rkey, d, (uint32_t)sizeof(T),
-                     signaled ? CTRL_CQ_UPDATE : 0, 0);
+                     wr_flags(signaled, fence), 0);
   });
 }
 

@@ -34,6 +34,7 @@ struct StreamArgs {
                            //    engine / NIC cannot make progress while this kernel is resident)
   uint64_t slot_stride;    // each iteration i uses offset (i % nslots) * slot_stride
   uint32_t nslots;
+  uint32_t fence_every;    // 0: no WR fenced; k: WRs k-1, 2k-1, ... of each QP carry CTRL_FENCE
   uint64_t timeout_ns;
   unsigned long long* out; // per CTA: [status, t_start, t_end, done, first_idx, last_idx, 0, 0]
 };
@@ -115,6 +116,7 @@ __global__ void __launch_bounds__(32, 1) rdma_stream_kernel(StreamArgs a) {
               a.out + (size_t)blockIdx.x * 8,
               [&](uint8_t* slot, uint16_t idx, uint32_t qpn, uint32_t i, uint32_t, uint8_t flags) {
                 const uint64_t off = (uint64_t)(i % a.nslots) * a.slot_stride;
+                if (a.fence_every && (i + 1) % a.fence_every == 0) flags |= CTRL_FENCE;
                 Wqe64 w;
                 if (a.opcode == OP_SEND) {
                   build_send_wqe(&w, OP_SEND, idx, qpn, lbase + off, a.lkey, a.bytes, flags, 0);
@@ -141,7 +143,7 @@ RN_API void rn_stream_clamp(uint32_t window, uint32_t* burst, uint32_t* signal_e
 RN_API int rn_k_rdma_stream(uint64_t stream, const uint64_t* qps_host, uint32_t nqp, uint32_t opcode, uint64_t laddr,
                             uint32_t lkey, uint64_t raddr, uint32_t rkey, uint64_t stride, uint32_t bytes,
                             uint32_t iters, uint32_t window, uint32_t signal_every, uint32_t burst, uint64_t slot_stride,
-                            uint32_t nslots, uint64_t timeout_ms, uint64_t out_dev) {
+                            uint32_t nslots, uint64_t timeout_ms, uint64_t out_dev, uint32_t fence_every) {
   StreamArgs a;
   if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps) return -22;
   for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
@@ -151,9 +153,70 @@ RN_API int rn_k_rdma_stream(uint64_t stream, const uint64_t* qps_host, uint32_t 
   rn_stream_clamp(window, &burst, &signal_every);
   a.signal_every = signal_every; a.burst = burst;
   a.slot_stride = slot_stride; a.nslots = nslots ? nslots : 1;
+  a.fence_every = fence_every;
   a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
   a.out = (unsigned long long*)out_dev;
   rdma_stream_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------- a WRITE and a dependent READ
+// One thread, `iters` times: an RDMA WRITE of `bytes` from laddr to raddr, then an RDMA READ of those bytes back from raddr
+// into back, and wait for the READ's completion.  How the READ is kept behind the WRITE:
+//   mode 0  the READ is fenced; both WQEs go out under ONE doorbell (exclusive poster)
+//   mode 1  the WRITE is signaled and its CQE awaited before the READ is posted (what ordering costs without the fence)
+//   mode 2  dev::rdma_write, then dev::rdma_read(..., fence = true) through the shared submit, then sq_wait
+// out: [status, t_start, t_end, pairs done, sum of pair ns, min pair ns, 0, 0]
+__global__ void __launch_bounds__(32, 1) write_read_kernel(QpDev* qp, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
+                                                           uint64_t back, uint32_t back_lkey, uint32_t bytes, uint32_t iters,
+                                                           uint32_t mode, unsigned long long timeout_ns, unsigned long long* out) {
+  if (threadIdx.x != 0) return;
+  int status = qp->state == QPS_ERR ? WAIT_QP_ERROR : WAIT_OK;
+  unsigned long long sum = 0, mn = ~0ull;
+  uint32_t done = 0;
+  const unsigned long long t0 = globaltimer_ns();
+  if (mode == 2) {
+    for (; done < iters && status == WAIT_OK; ++done) {
+      const unsigned long long ts = globaltimer_ns();
+      const unsigned long long i0 = rdma_write(qp, laddr, lkey, raddr, rkey, bytes, false);
+      const unsigned long long i1 = i0 == ~0ull ? ~0ull : rdma_read(qp, back, back_lkey, raddr, rkey, bytes, true, true);
+      if (i1 == ~0ull) { status = WAIT_TIMEOUT; break; }
+      status = sq_wait(qp, i1, timeout_ns);
+      const unsigned long long dt = globaltimer_ns() - ts;
+      sum += dt; mn = dt < mn ? dt : mn;
+    }
+  } else {
+    Poster p = poster_open(qp);
+    for (; done < iters && status == WAIT_OK; ++done) {
+      const unsigned long long ts = globaltimer_ns();
+      Wqe64 w;
+      unsigned long long idx = poster_reserve(p, 2, timeout_ns);
+      if (idx == ~0ull) { status = WAIT_TIMEOUT; break; }
+      build_rdma_wqe(&w, OP_RDMA_WRITE, (uint16_t)idx, p.qpn, laddr, lkey, raddr, rkey, bytes, mode == 0 ? 0 : CTRL_CQ_UPDATE, 0);
+      store_wqe(poster_slot(p, idx), w);
+      if (mode == 1) {
+        poster_ring(p, idx + 1);
+        if ((status = poster_wait(p, idx, timeout_ns)) != WAIT_OK) break;
+      }
+      build_rdma_wqe(&w, OP_RDMA_READ, (uint16_t)(idx + 1), p.qpn, back, back_lkey, raddr, rkey, bytes,
+                     mode == 0 ? (CTRL_CQ_UPDATE | CTRL_FENCE) : CTRL_CQ_UPDATE, 0);
+      store_wqe(poster_slot(p, idx + 1), w);
+      poster_ring(p, idx + 2);
+      if ((status = poster_wait(p, idx + 1, timeout_ns)) != WAIT_OK) break;
+      const unsigned long long dt = globaltimer_ns() - ts;
+      sum += dt; mn = dt < mn ? dt : mn;
+    }
+    poster_close(p);
+  }
+  out[0] = (unsigned long long)(long long)status;
+  out[1] = t0; out[2] = globaltimer_ns(); out[3] = done; out[4] = sum; out[5] = mn;
+}
+RN_API int rn_k_write_read(uint64_t stream, uint64_t qp_dev, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
+                           uint64_t back, uint32_t back_lkey, uint32_t bytes, uint32_t iters, uint32_t mode, uint64_t timeout_ms,
+                           uint64_t out_dev) {
+  if (mode > 2) return -22;
+  write_read_kernel<<<1, 32, 0, (cudaStream_t)stream>>>((QpDev*)qp_dev, laddr, lkey, raddr, rkey, back, back_lkey, bytes, iters, mode,
+                                                        (timeout_ms ? timeout_ms : 2000) * 1000000ull, (unsigned long long*)out_dev);
   return (int)cudaGetLastError();
 }
 
@@ -652,6 +715,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncGetAttributes(&a, rdma_stream_kernel);
   cudaFuncGetAttributes(&a, recv_consume_kernel);
   cudaFuncGetAttributes(&a, shared_post_stress_kernel);
+  cudaFuncGetAttributes(&a, write_read_kernel);
   cudaFuncGetAttributes(&a, atomic_stream_kernel);
   cudaFuncGetAttributes(&a, put_signal_kernel);
   cudaFuncGetAttributes(&a, put_inline_kernel);

@@ -455,9 +455,14 @@ RN_API int rn_verbs_set_state(void* qp, uint32_t state) {
 }
 
 // ------------------------------------------------------------------ host-posted verbs (baselines B0 / B2)
-// opcode is the mlx5 WQE opcode the rest of the project uses (wire.OP_*).
+// opcode is the mlx5 WQE opcode the rest of the project uses (wire.OP_*).  flags: RN_WR_SIGNALED (bit 0, so the 1 that
+// used to mean "signaled" still does) and RN_WR_FENCE (IBV_SEND_FENCE).
+enum : int { RN_WR_SIGNALED = 1, RN_WR_FENCE = 2 };
+static unsigned send_flags(int flags) {
+  return ((flags & RN_WR_SIGNALED) ? IBV_SEND_SIGNALED : 0u) | ((flags & RN_WR_FENCE) ? IBV_SEND_FENCE : 0u);
+}
 RN_API int rn_verbs_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey, uint32_t len,
-                              int signaled, uint32_t imm, uint64_t* wr_id_out) {
+                              int flags, uint32_t imm, uint64_t* wr_id_out) {
   QpH* q = (QpH*)qp;
   if (q->raw_owned) return why(-16, "this QP's queues are owned by the GPU poster; host posting would corrupt the producer index");
   ibv_sge sge = {laddr, len, lkey};
@@ -473,7 +478,7 @@ RN_API int rn_verbs_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_
     case 0x10: wr.opcode = IBV_WR_RDMA_READ; break;
     default: return why(-22, "unsupported opcode 0x%x for a host post", opcode);
   }
-  wr.send_flags = signaled ? IBV_SEND_SIGNALED : 0;
+  wr.send_flags = send_flags(flags);
   wr.imm_data = __builtin_bswap32(imm);            // host value -> network order
   wr.wr.rdma.remote_addr = raddr; wr.wr.rdma.rkey = rkey;
   int rc = ibv_post_send(q->qp, &wr, &bad);
@@ -484,7 +489,7 @@ RN_API int rn_verbs_post_send(void* qp, uint32_t opcode, uint64_t laddr, uint32_
 // 8-byte remote atomic (opcode OP_ATOMIC_FA: add = swap_add; OP_ATOMIC_CS: swap = swap_add, compare): the original
 // remote value lands in the 8 local bytes at laddr.
 RN_API int rn_verbs_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
-                                uint64_t swap_add, uint64_t compare, int signaled, uint64_t* wr_id_out) {
+                                uint64_t swap_add, uint64_t compare, int flags, uint64_t* wr_id_out) {
   QpH* q = (QpH*)qp;
   if (q->raw_owned) return why(-16, "this QP's queues are owned by the GPU poster; host posting would corrupt the producer index");
   ibv_sge sge = {laddr, 8, lkey};
@@ -497,7 +502,7 @@ RN_API int rn_verbs_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint3
     case 0x12: wr.opcode = IBV_WR_ATOMIC_FETCH_AND_ADD; wr.wr.atomic.compare_add = swap_add; break;
     default: return why(-22, "opcode 0x%x is not an atomic", opcode);
   }
-  wr.send_flags = signaled ? IBV_SEND_SIGNALED : 0;
+  wr.send_flags = send_flags(flags);
   wr.wr.atomic.remote_addr = raddr; wr.wr.atomic.rkey = rkey;
   int rc = ibv_post_send(q->qp, &wr, &bad);
   if (rc) return why(-rc, "ibv_post_send failed: %d (%s)", rc, strerror(rc));
@@ -508,7 +513,7 @@ RN_API int rn_verbs_post_atomic(void* qp, uint32_t opcode, uint64_t laddr, uint3
 // the caller's n host bytes; the provider copies them into the WQE, so no lkey is needed and the bytes may be reused at once.
 // The provider is the judge of what may be inline (length, opcode): its error comes back as -errno.
 RN_API int rn_verbs_post_inline(void* qp, uint32_t opcode, uint64_t raddr, uint32_t rkey, const void* data, uint32_t n,
-                                int signaled, uint32_t imm, uint64_t* wr_id_out) {
+                                int flags, uint32_t imm, uint64_t* wr_id_out) {
   QpH* q = (QpH*)qp;
   if (q->raw_owned) return why(-16, "this QP's queues are owned by the GPU poster; host posting would corrupt the producer index");
   ibv_sge sge = {(uint64_t)(uintptr_t)data, n, 0};
@@ -524,7 +529,7 @@ RN_API int rn_verbs_post_inline(void* qp, uint32_t opcode, uint64_t raddr, uint3
     case 0x10: wr.opcode = IBV_WR_RDMA_READ; break;
     default: return why(-22, "unsupported opcode 0x%x for a host post", opcode);
   }
-  wr.send_flags = IBV_SEND_INLINE | (signaled ? IBV_SEND_SIGNALED : 0);
+  wr.send_flags = IBV_SEND_INLINE | send_flags(flags);
   wr.imm_data = __builtin_bswap32(imm);
   wr.wr.rdma.remote_addr = raddr; wr.wr.rdma.rkey = rkey;
   int rc = ibv_post_send(q->qp, &wr, &bad);

@@ -68,11 +68,14 @@ class StreamResult:
 
 def rdma_stream(qps, opcode: int, src_mr, dst_mr, nbytes: int, iters: int = 1, window: int = 0,
                 signal_every: int = 1, burst: int = 1, stride: int = 0, slot_stride: int = 0, nslots: int = 1,
-                timeout_ms: int = 2000, stream=None, sync: bool = True, out=None, post_only: bool = False):
+                timeout_ms: int = 2000, stream=None, sync: bool = True, out=None, post_only: bool = False,
+                fence_every: int = 0):
     """Launch the device poster: one CTA per QP posts ``iters`` work requests of
     ``nbytes`` (window-limited), polls its CQ on the device and returns device times.
     ``burst`` work requests share one slot reservation and one doorbell (perftest ``--post_list``),
     ``signal_every`` is the CQ moderation (``--cq-mod``); both are clamped so the window can always drain.
+    ``fence_every=k`` sets the fence flag (``IBV_SEND_FENCE``) on every k-th work request of each QP (the k-th, 2k-th,
+    ...): it moves no byte before every earlier work request of its QP has finished.  0 fences nothing.
 
     For RDMA_READ ``src_mr`` is the local destination and ``dst_mr`` the remote source,
     mirroring the laddr/raddr roles in the WQE.  ``post_only`` skips the final completion wait (``iters`` must fit
@@ -88,7 +91,8 @@ def rdma_stream(qps, opcode: int, src_mr, dst_mr, nbytes: int, iters: int = 1, w
     out_addr, out_view = ctx.scratch(nq * 64) if out is None else out
     rc = lib.rn_k_rdma_stream(_stream_ptr(ws), qp_arr, nq, opcode | (0x80000000 if post_only else 0), src_mr.addr, src_mr.lkey,
                               dst_mr.addr if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
-                              stride, nbytes, iters, window, signal_every, burst, slot_stride, nslots, timeout_ms, out_addr)
+                              stride, nbytes, iters, window, signal_every, burst, slot_stride, nslots, timeout_ms, out_addr,
+                              fence_every)
     if rc:
         raise N.NativeError(f"rdma_stream launch failed: cuda error {rc}")
     if not sync:
@@ -102,6 +106,30 @@ def parse_stream_out(out, nqp: int, nbytes: int) -> StreamResult:
     o = [list(words[i * 8:(i + 1) * 8]) for i in range(nqp)]
     return StreamResult(status=[WAIT_STATUS.get(r[0], str(r[0])) for r in o], t_start_ns=[r[1] for r in o],
                         t_end_ns=[r[2] for r in o], done=[r[3] for r in o], bytes_per_msg=nbytes)
+
+
+WRITE_READ_MODES = {"fenced": 0, "wait": 1, "one_call": 2}
+
+
+def write_read(qp, src_mr, dst_mr, back_mr, nbytes: int, iters: int = 1, mode: str = "fenced", timeout_ms: int = 2000,
+               stream=None, scratch_off: int = 32768) -> dict:
+    """A WRITE followed by a READ of the same bytes, posted from one GPU thread ``iters`` times: ``nbytes`` from
+    ``src_mr`` to ``dst_mr``, then back from ``dst_mr`` into ``back_mr`` (all at offset 0), waiting for the READ's
+    completion each time.  ``mode`` says how the READ is kept behind the WRITE: ``"fenced"`` posts both under one doorbell
+    with the READ fenced; ``"wait"`` waits for the WRITE's completion before posting the READ (the only way without the
+    fence); ``"one_call"`` posts them with ``dev::rdma_write`` and ``dev::rdma_read(..., fence=true)``.  Returns
+    ``dict(status, done, device_ns, mean_ns, min_ns)`` (per pair: post to the READ's completion)."""
+    ctx = qp.ctx
+    ws = work_stream(ctx, stream)
+    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    rc = N.load().rn_k_write_read(_stream_ptr(ws), qp.dev_ptr, src_mr.addr, src_mr.lkey, dst_mr.addr, dst_mr.rkey, back_mr.addr,
+                                  back_mr.lkey, nbytes, iters, WRITE_READ_MODES[mode], timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"write_read launch failed ({rc})")
+    ws.synchronize()
+    w = (C.c_int64 * 8).from_buffer(out_view)
+    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), done=w[3], device_ns=w[2] - w[1], mean_ns=w[4] / max(w[3], 1),
+                min_ns=w[5] if w[3] else 0)
 
 
 def fill_random(t: torch.Tensor, seed: int = 1, stream=None):
