@@ -29,59 +29,51 @@
 #include <cuda_runtime.h>
 #include "hca_types.h"
 #include "post.cuh"
+#include "kernels/sm90.cuh"
 
 namespace rn {
 namespace eng {
 
 using namespace rn::dev;
+using namespace rn::sm90;
 
 constexpr int kThreads = 128;
 constexpr uint32_t kSub = 16384;        // bytes per TMA bulk transaction
 constexpr int kStages = 12;             // smem ring: 12 x 16 KiB
-// ring split: EngineCtl::stores_in_flight stages (default kSifDefault) may hold a TMA store that is still reading smem,
-// the others hold loads in flight (move_chunks<kSif>)
-constexpr int kMaxSif = 8;             // largest stores_in_flight
-constexpr int kSifDefault = 2;         // 10 loads + 2 stores: as fast as 1 or 3 stores, faster than 4 (DESIGN.md 3.1)
+// Ring split: kSif stages may hold a TMA store that is still reading smem, the other kStages - kSif hold loads in flight.
+// 10 loads + 2 stores: as fast as 1 or 3 stores, faster than 4 (DESIGN.md 3.1).
+constexpr int kSif = 2;
 constexpr uint32_t kBulkMin = 4096;     // below this the generic path is as fast
+// A queued chunk of at most this many bytes is waited for before control scans again (DESIGN.md 3.1).
+constexpr uint32_t kSmallChunk = 64 * 1024;
 
-// ------------------------------------------------------------------ PTX helpers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
+// ------------------------------------------------------------------ PTX helpers (the rest are sm90's)
+// try_wait without a suspend-time hint (sm90::mbar_try passes one)
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
       "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+      : "=r"(ok) : "r"(s32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
+          s32(smem_dst)),
+      "l"(gsrc), "r"(bytes), "r"(s32(bar))
       : "memory");
 }
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst),
-               "r"(smem_u32(smem_src)), "r"(bytes)
+               "r"(s32(smem_src)), "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------ MKey lookup
 // Returns the engine-reachable pointer for [addr, addr+len) under `key`, or 0 with
@@ -186,11 +178,8 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
       "{\n\t.reg .pred p;\n\t"
       "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
       "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+      : "=r"(ok) : "r"(s32(bar)), "r"(parity) : "memory");
   return ok != 0;
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {   // release at CTA scope
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 template <int N>
 __device__ __forceinline__ void bulk_wait() {
@@ -208,7 +197,7 @@ __device__ __forceinline__ void generic_bar() { asm volatile("bar.sync 1, %0;" :
 // Chunks need 16-byte aligned src, dst and len.  Returns false when a load never landed (bad mapping: bounded, the SM is
 // not wedged); true when control queued the quit entry.
 // kProf: add %globaltimer ns per wait to prof[MoverProf] (this CTA's row), written once on exit.
-template <int kSif, bool kProf>
+template <bool kProf>
 __device__ __noinline__ bool move_chunks(Smem& s, unsigned long long* prof) {
   constexpr uint32_t P = kStages - kSif;
   uint32_t ring_ph = 0, q_ph = 0;            // parity of the next wait, per ring stage / per queue entry
@@ -307,15 +296,9 @@ __device__ __noinline__ bool move_chunks(Smem& s, unsigned long long* prof) {
   }
 }
 
-// Control's choice of mover: the stores-in-flight split, or the profiled default split when EngineCtl::mover_prof is set.
-__device__ __forceinline__ bool run_mover(Smem& s, unsigned sif, unsigned long long* prof) {
-  if (prof) return move_chunks<kSifDefault, true>(s, prof);
-  switch (sif) {
-    case 8: return move_chunks<8, false>(s, nullptr);
-    case 6: return move_chunks<6, false>(s, nullptr);
-    case 4: return move_chunks<4, false>(s, nullptr);
-    default: return move_chunks<kSifDefault, false>(s, nullptr);
-  }
+// The profiled mover when EngineCtl::mover_prof is set.
+__device__ __forceinline__ bool run_mover(Smem& s, unsigned long long* prof) {
+  return prof ? move_chunks<true>(s, prof) : move_chunks<false>(s, nullptr);
 }
 
 // Generic path: any alignment; thread t of the n threads of warps 0, 2 and 3.
@@ -719,6 +702,97 @@ __device__ __forceinline__ bool draw_chunk(QpDev* qp, Resolved* res, unsigned lo
   return true;
 }
 
+// ---- the ordered section, entered in WQE order by the parse_seq turn
+// Wait until parse_seq names w and return it.  The turn word also carries "QP already failed" (PARSE_ERR_BIT), so the
+// common path is one poll, no fence.
+__device__ __forceinline__ unsigned long long wait_turn(EngineCtl* ctl, QpDev* qp, unsigned long long w) {
+  unsigned long long turn = ld_u64_volatile(&qp->parse_seq);
+  if ((turn & ~PARSE_ERR_BIT) != w) {
+    unsigned long long t0 = globaltimer_ns();
+    while (((turn = ld_u64_volatile(&qp->parse_seq)) & ~PARSE_ERR_BIT) != w) {
+      if (globaltimer_ns() - t0 > 4000000000ull) { ctl->fatal = 2; break; }   // predecessor died
+    }
+  }
+  return turn;
+}
+
+struct Committed {
+  uint8_t syn;            // final syndrome
+  uint32_t n, chunk;      // chunk count and granule of resolved[w]
+  uint64_t dst;           // the destination (a SEND's is the receive buffer matched here)
+  bool fenced, closed;    // fence_gated, and its gate still closed
+};
+
+// Commit WQE w, holding the turn.  The parallel part already published resolved[w] (n chunks of `chunk` bytes) unless
+// the WQE needs a receive.  err: the QP has failed; a WQE that fails here sets it.  The caller arms the ticket and passes
+// the turn on.  release_rq: release rq_head here, because the single path passes the turn of a one-chunk WQE with a
+// relaxed store (the batch path's closing fence releases it instead).
+__device__ __forceinline__ Committed commit_wqe(EngineCtl* ctl, QpDev* qp, unsigned long long w, const Parsed& p, bool recv,
+                                                uint32_t n, uint32_t chunk, bool& err, bool release_rq) {
+  Committed c{p.syn, n, chunk, p.dst, false, false};
+  if (err) {
+    // flushed: nothing moves, whatever the parse said
+    c.syn = SYN_WR_FLUSH_ERR;
+    c.n = write_resolved(qp, w, p.v, c.syn, 0, 0, 0, 0, &c.chunk);
+  } else if (recv) {
+    fence_gpu();  // acquire rq_head from the previous receive-consuming WQE
+    uint64_t rq_idx = 0;
+    uint8_t rq_taken = 0;
+    match_recv(ctl, qp, p.v, &c.syn, &c.dst, &rq_idx, &rq_taken);
+    c.n = write_resolved(qp, w, p.v, c.syn, p.src, c.dst, rq_idx, rq_taken, &c.chunk);
+    if (release_rq) fence_gpu();  // release rq_head
+  }
+  if (c.syn != SYN_OK && !err) { qp->state = QPS_ERR; err = true; }
+  // A fenced WQE whose gate is still closed is not moved by its claimer: even with one chunk it gets a gated ticket,
+  // which the helpers' offer scan stops at and opens once the retirer reaches it.  An open gate's fence orders the
+  // ticket after it.
+  c.fenced = fence_gated(p.v, c.syn);
+  c.closed = c.fenced && !gate_open(qp, w);
+  if (c.closed) atomicAdd(&qp->n_fence_waits, 1ull);
+  return c;
+}
+
+// Single claim of WQE w (the caller won the cursor CAS and took its acquire).  st: the QP state try_claim loaded.  The
+// claimer moves chunk 0 itself with the descriptor computed here, so only a WQE with more chunks, or a closed gate, gets a
+// ticket for the helpers.  Returns 1 with *out = chunk 0, or 0 when the gate is closed.
+__device__ __forceinline__ int claim_one(EngineCtl* ctl, QpDev* qp, unsigned long long w, uint32_t st, uint32_t pending,
+                                         Work* out, bool* saw_pending) {
+  trace_stamp(qp, w, TR_CLAIM);
+  // ordering audit: the doorbell record must already cover what the register announced
+  uint32_t dbr16 = be32(ld_u32_volatile(&qp->dbr[DBR_SND])) & 0xffff;
+  if (((dbr16 - (uint32_t)w) & 0xffff) < pending && ((dbr16 - (uint32_t)w) & 0xffff) < 0x8000)
+    atomicAdd(&qp->n_db_order_violations, 1ull);
+  // ---- parallel part
+  Parsed p;
+  parse_wqe(ctl, qp, w, &p);
+  const bool recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
+  uint32_t n = 1, chunk_sz = 0;
+  if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, &chunk_sz);
+  // ---- ordered part
+  const unsigned long long turn = wait_turn(ctl, qp, w);
+  bool err = (turn & PARSE_ERR_BIT) != 0 || st == QPS_ERR;
+  const Committed c = commit_wqe(ctl, qp, w, p, recv, n, chunk_sz, err, true);
+  Resolved* res = qp->resolved + (w & ((1u << qp->sq_log) - 1));
+  const unsigned long long next = (w + 1) | (err ? (unsigned long long)PARSE_ERR_BIT : 0ull);
+  if (c.n > 1 || c.closed) {
+    fence_gpu();  // release resolved[w] before the ticket that lets helpers read it
+    st_u64_relaxed(&res->ticket, (c.closed ? TICKET_GATED : TICKET_ONE) | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | c.n);
+    st_u64_release_scope(&qp->parse_seq, next, false);   // helpers trust: committed => ticket armed
+  } else {
+    st_u64_relaxed(&qp->parse_seq, next);
+  }
+  trace_stamp(qp, w, TR_PARSED);
+  if (c.closed) {
+    *saw_pending = true;
+    return 0;
+  }
+  const uint32_t bytes = c.syn == SYN_OK ? p.v.bytes : 0;
+  out->qp = qp; out->w = w; out->chunk = 0;
+  out->have_desc = 1; out->nch = c.n; out->src = p.src; out->dst = c.dst; out->fenced = c.fenced;
+  out->len = bytes < c.chunk ? bytes : c.chunk;     // chunk 0
+  return 1;
+}
+
 // Returns 0: nothing, 1: *out is a chunk to move, 2: a BATCH of out->chunk WQEs starting at out->w was
 // claimed and still has to be parsed (claim_batch, warp-collective).
 constexpr uint32_t kClaimBatch = 16;
@@ -749,71 +823,8 @@ __device__ __forceinline__ int try_claim(EngineCtl* ctl, QpDev* qp, Work* out, b
         return 2;
       }
     } else if (atomicCAS(&qp->cursor, c, c + 1) == c) {
-      const unsigned long long w = c;
       fence_scope(sys);  // acquire: WQE bytes the doorbell announced
-      trace_stamp(qp, w, TR_CLAIM);
-      // ordering audit: the doorbell record must already cover what the register announced
-      uint32_t dbr16 = be32(ld_u32_volatile(&qp->dbr[DBR_SND])) & 0xffff;
-      if (((dbr16 - (uint32_t)w) & 0xffff) < pending && ((dbr16 - (uint32_t)w) & 0xffff) < 0x8000)
-        atomicAdd(&qp->n_db_order_violations, 1ull);
-      // ---- parallel part
-      Parsed p;
-      parse_wqe(ctl, qp, w, &p);
-      const bool recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
-      uint32_t n = 1, chunk_sz = 0;
-      uint64_t fsrc = p.src, fdst = p.dst;
-      if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, &chunk_sz);
-      // ---- ordered part: wait for the turn.  The turn word also carries "QP already failed",
-      //      so the common path is one poll + one store, no fence.
-      unsigned long long turn = ld_u64_volatile(&qp->parse_seq);
-      if ((turn & ~PARSE_ERR_BIT) != w) {
-        unsigned long long t0 = globaltimer_ns();
-        while (((turn = ld_u64_volatile(&qp->parse_seq)) & ~PARSE_ERR_BIT) != w) {
-          if (globaltimer_ns() - t0 > 4000000000ull) { ctl->fatal = 2; break; }   // predecessor died
-        }
-      }
-      bool err = (turn & PARSE_ERR_BIT) != 0 || st == QPS_ERR;
-      uint8_t syn = p.syn;
-      if (err) {
-        // flushed: nothing moves, whatever the parse said
-        syn = SYN_WR_FLUSH_ERR;
-        n = write_resolved(qp, w, p.v, syn, 0, 0, 0, 0, &chunk_sz);
-      } else if (recv) {
-        fence_gpu();  // acquire rq_head from the previous receive-consuming WQE
-        uint64_t dst = p.dst, rq_idx = 0;
-        uint8_t rq_taken = 0;
-        match_recv(ctl, qp, p.v, &syn, &dst, &rq_idx, &rq_taken);
-        n = write_resolved(qp, w, p.v, syn, p.src, dst, rq_idx, rq_taken, &chunk_sz);
-        fdst = dst;
-        fence_gpu();  // release rq_head
-      }
-      if (syn != SYN_OK && !err) { qp->state = QPS_ERR; err = true; }
-      // A fenced WQE whose gate is still closed is not moved by its claimer: even with one chunk it gets a gated ticket,
-      // which the helpers' offer scan stops at and opens once the retirer reaches it.
-      const bool fenced = fence_gated(p.v, syn);
-      const bool closed = fenced && !gate_open(qp, w);
-      Resolved* res = qp->resolved + (w & mask);
-      const unsigned long long next = (w + 1) | (err ? (unsigned long long)PARSE_ERR_BIT : 0ull);
-      if (n > 1 || closed) {
-        fence_gpu();  // release resolved[w] before the ticket that lets helpers read it
-        st_u64_relaxed(&res->ticket, (closed ? TICKET_GATED : TICKET_ONE) | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | n);
-        st_u64_release_scope(&qp->parse_seq, next, false);   // helpers trust: committed => ticket armed
-      } else {
-        st_u64_relaxed(&qp->parse_seq, next);
-      }
-      trace_stamp(qp, w, TR_PARSED);
-      if (closed) {
-        atomicAdd(&qp->n_fence_waits, 1ull);
-        *saw_pending = true;
-        return 0;
-      }
-      out->qp = qp; out->w = w; out->chunk = 0;
-      {
-        const uint32_t bytes = syn == SYN_OK ? p.v.bytes : 0;
-        out->have_desc = 1; out->nch = n; out->src = fsrc; out->dst = fdst; out->fenced = fenced;
-        out->len = bytes < chunk_sz ? bytes : chunk_sz;     // chunk 0
-      }
-      return 1;
+      return claim_one(ctl, qp, c, st, pending, out, saw_pending);
     }
   }
   // ---- help.  The tickets of the 8 oldest committed WQEs are peeked with independent loads (one round
@@ -877,50 +888,28 @@ __device__ __forceinline__ void claim_batch(EngineCtl* ctl, QpDev* qp, unsigned 
   const uint32_t mask = (1u << qp->sq_log) - 1;
   const unsigned long long w = w0 + lane;
   Parsed p;
-  uint32_t n = 1;
+  uint32_t n = 1, chunk = 0;
   bool recv = false;
   if (lane < k) {
     trace_stamp(qp, w, TR_CLAIM);
     parse_wqe(ctl, qp, w, &p);
     recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
-    if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0);
+    if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, &chunk);
   }
   __syncwarp();
   unsigned long long turn = 0;
-  if (lane == 0) {
-    turn = ld_u64_volatile(&qp->parse_seq);
-    if ((turn & ~PARSE_ERR_BIT) != w0) {
-      unsigned long long t0 = globaltimer_ns();
-      while (((turn = ld_u64_volatile(&qp->parse_seq)) & ~PARSE_ERR_BIT) != w0) {
-        if (globaltimer_ns() - t0 > 4000000000ull) { ctl->fatal = 2; break; }   // predecessor died
-      }
-    }
-  }
+  if (lane == 0) turn = wait_turn(ctl, qp, w0);
   turn = __shfl_sync(0xffffffffu, turn, 0);
-  int err = ((turn & PARSE_ERR_BIT) != 0 || *(volatile uint32_t*)&qp->state == QPS_ERR) ? 1 : 0;
+  bool err = (turn & PARSE_ERR_BIT) != 0 || *(volatile uint32_t*)&qp->state == QPS_ERR;
   for (uint32_t i = 0; i < k; ++i) {
     if (lane == i) {
-      uint8_t syn = p.syn;
-      if (err) {
-        syn = SYN_WR_FLUSH_ERR;
-        n = write_resolved(qp, w, p.v, syn, 0, 0, 0, 0);
-      } else if (recv) {
-        fence_gpu();  // acquire rq_head from the previous receive-consuming WQE
-        uint64_t dst = p.dst, rq_idx = 0;
-        uint8_t rq_taken = 0;
-        match_recv(ctl, qp, p.v, &syn, &dst, &rq_idx, &rq_taken);
-        n = write_resolved(qp, w, p.v, syn, p.src, dst, rq_idx, rq_taken);
-      }
-      if (syn != SYN_OK && !err) { qp->state = QPS_ERR; err = 1; }
+      const Committed c = commit_wqe(ctl, qp, w, p, recv, n, chunk, err, false);
       Resolved* res = qp->resolved + (w & mask);
-      // a fenced WQE is armed gated unless its gate is already open (gate_open's fence then orders it before the ticket)
-      const bool closed = fence_gated(p.v, syn) && !gate_open(qp, w);
-      if (closed) atomicAdd(&qp->n_fence_waits, 1ull);
-      st_u64_relaxed(&res->ticket, (closed ? TICKET_GATED : 0ull) | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | n);    // chunk counter starts at 0
+      st_u64_relaxed(&res->ticket, (c.closed ? TICKET_GATED : 0ull) | ((w & TICKET_FIELD_MASK) << TICKET_GEN_SHIFT) | c.n);    // chunk counter starts at 0
       trace_stamp(qp, w, TR_PARSED);
     }
     __syncwarp();
-    err = __shfl_sync(0xffffffffu, err, i);
+    err = __shfl_sync(0xffffffffu, (int)err, i) != 0;
   }
   if (lane == 0) {
     fence_gpu();  // release: every lane's resolved[] / ticket / rq_head (ordered before this by the __syncwarp chain)
@@ -960,6 +949,16 @@ __device__ __forceinline__ bool complete_chunk(QpDev* qp, unsigned long long w, 
   return false;
 }
 
+// What control's lane 0 found to do in one iteration; the whole warp acts on it.
+enum Act : int {
+  ACT_LEAVE = -1,
+  ACT_NONE = 0,          // nothing claimed
+  ACT_QUEUED,            // a chunk queued for the mover
+  ACT_GENERIC,           // a generic copy for warps 0, 2 and 3
+  ACT_NO_BYTES,          // a claimed chunk with nothing to move
+  ACT_QUEUED_SMALL,      // queued, at most kSmallChunk: wait for it before scanning again
+};
+
 __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
@@ -973,7 +972,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
   if (warp == 1) {
     if (lane == 0) {
       unsigned long long* prof = ctl->mover_prof;
-      const bool ok = run_mover(s, ctl->stores_in_flight, prof ? prof + (size_t)blockIdx.x * MOVER_PROF_N : nullptr);
+      const bool ok = run_mover(s, prof ? prof + (size_t)blockIdx.x * MOVER_PROF_N : nullptr);
       if (!ok) { ctl->fatal = 1; *(volatile int*)&s.mover_fatal = 1; }
     }
     return;
@@ -1029,8 +1028,8 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
   };
   for (;;) {
     if (!reap(false)) { fatal = true; break; }
-    int batch_k = 0, act = 0;   // act: -1 leave, 0 nothing, 1 queued for the mover, 2 generic copy, 3 nothing to move,
-                                // 4 queued, small: wait for it
+    int batch_k = 0;
+    Act act = ACT_NONE;
     Work work;
     uint32_t nch = 0;
     if (lane == 0) {
@@ -1087,7 +1086,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
         last_activity = globaltimer_ns();
         spins = 0;
         if (len == 0) {
-          act = 3;
+          act = ACT_NO_BYTES;
         } else if (len >= kBulkMin && (((csrc | cdst) & 15) == 0) && ((len & 15) == 0)) {
           // reap() left room: outstanding < kQueue
           if (fenced) fence_proxy_async_global();   // the mover's TMA loads see what the gate's acquire made visible
@@ -1099,10 +1098,10 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
           atomicAdd(&ctl->n_bulk_chunks, 1ull);
           // A chunk the ring holds at once gains nothing from streaming; finishing it before the next scan keeps
           // small-message latency what it was (a 4 KiB WQE otherwise waits for the scan to be counted).
-          act = len <= kSub * (kStages - kMaxSif) ? 4 : 1;
+          act = len <= kSmallChunk ? ACT_QUEUED_SMALL : ACT_QUEUED;
         } else {
           s.gsrc = csrc; s.gdst = cdst; s.glen = len;
-          act = 2;
+          act = ACT_GENERIC;
         }
       } else {
         ++spins;
@@ -1116,7 +1115,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
           else if (host_watcher && globaltimer_ns() - last_activity > ctl->idle_timeout_ns) { quit = true; ctl->exited_idle = 1; ctl->quit_all = 1; }
         }
         if (spins > 256) __nanosleep(200);
-        if (quit) act = -1;
+        if (quit) act = ACT_LEAVE;
       }
     }
     // a batch claim is parsed by the whole warp; its chunks are then drawn like anybody else's
@@ -1125,15 +1124,15 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
       QpDev* bqp = (QpDev*)__shfl_sync(0xffffffffu, (unsigned long long)work.qp, 0);
       claim_batch(ctl, bqp, __shfl_sync(0xffffffffu, work.w, 0), (uint32_t)batch_k, lane);
     }
-    act = __shfl_sync(0xffffffffu, act, 0);
-    if (act < 0) break;
-    if (act == 2) {
+    act = (Act)__shfl_sync(0xffffffffu, (int)act, 0);
+    if (act == ACT_LEAVE) break;
+    if (act == ACT_GENERIC) {
       generic_bar();
       copy_generic(s.gsrc, s.gdst, s.glen, lane, kGenericThreads);
       generic_bar();   // every generic thread's stores before lane 0's release in complete_chunk
     }
-    if (act == 4 && !reap(true)) { fatal = true; break; }
-    if (act == 2 || act == 3) finish(work.qp, work.w, nch);
+    if (act == ACT_QUEUED_SMALL && !reap(true)) { fatal = true; break; }
+    if (act == ACT_GENERIC || act == ACT_NO_BYTES) finish(work.qp, work.w, nch);
   }
   // Leaving.  Every chunk handed to the mover is a claim that must be completed; after a mover fault nothing is
   // completed (the host sees ctl->fatal).
@@ -1157,7 +1156,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
 // dst + b * span as ONE queued chunk -- no claims, no chunk boundaries, no completion bookkeeping.  The distance between
 // this and the engine on the same CTA count is what the per-chunk work costs (tools/engine_pipeline.py).
 // prof (may be null): the mover's stall profile, MOVER_PROF_N counters per CTA, as the engine's.
-__global__ void __launch_bounds__(kThreads, 1) engine_ceiling_kernel(uint64_t src, uint64_t dst, uint32_t span, unsigned sif,
+__global__ void __launch_bounds__(kThreads, 1) engine_ceiling_kernel(uint64_t src, uint64_t dst, uint32_t span,
                                                                     unsigned int* fatal, unsigned long long* prof) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
@@ -1170,7 +1169,7 @@ __global__ void __launch_bounds__(kThreads, 1) engine_ceiling_kernel(uint64_t sr
     s.q[1].len = kQuitLen;
     mbar_arrive(&s.qfull[1]);
   } else if (threadIdx.x == 32) {
-    const bool ok = run_mover(s, sif, prof ? prof + (size_t)blockIdx.x * MOVER_PROF_N : nullptr);
+    const bool ok = run_mover(s, prof ? prof + (size_t)blockIdx.x * MOVER_PROF_N : nullptr);
     if (!ok && fatal) atomicAdd(fatal, 1u);
   }
 }

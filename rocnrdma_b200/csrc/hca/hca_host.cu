@@ -1006,12 +1006,7 @@ RN_API int rn_engine_start(void* hca, int n_ctas, uint64_t idle_timeout_ms, uint
   c.oneshot = h->oneshot;
   c.host_native_atomics = h->host_native_atomics ? 1u : 0u;
   {
-    const char* e = getenv("RN_ENGINE_STORES_IN_FLIGHT");
-    int v = e ? atoi(e) : 0;
-    c.stores_in_flight = (v == 2 || v == 4 || v == 6 || v == 8) ? (unsigned)v : (unsigned)eng::kSifDefault;
-  }
-  {
-    // The mover's stall profile (rn_engine_mover_profile); off, the engine runs the unprofiled movers.
+    // The mover's stall profile (rn_engine_mover_profile); off, the engine runs the unprofiled mover.
     const char* e = getenv("RN_ENGINE_PROFILE");
     h->prof_on = e && atoi(e) == 1;
     if (h->prof_on) {
@@ -1052,10 +1047,7 @@ RN_API int rn_k_engine_ceiling(uint64_t stream, uint64_t src, uint64_t dst, uint
     return fail(-22, "engine_ceiling: need ctas > 0 and a 16-byte aligned span below 4 GiB");
   const size_t smem = eng::engine_smem_bytes();
   CU_OK(cudaFuncSetAttribute(eng::engine_ceiling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const char* e = getenv("RN_ENGINE_STORES_IN_FLIGHT");
-  const int v = e ? atoi(e) : 0;
-  const unsigned sif = (v == 2 || v == 4 || v == 6 || v == 8) ? (unsigned)v : (unsigned)eng::kSifDefault;
-  eng::engine_ceiling_kernel<<<ctas, eng::kThreads, smem, (cudaStream_t)stream>>>(src, dst, (uint32_t)span, sif,
+  eng::engine_ceiling_kernel<<<ctas, eng::kThreads, smem, (cudaStream_t)stream>>>(src, dst, (uint32_t)span,
                                                                                   (unsigned int*)fatal_dev,
                                                                                   (unsigned long long*)prof_dev);
   CU_OK(cudaGetLastError());

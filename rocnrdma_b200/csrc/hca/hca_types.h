@@ -157,7 +157,6 @@ struct EngineCtl {
   unsigned int exited_idle;        // set when the watchdog ended the engine
   unsigned int fatal;              // a DMA never completed; engine bailed out
   unsigned int quit_all;           // the host-doorbell watcher found the engine idle / drained: everybody leaves
-  unsigned int stores_in_flight;   // smem ring split: this many TMA stores may still be reading smem, the rest of the ring holds loads (2, 4, 6 or 8)
   unsigned int oneshot;            // exit as soon as every queue is drained (profiling under ncu: kernels are serialised there)
   unsigned int host_native_atomics;  // cudaDevAttrHostNativeAtomicSupported: a GPU atomic on pinned host memory is atomic there
   unsigned long long n_bulk_chunks;     // chunks moved through the TMA bulk path

@@ -1,5 +1,6 @@
-// Hopper (sm_90a) building blocks shared by the two GEMM files: mbarriers, TMA tensor loads (plain and cluster
-// multicast) and stores, warpgroup MMA (wgmma) with shared-memory descriptors, cluster helpers.
+// Hopper (sm_90a) building blocks shared by the two GEMM files and the software HCA's engine (hca/engine.cuh): mbarriers,
+// bulk-copy groups, TMA tensor loads (plain and cluster multicast) and stores, warpgroup MMA (wgmma) with shared-memory
+// descriptors, cluster helpers.
 //
 // Operand tiles are K-major with 128-byte rows, loaded by TMA with SWIZZLE_128B: 8-row groups 1024 bytes apart.  A
 // wgmma descriptor of such a tile steps along K by adding bytes / 16 to its start-address field (32 bytes = +2 per

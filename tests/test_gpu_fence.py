@@ -179,19 +179,17 @@ def test_device_posted_write_then_fenced_read(ctx, mode, nbytes):
     GATE_WAITS.append(c["n_fence_waits"])
 
 
-@pytest.mark.parametrize("ctas,sif,chunk,qmem,dmem,oneshot", CONFIGS,
-                         ids=[f"c{c}-s{s}-k{k // K}-q{q}-d{d}-{'oneshot' if o else 'live'}" for c, s, k, q, d, o in CONFIGS])
-def test_random_fenced_programs_on_the_softhca(monkeypatch, ctas, sif, chunk, qmem, dmem, oneshot):
-    if sif == "prof":
+@pytest.mark.parametrize("ctas,prof,chunk,qmem,dmem,oneshot", CONFIGS,
+                         ids=[f"c{c}-{'prof-' if p else ''}k{k // K}-q{q}-d{d}-{'oneshot' if o else 'live'}" for c, p, k, q, d, o in CONFIGS])
+def test_random_fenced_programs_on_the_softhca(monkeypatch, ctas, prof, chunk, qmem, dmem, oneshot):
+    if prof:
         monkeypatch.setenv("RN_ENGINE_PROFILE", "1")
-        monkeypatch.delenv("RN_ENGINE_STORES_IN_FLIGHT", raising=False)
     else:
         monkeypatch.delenv("RN_ENGINE_PROFILE", raising=False)
-        monkeypatch.setenv("RN_ENGINE_STORES_IN_FLIGHT", str(sif))
     cfg = {"wire": "softhca", "max_wrs": 100, "max_len": 4 << 20, "big_budget": 12 << 20, "ctas": ctas,
            "chunk_bytes": chunk, "data_mem": dmem, "allow_rnr": not oneshot, "fences": True}
     s = M.replay_seed()
-    for seed in [s] if s is not None else [70_000 + 100 * CONFIGS.index((ctas, sif, chunk, qmem, dmem, oneshot)) + i
+    for seed in [s] if s is not None else [70_000 + 100 * CONFIGS.index((ctas, prof, chunk, qmem, dmem, oneshot)) + i
                                            for i in range(M.soak_seeds(2))]:
         F.check_seed(seed, cfg, lambda: _CountingWire(0, ctas, chunk, qmem, oneshot))
 

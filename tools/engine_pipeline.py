@@ -187,7 +187,6 @@ def main():
                      "us_per_granule_ceiling": round(t_a, 2), "us_per_granule_engine": round(t_b, 2),
                      "dead_us_per_chunk": round(t_b - t_a, 2)})
     out = {"card": card(), "msg_bytes": MSG, "window": 8, "nslots": NSLOTS, "reps": args.reps,
-           "stores_in_flight": int(os.environ.get("RN_ENGINE_STORES_IN_FLIGHT", "2") or 2),
            "memcpy_d2d_gbps": summary(runs[("memcpy", 0)]), "rows": rows}
     if profiles:
         out["mover_profile"] = profiles
