@@ -133,6 +133,7 @@ _SIGS = {
     "rn_k_write_read": (i32, [u64, u64, u64, u32, u64, u32, u64, u32, u32, u32, u32, u64, u64]),
     "rn_stream_clamp": (None, [u32, C.POINTER(u32), C.POINTER(u32)]),
     "rn_wire_build_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, u64, u32, u32, u32, u32]),
+    "rn_wire_build_cqe": (None, [C.POINTER(u8), u32, u32, u32, u32, u32, u32, u32, u32, u32, u64]),
     "rn_wire_decode_cqe": (i32, [C.POINTER(u8), C.POINTER(RnWc)]),
     "rn_wire_build_atomic_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, u64, u32, u64, u64, u32]),
     "rn_wire_decode_wqe": (i32, [C.POINTER(u8), C.POINTER(u64)]),

@@ -120,22 +120,16 @@ __device__ __forceinline__ uint8_t* cqe_slot(uint8_t* ring, uint32_t log_n, unsi
   return ring + ((size_t)(slot & ((1u << log_n) - 1)) << 6);
 }
 __device__ __forceinline__ void cqe_body(uint8_t* cqe, uint8_t opcode, uint32_t byte_cnt, uint32_t imm) {
-  const bool err = (opcode == CQE_REQ_ERR || opcode == CQE_RESP_ERR);
+  const uint4 mid = encode_cqe_mid(opcode, byte_cnt, imm);
   st_v4(cqe + 0, 0u, 0u, 0u, 0u);
   st_v4(cqe + 16, 0u, 0u, 0u, 0u);
-  if (!err) st_v4(cqe + 32, 0u, be32(imm), 0u, be32(byte_cnt));
-  else st_v4(cqe + 32, 0u, 0u, 0u, 0u);
+  st_v4(cqe + CQE_MID_OFF, mid.x, mid.y, mid.z, mid.w);
 }
+// The engine's vendor syndrome is 0.
 __device__ __forceinline__ void cqe_tail(uint8_t* cqe, uint32_t log_n, unsigned int slot, uint8_t opcode, uint8_t wqe_opcode,
                                          uint32_t qpn, uint16_t wqe_counter, uint8_t syndrome, unsigned long long now) {
-  const bool err = (opcode == CQE_REQ_ERR || opcode == CQE_RESP_ERR);
-  const uint8_t owner = (uint8_t)((slot >> log_n) & 1u);
-  // err view: byte 54 = vendor_err_synd, byte 55 = syndrome (top byte of the word at 52)
-  uint32_t w48 = err ? 0u : be32((uint32_t)(now >> 32));
-  uint32_t w52 = err ? ((uint32_t)syndrome << 24) : be32((uint32_t)now);
-  uint32_t w56 = be32(((uint32_t)wqe_opcode << 24) | (qpn & 0xffffff));
-  uint32_t w60 = (uint32_t)be16(wqe_counter) | ((uint32_t)cqe_op_own(opcode, owner) << 24);
-  st_v4(cqe + 48, w48, w52, w56, w60);
+  const uint4 t = encode_cqe_tail(opcode, (uint8_t)((slot >> log_n) & 1u), wqe_counter, qpn, wqe_opcode, syndrome, 0, now);
+  st_v4(cqe + CQE_TAIL_OFF, t.x, t.y, t.z, t.w);
 }
 
 // ------------------------------------------------------------------ chunk copy
@@ -449,8 +443,7 @@ __device__ __forceinline__ void match_recv(EngineCtl* ctl, QpDev* qp, const WqeV
   // is only fetched when the opcode actually needs the buffer it names (SEND, not WRITE_IMM).
   bool have = head < qp->rq_cached_pi;
   while (!have) {
-    uint32_t rpi16 = be32(ld_u32_volatile(&qp->r.rq_dbr[DBR_RCV])) & 0xffff;
-    qp->rq_cached_pi = head + ((rpi16 - (uint32_t)head) & 0xffff);
+    qp->rq_cached_pi = expand16(wq_dbr_index(ld_u32_volatile(&qp->r.rq_dbr[DBR_RCV])), head);
     if (head < qp->rq_cached_pi) { have = true; break; }
     unsigned long long now = globaltimer_ns();
     if (t0 == 0) { t0 = now; atomicAdd(&qp->n_rnr, 1ull); }
@@ -466,14 +459,12 @@ __device__ __forceinline__ void match_recv(EngineCtl* ctl, QpDev* qp, const WqeV
   }
   fence_scope(qp->sys_scope != 0);
   const uint8_t* rs = qp->r.rq + ((head & ((1ull << qp->r.rq_log) - 1)) << 4);
-  uint4 d = ld_v4_volatile(rs);
-  uint32_t rbytes = be32(d.x) & 0x7fffffffu, rlkey = be32(d.y);
-  uint64_t raddr = ((uint64_t)be32(d.z) << 32) | be32(d.w);
+  const uint4 d = ld_v4_volatile(rs);
   *rq_idx = head;
   *rq_taken = 1;
   qp->rq_head = head + 1;
-  if (rbytes < v.bytes) *syn = SYN_REMOTE_INVAL_REQ_ERR;
-  else *dst = translate(qp->r.rkeys, qp->r.n_rkeys, rlkey, raddr, v.bytes, ACC_LOCAL_WRITE, true, syn);
+  if (recv_wqe_bytes(d) < v.bytes) *syn = SYN_REMOTE_INVAL_REQ_ERR;
+  else *dst = translate(qp->r.rkeys, qp->r.n_rkeys, recv_wqe_lkey(d), recv_wqe_addr(d), v.bytes, ACC_LOCAL_WRITE, true, syn);
 }
 
 // ------------------------------------------------------------------ retire
@@ -497,8 +488,8 @@ __device__ __forceinline__ bool cq_would_overrun(CqDev* cq, unsigned int end_pi,
   const unsigned int depth = 1u << log_n;
   unsigned int ci = *(volatile unsigned int*)&cq->ci_seen;
   if (end_pi - ci <= depth) return false;
-  const unsigned int ci24 = be32(ld_u32_volatile(cq->dbrec)) & 0xffffffu;
-  ci = end_pi - ((end_pi - ci24) & 0xffffffu);
+  // the record holds 24 bits of ci: the consumer is (end_pi - ci24) mod 2^24 behind the producer
+  ci = end_pi - ((end_pi - cq_dbr_index(ld_u32_volatile(cq->dbrec))) & 0xffffffu);
   *(volatile unsigned int*)&cq->ci_seen = ci;
   return end_pi - ci > depth;
 }
@@ -759,8 +750,8 @@ __device__ __forceinline__ int claim_one(EngineCtl* ctl, QpDev* qp, unsigned lon
                                          Work* out, bool* saw_pending) {
   trace_stamp(qp, w, TR_CLAIM);
   // ordering audit: the doorbell record must already cover what the register announced
-  uint32_t dbr16 = be32(ld_u32_volatile(&qp->dbr[DBR_SND])) & 0xffff;
-  if (((dbr16 - (uint32_t)w) & 0xffff) < pending && ((dbr16 - (uint32_t)w) & 0xffff) < 0x8000)
+  const uint16_t ahead = (uint16_t)(wq_dbr_index(ld_u32_volatile(&qp->dbr[DBR_SND])) - (uint16_t)w);
+  if (ahead < pending && ahead < 0x8000)
     atomicAdd(&qp->n_db_order_violations, 1ull);
   // ---- parallel part
   Parsed p;
@@ -808,8 +799,7 @@ __device__ __forceinline__ int try_claim(EngineCtl* ctl, QpDev* qp, Work* out, b
   unsigned long long db = look_at_doorbell ? ld_u64_volatile(qp->bf) : 0ull;
   unsigned long long off = ld_u64_volatile(&qp->offer);
   unsigned long long ps = ld_u64_volatile(&qp->parse_seq) & ~PARSE_ERR_BIT;
-  uint32_t idx16 = (be32((uint32_t)db) >> 8) & 0xffff;
-  uint32_t pending = look_at_doorbell ? ((idx16 + 1 - (uint32_t)c) & 0xffff) : 0u;
+  uint32_t pending = look_at_doorbell ? (uint16_t)(doorbell_index(db) + 1 - (uint16_t)c) : 0u;
   if (pending != 0 && pending < 0x8000) {
     *saw_pending = true;
     // Every engine CTA races for the same word with a value it loaded one L2 round trip ago, so only

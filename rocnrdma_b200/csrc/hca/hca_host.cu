@@ -501,9 +501,8 @@ RN_API int rn_create_cq(void* hca, uint32_t ncqe, uint32_t mem, void** out) {
   uint32_t* dbrec = (uint32_t*)arena_alloc(h, 64, host);
   c->d = (CqDev*)arena_alloc(h, sizeof(CqDev), false);
   if (!ring || !dbrec || !c->d) { delete c; return fail(-12, "create_cq: control arena exhausted"); }
-  // every CQE starts INVALID with owner = 1 (the first hardware pass writes owner 0)
-  std::vector<uint8_t> init((size_t)ncqe * 64, 0);
-  for (uint32_t i = 0; i < ncqe; ++i) init[(size_t)i * 64 + 63] = cqe_op_own(CQE_INVALID, 1);
+  std::vector<uint8_t> init((size_t)ncqe * CQE_SIZE);
+  init_cq_ring(init.data(), ncqe);
   if (host) memcpy(ring, init.data(), init.size());
   else { int rc = push(h, ring, init.data(), init.size()); if (rc) { delete c; return rc; } }
   c->ring_host = host ? ring : nullptr;
@@ -532,7 +531,7 @@ RN_API int rn_poll_cq(void* cq, int max, RnWc* out) {
     size_t off = (size_t)(c->h_ci & ((1u << c->h.log_n) - 1)) << 6;
     if (c->ring_host) {
       volatile uint8_t* p = c->ring_host + off;
-      uint8_t oo = p[63];
+      uint8_t oo = p[CQE_OP_OWN_OFF];
       if (!cqe_valid(oo, c->h_ci, c->h.log_n)) break;
       __sync_synchronize();
       memcpy(&cqe, (const void*)p, 64);
@@ -550,10 +549,10 @@ RN_API int rn_poll_cq(void* cq, int max, RnWc* out) {
     for (auto* q : h->qps) {
       if (q->h.qpn != v.qpn) continue;
       if (v.opcode == CQE_REQ || v.opcode == CQE_REQ_ERR) {
-        uint64_t done = q->h_sq_done + (uint16_t)(v.wqe_counter + 1 - (uint16_t)q->h_sq_done);
+        uint64_t done = expand16(v.wqe_counter + 1u, q->h_sq_done);
         if (done <= q->h_sq_pi) q->h_sq_done = done;
       } else if (q->rcq == c) {
-        uint64_t done = q->h_rq_done + (uint16_t)(v.wqe_counter + 1 - (uint16_t)q->h_rq_done);
+        uint64_t done = expand16(v.wqe_counter + 1u, q->h_rq_done);
         if (done <= q->h_rq_pi) q->h_rq_done = done;
       }
       break;
@@ -562,7 +561,7 @@ RN_API int rn_poll_cq(void* cq, int max, RnWc* out) {
     ++c->h_ci;
   }
   if (n) {
-    uint32_t rec = be32(c->h_ci & 0xffffff);
+    uint32_t rec = cq_dbr_word(c->h_ci);
     if (c->ring_host) *(volatile uint32_t*)c->h.dbrec = rec;
     else push(h, c->h.dbrec, &rec, 4);
   }
@@ -856,7 +855,7 @@ static int host_sq_publish(Qp* q, const Wqe64& w, uint64_t idx, uint64_t* idx_ou
   int rc = host_store(q, slot, &w, 64);
   if (rc) return rc;
   __sync_synchronize();
-  uint32_t rec = be32((uint32_t)((idx + 1) & 0xffff));
+  uint32_t rec = wq_dbr_word(idx + 1);
   rc = host_store(q, &q->h.dbr[DBR_SND], &rec, 4);
   if (rc) return rc;
   __sync_synchronize();
@@ -942,12 +941,11 @@ RN_API int rn_post_recv(void* qp, uint64_t addr, uint32_t lkey, uint32_t bytes) 
       return fail(-12, "post_recv: receive queue full (%llu posted, %llu consumed): poll the receive CQ first",
                   (unsigned long long)i, (unsigned long long)q->h_rq_done);
   }
-  RecvWqe w;
-  encode_data(&w.data, addr, lkey, bytes);
+  const Words16 w = recv_wqe_words(addr, lkey, bytes);
   int rc = host_store(q, q->h.rq + ((i & ((1ull << q->h.rq_log) - 1)) << 4), &w, 16);
   if (rc) return rc;
   __sync_synchronize();
-  uint32_t rec = be32((uint32_t)((i + 1) & 0xffff));
+  uint32_t rec = wq_dbr_word(i + 1);
   rc = host_store(q, &q->h.dbr[DBR_RCV], &rec, 4);
   if (rc) return rc;
   q->h_rq_pi = i + 1;
@@ -1099,6 +1097,15 @@ RN_API void rn_wire_build_atomic_wqe(uint8_t* out64, uint32_t opcode, uint32_t i
   Wqe64 w;
   build_atomic_wqe(&w, (uint8_t)opcode, (uint16_t)idx, qpn, laddr, lkey, raddr, rkey, swap_add, compare, (uint8_t)flags);
   memcpy(out64, &w, 64);
+}
+// The CQE the engine and the mock ConnectX write, from the encoder they share.
+RN_API void rn_wire_build_cqe(uint8_t* out64, uint32_t opcode, uint32_t owner, uint32_t wqe_counter, uint32_t qpn,
+                              uint32_t wqe_opcode, uint32_t byte_cnt, uint32_t imm, uint32_t syndrome, uint32_t vendor_synd,
+                              uint64_t timestamp) {
+  Cqe64 c;
+  encode_cqe(&c, (uint8_t)opcode, (uint8_t)owner, (uint16_t)wqe_counter, qpn, (uint8_t)wqe_opcode, byte_cnt, imm,
+             (uint8_t)syndrome, (uint8_t)vendor_synd, timestamp);
+  memcpy(out64, &c, 64);
 }
 // Decode a WQE with the engine's decoder: returns 1 if it is well formed.  out[] = opcode, wqe_idx, qpn, ds,
 // fm_ce_se, imm, raddr, rkey, laddr, lkey, bytes, swap_add, compare.

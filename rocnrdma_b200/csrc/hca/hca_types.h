@@ -87,7 +87,7 @@ struct RemoteView {
   MKeyEntry* rkeys;           // responder's MKey table
   uint32_t n_rkeys;
   uint32_t qpn;
-  uint8_t* rq;                // responder receive ring (16-byte RecvWqe strides)
+  uint8_t* rq;                // responder receive ring (16-byte receive WQEs)
   uint32_t* rq_dbr;           // responder doorbell record ([DBR_RCV] = be32 count)
   uint32_t rq_log;
   uint32_t connected;         // bit 0: connected; bit 1: responder CQ's consumer record addressable (same process)

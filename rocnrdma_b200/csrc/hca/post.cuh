@@ -140,7 +140,7 @@ __device__ __forceinline__ void st_u64_release_scope(void* p, unsigned long long
 // Ring the doorbell for every WQE below `to`: record, then register.
 __device__ __forceinline__ void ring_doorbell(uint32_t* dbr, unsigned long long* bf, uint32_t qpn, unsigned long long to,
                                               bool sys) {
-  st_u32_volatile(&dbr[DBR_SND], be32((uint32_t)(to & 0xffff)));
+  st_u32_volatile(&dbr[DBR_SND], wq_dbr_word(to));
   // The doorbell register store is a RELEASE: WQE bytes and the doorbell record are visible before
   // it (what the engine audits, and what a ConnectX requires: it may fetch the record and the WQE as
   // soon as the MMIO write lands).
@@ -207,17 +207,15 @@ __device__ __forceinline__ int sq_submit(QpDev* qp, unsigned long long idx, uint
 // requester completion of another QP, is NOT ours -- its wqe_counter is an index into another queue, so crediting it to
 // sq_cons would hand out SQ slots that have not executed yet.  Leave it at the head for its own consumer (recv_wait /
 // the other QP's poller).
-__device__ __forceinline__ uint8_t cqe_tail_op_own(const uint4& tail) { return (uint8_t)(tail.w >> 24); }
 __device__ __forceinline__ bool req_cqe(const uint4& tail, uint32_t qpn, int& rc) {
-  const uint8_t opc = cqe_opcode(cqe_tail_op_own(tail));
-  if ((opc != CQE_REQ && opc != CQE_REQ_ERR) || (be32(tail.z) & 0xffffffu) != qpn) return false;
+  const uint8_t opc = cqe_tail_opcode(tail);
+  if ((opc != CQE_REQ && opc != CQE_REQ_ERR) || cqe_tail_qpn(tail) != qpn) return false;
   if (opc == CQE_REQ_ERR) rc = WAIT_CQE_ERROR;
   return true;
 }
-// The completed index after an accepted CQE: its 16-bit wqe_counter expanded against the consumer position `cons`.
+// The completed index after an accepted CQE: its 16-bit wqe_counter + 1 expanded against the consumer position `cons`.
 __device__ __forceinline__ unsigned long long req_cqe_done(const uint4& tail, unsigned long long cons) {
-  const uint16_t wqe_counter = be16((uint16_t)(tail.w & 0xffff));
-  return cons + (unsigned long long)((uint16_t)(wqe_counter + 1 - (uint16_t)cons));
+  return expand16(cqe_tail_counter(tail) + 1u, cons);
 }
 
 // Consume at most one CQE of the QP's send CQ.  Returns 1 if one was consumed, 0 if
@@ -226,7 +224,7 @@ __device__ __forceinline__ int cq_poll_once(QpDev* qp) {
   CqDev* cq = qp->scq;
   unsigned int ci = *(volatile unsigned int*)&cq->ci;
   const uint8_t* cqe = cq->buf + ((size_t)(ci & ((1u << cq->log_n) - 1)) << 6);
-  const uint4 tail = ld_v4_volatile(cqe + 48);
+  const uint4 tail = ld_v4_volatile(cqe + CQE_TAIL_OFF);
   if (!cqe_valid(cqe_tail_op_own(tail), ci, cq->log_n)) return 0;
   __threadfence();  // acquire: payload and the rest of the CQE are visible past this point
   int rc = 1;
@@ -235,7 +233,7 @@ __device__ __forceinline__ int cq_poll_once(QpDev* qp) {
   if (atomicCAS(&cq->ci, ci, ci + 1) == ci) {
     trace_stamp(qp, done - 1, TR_SEEN);
     atomicMax(&qp->sq_cons, done);
-    st_u32_volatile(&cq->dbrec[0], be32((ci + 1) & 0xffffff));
+    st_u32_volatile(&cq->dbrec[0], cq_dbr_word(ci + 1));
   }
   return rc;
 }
@@ -296,7 +294,7 @@ __device__ __forceinline__ void poster_close(Poster& p) {
   st_u64_relaxed(&p.qp->ready_head, p.head);
   st_u64_relaxed(&p.qp->sq_cons, p.cons);
   *(volatile unsigned int*)&p.cq->ci = p.ci;
-  st_u32_volatile(&p.cq->dbrec[0], be32(p.ci & 0xffffff));
+  st_u32_volatile(&p.cq->dbrec[0], cq_dbr_word(p.ci));
 }
 // Consume CQEs that are ready now.  Returns <0 on an error completion (the rest of the run is still
 // consumed), else the number consumed.  A CQE that is not a requester completion of this QP stops the
@@ -305,7 +303,7 @@ __device__ __forceinline__ int poster_poll(Poster& p, int max_cqes = 8) {
   int n = 0, rc = 0;
   while (n < max_cqes) {
     const uint8_t* cqe = p.cq_buf + ((size_t)(p.ci & ((1u << p.cq_log) - 1)) << 6);
-    const uint4 tail = ld_v4_volatile(cqe + 48);
+    const uint4 tail = ld_v4_volatile(cqe + CQE_TAIL_OFF);
     if (!cqe_valid(cqe_tail_op_own(tail), p.ci, p.cq_log)) break;
     if (!req_cqe(tail, p.qpn, rc)) break;
     p.cons = req_cqe_done(tail, p.cons);
@@ -315,7 +313,7 @@ __device__ __forceinline__ int poster_poll(Poster& p, int max_cqes = 8) {
   }
   if (n) {
     __threadfence();                                              // acquire: payload behind the CQEs just seen
-    st_u32_volatile(&p.cq->dbrec[0], be32(p.ci & 0xffffff));      // consumer record (what a NIC checks for overrun)
+    st_u32_volatile(&p.cq->dbrec[0], cq_dbr_word(p.ci));          // consumer record (what a NIC checks for overrun)
     *(volatile unsigned int*)&p.cq->ci = p.ci;
   }
   return rc < 0 ? rc : n;
@@ -325,7 +323,7 @@ __device__ __forceinline__ int poster_poll(Poster& p, int max_cqes = 8) {
 // has the CQE load in flight while the release in front of the doorbell waits for the WQE stores to be acknowledged:
 // the two L2 round trips of a post-one / poll-one iteration overlap instead of adding up.
 __device__ __forceinline__ uint4 poster_peek(const Poster& p) {
-  return ld_v4_volatile(p.cq_buf + ((size_t)(p.ci & ((1u << p.cq_log) - 1)) << 6) + 48);
+  return ld_v4_volatile(p.cq_buf + ((size_t)(p.ci & ((1u << p.cq_log) - 1)) << 6) + CQE_TAIL_OFF);
 }
 // Consume the CQE whose tail was loaded by poster_peek, if it was ready and ours.  Returns 1 / 0 / WAIT_CQE_ERROR.
 __device__ __forceinline__ int poster_take(Poster& p, const uint4 tail) {
@@ -336,7 +334,7 @@ __device__ __forceinline__ int poster_take(Poster& p, const uint4 tail) {
   if (p.trace) trace_stamp(p.qp, p.cons - 1, TR_SEEN);
   ++p.ci;
   __threadfence();                                                // acquire: payload behind the CQE
-  st_u32_volatile(&p.cq->dbrec[0], be32(p.ci & 0xffffff));
+  st_u32_volatile(&p.cq->dbrec[0], cq_dbr_word(p.ci));
   return rc;
 }
 
@@ -496,10 +494,11 @@ __device__ __forceinline__ int post_flush(QpDev* qp, bool post_only, unsigned lo
 __device__ __forceinline__ void post_recv(QpDev* qp, uint64_t addr, uint32_t lkey, uint32_t bytes) {
   unsigned long long i = qp->rq_pi;
   uint8_t* slot = qp->rq + ((i & ((1ull << qp->rq_log) - 1)) << 4);
-  st_v4(slot, be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(addr >> 32)), be32((uint32_t)addr));
+  const uint4 r = recv_wqe_words(addr, lkey, bytes);
+  st_v4(slot, r.x, r.y, r.z, r.w);
   fence_sys();
   qp->rq_pi = i + 1;
-  st_u32_volatile(&qp->dbr[DBR_RCV], be32((uint32_t)((i + 1) & 0xffff)));
+  st_u32_volatile(&qp->dbr[DBR_RCV], wq_dbr_word(i + 1));
   fence_sys();
 }
 
@@ -511,21 +510,20 @@ __device__ __forceinline__ long long recv_wait(QpDev* qp, uint32_t* imm, unsigne
   for (unsigned it = 0;; ++it) {
     unsigned int ci = *(volatile unsigned int*)&cq->ci;
     const uint8_t* cqe = cq->buf + ((size_t)(ci & ((1u << cq->log_n) - 1)) << 6);
-    uint4 tail = ld_v4_volatile(cqe + 48);
-    uint8_t op_own = (uint8_t)(tail.w >> 24);
-    if (cqe_valid(op_own, ci, cq->log_n)) {
+    const uint4 tail = ld_v4_volatile(cqe + CQE_TAIL_OFF);
+    if (cqe_valid(cqe_tail_op_own(tail), ci, cq->log_n)) {
       __threadfence();
-      uint4 mid = ld_v4_volatile(cqe + 32);  // srqn | imm | rsvd | byte_cnt
-      uint8_t opc = cqe_opcode(op_own);
+      const uint4 mid = ld_v4_volatile(cqe + CQE_MID_OFF);
+      const uint8_t opc = cqe_tail_opcode(tail);
       if (opc == CQE_REQ || opc == CQE_REQ_ERR) {      // shared CQ: a send completion is at the head; its poller takes it
         if ((it & 15) == 15 && globaltimer_ns() - t0 > timeout_ns) return WAIT_TIMEOUT;
         continue;
       }
       if (atomicCAS(&cq->ci, ci, ci + 1) != ci) continue;
-      st_u32_volatile(&cq->dbrec[0], be32((ci + 1) & 0xffffff));
-      if (opc == CQE_RESP_ERR || opc == CQE_REQ_ERR) return WAIT_CQE_ERROR;
-      if (imm) *imm = be32(mid.y);
-      return (long long)be32(mid.w);
+      st_u32_volatile(&cq->dbrec[0], cq_dbr_word(ci + 1));
+      if (cqe_is_error(opc)) return WAIT_CQE_ERROR;
+      if (imm) *imm = cqe_mid_imm(mid);
+      return (long long)cqe_mid_byte_cnt(mid);
     }
     if ((it & 15) == 15 && globaltimer_ns() - t0 > timeout_ns) return WAIT_TIMEOUT;
   }

@@ -558,14 +558,14 @@ __global__ void __launch_bounds__(kCqWatchThreads, 1) cq_watch_kernel(const CqDe
     if (threadIdx.x == 0) {
       const uint8_t* cqe = buf + ((size_t)(k & ((1u << log_n) - 1)) << 6);
       const unsigned long long tw = globaltimer_ns();
-      uint4 t = ld_v4_volatile(cqe + 48);
-      while (!cqe_valid((uint8_t)(t.w >> 24), k, log_n)) {
+      uint4 t = ld_v4_volatile(cqe + CQE_TAIL_OFF);
+      while (!cqe_valid(cqe_tail_op_own(t), k, log_n)) {
         if (globaltimer_ns() - tw > timeout_ns) { s_status = WAIT_TIMEOUT; break; }
-        t = ld_v4_volatile(cqe + 48);
+        t = ld_v4_volatile(cqe + CQE_TAIL_OFF);
       }
       fence_sys();   // acquire: the payload the CQE announces
-      s_counter = be16((uint16_t)(t.w & 0xffff));
-      if (cqe_opcode((uint8_t)(t.w >> 24)) == CQE_REQ_ERR) ++s_errs;
+      s_counter = cqe_tail_counter(t);
+      if (cqe_tail_opcode(t) == CQE_REQ_ERR) ++s_errs;
     }
     __syncthreads();   // thread 0's acquire, then the barrier: every thread's loads below see the message
     if (s_status != WAIT_OK) break;

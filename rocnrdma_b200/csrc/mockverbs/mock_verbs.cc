@@ -57,7 +57,6 @@
 #include "../wire/mlx5_wire.h"
 
 using namespace rnabi;
-using rn::be16;
 using rn::be32;
 using rn::be64;
 
@@ -373,12 +372,12 @@ bool nic_atomic(uint8_t opcode, uint64_t tgt, MockMr* mr, uint64_t swap_add, uin
 }
 
 // ------------------------------------------------------------------ CQE writer
-void write_cqe(MockCq* cq, uint8_t opcode, uint8_t wqe_opcode, uint32_t qpn, uint16_t counter, uint32_t bytes, uint32_t imm_be,
+void write_cqe(MockCq* cq, uint8_t opcode, uint8_t wqe_opcode, uint32_t qpn, uint16_t counter, uint32_t bytes, uint32_t imm,
                uint8_t syndrome) {
   const uint32_t depth = 1u << cq->log_n;
   const uint32_t slot = cq->pi.load(std::memory_order_relaxed);
-  const uint32_t ci = be32(*(volatile uint32_t*)&cq->dbrec[0]) & 0xffffffu;
-  if (((slot - ci) & 0xffffffu) >= depth) {
+  const uint32_t ci = rn::cq_dbr_index(*(volatile uint32_t*)&cq->dbrec[0]);
+  if (((slot - ci) & 0xffffffu) >= depth) {   // the record holds 24 bits of ci: distance mod 2^24
     // CQ overrun: the consumer has not freed the slot.  A ConnectX raises a CQ error; the mock counts it and
     // drops the completion (the consumer's bounded wait then reports the loss) rather than corrupting the ring.
     cq->overruns++;
@@ -386,21 +385,10 @@ void write_cqe(MockCq* cq, uint8_t opcode, uint8_t wqe_opcode, uint32_t qpn, uin
   }
   uint8_t* p = cq->buf + ((size_t)(slot & (depth - 1)) << 6);
   rn::Cqe64 c;
-  memset(&c, 0, sizeof c);
-  c.imm_inval_pkey = imm_be;
-  c.byte_cnt = be32(bytes);
-  const uint64_t t = now_ns();
-  c.timestamp_h = be32((uint32_t)(t >> 32)); c.timestamp_l = be32((uint32_t)t);
-  c.sop_drop_qpn = be32(((uint32_t)wqe_opcode << 24) | (qpn & 0xffffffu));
-  c.wqe_counter = be16(counter);
-  if (syndrome) {
-    rn::ErrCqe* e = reinterpret_cast<rn::ErrCqe*>(&c);
-    e->syndrome = syndrome; e->vendor_err_synd = 0x5a;
-    e->s_wqe_opcode_qpn = c.sop_drop_qpn; e->wqe_counter = c.wqe_counter;
-  }
-  memcpy(p, &c, 63);
+  rn::encode_cqe(&c, opcode, (uint8_t)((slot >> cq->log_n) & 1u), counter, qpn, wqe_opcode, bytes, imm, syndrome, 0x5a, now_ns());
+  memcpy(p, &c, rn::CQE_OP_OWN_OFF);
   // owner bit last, released: a poller (host, or a GPU reading this page over PCIe) that sees it sees the body
-  __atomic_store_n(p + 63, rn::cqe_op_own(opcode, (slot >> cq->log_n) & 1u), __ATOMIC_RELEASE);
+  __atomic_store_n(p + rn::CQE_OP_OWN_OFF, c.op_own, __ATOMIC_RELEASE);
   cq->pi.store(slot + 1, std::memory_order_release);
 }
 
@@ -408,7 +396,7 @@ void write_cqe(MockCq* cq, uint8_t opcode, uint8_t wqe_opcode, uint32_t qpn, uin
 // receive, up to the RNR timeout.  Returns 1 when a receive is there, 0 while the WQE must be retried later, -1 once the
 // timeout has passed.
 int recv_wait(MockQp* qp, MockQp* peer) {
-  const uint16_t rpi = (uint16_t)be32(*(volatile uint32_t*)&peer->dbrec[rn::DBR_RCV]);
+  const uint16_t rpi = rn::wq_dbr_index(*(volatile uint32_t*)&peer->dbrec[rn::DBR_RCV]);
   if ((uint16_t)(rpi - (uint16_t)peer->hw_rq_cons) != 0) return 1;
   const uint64_t t = now_ns();
   if (!qp->rnr_since_ns) { qp->rnr_since_ns = t; qp->n_rnr++; }
@@ -491,13 +479,12 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         if (r < 0) { syn = rn::SYN_RNR_RETRY_EXC_ERR; break; }
         std::atomic_thread_fence(std::memory_order_acquire);
         const uint8_t* rs = peer->rq + ((peer->hw_rq_cons & (peer->rq_cnt - 1)) << 4);
-        rn::DataSeg ds;
-        memcpy(&ds, rs, 16);
-        const uint32_t rbytes = be32(ds.byte_count) & 0x7fffffffu, rlkey = be32(ds.lkey);
-        const uint64_t raddr = be64(ds.addr);
+        rn::Words16 rw;
+        memcpy(&rw, rs, 16);
         consumed_rq = true; rq_index = (uint16_t)peer->hw_rq_cons++;
-        if (rbytes < v.bytes) syn = rn::SYN_REMOTE_INVAL_REQ_ERR;
-        uint64_t dst = syn == rn::SYN_OK ? translate(rdev, rlkey, raddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, true, &syn, &rmr) : 0;
+        if (rn::recv_wqe_bytes(rw) < v.bytes) syn = rn::SYN_REMOTE_INVAL_REQ_ERR;
+        uint64_t dst = syn == rn::SYN_OK ? translate(rdev, rn::recv_wqe_lkey(rw), rn::recv_wqe_addr(rw), v.bytes, IBV_ACCESS_LOCAL_WRITE,
+                                                     true, &syn, &rmr) : 0;
         if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, rmr, src, lmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) moved = v.bytes;
         break;
@@ -523,7 +510,7 @@ bool nic_execute(MockQp* qp, uint64_t w) {
   if (consumed_rq && peer && peer->rcq) {
     const uint8_t rop = err ? rn::CQE_RESP_ERR
                             : (opc == rn::OP_SEND ? rn::CQE_RESP_SEND : (opc == rn::OP_SEND_IMM ? rn::CQE_RESP_SEND_IMM : rn::CQE_RESP_WR_IMM));
-    write_cqe(peer->rcq, rop, 0, peer->v.qp_num, rq_index, moved, wqe.ctrl.imm, err ? syn : 0);
+    write_cqe(peer->rcq, rop, 0, peer->v.qp_num, rq_index, moved, be32(wqe.ctrl.imm), err ? syn : 0);
   }
   if (err || (ok && (v.fm_ce_se & rn::CTRL_CQ_UPDATE)) || qp->sq_sig_all) {
     write_cqe(qp->scq, err ? rn::CQE_REQ_ERR : rn::CQE_REQ, opc, qp->v.qp_num, (uint16_t)w, moved, 0, err ? syn : 0);
@@ -553,7 +540,7 @@ bool nic_sweep() {
         const unsigned long long val = __atomic_load_n((unsigned long long*)(qp->uar + kBfOffset + r * kBfSize), __ATOMIC_ACQUIRE);
         if (val != qp->bf_seen[r]) { qp->bf_seen[r] = val; rung = true; rung_val = val; }
       }
-      const uint16_t pi16 = (uint16_t)be32(*(volatile uint32_t*)&qp->dbrec[rn::DBR_SND]);
+      const uint16_t pi16 = rn::wq_dbr_index(*(volatile uint32_t*)&qp->dbrec[rn::DBR_SND]);
       uint16_t pending = (uint16_t)(pi16 - (uint16_t)qp->hw_sq_cons);
       if (rung) {
         qp->n_doorbells++;
@@ -561,7 +548,7 @@ bool nic_sweep() {
         // register, must already cover that WQE -- otherwise the register store overtook the record store (ordering bug in
         // the poster).  ("Nothing pending" is not the test: an earlier sweep may already have executed this WQE off a
         // record that was ahead of its doorbell, which is legal.)
-        const uint16_t bell_idx = (uint16_t)(be32((uint32_t)rung_val) >> 8);
+        const uint16_t bell_idx = rn::doorbell_index(rung_val);
         if ((uint16_t)(pi16 - (uint16_t)(bell_idx + 1)) >= 0x8000u) qp->n_db_no_progress++;
       }
       // Work is only fetched on a doorbell (a real NIC does not look at the record unprompted); a WQE that had
@@ -654,7 +641,7 @@ int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
     // doorbell record, then the doorbell: first 8 bytes of the last WQE's ctrl segment into the BlueFlame
     // register, alternating between the two registers as libmlx5 does
     std::atomic_thread_fence(std::memory_order_release);
-    *(volatile uint32_t*)&qp->dbrec[rn::DBR_SND] = be32((uint32_t)(head & 0xffff));
+    *(volatile uint32_t*)&qp->dbrec[rn::DBR_SND] = rn::wq_dbr_word(head);
     std::atomic_thread_fence(std::memory_order_release);
     unsigned long long db;
     memcpy(&db, qp->sq + (((head - 1) & (qp->sq_cnt - 1)) << 6), 8);
@@ -674,15 +661,14 @@ int mock_post_recv(ibv_qp* q, ibv_recv_wr* wr, ibv_recv_wr** bad) {
   for (; wr; wr = wr->next) {
     if (head - qp->rq_tail >= qp->rq_cnt) { if (bad) *bad = wr; rc = ENOMEM; break; }
     if (wr->num_sge != 1) { if (bad) *bad = wr; rc = EINVAL; break; }
-    rn::RecvWqe r;
-    rn::encode_data(&r.data, wr->sg_list[0].addr, wr->sg_list[0].lkey, wr->sg_list[0].length);
+    const rn::Words16 r = rn::recv_wqe_words(wr->sg_list[0].addr, wr->sg_list[0].lkey, wr->sg_list[0].length);
     memcpy(qp->rq + ((head & (qp->rq_cnt - 1)) << 4), &r, 16);
     qp->rq_wrid[head & (qp->rq_cnt - 1)] = wr->wr_id;
     ++head;
   }
   if (head != qp->rq_head) {
     std::atomic_thread_fence(std::memory_order_release);
-    *(volatile uint32_t*)&qp->dbrec[rn::DBR_RCV] = be32((uint32_t)(head & 0xffff));
+    *(volatile uint32_t*)&qp->dbrec[rn::DBR_RCV] = rn::wq_dbr_word(head);
     qp->rq_head = head;
   }
   return rc;
@@ -714,7 +700,7 @@ int mock_poll_cq(ibv_cq* c, int n, ibv_wc* wc) {
   int got = 0;
   while (got < n) {
     const uint8_t* p = cq->buf + ((size_t)(cq->ci & ((1u << cq->log_n) - 1)) << 6);
-    const uint8_t oo = __atomic_load_n(p + 63, __ATOMIC_ACQUIRE);
+    const uint8_t oo = __atomic_load_n(p + rn::CQE_OP_OWN_OFF, __ATOMIC_ACQUIRE);
     if (!rn::cqe_valid(oo, cq->ci, cq->log_n)) break;
     rn::Cqe64 e;
     memcpy(&e, p, 64);
@@ -732,11 +718,11 @@ int mock_poll_cq(ibv_cq* c, int n, ibv_wc* wc) {
       std::lock_guard<std::mutex> g(qp->post_mu);
       if (req) {
         o.wr_id = qp->sq_wrid[v.wqe_counter & (qp->sq_cnt - 1)];
-        const uint64_t done = qp->sq_tail + (uint16_t)(v.wqe_counter + 1 - (uint16_t)qp->sq_tail);
+        const uint64_t done = rn::expand16(v.wqe_counter + 1u, qp->sq_tail);
         if (done <= qp->sq_head) qp->sq_tail = done;     // unsignaled predecessors are complete too (RC is in order)
       } else {
         o.wr_id = qp->rq_wrid[v.wqe_counter & (qp->rq_cnt - 1)];
-        const uint64_t done = qp->rq_tail + (uint16_t)(v.wqe_counter + 1 - (uint16_t)qp->rq_tail);
+        const uint64_t done = rn::expand16(v.wqe_counter + 1u, qp->rq_tail);
         if (done <= qp->rq_head) qp->rq_tail = done;
       }
     }
@@ -753,7 +739,7 @@ int mock_poll_cq(ibv_cq* c, int n, ibv_wc* wc) {
     ++cq->ci;
     ++got;
   }
-  if (got) *(volatile uint32_t*)&cq->dbrec[0] = be32(cq->ci & 0xffffffu);
+  if (got) *(volatile uint32_t*)&cq->dbrec[0] = rn::cq_dbr_word(cq->ci);
   // A real NIC needs no CPU; this one is a thread.  A caller that spins on an empty CQ from the core the NIC
   // thread was placed on would starve it for a scheduler tick at a time, so an empty poll gives the core away
   // now and then.
@@ -949,7 +935,7 @@ MOCK_API ibv_cq* ibv_create_cq(ibv_context* c, int cqe, void* cq_context, ibv_co
   q->buf = (uint8_t*)page_alloc((size_t)n * 64);
   q->dbrec = (uint32_t*)page_alloc(64);
   if (!q->buf || !q->dbrec) { free(q->buf); free(q->dbrec); delete q; errno = ENOMEM; return nullptr; }
-  for (uint32_t i = 0; i < n; ++i) q->buf[(size_t)i * 64 + 63] = rn::cqe_op_own(rn::CQE_INVALID, 1);
+  rn::init_cq_ring(q->buf, n);
   q->v.context = c; q->v.channel = ch; q->v.cq_context = cq_context; q->v.handle = cqn; q->v.cqe = (int)n - 1;
   pthread_mutex_init(&q->v.mutex, nullptr);
   pthread_cond_init(&q->v.cond, nullptr);

@@ -1,4 +1,4 @@
-// mlx5 work-queue wire format: WQE segments, CQE64, doorbell record.
+// mlx5 work-queue wire format: WQE segments, receive WQEs, CQE64, doorbell and CQ consumer records.
 //
 // Everything a ConnectX HCA reads or writes in a send queue / completion queue,
 // byte-exact and big-endian, usable from host C++, CUDA device code and (through
@@ -11,6 +11,7 @@
 // (README.md:67).  SURVEY.md N3/K1 asks for the GPU to build these itself.
 #pragma once
 #include <stdint.h>
+#include <string.h>
 
 #if defined(__CUDACC__)
 #define RN_HD __host__ __device__ __forceinline__
@@ -150,10 +151,6 @@ enum : uint32_t { INLINE_OFF_RDMA = 36, INLINE_OFF_SEND = 20 };
 static_assert(__builtin_offsetof(Wqe64, rdma_inl.data) == INLINE_OFF_RDMA, "rdma inline payload");
 static_assert(__builtin_offsetof(Wqe64, send_inl.data) == INLINE_OFF_SEND, "send inline payload");
 
-// Receive WQE: a bare scatter list; we use one data segment per 16-byte stride.
-struct alignas(16) RecvWqe { DataSeg data; };
-static_assert(sizeof(RecvWqe) == 16, "recv wqe");
-
 struct alignas(64) Cqe64 {       // mlx5_cqe64
   uint8_t outer_l3_tunneled;
   uint8_t rsvd0;
@@ -206,6 +203,8 @@ RN_HD uint32_t ctrl_word1(uint32_t qpn, uint8_t ds) { return be32((qpn << 8) | (
 RN_HD uint64_t doorbell_word(uint32_t qpn, uint16_t last) {
   return (uint64_t)ctrl_word0(OP_NOP, last) | ((uint64_t)ctrl_word1(qpn, 0) << 32);
 }
+// The last WQE index a doorbell register word names.
+RN_HD uint16_t doorbell_index(uint64_t db) { return (uint16_t)(be32((uint32_t)db) >> 8); }
 
 RN_HD void encode_ctrl(CtrlSeg* c, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, uint8_t ds,
                        uint8_t fm_ce_se, uint32_t imm) {
@@ -369,6 +368,61 @@ RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
 RN_HD uint8_t cqe_op_own(uint8_t opcode, uint8_t owner) { return (uint8_t)((opcode << 4) | (owner & 1)); }
 RN_HD uint8_t cqe_opcode(uint8_t op_own) { return op_own >> 4; }
 RN_HD uint8_t cqe_owner(uint8_t op_own) { return op_own & 1; }
+RN_HD bool cqe_is_error(uint8_t opcode) { return opcode == CQE_REQ_ERR || opcode == CQE_RESP_ERR; }
+
+// ---------------------------------------------------------------- CQEs as 16-byte parts
+// A CQE is written and read as 16-byte parts of four words in memory order (a uint4 in CUDA code); bytes 0-31 are zero.
+//   mid  = bytes 32-47: srqn | imm | reserved | byte_cnt   (imm and byte_cnt are reserved, so zero, in an error CQE)
+//   tail = bytes 48-63: timestamp_h | timestamp_l | sop_drop_qpn | wqe_counter, signature, op_own.  An error CQE has
+//          zero, then reserved[2], vendor_err_synd, syndrome for the timestamp.  op_own holds the owner bit: tail last.
+#if defined(__CUDACC__)
+typedef uint4 Words16;
+#else
+struct alignas(16) Words16 { uint32_t x, y, z, w; };
+#endif
+enum : uint32_t { CQE_MID_OFF = 32, CQE_TAIL_OFF = 48, CQE_OP_OWN_OFF = 63 };
+static_assert(__builtin_offsetof(Cqe64, srqn) == CQE_MID_OFF, "cqe mid");
+static_assert(__builtin_offsetof(Cqe64, timestamp_h) == CQE_TAIL_OFF, "cqe tail");
+static_assert(__builtin_offsetof(Cqe64, op_own) == CQE_OP_OWN_OFF, "cqe op_own");
+static_assert(__builtin_offsetof(ErrCqe, vendor_err_synd) == CQE_TAIL_OFF + 6, "err cqe syndromes");
+
+RN_HD Words16 encode_cqe_mid(uint8_t opcode, uint32_t byte_cnt, uint32_t imm) {
+  const bool err = cqe_is_error(opcode);
+  return Words16{0u, err ? 0u : be32(imm), 0u, err ? 0u : be32(byte_cnt)};
+}
+// vendor_synd: the vendor syndrome of an error CQE (bits of no meaning to a consumer).
+RN_HD Words16 encode_cqe_tail(uint8_t opcode, uint8_t owner, uint16_t wqe_counter, uint32_t qpn, uint8_t wqe_opcode,
+                              uint8_t syndrome, uint8_t vendor_synd, uint64_t timestamp) {
+  const bool err = cqe_is_error(opcode);
+  return Words16{err ? 0u : be32((uint32_t)(timestamp >> 32)),
+                 err ? ((uint32_t)syndrome << 24) | ((uint32_t)vendor_synd << 16) : be32((uint32_t)timestamp),
+                 be32(((uint32_t)wqe_opcode << 24) | (qpn & 0xffffff)),
+                 (uint32_t)be16(wqe_counter) | ((uint32_t)cqe_op_own(opcode, owner) << 24)};
+}
+// The whole CQE (host producers and the test hook).
+RN_HD void encode_cqe(Cqe64* c, uint8_t opcode, uint8_t owner, uint16_t wqe_counter, uint32_t qpn, uint8_t wqe_opcode,
+                      uint32_t byte_cnt, uint32_t imm, uint8_t syndrome, uint8_t vendor_synd, uint64_t timestamp) {
+  const Words16 mid = encode_cqe_mid(opcode, byte_cnt, imm);
+  const Words16 tail = encode_cqe_tail(opcode, owner, wqe_counter, qpn, wqe_opcode, syndrome, vendor_synd, timestamp);
+  memset(c, 0, CQE_MID_OFF);
+  memcpy(reinterpret_cast<uint8_t*>(c) + CQE_MID_OFF, &mid, 16);
+  memcpy(reinterpret_cast<uint8_t*>(c) + CQE_TAIL_OFF, &tail, 16);
+}
+// Every slot of a new CQ ring: zero, opcode INVALID, owner 1 (the producer's first pass writes owner 0).
+RN_HD void init_cq_ring(uint8_t* ring, uint32_t ncqe) {
+  memset(ring, 0, (size_t)ncqe * CQE_SIZE);
+  for (uint32_t i = 0; i < ncqe; ++i) ring[(size_t)i * CQE_SIZE + CQE_OP_OWN_OFF] = cqe_op_own(CQE_INVALID, 1);
+}
+
+RN_HD uint8_t cqe_tail_op_own(const Words16& tail) { return (uint8_t)(tail.w >> 24); }
+RN_HD uint8_t cqe_tail_opcode(const Words16& tail) { return cqe_opcode(cqe_tail_op_own(tail)); }
+RN_HD uint16_t cqe_tail_counter(const Words16& tail) { return be16((uint16_t)tail.w); }
+RN_HD uint32_t cqe_tail_qpn(const Words16& tail) { return be32(tail.z) & 0xffffff; }
+RN_HD uint8_t cqe_tail_wqe_opcode(const Words16& tail) { return (uint8_t)(be32(tail.z) >> 24); }
+RN_HD uint8_t cqe_tail_syndrome(const Words16& tail) { return (uint8_t)(tail.y >> 24); }         // error CQEs only
+RN_HD uint8_t cqe_tail_vendor_synd(const Words16& tail) { return (uint8_t)(tail.y >> 16); }      // error CQEs only
+RN_HD uint32_t cqe_mid_imm(const Words16& mid) { return be32(mid.y); }
+RN_HD uint32_t cqe_mid_byte_cnt(const Words16& mid) { return be32(mid.w); }
 
 struct CqeView {
   uint8_t opcode, owner, syndrome, vendor_synd, wqe_opcode;
@@ -377,24 +431,43 @@ struct CqeView {
   bool is_error;
 };
 RN_HD void decode_cqe(const Cqe64* c, CqeView* v) {
-  v->opcode = cqe_opcode(c->op_own);
-  v->owner = cqe_owner(c->op_own);
-  v->wqe_counter = be16(c->wqe_counter);
-  uint32_t sq = be32(c->sop_drop_qpn);
-  v->qpn = sq & 0xffffff;
-  v->wqe_opcode = (uint8_t)(sq >> 24);
-  v->byte_cnt = be32(c->byte_cnt);
-  v->imm = be32(c->imm_inval_pkey);
-  v->is_error = (v->opcode == CQE_REQ_ERR || v->opcode == CQE_RESP_ERR);
-  const ErrCqe* e = reinterpret_cast<const ErrCqe*>(c);
-  v->syndrome = v->is_error ? e->syndrome : 0;
-  v->vendor_synd = v->is_error ? e->vendor_err_synd : 0;
+  Words16 mid, tail;
+  memcpy(&mid, reinterpret_cast<const uint8_t*>(c) + CQE_MID_OFF, 16);
+  memcpy(&tail, reinterpret_cast<const uint8_t*>(c) + CQE_TAIL_OFF, 16);
+  v->opcode = cqe_tail_opcode(tail);
+  v->owner = cqe_owner(cqe_tail_op_own(tail));
+  v->wqe_counter = cqe_tail_counter(tail);
+  v->qpn = cqe_tail_qpn(tail);
+  v->wqe_opcode = cqe_tail_wqe_opcode(tail);
+  v->byte_cnt = cqe_mid_byte_cnt(mid);
+  v->imm = cqe_mid_imm(mid);
+  v->is_error = cqe_is_error(v->opcode);
+  v->syndrome = v->is_error ? cqe_tail_syndrome(tail) : 0;
+  v->vendor_synd = v->is_error ? cqe_tail_vendor_synd(tail) : 0;
 }
 
-// A CQE at consumer index `ci` of a 2^log_n ring is valid when its opcode is not
-// INVALID and its owner bit equals the pass parity of ci.
+// A CQE at consumer index `ci` of a 2^log_n ring is valid when its opcode is not INVALID and its owner bit is ci's pass parity.
 RN_HD bool cqe_valid(uint8_t op_own, uint32_t ci, uint32_t log_n) {
   return cqe_opcode(op_own) != CQE_INVALID && cqe_owner(op_own) == ((ci >> log_n) & 1u);
 }
+
+// ---------------------------------------------------------------- index records and counters
+// A 16-bit wire counter (a CQE's wqe_counter, a doorbell record) expanded to the 64-bit index at or above `near` that
+// it names (wire.expand16).  Only the low 16 bits of `counter` count, so a caller may pass wqe_counter + 1 unwrapped.
+RN_HD uint64_t expand16(uint32_t counter, uint64_t near) { return near + ((counter - (uint32_t)near) & 0xffffu); }
+// SQ / RQ doorbell record: be32 of the producer index's low 16 bits.
+RN_HD uint32_t wq_dbr_word(uint64_t pi) { return be32((uint32_t)(pi & 0xffff)); }
+RN_HD uint16_t wq_dbr_index(uint32_t rec) { return (uint16_t)be32(rec); }
+// CQ consumer record: be32 of the consumer index's low 24 bits.
+RN_HD uint32_t cq_dbr_word(uint32_t ci) { return be32(ci & 0xffffff); }
+RN_HD uint32_t cq_dbr_index(uint32_t rec) { return be32(rec) & 0xffffff; }
+
+// A receive WQE: one data segment (what encode_data writes) per 16-byte stride.
+RN_HD Words16 recv_wqe_words(uint64_t addr, uint32_t lkey, uint32_t bytes) {
+  return Words16{be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(addr >> 32)), be32((uint32_t)addr)};
+}
+RN_HD uint32_t recv_wqe_bytes(const Words16& d) { return be32(d.x) & 0x7fffffffu; }
+RN_HD uint32_t recv_wqe_lkey(const Words16& d) { return be32(d.y); }
+RN_HD uint64_t recv_wqe_addr(const Words16& d) { return ((uint64_t)be32(d.z) << 32) | be32(d.w); }
 
 }  // namespace rn

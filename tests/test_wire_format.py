@@ -99,3 +99,26 @@ def test_native_encoder_matches_python_mirror():
         assert bytes(buf) == W.rdma_wqe(op, idx, qpn, la, lk, ra, rk, nb, fl, imm)
     lib.rn_wire_build_wqe(buf, W.OP_SEND, 3, 0x100, 0x1000, 0x5, 0, 0, 100, W.CTRL_CQ_UPDATE, 0)
     assert bytes(buf) == W.send_wqe(W.OP_SEND, 3, 0x100, 0x1000, 0x5, 100)
+
+
+@pytest.mark.parametrize("op", [W.CQE_REQ, W.CQE_RESP_WR_IMM, W.CQE_RESP_SEND, W.CQE_RESP_SEND_IMM, W.CQE_REQ_ERR,
+                                W.CQE_RESP_ERR])
+def test_native_cqe_encoder_matches_python_mirror(op):
+    """The CQE encoder the engine and the mock ConnectX share writes wire.cqe()'s bytes.  An error CQE keeps only the
+    syndromes where a good one has imm, byte_cnt and the timestamp: every other byte of it is reserved and zero."""
+    from rocnrdma_b200 import _native as N
+    lib = N.load()
+    buf = (C.c_uint8 * 64)()
+    err = op in (W.CQE_REQ_ERR, W.CQE_RESP_ERR)
+    for owner, ctr, qpn, wop, bc, imm, syn, ts in [
+        (0, 0, 0, 0, 0, 0, 0, 0),
+        (1, 0xBEEF, 0x123456, W.OP_RDMA_WRITE, 4096, 9, W.SYN["REMOTE_ACCESS_ERR"], 0x0102030405060708),
+        (1, 0xFFFF, 0xFFFFFF, 0xFF, 0xFFFFFFFF, 0xFFFFFFFF, 0xFF, 2 ** 64 - 1),
+    ]:
+        lib.rn_wire_build_cqe(buf, op, owner, ctr, qpn, wop, bc, imm, syn, 0, ts)
+        assert bytes(buf) == W.cqe(op, owner, ctr, qpn, wop, bc, imm, syn, ts)
+        lib.rn_wire_build_cqe(buf, op, owner, ctr, qpn, wop, bc, imm, syn, 0x5A, ts)
+        if err:    # the vendor syndrome is byte 54; every byte before it stays zero
+            assert bytes(buf)[:56] == bytes(54) + bytes([0x5A, syn])
+        else:      # a good CQE carries no syndrome
+            assert bytes(buf) == W.cqe(op, owner, ctr, qpn, wop, bc, imm, syn, ts)

@@ -51,9 +51,16 @@ err_cqe_ops = st.sampled_from([W.CQE_REQ_ERR, W.CQE_RESP_ERR])
 
 
 @settings(max_examples=300, deadline=None)
-@given(op=st.one_of(good_cqe_ops, err_cqe_ops), owner=st.integers(0, 1), ctr=u16, qpn=u24, wop=u8, bc=u32, imm=u32, syn=u8, ts=u64)
-def test_cqe_decoders_agree(lib, op, owner, ctr, qpn, wop, bc, imm, syn, ts):
+@given(op=st.one_of(good_cqe_ops, err_cqe_ops), owner=st.integers(0, 1), ctr=u16, qpn=u24, wop=u8, bc=u32, imm=u32, syn=u8, ts=u64,
+       vendor=u8)
+def test_cqe_decoders_agree(lib, op, owner, ctr, qpn, wop, bc, imm, syn, ts, vendor):
+    """The native encoder writes wire.cqe()'s bytes, and both decoders read them back."""
     raw = W.cqe(op, owner, ctr, qpn, wop, bc, imm, syn, ts)
+    buf = (C.c_uint8 * 64)()
+    lib.rn_wire_build_cqe(buf, op, owner, ctr, qpn, wop, bc, imm, syn, vendor, ts)
+    # the vendor syndrome (byte 54, which wire.cqe leaves 0) is the only byte the Python mirror does not model
+    want = raw[:54] + bytes([vendor]) + raw[55:] if op in (W.CQE_REQ_ERR, W.CQE_RESP_ERR) else raw
+    assert bytes(buf) == want
     wc = N.RnWc()
     assert lib.rn_wire_decode_cqe((C.c_uint8 * 64)(*raw), C.byref(wc)) == 0
     py = W.decode_cqe(raw)
