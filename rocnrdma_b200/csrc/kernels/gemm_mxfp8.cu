@@ -58,20 +58,21 @@ struct MxArgs {
   uint32_t M, N, K;
   unsigned long long* out;   // [status, t_start, t_end, tiles, 0...]: mapped pinned HOST memory -- written by the last CTA only
   unsigned int* done;        // device scratch (zeroed, self-cleaning): CTAs finished
-  // Receive-side fusion ("the panel arrives -> its tiles start"): one word per 128-row panel of A, nonzero once the panel's
-  // record has landed in this GPU's memory (recv_consume_kernel stamps it when the panel's receive completion shows up).
-  // nullptr: A is complete before the launch.  The TMA producer and the scale loaders wait for the word of the panel
-  // they are about to read; every wait is bounded.
+  // Receive-side fusion ("the record arrives -> its tiles start"): one word per record of A (a K4 panel record, a K3
+  // chunk record, or the whole matrix when A is plain), nonzero once that record has landed in this GPU's memory
+  // (recv_consume_kernel stamps word `imm` when the record's receive completion shows up; the immediate is the panel or
+  // chunk id).  nullptr: A is complete before the launch.  The TMA producer and the scale loaders wait for the word of the
+  // record they are about to read; every wait is bounded.
   const unsigned long long* a_ready;
   uint64_t ready_timeout_ns;
 };
-// bounded wait for a panel's arrival word; the acquire orders it before the loads of the panel, the proxy fence extends
-// that to the async proxy (TMA reads the panel)
-__device__ __forceinline__ bool wait_panel(const unsigned long long* ready, uint32_t panel, uint64_t timeout_ns, volatile int* abort) {
+// bounded wait for a record's arrival word; the acquire orders it before the loads of the record, the proxy fence extends
+// that to the async proxy (TMA reads the record)
+__device__ __forceinline__ bool wait_record(const unsigned long long* ready, uint32_t rec, uint64_t timeout_ns, volatile int* abort) {
   if (!ready) return true;
   unsigned long long v, t0 = 0;
   for (unsigned n = 0;; ++n) {
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ready + panel) : "memory");
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ready + rec) : "memory");
     if (v) break;
     if (*abort) return false;
     if ((n & 63) == 63) {
@@ -135,8 +136,11 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
     uint32_t stage = 0, phase = 0;
     for (uint32_t tile = unit; tile < n_tiles && !s.abort; tile += n_units) {
       const uint32_t m_blk = (tile / n_blks) * CTAS + rank, n_blk = tile % n_blks;
-      if (!wait_panel(g.a_ready, m_blk, g.ready_timeout_ns, &s.abort)) break;   // the scales travel in the same record
       const uint32_t ar = m_blk * BM, br = n_blk * BN;                       // rows of a tile never straddle records
+      // wait for the record that holds rows ar.. (the scales travel in it too).  A tile that starts at or past row M -- the
+      // pair kernel's second CTA when ceil(M / 128) is odd -- reads only zero-filled rows and neutral scales: no record
+      // holds them, so there is nothing to wait for (and no arrival word to read).
+      if (ar < g.M && !wait_record(g.a_ready, ar / g.a_rows_per_rec, g.ready_timeout_ns, &s.abort)) break;
       for (uint32_t kb = 0; kb < k_blks; ++kb) {
         const uint32_t sa = load_scales(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, ks, ar + t, kb);
         const uint32_t sb = load_scales(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, ks, br + t, kb);

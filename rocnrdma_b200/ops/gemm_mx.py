@@ -74,18 +74,22 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
     Any M and N; K a multiple of 32 (one MX block) and of 16 bytes.
     ``cta_group``: 2 = CTA-pair kernel (256 x 128 per 2-CTA cluster, B multicast: half the B traffic per FLOP), 1 = single-CTA kernel
     (128 x 128), 0 = pair for M > 128.  ``RN_MX_CTA_GROUP`` overrides (A/B switch).
-    ``a_ready``: receive-side fusion.  An int64 tensor with one word per 128-row panel of ``a`` (``a`` living in panel or chunk
-    records of a registered receive buffer); the kernel starts a tile only once the word of the panel it reads is nonzero --
-    ``ops.recv_consume(..., stamps=a_ready)`` sets it when the panel's receive completion arrives -- so the product overlaps
-    the transfer panel by panel.  Launch with a ``grid`` that leaves SMs for whatever produces the panels (a persistent
-    kernel spinning on all SMs would starve it)."""
+    ``a_ready``: receive-side fusion.  An int64 CUDA tensor with one word per record of ``a``, nonzero once that record has
+    landed (``a`` living in panel or chunk records of a registered receive buffer; a plain ``a`` is one record).  The
+    kernel starts a tile only once the word of the record it reads is nonzero, so the product overlaps the transfer record
+    by record.  ``ops.recv_consume(..., stamps=a_ready)`` produces exactly these words when every record arrives by
+    RDMA_WRITE_IMM with its index as the immediate: the chunk id for K3 records, the panel id for K4 records.  Launch with
+    a ``grid`` that leaves SMs for whatever produces the records (a persistent kernel spinning on all SMs would starve it)."""
     import os
     if os.environ.get("RN_MX_CTA_GROUP"):
         cta_group = int(os.environ["RN_MX_CTA_GROUP"])
     M, Nn, K = a.rows, b.rows, a.K
     assert b.K == K and c.dtype == torch.bfloat16 and tuple(c.shape) == (M, Nn) and c.is_contiguous()
     if a_ready is not None:
-        assert a_ready.dtype == torch.int64 and a_ready.numel() >= -(-M // PANEL_ROWS) and a_ready.is_cuda
+        n_rec = -(-M // (a.rows_per_rec or M))
+        if a_ready.dtype != torch.int64 or not a_ready.is_cuda or a_ready.numel() < n_rec:
+            raise ValueError(f"a_ready must be an int64 CUDA tensor with one word per record of a ({n_rec}), "
+                             f"got {a_ready.dtype} x {a_ready.numel()} on {a_ready.device}")
     lib = N.load()
     ws = work_stream(ctx, stream)
     out_addr, out_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)

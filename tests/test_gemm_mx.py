@@ -1,6 +1,8 @@
 """K7: the block-scaled fp8 GEMM (e4m3 wgmma, block scales applied in registers) against a PyTorch fp32 reference of the
 same op: dequantise both operands (e4m3 * 2^(scale - 127) per 32-element block), multiply in fp32.  The kernel's
 only rounding beyond that is fp32 accumulation order and the bf16 store."""
+import ctypes as C
+
 import pytest
 import torch
 
@@ -113,7 +115,10 @@ def test_mxfp8_consumes_chunk_records_of_the_fused_pack(ctx):
 def test_mxfp8_starts_tiles_as_their_panels_arrive(ctx):
     """Receive-side fusion on one GPU: GEMM 1's fp8 panels travel through the wire (RDMA_WRITE_IMM per panel), a consumer
     kernel stamps each arrival, and GEMM 2 -- launched BEFORE anything has arrived -- starts each tile when the panel it
-    reads is there.  Everything is resident at once (engine 16 SMs, GEMM 1 on 48, consumer 1, GEMM 2 on 64)."""
+    reads is there.  Everything is resident at once (engine 16 SMs, GEMM 1 on 48, consumer 1, GEMM 2 on 64: 129 of 132).
+    The receive buffer holds poison until a panel lands (e4m3 448 under scale 2^127), and the result must equal bit for
+    bit the same call made after every panel is in place: a tile that read its panel early changes bits.
+    tests/test_gpu_receive_fusion.py checks the same chain with exact operands at odd and ragged panel counts."""
     M, K1, N1, N2 = 1024, 512, 1024, 512
     p, q = _rand(M, K1, spread=False), _rand(N1, K1, spread=False)
     w = _rand(N2, N1)
@@ -121,8 +126,11 @@ def test_mxfp8_starts_tiles_as_their_panels_arrive(ctx):
     panels = M // 128
     nb = panels * ops.panel_record_bytes(N1)
     snd = torch.zeros(nb, dtype=torch.uint8, device="cuda")
-    rcv = torch.zeros(nb, dtype=torch.uint8, device="cuda")
-    stamps = torch.zeros(panels, dtype=torch.int64, device="cuda")
+    rcv = torch.full((panels, nb // panels), 0xFE, dtype=torch.uint8, device="cuda")
+    rcv[:, :128 * N1] = 0x7E
+    rcv = rcv.reshape(-1)
+    words = torch.zeros(panels + 8, dtype=torch.int64, device="cuda")     # zero words behind the arrival words
+    stamps = words[:panels]
     y = torch.zeros(M, N2, device="cuda", dtype=torch.bfloat16)
     sm, rm = ctx.reg_mr(snd), ctx.reg_mr(rcv)
     qp = ctx.loopback_qp(depth=64)
@@ -141,8 +149,14 @@ def test_mxfp8_starts_tiles_as_their_panels_arrive(ctx):
         ctx.engine_stop()
     assert r1.ok and r1.panels_posted == panels
     assert ops.parse_recv(view)["seen"] == panels
-    assert torch.all(stamps != 0)
+    assert torch.all(stamps != 0) and torch.all(words[panels:] == 0)
     assert torch.equal(snd, rcv)
+    status = (C.c_int64 * 8).from_buffer(out2)[0]                       # read before the next call reuses the slot
+    assert status == 0, f"on-arrival GEMM: {status}"
+    y_after = torch.zeros_like(y)
+    assert ops.gemm_mxfp8(ctx, MX.MxOperand.from_panel_records(rcv, M, N1), MX.MxOperand.from_tensors(wq, ws), y_after).ok
+    diff = (y.view(torch.int16) != y_after.view(torch.int16)).sum().item()
+    assert diff == 0, f"{diff} elements differ between the product on arrival and after arrival"
     xq = rcv.reshape(panels, -1)[:, :128 * N1].reshape(M, N1)
     xs = rcv.reshape(panels, -1)[:, 128 * N1:].reshape(M, N1 // 32)
     _check(y, xq, xs, wq, ws, N1)
