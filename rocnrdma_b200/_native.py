@@ -186,6 +186,7 @@ _SIGS = {
     "rn_verbs_dev_name": (C.c_char_p, [vp]),
     "rn_verbs_port_active": (i32, [vp]),
     "rn_verbs_link_layer": (i32, [vp]),
+    "rn_verbs_max_msg": (u32, [vp]),
     "rn_verbs_local_addr": (i32, [vp, C.POINTER(u16), C.POINTER(u8)]),
     "rn_verbs_reg_mr": (vp, [vp, u64, u64, i32, i32, u64, u32, C.POINTER(u32), C.POINTER(u32)]),
     "rn_verbs_dereg_mr": (i32, [vp]),
@@ -286,6 +287,15 @@ def load():
         _bind(lib, name, res, args, optional=True)
     _LIB = lib
     return lib
+
+
+def byte_count(n, what: str = "nbytes") -> int:
+    """``n`` as the 32-bit byte count the native entry points take: ``ValueError`` outside ``[0, 2**32)``, where ctypes
+    would silently wrap it to a shorter length.  (What fits but exceeds the maximum message length fails on the wire.)"""
+    n = int(n)
+    if not 0 <= n < 1 << 32:
+        raise ValueError(f"{what}={n}: a byte count must lie in [0, 2**32)")
+    return n
 
 
 def check(rc: int, what: str = ""):

@@ -264,6 +264,7 @@ class QueuePair:
     def _post(self, opcode, laddr, lkey, raddr, rkey, nbytes, signaled=True, imm=0, fence=False) -> int:
         idx = C.c_uint64()
         flags = _ctrl_flags(signaled, fence)
+        nbytes = N.byte_count(nbytes)
         self.ctx.sweep_revoked()          # a freed allocation must not be reachable through a stale key
         N.check(self.ctx._lib.rn_post_send(self._q, opcode, laddr, lkey, raddr, rkey, nbytes, flags, imm,
                                            C.byref(idx)), "post_send")
@@ -348,8 +349,9 @@ class QueuePair:
         return self._post_inline(W.OP_SEND if imm is None else W.OP_SEND_IMM, 0, 0, buf, signaled, imm or 0, fence)
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
-        """Post one receive buffer (consumed in order by SEND / WRITE_WITH_IMM)."""
-        n = dst.length - off if nbytes is None else nbytes
+        """Post one receive buffer (consumed in order by SEND / WRITE_WITH_IMM).  A buffer longer than
+        ``Context.max_msg_bytes`` holds any message."""
+        n = N.byte_count(dst.length - off if nbytes is None else nbytes)
         N.check(self.ctx._lib.rn_post_recv(self._q, dst.addr + off, dst.lkey, n), "post_recv")
 
     def set_flags(self, sys_scope: Optional[bool] = None, trace: Optional[bool] = None):
@@ -470,6 +472,7 @@ class VerbsQueuePair(QueuePair):
 
     def _post(self, opcode, laddr, lkey, raddr, rkey, nbytes, signaled=True, imm=0, fence=False) -> int:
         wr = C.c_uint64()
+        nbytes = N.byte_count(nbytes)
         self._vcheck(self.ctx._lib.rn_verbs_post_send(self._vq, opcode, laddr, lkey, raddr, rkey, nbytes, _verbs_flags(signaled, fence),
                                                       imm, C.byref(wr)), "post_send")
         return wr.value
@@ -494,7 +497,7 @@ class VerbsQueuePair(QueuePair):
         return wr.value
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
-        n = dst.length - off if nbytes is None else nbytes
+        n = N.byte_count(dst.length - off if nbytes is None else nbytes)
         self._vcheck(self.ctx._lib.rn_verbs_post_recv(self._vq, dst.addr + off, dst.lkey, n, None), "post_recv")
 
     def set_flags(self, sys_scope: Optional[bool] = None, trace: Optional[bool] = None):
@@ -577,6 +580,15 @@ class Context:
         sz = C.c_uint64()
         self._scratch_ptr = self._lib.rn_hca_scratch(self._h, C.byref(sz)) if self._h else 0
         self._scratch_size = sz.value
+
+    @property
+    def max_msg_bytes(self) -> int:
+        """The longest message, inclusive, a WRITE, WRITE_WITH_IMM, READ, SEND or SEND_WITH_IMM may carry: 2^30 bytes on
+        the software HCA, the port's ``max_msg_sz`` on the verbs wire.  A longer one completes with ``LOCAL_LENGTH_ERR``
+        and moves nothing; a byte count outside ``[0, 2**32)`` is refused with ``ValueError`` before it is posted."""
+        if self._vdev:
+            return int(self._lib.rn_verbs_max_msg(self._vdev))
+        return W.MAX_MSG
 
     @property
     def aux_stream(self):
@@ -757,7 +769,7 @@ class Context:
 
     def create_qp(self, scq: CompletionQueue, rcq: Optional[CompletionQueue] = None, sq_depth: int = 256,
                   rq_depth: int = 256, sq_mem: int = W.MEM_DEVICE, chunk_bytes: int = 512 << 10) -> QueuePair:
-        """``ibv_create_qp`` (RC).  ``sq_mem`` places the rings and doorbells in device memory (posted by kernels) or pinned host memory (posted by the CPU); ``chunk_bytes`` is the engine's minimum work granule for this QP."""
+        """``ibv_create_qp`` (RC).  ``sq_mem`` places the rings and doorbells in device memory (posted by kernels) or pinned host memory (posted by the CPU); ``chunk_bytes`` is the engine's minimum work granule for this QP: a multiple of 16, at most ``max_msg_bytes``."""
         q = C.c_void_p()
         rcq = rcq or scq
         if self.wire == "verbs":
@@ -767,7 +779,8 @@ class Context:
             qp = VerbsQueuePair(self, vq, scq, rcq, sq_depth, rq_depth, sq_mem)
             self._vqps.append(qp)
             return qp
-        N.check(self._lib.rn_create_qp(self._h, scq._c, rcq._c, sq_depth, rq_depth, sq_mem, chunk_bytes, C.byref(q)),
+        N.check(self._lib.rn_create_qp(self._h, scq._c, rcq._c, sq_depth, rq_depth, sq_mem,
+                                       N.byte_count(chunk_bytes, "chunk_bytes"), C.byref(q)),
                 "create_qp")
         return QueuePair(self, q, scq, rcq, sq_depth, rq_depth, sq_mem)
 

@@ -359,6 +359,10 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
     p->syn = SYN_LOCAL_QP_OP_ERR;
   } else if (!qp->r.connected && v.opcode != OP_NOP) {
     p->syn = SYN_LOCAL_QP_OP_ERR;
+  } else if (v.bytes > MAX_MSG) {
+    // over-long message, before any key is looked at (DESIGN.md 3.1); a NOP decodes to 0 bytes and an atomic of more
+    // than 8 bytes fails with this syndrome anyway
+    p->syn = SYN_LOCAL_LENGTH_ERR;
   } else {
     switch (v.opcode) {
       case OP_NOP: v.bytes = 0; break;

@@ -582,6 +582,8 @@ RN_API int rn_create_qp(void* hca, void* scq, void* rcq, uint32_t nsq, uint32_t 
   if (h->qps.size() >= h->max_qps) return fail(-12, "create_qp: QP table full");
   if (chunk_bytes == 0) chunk_bytes = 512u << 10;
   if (chunk_bytes & 15) return fail(-22, "create_qp: chunk_bytes must be a multiple of 16");
+  // A granule longer than the longest message means nothing; bounded by it, the engine's granule sums stay below 2^31.
+  if (chunk_bytes > MAX_MSG) return fail(-22, "create_qp: chunk_bytes must not exceed the maximum message length (2^30)");
   bool host = sq_mem == MEM_HOST_PINNED;
   Qp* q = new Qp();
   q->hca = h; q->sq_mem = sq_mem; q->scq = (Cq*)scq; q->rcq = (Cq*)rcq;

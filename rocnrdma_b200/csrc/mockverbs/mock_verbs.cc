@@ -427,6 +427,8 @@ bool nic_execute(MockQp* qp, uint64_t w) {
     syn = rn::SYN_WR_FLUSH_ERR;
   } else if (!ok || v.qpn != qp->v.qp_num || v.wqe_idx != (uint16_t)w) {
     syn = rn::SYN_LOCAL_QP_OP_ERR;
+  } else if (v.bytes > rn::MAX_MSG) {            // the max_msg_sz ibv_query_port reports
+    syn = rn::SYN_LOCAL_LENGTH_ERR;                // over-long message, before any key or the peer (DESIGN.md 3.1)
   } else if (v.opcode == rn::OP_NOP) {
   } else if (!peer || (peer->v.state != IBV_QPS_RTR && peer->v.state != IBV_QPS_RTS)) {
     syn = rn::SYN_TRANSPORT_RETRY_EXC_ERR;        // nobody answers: what a dead peer looks like on RC
@@ -792,7 +794,7 @@ MOCK_API int ibv_query_port(ibv_context* c, uint8_t port, ibv_port_attr* a) {
   if (port != 1) return EINVAL;
   MockDev* dev = reinterpret_cast<MockCtx*>(c)->dev;
   a->state = IBV_PORT_ACTIVE; a->max_mtu = IBV_MTU_4096; a->active_mtu = IBV_MTU_4096; a->gid_tbl_len = 8;
-  a->port_cap_flags = 0; a->max_msg_sz = 1u << 30; a->bad_pkey_cntr = 0; a->qkey_viol_cntr = 0; a->pkey_tbl_len = 1;
+  a->port_cap_flags = 0; a->max_msg_sz = rn::MAX_MSG; a->bad_pkey_cntr = 0; a->qkey_viol_cntr = 0; a->pkey_tbl_len = 1;
   a->lid = dev->lid; a->sm_lid = 1; a->lmc = 0; a->max_vl_num = 4; a->sm_sl = 0; a->subnet_timeout = 18; a->init_type_reply = 0;
   a->active_width = 2 /* 4x */; a->active_speed = 128 /* NDR */; a->phys_state = 5 /* LinkUp */;
   a->link_layer = IBV_LINK_LAYER_INFINIBAND; a->flags = 0;

@@ -296,6 +296,7 @@ RN_API int rn_verbs_close(void* dev) {
 RN_API const char* rn_verbs_dev_name(void* dev) { return ((Dev*)dev)->name; }
 RN_API int rn_verbs_port_active(void* dev) { return ((Dev*)dev)->pattr.state == IBV_PORT_ACTIVE; }
 RN_API int rn_verbs_link_layer(void* dev) { return ((Dev*)dev)->pattr.link_layer; }
+RN_API uint32_t rn_verbs_max_msg(void* dev) { return ((Dev*)dev)->pattr.max_msg_sz; }
 RN_API int rn_verbs_local_addr(void* dev, uint16_t* lid, uint8_t* gid16) {
   Dev* d = (Dev*)dev;
   *lid = d->pattr.lid;

@@ -45,6 +45,8 @@ enum : uint32_t {
   CQE_SIZE = 64,
   MAX_INLINE = 28,   // largest inline payload: ctrl + raddr + a 4-byte inline header + 28 bytes fill one WQEBB
   INLINE_SEG = 0x80000000u,   // byte_count flag: the payload follows in the WQE itself
+  MAX_BYTE_COUNT = 0x7fffffffu,   // largest byte count a gather data segment carries (bit 31 is INLINE_SEG)
+  MAX_MSG = 1u << 30,         // longest message, inclusive (DESIGN.md 3.1); longer WRITE / READ / SEND: LOCAL_LENGTH_ERR
 };
 
 enum Opcode : uint8_t {  // ctrl.opmod_idx_opcode[7:0]
@@ -220,8 +222,11 @@ RN_HD void encode_raddr(RaddrSeg* r, uint64_t raddr, uint32_t rkey) {
   r->rkey = be32(rkey);
   r->reserved = 0;
 }
+// A byte count the segment cannot carry saturates, so it reaches the HCA as longer than MAX_MSG and fails there; masking
+// it would post a shorter, valid message.
+RN_HD uint32_t data_byte_count(uint32_t bytes) { return bytes > MAX_BYTE_COUNT ? MAX_BYTE_COUNT : bytes; }
 RN_HD void encode_data(DataSeg* d, uint64_t addr, uint32_t lkey, uint32_t bytes) {
-  d->byte_count = be32(bytes & 0x7fffffffu);
+  d->byte_count = be32(data_byte_count(bytes));
   d->lkey = be32(lkey);
   d->addr = be64(addr);
 }
@@ -462,9 +467,10 @@ RN_HD uint16_t wq_dbr_index(uint32_t rec) { return (uint16_t)be32(rec); }
 RN_HD uint32_t cq_dbr_word(uint32_t ci) { return be32(ci & 0xffffff); }
 RN_HD uint32_t cq_dbr_index(uint32_t rec) { return be32(rec) & 0xffffff; }
 
-// A receive WQE: one data segment (what encode_data writes) per 16-byte stride.
+// A receive WQE: one data segment (what encode_data writes) per 16-byte stride.  A buffer longer than the segment can
+// say saturates too: it still holds any message.
 RN_HD Words16 recv_wqe_words(uint64_t addr, uint32_t lkey, uint32_t bytes) {
-  return Words16{be32(bytes & 0x7fffffffu), be32(lkey), be32((uint32_t)(addr >> 32)), be32((uint32_t)addr)};
+  return Words16{be32(data_byte_count(bytes)), be32(lkey), be32((uint32_t)(addr >> 32)), be32((uint32_t)addr)};
 }
 RN_HD uint32_t recv_wqe_bytes(const Words16& d) { return be32(d.x) & 0x7fffffffu; }
 RN_HD uint32_t recv_wqe_lkey(const Words16& d) { return be32(d.y); }

@@ -80,7 +80,10 @@ def rdma_stream(qps, opcode: int, src_mr, dst_mr, nbytes: int, iters: int = 1, w
     For RDMA_READ ``src_mr`` is the local destination and ``dst_mr`` the remote source,
     mirroring the laddr/raddr roles in the WQE.  ``post_only`` skips the final completion wait (``iters`` must fit
     the window): the work is reaped later -- by ``Context.engine_run_oneshot`` under a profiler, or by the caller.
+    A work request longer than ``Context.max_msg_bytes`` completes with ``LOCAL_LENGTH_ERR`` (status ``CQE_ERROR``);
+    ``nbytes`` outside ``[0, 2**32)`` raises ``ValueError``.
     """
+    nbytes = N.byte_count(nbytes)
     lib = N.load()
     if not isinstance(qps, (list, tuple)):
         qps = [qps]
@@ -118,7 +121,9 @@ def write_read(qp, src_mr, dst_mr, back_mr, nbytes: int, iters: int = 1, mode: s
     completion each time.  ``mode`` says how the READ is kept behind the WRITE: ``"fenced"`` posts both under one doorbell
     with the READ fenced; ``"wait"`` waits for the WRITE's completion before posting the READ (the only way without the
     fence); ``"one_call"`` posts them with ``dev::rdma_write`` and ``dev::rdma_read(..., fence=true)``.  Returns
-    ``dict(status, done, device_ns, mean_ns, min_ns)`` (per pair: post to the READ's completion)."""
+    ``dict(status, done, device_ns, mean_ns, min_ns)`` (per pair: post to the READ's completion).  ``nbytes`` as in
+    :func:`rdma_stream`."""
+    nbytes = N.byte_count(nbytes)
     ctx = qp.ctx
     ws = work_stream(ctx, stream)
     out_addr, out_view = ctx.scratch(64, offset=scratch_off)
@@ -257,7 +262,8 @@ def put_signal(qp, src_mr, dst_mr, nbytes: int, sig_mr, sig_off: int = 0, fetch_
     values go to ``fetch_mr`` (message ``i`` at ``(i % (fetch_mr.length // 8)) * 8``); by default to a small buffer the
     context registers the first time it is needed -- pass ``fetch_mr`` when the engine is already running, since a
     first allocation then waits for it.  ``window`` bounds the messages in flight (0: the send queue does).  Returns a
-    :class:`StreamResult` (``us_per_msg`` = device time per message)."""
+    :class:`StreamResult` (``us_per_msg`` = device time per message).  ``nbytes`` as in :func:`rdma_stream`."""
+    nbytes = N.byte_count(nbytes)
     lib = N.load()
     ctx = qp.ctx
     if fetch_mr is None:

@@ -14,6 +14,8 @@ WQEBB = 64
 CQE_SIZE = 64
 MAX_INLINE = 28            # largest inline payload: ctrl + raddr + a 4-byte inline header + 28 bytes fill one WQEBB
 INLINE_SEG = 0x80000000    # byte_count flag of an inline data segment
+MAX_BYTE_COUNT = 0x7FFFFFFF  # largest byte count a gather data segment carries
+MAX_MSG = 1 << 30          # longest message, inclusive; a longer WRITE / READ / SEND completes with LOCAL_LENGTH_ERR
 
 OP_NOP = 0x00
 OP_SEND_INVAL = 0x01
@@ -66,7 +68,9 @@ def raddr_seg(raddr: int, rkey: int) -> bytes:
 
 
 def data_seg(addr: int, lkey: int, nbytes: int) -> bytes:
-    return struct.pack(">IIQ", nbytes & 0x7FFFFFFF, lkey, addr)
+    """A gather data segment.  A byte count past ``MAX_BYTE_COUNT`` saturates (it then fails as over-long, rather than
+    reaching the HCA as a shorter valid message)."""
+    return struct.pack(">IIQ", min(nbytes, MAX_BYTE_COUNT), lkey, addr)
 
 
 def rdma_wqe(opcode, wqe_idx, qpn, laddr, lkey, raddr, rkey, nbytes, fm_ce_se=CTRL_CQ_UPDATE, imm=0) -> bytes:

@@ -11,6 +11,9 @@ The model is plain Python and numpy and is written from the contract in DESIGN.m
   included.  SEND and WRITE_IMM consume receives in order; a WR that fails a requester-side check consumes none.
 * Atomics execute in WR order and see every byte written by earlier WRITEs of the QP.
 * Zero-length WRITE, WRITE_IMM and READ check no key and move nothing (WRITE_IMM still consumes a receive).
+* A WRITE, WRITE_IMM, READ, SEND or SEND_IMM longer than the maximum message length (2^30 bytes, inclusive) fails with
+  LOCAL_LENGTH_ERR before any key is looked at: it moves nothing and consumes no receive.  ``cfg["max_msg"]`` (that
+  length) makes the generator build such WRs (fault ``too_long``); without it the programs are what they always were.
 
 Programs address memory as (MR name, offset from the MR's start), so the runner only has to turn MR names into keys and
 addresses; the model itself never sees a pointer.  Every buffer base is 16-byte aligned, so an offset's residue mod 16 is
@@ -34,6 +37,13 @@ ACC_ALL = 15
 NO_LOCAL_WRITE = ACC_REMOTE_READ
 RDMA_OPS = ("WRITE", "WRITE_IMM", "READ")
 RECV_OPS = ("SEND", "SEND_IMM", "WRITE_IMM")
+MSG_OPS = ("WRITE", "WRITE_IMM", "READ", "SEND", "SEND_IMM")
+MAX_MSG = 1 << 30
+
+
+def too_long_lengths(max_msg):
+    """Byte counts past the maximum message length: just past it, and where a 31-bit byte count would wrap."""
+    return [max_msg + 1, max_msg + 16, 2**31 - 1, 2**31, 2**31 + 64, 2**32 - 16]
 
 
 def _chunks(nbytes, ctas, chunk_bytes):
@@ -165,6 +175,7 @@ def run_model(prog: Program, host_native_atomics: bool = True, resolve_cas: bool
     With ``resolve_cas`` a CS whose compare is still None gets one that hits (``cas_hit``) or misses the word's current
     value: that is how the generator makes half of the CAS succeed."""
     cfg = prog.cfg
+    max_msg = cfg.get("max_msg") or MAX_MSG
     mem = {k: b.init.copy() for k, b in prog.bufs.items()}
     out = Outcome(mem, [QpOutcome() for _ in prog.qps])
 
@@ -184,7 +195,9 @@ def run_model(prog: Program, host_native_atomics: bool = True, resolve_cas: bool
                 continue
             syn, nbytes = None, w.n
             recv_taken = None
-            if w.op == "NOP":
+            if w.op in MSG_OPS and w.n > max_msg:
+                syn = "LOCAL_LENGTH_ERR"                # before any key, and before a receive is matched
+            elif w.op == "NOP":
                 nbytes = 0
             elif w.op in RDMA_OPS and w.n == 0:
                 # zero-length RDMA: no key is looked at, nothing moves; WRITE_IMM still needs and takes a receive
@@ -358,7 +371,7 @@ def generate(seed: int, cfg: dict) -> Program:
         fault_at = int(rng.integers(0, n_wr)) if fault_prog else -1
         fault_kind = None
         if fault_prog:
-            kinds = [f for f in FAULTS if not (verbs and f == "atomic_len4")]
+            kinds = [f for f in FAULTS if not (verbs and f == "atomic_len4")] + ["too_long"] * (len(FAULTS) if cfg.get("max_msg") else 0)
             fault_kind = kinds[int(rng.integers(0, len(kinds)))]
         exact_fits = 0 if fault_prog else int(rng.integers(1, 4))
         exact_at = set(int(x) for x in rng.choice(n_wr, size=min(exact_fits, n_wr), replace=False)) if exact_fits else set()
@@ -395,6 +408,8 @@ def generate(seed: int, cfg: dict) -> Program:
                 op = str(rng.choice(["READ", "FA"]))
             elif fault in ("send_too_long", "recv_no_local_write"):
                 op = str(rng.choice(["SEND", "SEND_IMM", "ISEND"]))
+            elif fault == "too_long":
+                op = str(rng.choice(MSG_OPS))
             elif exact:
                 op = str(rng.choice(["WRITE", "READ", "SEND"]))
             if rnr_prog and i == n_wr - 1:
@@ -446,6 +461,16 @@ def generate(seed: int, cfg: dict) -> Program:
                 elif fault == "remote_past_end":
                     w.rmr = new_mr("atom7", p + "ATOM", 8 * word, 7, ACC_ALL, "remote")
                     w.roff = 0
+            elif fault == "too_long":
+                # far longer than its MRs, which the length-first rule makes harmless: nothing may be looked at or moved
+                w.n = int(rng.choice(too_long_lengths(cfg["max_msg"])))
+                if base == "READ":
+                    w.lmr, w.loff = p + "dst_l", dst.take(64) - 64
+                    w.rmr, w.roff = p + "src_r", src_off(64)
+                else:
+                    w.lmr, w.loff = p + "src_l", src_off(64)
+                    if base.startswith("WRITE"):
+                        w.rmr, w.roff = p + "dst_r", dst.take(64) - 64
             else:
                 n = pick_len(min(cfg["max_len"], max(1, big_left)))
                 if exact or fault:
@@ -511,7 +536,7 @@ def generate(seed: int, cfg: dict) -> Program:
                     w.bad_rkey = True
             # its receive, on the responder's queue
             if base in RECV_OPS and not (rnr_prog and i == n_wr - 1):
-                if base == "WRITE_IMM":
+                if base == "WRITE_IMM" or fault == "too_long":
                     recvs.append(Recv(p + "rcv", dst.take(16) - 64, 16))
                 else:
                     if fault == "send_too_long":

@@ -5,7 +5,8 @@ The software HCA runs a covering set of configs: engine CTAs, the plain or the p
 queues and data in device or pinned host memory, and everything pre-posted before a one-shot engine (batched claims) or
 posted while the engine runs (single claims).  Besides bytes, completions and QP state, each run checks that the engine
 left cleanly and moved exactly the number of bulk chunks the model predicts, so a program provably went down the copy
-paths it was generated for.  The mock ConnectX runs the same kind of programs with its data in HBM.  ``RN_RC_SEED=<n>`` replays one seed; ``RN_RC_SOAK=<n>`` runs n seeds per config."""
+paths it was generated for.  Every config also builds WRs longer than the maximum message length (``cfg["max_msg"]``),
+which must fail before any key is looked at.  The mock ConnectX runs the same kind of programs with its data in HBM.  ``RN_RC_SEED=<n>`` replays one seed; ``RN_RC_SOAK=<n>`` runs n seeds per config."""
 import time
 
 import pytest
@@ -45,7 +46,7 @@ def test_softhca_matches_the_model(monkeypatch, ctas, prof, chunk, qmem, dmem, o
     else:
         monkeypatch.delenv("RN_ENGINE_PROFILE", raising=False)
     cfg = {"wire": "softhca", "max_wrs": 150, "max_len": 4 << 20, "big_budget": 12 << 20, "ctas": ctas,
-           "chunk_bytes": chunk, "data_mem": dmem, "allow_rnr": not oneshot}
+           "chunk_bytes": chunk, "data_mem": dmem, "allow_rnr": not oneshot, "max_msg": M.MAX_MSG}
     t0 = time.monotonic()
     bulk = 0
     for seed in _seeds(4, 1000 * CONFIGS.index((ctas, prof, chunk, qmem, dmem, oneshot))):
@@ -55,6 +56,6 @@ def test_softhca_matches_the_model(monkeypatch, ctas, prof, chunk, qmem, dmem, o
 
 
 def test_mock_connectx_matches_the_model_on_hbm():
-    cfg = {"wire": "verbs", "max_wrs": 100, "max_len": 1 << 20, "big_budget": 4 << 20, "allow_rnr": True}
+    cfg = {"wire": "verbs", "max_wrs": 100, "max_len": 1 << 20, "big_budget": 4 << 20, "allow_rnr": True, "max_msg": M.MAX_MSG}
     for seed in _seeds(6, 50_000):
         M.check_seed(seed, cfg, lambda: M.VerbsWire(device=0))

@@ -121,6 +121,20 @@ def test_one_syndrome_per_fault_class():
     assert _req(o) == [(0, "OK", 8)]
 
 
+def test_too_long_fails_before_any_key_and_takes_no_receive():
+    """Longer than the maximum message length: LOCAL_LENGTH_ERR even with bad keys and an MR far too short, nothing moves,
+    the receive stays for later, and the next WR is flushed.  The limit itself is a legal length."""
+    for op in M.MSG_OPS:
+        for n in M.too_long_lengths(M.MAX_MSG):
+            w = WR(op, n, "dst" if op == "READ" else "src", 0, None if op.startswith("SEND") else ("src" if op == "READ" else "dst"),
+                   0, bad_lkey=True, bad_rkey=True)
+            o = M.run_model(_prog([w, WR("WRITE", 4, "src", 0, "dst", 0)], recvs=[Recv("dst", 0, 48)]))
+            assert _req(o) == [(0, "LOCAL_LENGTH_ERR"), (1, "WR_FLUSH_ERR")], (op, n)
+            assert _resp(o) == [] and not o.mem["DST"].any()
+    o = M.run_model(_prog([WR("SEND", M.MAX_MSG, "src", 0)], recvs=[Recv("dst", 0, 48)]))
+    assert _req(o) == [(0, "LOCAL_PROT_ERR")]        # at the limit the length passes and the key check fails
+
+
 def test_mr_edges():
     """An access ending at the MR's last byte succeeds; one byte more is a remote access error; canaries stay."""
     ok = M.run_model(_prog([WR("WRITE", 16, "src", 0, "dst", 32)]))
@@ -141,14 +155,13 @@ def test_bulk_chunk_prediction():
     assert M.bulk_chunks(4097, 0, 0, 1, 1 << 16) == 0                     # length not a multiple of 16
 
 
-@pytest.mark.parametrize("wire", ["verbs", "softhca"])
-def test_generated_programs_keep_their_promises(wire):
-    """Write targets never overlap each other or a source, a fault program fails exactly once where it was built to,
-    and the generator reaches every fault class, exact fits, atomics on written words and zero-length RDMA."""
+def _check_promises(wire, extra):
+    """Write targets never overlap each other or a source, a fault program fails exactly once where it was built to;
+    returns the fault classes and special cases the programs reached."""
     seen = set()
     for seed in range(150):
         p = M.generate(seed, {"wire": wire, "max_wrs": 60, "max_len": 1 << 18, "big_budget": 1 << 20, "allow_rnr": True,
-                              "ctas": 3, "chunk_bytes": (20 << 10) + 16})
+                              "ctas": 3, "chunk_bytes": (20 << 10) + 16, **extra})
         o = M.run_model(p)
         for qi, (qp, q) in enumerate(zip(p.qps, o.qps)):
             faults = [i for i, w in enumerate(qp.wrs) if w.fault]
@@ -169,12 +182,31 @@ def test_generated_programs_keep_their_promises(wire):
                     seen.add("zero_length_bad_keys")
                 if w.rmr and "dstfit" in w.rmr and not w.fault:
                     seen.add("exact_fit")
+                if w.fault == "too_long":
+                    assert w.n > M.MAX_MSG and w.op in M.MSG_OPS, (seed, qi, i)
+                    seen.add(("too_long", w.op))
+    return seen
+
+
+@pytest.mark.parametrize("wire", ["verbs", "softhca"])
+def test_generated_programs_keep_their_promises(wire):
+    """... and the generator reaches every fault class, exact fits, atomics on written words and zero-length RDMA."""
+    seen = _check_promises(wire, {})
     want = set(M.FAULTS) - ({"atomic_len4"} if wire == "verbs" else set())
     assert want | {"zero_length_bad_keys", "exact_fit"} <= seen, sorted(want - seen)
+    assert not any(isinstance(x, tuple) for x in seen)           # no over-long WR unless asked for
+
+
+@pytest.mark.parametrize("wire", ["verbs", "softhca"])
+def test_generated_programs_with_max_msg_reach_every_too_long_opcode(wire):
+    seen = _check_promises(wire, {"max_msg": M.MAX_MSG})
+    want = {("too_long", op) for op in M.MSG_OPS}
+    assert want <= seen, sorted(want - seen)
 
 
 # ---------------------------------------------------------------------------------------------------------------- the mock ConnectX
 MOCK_CFG = {"wire": "verbs", "max_wrs": 60, "max_len": 1 << 18, "big_budget": 1 << 20, "allow_rnr": True}
+MAX_MSG_EVERY = 3      # every third seed also builds over-long WRs (cfg["max_msg"])
 
 
 @pytest.fixture(scope="module")
@@ -194,7 +226,8 @@ def _seeds(n):
 def test_mock_connectx_matches_the_model_on_host_dram(verbs_lib):
     checked = 0
     for seed in _seeds(120):
-        M.check_seed(seed, MOCK_CFG, lambda: M.VerbsWire(device=None))
+        cfg = dict(MOCK_CFG, max_msg=M.MAX_MSG) if seed % MAX_MSG_EVERY == MAX_MSG_EVERY - 1 else MOCK_CFG
+        M.check_seed(seed, cfg, lambda: M.VerbsWire(device=None))
         checked += 1
     assert checked >= 1
 

@@ -101,6 +101,22 @@ def test_native_encoder_matches_python_mirror():
     assert bytes(buf) == W.send_wqe(W.OP_SEND, 3, 0x100, 0x1000, 0x5, 100)
 
 
+@pytest.mark.parametrize("nb", [W.MAX_MSG, W.MAX_MSG + 1, 2**31 - 1, 2**31, 2**31 + 64, 2**32 - 16, 2**32 - 1])
+@pytest.mark.parametrize("op", [W.OP_RDMA_WRITE, W.OP_RDMA_READ, W.OP_SEND])
+def test_byte_counts_past_31_bits_saturate(op, nb):
+    """A byte count the data segment cannot carry is posted as 2^31 - 1 -- longer than any message, so it fails at the
+    HCA -- never as its low 31 bits (2^31 + 64 would be a valid 64-byte message, 2^31 an empty one).  Both encoders."""
+    from rocnrdma_b200 import _native as N
+    lib = N.load()
+    buf = (C.c_uint8 * 64)()
+    lib.rn_wire_build_wqe(buf, op, 1, 0x100, 0x1000, 0x5, 0x2000, 0x6, nb, W.CTRL_CQ_UPDATE, 0)
+    want = (W.send_wqe(op, 1, 0x100, 0x1000, 0x5, nb) if op == W.OP_SEND else
+            W.rdma_wqe(op, 1, 0x100, 0x1000, 0x5, 0x2000, 0x6, nb))
+    assert bytes(buf) == want
+    sent = W.decode_wqe(bytes(buf)).nbytes
+    assert sent == min(nb, W.MAX_BYTE_COUNT) and (sent > W.MAX_MSG) == (nb > W.MAX_MSG)
+
+
 @pytest.mark.parametrize("op", [W.CQE_REQ, W.CQE_RESP_WR_IMM, W.CQE_RESP_SEND, W.CQE_RESP_SEND_IMM, W.CQE_REQ_ERR,
                                 W.CQE_RESP_ERR])
 def test_native_cqe_encoder_matches_python_mirror(op):

@@ -1,5 +1,6 @@
 """Property tests (hypothesis): the C encoders / decoders the engine and the posters use (csrc/wire/mlx5_wire.h,
-reached through the CPU test hooks) agree with the Python mirror on EVERY field value, not just on hand-picked ones."""
+reached through the CPU test hooks) agree with the Python mirror on EVERY field value, not just on hand-picked ones.
+Byte counts range over all 32 bits: one the data segment cannot carry saturates at 2^31 - 1 in both encoders."""
 import ctypes as C
 
 import pytest
@@ -22,28 +23,30 @@ def lib():
 
 
 @settings(max_examples=300, deadline=None)
-@given(op=rdma_ops, idx=u16, qpn=u24, la=u64, lk=u32, ra=u64, rk=u32, nb=u31, fl=flags, imm=u32)
+@given(op=rdma_ops, idx=u16, qpn=u24, la=u64, lk=u32, ra=u64, rk=u32, nb=st.one_of(u31, u32), fl=flags, imm=u32)
 def test_rdma_wqe_bytes_and_roundtrip(lib, op, idx, qpn, la, lk, ra, rk, nb, fl, imm):
     buf = (C.c_uint8 * 64)()
     lib.rn_wire_build_wqe(buf, op, idx, qpn, la, lk, ra, rk, nb, fl, imm)
     raw = bytes(buf)
     assert raw == W.rdma_wqe(op, idx, qpn, la, lk, ra, rk, nb, fl, imm)
     v = W.decode_wqe(raw)
-    assert (v.opcode, v.wqe_idx, v.qpn, v.laddr, v.lkey, v.raddr, v.rkey, v.nbytes, v.fm_ce_se) == (op, idx, qpn, la, lk, ra, rk, nb, fl)
+    assert (v.opcode, v.wqe_idx, v.qpn, v.laddr, v.lkey, v.raddr, v.rkey, v.fm_ce_se) == (op, idx, qpn, la, lk, ra, rk, fl)
+    assert v.nbytes == min(nb, W.MAX_BYTE_COUNT)
     assert v.ds == 3
     if op == W.OP_RDMA_WRITE_IMM:
         assert v.imm == imm
 
 
 @settings(max_examples=200, deadline=None)
-@given(op=send_ops, idx=u16, qpn=u24, la=u64, lk=u32, nb=u31, fl=flags, imm=u32)
+@given(op=send_ops, idx=u16, qpn=u24, la=u64, lk=u32, nb=st.one_of(u31, u32), fl=flags, imm=u32)
 def test_send_wqe_bytes_and_roundtrip(lib, op, idx, qpn, la, lk, nb, fl, imm):
     buf = (C.c_uint8 * 64)()
     lib.rn_wire_build_wqe(buf, op, idx, qpn, la, lk, 0, 0, nb, fl, imm)
     raw = bytes(buf)
     assert raw == W.send_wqe(op, idx, qpn, la, lk, nb, fl, imm)
     v = W.decode_wqe(raw)
-    assert (v.opcode, v.wqe_idx, v.qpn, v.laddr, v.lkey, v.nbytes, v.fm_ce_se, v.ds) == (op, idx, qpn, la, lk, nb, fl, 2)
+    assert (v.opcode, v.wqe_idx, v.qpn, v.laddr, v.lkey, v.nbytes, v.fm_ce_se, v.ds) == (op, idx, qpn, la, lk, min(nb, W.MAX_BYTE_COUNT),
+                                                                                        fl, 2)
 
 
 good_cqe_ops = st.sampled_from([W.CQE_REQ, W.CQE_RESP_WR_IMM, W.CQE_RESP_SEND, W.CQE_RESP_SEND_IMM])

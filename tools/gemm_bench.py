@@ -45,7 +45,7 @@ for (M, N, K) in shapes:
             with torch.cuda.stream(ctx.stream):
                 ev[0].record()
                 ops.gemm_send(ctx, a, b, c, grid=grid, sync=False)
-                ops.rdma_stream(qp, W.OP_RDMA_WRITE, cm, dm, min(2 * M * N, (1 << 31) - 65536), iters=1, sync=False)
+                ops.rdma_stream(qp, W.OP_RDMA_WRITE, cm, dm, min(2 * M * N, ctx.max_msg_bytes), iters=1, sync=False)
                 ev[1].record(); ev[1].synchronize()
             unf_us = min(unf_us, ev[0].elapsed_time(ev[1]) * 1e3)
         ctx.engine_stop()
