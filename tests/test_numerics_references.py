@@ -1,6 +1,6 @@
 """CPU checks of the fp8 references' edge rules (NaN, +-Inf, scale bytes 0x00 / 0xFF), of their finite behaviour against
-the formulas they had before the rules were added, and of the stream-K schedule model the GPU numerics tests choose
-their cases with."""
+the formulas they had before the rules were added, and of the schedule models (stream-K, and both GEMMs' tile loops) the
+GPU numerics tests choose their cases with."""
 import itertools
 
 import pytest
@@ -9,6 +9,7 @@ import torch
 from rocnrdma_b200.ops import gemm as G
 from rocnrdma_b200.ops import gemm_mx as MX
 from rocnrdma_b200.ops import pack as P
+from test_gpu_gemm_scale import K4_SCALE_CASES, K7_SCALE_CASES, Schedule
 from test_gpu_numerics import STREAM_K_CASES, StreamK
 
 NAN, INF = float("nan"), float("inf")
@@ -172,3 +173,67 @@ def test_stream_k_flag_is_not_the_same_as_a_split():
     every tail tile runs whole on one cluster."""
     m = StreamK(1024, 768, 128, 10, 1)
     assert m.stream_k and m.n_tail == m.R and not m.split_tiles()
+
+
+# ------------------------------------------------------------------ both GEMMs' tile schedules (launch rule + tile loop)
+def test_schedule_model_hand_counted_k4():
+    # one CTA per 128 x 256 tile, 4096^3 on 132 SMs: 32 x 16 = 512 tiles, 512 = 3 * 132 + 116; k_blks = 64 = 3 * 21 + 1, so
+    # a unit's tiles enter the 3-stage ring at stages 0, 1, 2, 0
+    s = Schedule("k4", 4096, 4096, 4096, 1, 0)
+    assert (s.grid, s.n_units, s.n_tiles, s.k_blks) == (132, 132, 512, 64)
+    assert [len(u) for u in s.units].count(4) == 116 and [len(u) for u in s.units].count(3) == 16
+    assert s.units[0] == [(0, 0, 64), (132, 0, 64), (264, 0, 64), (396, 0, 64)]
+    assert s.entry_stages()[:3] == [1, 2, 0]
+    # pair kernel at grid 13: 12 CTAs, 6 units; 8192 x 8192 pair tiles: 32 x 32 = 1024 = 170 * 6 + 4; k_blks 32 = 3 * 10 + 2
+    s = Schedule("k4", 8192, 8192, 2048, 2, 13)
+    assert (s.grid, s.n_units, s.ctas) == (12, 6, 2)
+    assert [len(u) for u in s.units] == [171] * 4 + [170] * 2
+    assert s.entry_stages()[:3] == [2, 1, 0] and not s.stream_k
+    # grid clamps: past the SM count -> SMs; never more CTAs than tiles (pairs: 2 per tile); a grid of 1 is the 1-CTA kernel
+    assert Schedule("k4", 300, 512, 64, 1, 200).grid == 6
+    assert (Schedule("k4", 256, 256, 64, 2, 0).grid, Schedule("k4", 256, 256, 64, 2, 0).n_units) == (2, 1)
+    assert Schedule("k4", 512, 256, 64, 2, 1).ctas == 1
+    # stream-K, 4096^3 at grid 13: 256 pair tiles = 42 * 6 + 4, the 4 * 64 tail k-blocks dealt in shares of 42 or 43: unit 0
+    # owns tile 252's first 42 k-blocks; unit 1 finishes tile 252 (22) and starts 253 (21)
+    s = Schedule("k4", 4096, 4096, 4096, 3, 13, stream_k=True)
+    assert s.stream_k and s.n_units == 6
+    assert s.units[0][42:] == [(252, 0, 42)] and s.units[1][42:] == [(252, 42, 64), (253, 0, 21)]
+    assert s.max_tiles_per_unit() == 44
+    # without stream-K the same launch leaves the 4 tail tiles whole on units 0..3
+    s = Schedule("k4", 4096, 4096, 4096, 3, 13)
+    assert not s.stream_k and s.units[3][-1] == (255, 0, 64) and len(s.units[4]) == 42
+
+
+def test_schedule_model_hand_counted_k7():
+    # 128 x 128 tiles, 4096 x 4096 x 1152 at grid 13: 1024 tiles = 78 * 13 + 10; k_blks = 9 = 4 * 2 + 1: stages 1, 2, 3, 0
+    s = Schedule("k7", 4096, 4096, 1152, 1, 13)
+    assert (s.grid, s.n_units, s.k_blks, s.stages) == (13, 13, 9, 4)
+    assert [len(u) for u in s.units] == [79] * 10 + [78] * 3
+    assert s.entry_stages()[:4] == [1, 2, 3, 0]
+    assert s.coords(130) == (4, 2)                                  # row-major: tile // n_blks, tile % n_blks
+    # pair kernel: 256 x 128 per cluster; cta_group 0 picks it for M > 128
+    s = Schedule("k7", 300, 200, 4096, 0, 0)
+    assert (s.ctas, s.n_tiles, s.grid, s.n_units) == (2, 4, 8, 4)
+    assert not any(Schedule("k7", 4096, 4096, 4096, cg, 13).facts()["mid_ring_entry"] for cg in (1, 2))   # k_blks % 4 == 0
+
+
+def test_schedule_model_panel_races():
+    # 512 x 512, one CTA per tile, group_m 1: tiles (m, n) = (t // 2, t % 2).  Grid 2: panel p completes in slot p, one
+    # after another; grid 4: panels 0 and 1 complete in slot 0 on different units, in an order the schedule leaves open
+    s = Schedule("k4", 512, 512, 64, 1, 2)
+    assert {p: v[0] for p, v in s.panel_done_slots().items()} == {p: p for p in range(4)} and not s.panels_race()
+    assert Schedule("k4", 512, 512, 64, 1, 4).panels_race()
+    assert not Schedule("k4", 512, 512, 64, 1, 1).panels_race()
+    assert Schedule("k4", 512, 512, 64, 2, 2).panels_race()          # a pair tile completes two panels at once
+
+
+def test_scale_cases_exercise_what_they_claim():
+    for (M, N, K), cg, gt in K4_SCALE_CASES:
+        grid = {"default": 0, "beside_engine": 132 - 32, "small": 13}[gt]
+        f = Schedule("k4", M, N, K, cg, grid, stream_k=cg == 3, group_m=8).facts()
+        assert f["mid_ring_entry"] and f["max_tiles_per_unit"] >= (8 if gt == "small" else 2), (M, N, K, cg, gt, f)
+        assert f["stream_k"] == (cg == 3), (M, N, K, cg, gt)
+    assert {(-(-K // 64)) % 3 for (_, _, K), _, _ in K4_SCALE_CASES} == {1, 2}
+    k7 = [Schedule("k7", M, N, K, cg, {"default": 0, "beside_engine": 100, "small": 13}[gt]).facts() for _, (M, N, K), cg, gt in K7_SCALE_CASES]
+    assert any(f["mid_ring_entry"] for f in k7) and max(f["max_tiles_per_unit"] for f in k7) >= 8
+    assert Schedule("k4", 8192, 8192, 2048, 2, 100, group_m=4).panels_race()
