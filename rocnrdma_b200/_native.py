@@ -61,6 +61,11 @@ class RnMockQpStats(C.Structure):
                 ("n_doorbells", u64), ("hw_sq_cons", u64), ("sq_cq_overruns", u64)]
 
 
+class RnSge(C.Structure):
+    """One scatter-gather entry (``rn::Sge``): ``bytes`` at ``addr`` under ``lkey``."""
+    _fields_ = [("addr", u64), ("lkey", u32), ("bytes", u32)]
+
+
 class RnEngineStats(C.Structure):
     _fields_ = [("n_bulk_chunks", u64), ("t_start", u64), ("t_exit", u64), ("running_ctas", u32),
                 ("exited_idle", u32), ("fatal", u32), ("n_qps", u32), ("ctas", u32), ("pad", u32)]
@@ -97,6 +102,8 @@ _SIGS = {
     "rn_post_recv": (i32, [vp, u64, u32, u32]),
     "rn_post_atomic": (i32, [vp, u32, u64, u32, u64, u32, u64, u64, u32, C.POINTER(u64)]),
     "rn_post_inline": (i32, [vp, u32, u64, u32, vp, u32, u32, u32, C.POINTER(u64)]),
+    "rn_post_wqe_bytes": (i32, [vp, C.POINTER(u8), C.POINTER(u64)]),
+    "rn_post_send_sg": (i32, [vp, u32, C.POINTER(RnSge), i32, u64, u32, u32, u32, C.POINTER(u64)]),
     "rn_hca_host_native_atomics": (i32, [vp]),
     "rn_host_stream": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, u64, u32, u64, C.POINTER(u64), C.POINTER(u32)]),
     "rn_host_staged_stream": (i32, [vp, u64, u64, u64, u32, u64, u32, u32, u32, u64, u32, u64, C.POINTER(u64)]),
@@ -139,12 +146,16 @@ _SIGS = {
     "rn_wire_decode_wqe": (i32, [C.POINTER(u8), C.POINTER(u64)]),
     "rn_wire_build_inline_wqe": (None, [C.POINTER(u8), u32, u32, u32, u64, u32, C.POINTER(u8), u32, u32, u32]),
     "rn_wire_decode_wqe_inline": (i32, [C.POINTER(u8), C.POINTER(u64)]),
+    "rn_wire_build_sg_wqe": (None, [C.POINTER(u8), u32, u32, u32, C.POINTER(RnSge), i32, u64, u32, u32, u32]),
+    "rn_wire_decode_wqe_sg": (i32, [C.POINTER(u8), C.POINTER(u64)]),
     "rn_k_atomic_stream": (i32, [u64, C.POINTER(u64), u32, u32, u32, u64, u32, u64, u64, u32, u64, u64, u64, u32, u32, u32, u32, u64, u64]),
     "rn_k_put_signal": (i32, [u64, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32, u32, u64, u64]),
     "rn_k_signal_wait": (i32, [u64, u64, u64, u64, u64, u64, u64, u64, u64, u64]),
     "rn_k_cq_watch": (i32, [u64, u64, u32, u64, u64, u64, u32, u64, u64, u64, u64, u64]),
     "rn_k_put_inline": (i32, [u64, C.POINTER(u64), u32, u64, u64, u32, u64, u32, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32,
                               u32, u32, u32, u64, u64]),
+    "rn_k_gather_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32, u32, u32,
+                                 u32, u32, u32, u64, u64]),
     "rn_gpu_page_size": (u64, []),
     "rn_dmabuf_export": (i32, [u64, u64, C.POINTER(i32)]),
     "rn_dmabuf_close": (i32, [i32]),
@@ -203,6 +214,8 @@ _SIGS = {
     "rn_verbs_post_atomic": (i32, [vp, u32, u64, u32, u64, u32, u64, u64, i32, C.POINTER(u64)]),
     "rn_verbs_post_inline": (i32, [vp, u32, u64, u32, vp, u32, i32, u32, C.POINTER(u64)]),
     "rn_verbs_qp_max_inline": (u32, [vp]),
+    "rn_verbs_post_sg": (i32, [vp, u32, C.POINTER(RnSge), i32, u64, u32, i32, u32, C.POINTER(u64)]),
+    "rn_verbs_qp_max_sge": (u32, [vp]),
     "rn_verbs_poll": (i32, [vp, i32, C.POINTER(RnVWc)]),
     "rn_verbs_host_stream": (i32, [vp, u32, u64, u32, u64, u32, u32, u32, u32, u64, u32, u64, C.POINTER(u64), C.POINTER(u32)]),
     "rn_verbs_host_staged_stream": (i32, [vp, u64, u64, u64, u32, u64, u32, u32, u32, u64, u32, u64, C.POINTER(u64)]),
@@ -214,6 +227,7 @@ _SIGS = {
     "rn_verbs_mock_declare_gpu_range": (i32, [u64, u64]),
     "rn_verbs_mock_gpu_free": (i32, [u64]),
     "rn_verbs_mock_set_rnr_timeout_ms": (i32, [u64]),
+    "rn_verbs_mock_post_wqe": (i32, [vp, C.POINTER(u8), C.POINTER(u64)]),
     "rn_verbs_mock_bridge_status": (C.c_char_p, []),
 }
 

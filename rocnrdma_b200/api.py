@@ -348,6 +348,52 @@ class QueuePair:
         buf = _inline_bytes(data, self.max_inline)
         return self._post_inline(W.OP_SEND if imm is None else W.OP_SEND_IMM, 0, 0, buf, signaled, imm or 0, fence)
 
+    @property
+    def max_send_sge(self) -> int:
+        """Scatter-gather entries a WRITE, READ or SEND may carry: 2 (ctrl + raddr + two data segments fill one WQEBB)."""
+        return W.MAX_SGE
+
+    def _sg_list(self, sges):
+        """``sges`` -- ``(MemoryRegion, offset, length)`` tuples -- as native entries; ``ValueError`` before anything is
+        posted when there are none or more than ``max_send_sge``, or a length lies outside ``[0, 2**32)``."""
+        sges = list(sges)
+        if not 1 <= len(sges) <= self.max_send_sge:
+            raise ValueError(f"{len(sges)} scatter-gather entries (1..{self.max_send_sge})")
+        arr = (N.RnSge * len(sges))()
+        for i, (mr, off, n) in enumerate(sges):
+            arr[i].addr, arr[i].lkey, arr[i].bytes = mr.addr + off, mr.lkey, N.byte_count(n, f"sges[{i}] length")
+        return arr
+
+    def _post_sg(self, opcode, arr, raddr, rkey, signaled, imm, fence) -> int:
+        idx = C.c_uint64()
+        self.ctx.sweep_revoked()
+        N.check(self.ctx._lib.rn_post_send_sg(self._q, opcode, arr, len(arr), raddr, rkey, _ctrl_flags(signaled, fence), imm,
+                                              C.byref(idx)), "post_send_sg")
+        return idx.value
+
+    def post_write_sg(self, sges, dst: MemoryRegion, dst_off=0, signaled=True, imm=None, fence=False) -> int:
+        """Gather RDMA WRITE (``imm`` not None: WRITE_WITH_IMM): the ``(MemoryRegion, offset, length)`` entries of
+        ``sges``, at most ``max_send_sge``, concatenated in list order, land at ``dst.addr + dst_off`` as one message of
+        their total length -- one work request, one completion.  Zero-length entries are dropped.  ``fence`` as in
+        :meth:`post_write`.  Returns the WQE index."""
+        arr = self._sg_list(sges)
+        op = W.OP_RDMA_WRITE if imm is None else W.OP_RDMA_WRITE_IMM
+        return self._post_sg(op, arr, dst.addr + dst_off, dst.rkey, signaled, imm or 0, fence)
+
+    def post_read_sg(self, sges, src_remote: MemoryRegion, remote_off=0, signaled=True, fence=False) -> int:
+        """Scatter RDMA READ: fetches the total length of ``sges`` from ``src_remote.addr + remote_off``; the first
+        entry's length goes to the first entry, the rest to the next (each registered with ``ACC_LOCAL_WRITE``).
+        Overlapping entries are undefined, as in IB.  ``fence`` as in :meth:`post_read`.  Returns the WQE index."""
+        arr = self._sg_list(sges)
+        return self._post_sg(W.OP_RDMA_READ, arr, src_remote.addr + remote_off, src_remote.rkey, signaled, 0, fence)
+
+    def post_send_sg(self, sges, signaled=True, imm=None, fence=False) -> int:
+        """Gather SEND (``imm`` not None: SEND_WITH_IMM): the entries of ``sges`` concatenated in list order land in the
+        responder's next receive buffer, which must hold their total.  ``fence`` as in :meth:`post_send`.  Returns the
+        WQE index."""
+        arr = self._sg_list(sges)
+        return self._post_sg(W.OP_SEND if imm is None else W.OP_SEND_IMM, arr, 0, 0, signaled, imm or 0, fence)
+
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):
         """Post one receive buffer (consumed in order by SEND / WRITE_WITH_IMM).  A buffer longer than
         ``Context.max_msg_bytes`` holds any message."""
@@ -494,6 +540,17 @@ class VerbsQueuePair(QueuePair):
         wr = C.c_uint64()
         self._vcheck(self.ctx._lib.rn_verbs_post_inline(self._vq, opcode, raddr, rkey, C.create_string_buffer(buf, len(buf)),
                                                         len(buf), _verbs_flags(signaled, fence), imm, C.byref(wr)), "post_inline")
+        return wr.value
+
+    @property
+    def max_send_sge(self) -> int:
+        """The send scatter-gather entries the provider granted, capped at 2 (one WQEBB)."""
+        return min(W.MAX_SGE, self.ctx._lib.rn_verbs_qp_max_sge(self._vq))
+
+    def _post_sg(self, opcode, arr, raddr, rkey, signaled, imm, fence) -> int:
+        wr = C.c_uint64()
+        self._vcheck(self.ctx._lib.rn_verbs_post_sg(self._vq, opcode, arr, len(arr), raddr, rkey, _verbs_flags(signaled, fence),
+                                                    imm, C.byref(wr)), "post_sg")
         return wr.value
 
     def post_recv(self, dst: MemoryRegion, nbytes=None, off=0):

@@ -317,8 +317,27 @@ __device__ __forceinline__ void copy_generic(uint64_t src, uint64_t dst, uint32_
 struct Parsed {
   WqeView v;
   uint64_t src, dst;
+  uint64_t local1;        // two-entry WQE: entry 1, translated
   uint8_t syn;
 };
+
+// A clean two-entry WQE that moves bytes: its chunks map through the slot's SgSide record.
+__device__ __forceinline__ bool is_sg(const WqeView& v, uint8_t syn) { return v.nsge == 2 && syn == SYN_OK && v.bytes != 0; }
+
+// Keys of a two-entry WQE (its total already passed the MAX_MSG check): each local entry over its own range, in list
+// order, with `lneed`; then, unless it is a SEND (whose remote side is the receive matched at commit), the remote key over
+// the whole message with `rneed`.  The three entries are loaded back to back (one round trip).  Returns the remote side;
+// *local0 and p->local1 receive the translated entries.
+__device__ __forceinline__ uint64_t parse_sg_keys(const QpDev* qp, Parsed* p, uint32_t lneed, uint32_t rneed, bool remote,
+                                                  uint64_t* local0) {
+  const WqeView& v = p->v;
+  const MKeyRaw l0 = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey), l1 = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey1);
+  const MKeyRaw rk = remote ? mkey_load(qp->r.rkeys, qp->r.n_rkeys, v.rkey) : MKeyRaw{};
+  *local0 = mkey_check(l0, v.lkey, v.laddr, v.len0, lneed, false, &p->syn);
+  if (*local0) p->local1 = mkey_check(l1, v.lkey1, v.laddr1, v.bytes - v.len0, lneed, false, &p->syn);
+  if (!p->local1 || !remote) return 0;
+  return mkey_check(rk, v.rkey, v.raddr, v.bytes, rneed, true, &p->syn);
+}
 
 // Atomic (CS / FA): both keys are checked here, nothing is moved; the retirer executes it in WQE order
 // (retire_atomics).  On success src = target word, dst = local fetch buffer, v.imm = RESOLVED_ATOMIC_* flags
@@ -352,7 +371,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
   wv[2] = ld_v4_volatile(slot + 32);
   wv[3] = ld_v4_volatile(slot + 48);
   p->syn = SYN_OK;
-  p->src = p->dst = 0;
+  p->src = p->dst = p->local1 = 0;
   bool ok = decode_wqe(&wqe, &p->v);
   WqeView& v = p->v;
   if (!ok || v.qpn != qp->qpn || v.wqe_idx != (uint16_t)w) {
@@ -376,6 +395,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
           if (p->dst) p->src = (uint64_t)(slot + v.inl_off);
           break;
         }
+        if (v.nsge == 2) { p->dst = parse_sg_keys(qp, p, 0, ACC_REMOTE_WRITE, true, &p->src); break; }
         const MKeyRaw lk = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey), rk = mkey_load(qp->r.rkeys, qp->r.n_rkeys, v.rkey);
         p->src = mkey_check(lk, v.lkey, v.laddr, v.bytes, 0, false, &p->syn);
         if (p->src) p->dst = mkey_check(rk, v.rkey, v.raddr, v.bytes, ACC_REMOTE_WRITE, true, &p->syn);
@@ -383,6 +403,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
       }
       case OP_RDMA_READ: {
         if (v.bytes == 0) { p->src = p->dst = 1; break; }
+        if (v.nsge == 2) { p->src = parse_sg_keys(qp, p, ACC_LOCAL_WRITE, ACC_REMOTE_READ, true, &p->dst); break; }
         const MKeyRaw lk = mkey_load(qp->lkeys, qp->n_lkeys, v.lkey), rk = mkey_load(qp->r.rkeys, qp->r.n_rkeys, v.rkey);
         p->dst = mkey_check(lk, v.lkey, v.laddr, v.bytes, ACC_LOCAL_WRITE, false, &p->syn);
         if (p->dst) p->src = mkey_check(rk, v.rkey, v.raddr, v.bytes, ACC_REMOTE_READ, true, &p->syn);
@@ -390,6 +411,7 @@ __device__ __forceinline__ void parse_wqe(const EngineCtl* ctl, QpDev* qp, unsig
       }
       case OP_SEND:
       case OP_SEND_IMM:
+        if (v.nsge == 2) { parse_sg_keys(qp, p, 0, 0, false, &p->src); break; }
         p->src = v.inl_off ? (uint64_t)(slot + v.inl_off) : translate(qp->lkeys, qp->n_lkeys, v.lkey, v.laddr, v.bytes, 0, false, &p->syn);
         break;
       case OP_ATOMIC_CS:
@@ -405,10 +427,12 @@ __device__ __forceinline__ bool needs_recv_wqe(uint8_t opcode) {
 
 // Publish resolved[w].  Runs in the parallel part for plain RDMA WRITE / READ / NOP and in
 // the ordered part for receive-consuming opcodes.  Returns the number of chunks.
+// local1: a two-entry WQE's translated entry 1 (is_sg), which goes to the slot's SgSide record.
 __device__ __forceinline__ uint32_t write_resolved(QpDev* qp, unsigned long long w, const WqeView& v, uint8_t syn,
                                                    uint64_t src, uint64_t dst, uint64_t rq_idx, uint8_t rq_taken,
-                                                   uint32_t* chunk_out = nullptr) {
-  Resolved* r = qp->resolved + (w & ((1u << qp->sq_log) - 1));
+                                                   uint64_t local1, uint32_t* chunk_out = nullptr) {
+  const uint32_t slot = (uint32_t)(w & ((1u << qp->sq_log) - 1));
+  Resolved* r = qp->resolved + slot;
   // Work granule: at least the QP's chunk_bytes, grown so that a very large message is cut
   // into ~8 claims per engine CTA (bounded claim traffic, still balances the tail).
   uint32_t chunk = qp->chunk_bytes;
@@ -419,6 +443,13 @@ __device__ __forceinline__ uint32_t write_resolved(QpDev* qp, unsigned long long
     if (want > chunk) chunk = want;
   }
   uint32_t nchunks = (syn == SYN_OK && v.bytes > 0) ? (v.bytes + chunk - 1) / chunk : 1;
+  const bool sg = is_sg(v, syn);
+  if (sg) {
+    // chunks never straddle an entry (SgSide)
+    const uint32_t n0 = (v.len0 + chunk - 1) / chunk;
+    nchunks = n0 + (v.bytes - v.len0 + chunk - 1) / chunk;
+    st_v4(qp->sg + slot, (uint32_t)local1, (uint32_t)(local1 >> 32), v.len0, n0);
+  }
   // a clean atomic keeps its operands where a chunked copy / a receive keeps its bookkeeping (hca_types.h)
   const bool atom = syn == SYN_OK && is_atomic(v.opcode);
   r->chunk = atom ? (uint32_t)(v.compare >> 32) : chunk;
@@ -427,7 +458,8 @@ __device__ __forceinline__ uint32_t write_resolved(QpDev* qp, unsigned long long
   r->bytes = (syn == SYN_OK) ? v.bytes : 0;
   r->nchunks = nchunks;
   r->imm = v.imm;
-  r->opcode = v.opcode; r->fm_ce_se = v.fm_ce_se; r->syndrome = syn; r->rq_consumed = rq_taken;
+  r->opcode = v.opcode; r->syndrome = syn; r->rq_consumed = rq_taken;
+  r->fm_ce_se = (uint8_t)((v.fm_ce_se & ~RESOLVED_SG) | (sg ? RESOLVED_SG : 0));
   r->rq_idx = atom ? v.swap_add : rq_idx;
   r->done = atom ? (uint32_t)v.compare : 0u;
   *(volatile unsigned long long*)&r->state = (w << 2) | 1ull;
@@ -728,13 +760,13 @@ __device__ __forceinline__ Committed commit_wqe(EngineCtl* ctl, QpDev* qp, unsig
   if (err) {
     // flushed: nothing moves, whatever the parse said
     c.syn = SYN_WR_FLUSH_ERR;
-    c.n = write_resolved(qp, w, p.v, c.syn, 0, 0, 0, 0, &c.chunk);
+    c.n = write_resolved(qp, w, p.v, c.syn, 0, 0, 0, 0, 0, &c.chunk);
   } else if (recv) {
     fence_gpu();  // acquire rq_head from the previous receive-consuming WQE
     uint64_t rq_idx = 0;
     uint8_t rq_taken = 0;
     match_recv(ctl, qp, p.v, &c.syn, &c.dst, &rq_idx, &rq_taken);
-    c.n = write_resolved(qp, w, p.v, c.syn, p.src, c.dst, rq_idx, rq_taken, &c.chunk);
+    c.n = write_resolved(qp, w, p.v, c.syn, p.src, c.dst, rq_idx, rq_taken, p.local1, &c.chunk);
     if (release_rq) fence_gpu();  // release rq_head
   }
   if (c.syn != SYN_OK && !err) { qp->state = QPS_ERR; err = true; }
@@ -762,7 +794,7 @@ __device__ __forceinline__ int claim_one(EngineCtl* ctl, QpDev* qp, unsigned lon
   parse_wqe(ctl, qp, w, &p);
   const bool recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
   uint32_t n = 1, chunk_sz = 0;
-  if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, &chunk_sz);
+  if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, p.local1, &chunk_sz);
   // ---- ordered part
   const unsigned long long turn = wait_turn(ctl, qp, w);
   bool err = (turn & PARSE_ERR_BIT) != 0 || st == QPS_ERR;
@@ -781,9 +813,16 @@ __device__ __forceinline__ int claim_one(EngineCtl* ctl, QpDev* qp, unsigned lon
     *saw_pending = true;
     return 0;
   }
-  const uint32_t bytes = c.syn == SYN_OK ? p.v.bytes : 0;
+  uint32_t bytes = c.syn == SYN_OK ? p.v.bytes : 0;
+  uint64_t src = p.src, dst = c.dst;
+  if (is_sg(p.v, c.syn)) {
+    // two entries: chunk 0 starts entry 0, or entry 1 when entry 0 is empty; the remote side starts at 0 either way
+    if (p.v.len0) bytes = p.v.len0;
+    else if (p.v.opcode == OP_RDMA_READ) dst = p.local1;
+    else src = p.local1;
+  }
   out->qp = qp; out->w = w; out->chunk = 0;
-  out->have_desc = 1; out->nch = c.n; out->src = p.src; out->dst = c.dst; out->fenced = c.fenced;
+  out->have_desc = 1; out->nch = c.n; out->src = src; out->dst = dst; out->fenced = c.fenced;
   out->len = bytes < c.chunk ? bytes : c.chunk;     // chunk 0
   return 1;
 }
@@ -888,7 +927,7 @@ __device__ __forceinline__ void claim_batch(EngineCtl* ctl, QpDev* qp, unsigned 
     trace_stamp(qp, w, TR_CLAIM);
     parse_wqe(ctl, qp, w, &p);
     recv = p.syn == SYN_OK && needs_recv_wqe(p.v.opcode);
-    if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, &chunk);
+    if (!recv) n = write_resolved(qp, w, p.v, p.syn, p.src, p.dst, 0, 0, p.local1, &chunk);
   }
   __syncwarp();
   unsigned long long turn = 0;
@@ -1068,11 +1107,26 @@ __global__ void __launch_bounds__(kThreads, 1) engine_kernel(EngineCtl* ctl) {
           const uint4 f = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r) + 16);   // bytes | nchunks | imm | flags
           const uint4 a = ld_v4_volatile(reinterpret_cast<const uint8_t*>(r));        // src | dst
           const uint32_t chunk = *(volatile uint32_t*)&r->chunk;
-          const uint64_t off = (uint64_t)work.chunk * chunk;
-          const uint32_t bytes = f.x;
+          uint32_t c = work.chunk, bytes = f.x;
+          csrc = ((uint64_t)a.y << 32) | a.x;
+          cdst = ((uint64_t)a.w << 32) | a.z;
+          if ((f.w >> 8) & RESOLVED_SG) {
+            // two entries: rebase onto the entry chunk c lies in (SgSide)
+            const uint4 g = ld_v4_volatile(work.qp->sg + (work.w & ((1u << work.qp->sq_log) - 1)));   // local1 | len0 | n0
+            if (c < g.w) {
+              bytes = g.z;
+            } else {
+              const uint64_t local1 = ((uint64_t)g.y << 32) | g.x;
+              c -= g.w;
+              bytes -= g.z;
+              if ((uint8_t)f.w == OP_RDMA_READ) { csrc += g.z; cdst = local1; }
+              else { csrc = local1; cdst += g.z; }
+            }
+          }
+          const uint64_t off = (uint64_t)c * chunk;
           len = bytes == 0 ? 0 : (uint32_t)((bytes - off < chunk) ? (bytes - off) : chunk);
-          csrc = (((uint64_t)a.y << 32) | a.x) + off;
-          cdst = (((uint64_t)a.w << 32) | a.z) + off;
+          csrc += off;
+          cdst += off;
           nch = f.y;
           fenced = ((f.w >> 8) & 0xe0u) == CTRL_FENCE;
         }

@@ -594,8 +594,9 @@ RN_API int rn_create_qp(void* hca, void* scq, void* rcq, uint32_t nsq, uint32_t 
   Resolved* res = (Resolved*)arena_alloc(h, (size_t)nsq * sizeof(Resolved), false);
   unsigned long long* trace = (unsigned long long*)arena_alloc(h, (size_t)nsq * 64, false);
   uint32_t* flags = (uint32_t*)arena_alloc(h, (size_t)nsq * 4, false);
+  SgSide* sg = (SgSide*)arena_alloc(h, (size_t)nsq * sizeof(SgSide), false);
   q->d = (QpDev*)arena_alloc(h, sizeof(QpDev), false);
-  if (!sq || !rq || !dbr || !bf || !res || !trace || !flags || !q->d) { delete q; return fail(-12, "create_qp: control arena exhausted"); }
+  if (!sq || !rq || !dbr || !bf || !res || !trace || !flags || !sg || !q->d) { delete q; return fail(-12, "create_qp: control arena exhausted"); }
   memset(&q->h, 0, sizeof q->h);
   q->h.qpn = h->next_qpn++;
   q->h.state = QPS_RESET;
@@ -607,6 +608,7 @@ RN_API int rn_create_qp(void* hca, void* scq, void* rcq, uint32_t nsq, uint32_t 
   q->h.resolved = res;
   q->h.trace = trace;
   q->h.ready_flags = flags;
+  q->h.sg = sg;
   q->h.trace_on = 0;
   q->h.sq_in_device = host ? 0 : 1;
   q->h.sys_scope = (host || q->scq->mem == MEM_HOST_PINNED || q->rcq->mem == MEM_HOST_PINNED) ? 1 : 0;
@@ -928,6 +930,40 @@ RN_API int rn_post_inline(void* qp, uint32_t opcode, uint64_t raddr, uint32_t rk
   return host_sq_publish(q, w, idx, idx_out);
 }
 
+// Host-posted gather WRITE / WRITE_IMM / SEND / SEND_IMM or scatter READ of n (1..MAX_SGE) entries: the message is the
+// entries concatenated in list order.  Zero-length entries are dropped; raddr / rkey are ignored for SEND.
+RN_API int rn_post_send_sg(void* qp, uint32_t opcode, const Sge* sg, int n, uint64_t raddr, uint32_t rkey, uint32_t flags,
+                           uint32_t imm, uint64_t* idx_out) {
+  Qp* q = (Qp*)qp;
+  const bool send = opcode == OP_SEND || opcode == OP_SEND_IMM;
+  if (!send && opcode != OP_RDMA_WRITE && opcode != OP_RDMA_WRITE_IMM && opcode != OP_RDMA_READ)
+    return fail(-22, "post_send_sg: opcode 0x%x takes no scatter-gather list", opcode);
+  if (n < 1 || n > (int)MAX_SGE) return fail(-22, "post_send_sg: %d entries (1..%u)", n, (unsigned)MAX_SGE);
+  uint64_t idx = 0;
+  int rc = host_sq_slot(q, "post_send_sg", &idx);
+  if (rc) return rc;
+  Wqe64 w;
+  if (send) build_send_sg_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, sg, n, (uint8_t)flags, imm);
+  else build_rdma_sg_wqe(&w, (uint8_t)opcode, (uint16_t)idx, q->h.qpn, sg, n, raddr, rkey, (uint8_t)flags, imm);
+  return host_sq_publish(q, w, idx, idx_out);
+}
+
+// Test hook: post a caller-built WQE through the host poster -- its 64 bytes as given, with this QP's number and the next
+// index written into the ctrl segment.  It hands the engine WQEs no poster makes (a two-segment list with a zero-length
+// segment).
+RN_API int rn_post_wqe_bytes(void* qp, const uint8_t* wqe64, uint64_t* idx_out) {
+  Qp* q = (Qp*)qp;
+  uint64_t idx = 0;
+  int rc = host_sq_slot(q, "post_wqe_bytes", &idx);
+  if (rc) return rc;
+  Wqe64 w;
+  memcpy(&w, wqe64, 64);
+  const uint32_t w0 = be32(w.ctrl.opmod_idx_opcode), w1 = be32(w.ctrl.qpn_ds);
+  w.ctrl.opmod_idx_opcode = ctrl_word0((uint8_t)w0, (uint16_t)idx, (uint8_t)(w0 >> 24));
+  w.ctrl.qpn_ds = ctrl_word1(q->h.qpn, (uint8_t)(w1 & 0x3f));
+  return host_sq_publish(q, w, idx, idx_out);
+}
+
 RN_API int rn_post_recv(void* qp, uint64_t addr, uint32_t lkey, uint32_t bytes) {
   Qp* q = (Qp*)qp;
   cudaSetDevice(q->hca->dev);
@@ -1136,6 +1172,26 @@ RN_API int rn_wire_decode_wqe_inline(const uint8_t* wqe64, uint64_t* out15) {
   const uint64_t f[15] = {v.opcode, v.wqe_idx, v.qpn, v.ds, v.fm_ce_se, v.imm, v.raddr, v.rkey, v.laddr, v.lkey, v.bytes,
                           v.swap_add, v.compare, v.inl_off != 0, v.inl_off};
   memcpy(out15, f, sizeof f);
+  return ok ? 1 : 0;
+}
+RN_API void rn_wire_build_sg_wqe(uint8_t* out64, uint32_t opcode, uint32_t idx, uint32_t qpn, const Sge* sg, int n,
+                                 uint64_t raddr, uint32_t rkey, uint32_t flags, uint32_t imm) {
+  Wqe64 w;
+  memset(&w, 0, sizeof w);
+  if (opcode == OP_SEND || opcode == OP_SEND_IMM) build_send_sg_wqe(&w, (uint8_t)opcode, (uint16_t)idx, qpn, sg, n, (uint8_t)flags, imm);
+  else build_rdma_sg_wqe(&w, (uint8_t)opcode, (uint16_t)idx, qpn, sg, n, raddr, rkey, (uint8_t)flags, imm);
+  memcpy(out64, &w, 64);
+}
+// rn_wire_decode_wqe's 13 fields (bytes is the total), then: the entry count, entry 0's length, entry 1's address and
+// key (the last three are 0 for a one-entry WQE).
+RN_API int rn_wire_decode_wqe_sg(const uint8_t* wqe64, uint64_t* out17) {
+  Wqe64 w;
+  memcpy(&w, wqe64, 64);
+  WqeView v;
+  const bool ok = decode_wqe(&w, &v);
+  const uint64_t f[17] = {v.opcode, v.wqe_idx, v.qpn, v.ds, v.fm_ce_se, v.imm, v.raddr, v.rkey, v.laddr, v.lkey, v.bytes,
+                          v.swap_add, v.compare, v.nsge, v.len0, v.laddr1, v.lkey1};
+  memcpy(out17, f, sizeof f);
   return ok ? 1 : 0;
 }
 RN_API int rn_wire_decode_cqe(const uint8_t* cqe64, RnWc* out) {

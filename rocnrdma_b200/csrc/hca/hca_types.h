@@ -80,6 +80,20 @@ static_assert(sizeof(Resolved) == 64, "Resolved is one cache-line pair slot");
 static_assert(offsetof(Resolved, done) == 32 && offsetof(Resolved, chunk) == 36 && offsetof(Resolved, rq_idx) == 40,
               "atomic operands are read back as one 16-byte load at offset 32");
 enum : uint32_t { RESOLVED_ATOMIC_SYS = 1u };   // Resolved::imm of an atomic: execute (and fence) at system scope
+// Resolved::fm_ce_se of a clean two-entry WQE (a bit the wire's fm_ce_se leaves reserved): its chunks map through the
+// slot's SgSide record.
+enum : uint8_t { RESOLVED_SG = 0x10 };
+
+// Per-SQ-slot side record of a two-entry WQE (gather WRITE / WRITE_IMM / SEND, scatter READ), written with its Resolved
+// record and read only when that record carries RESOLVED_SG.  Chunks never straddle an entry: chunk c < n0 covers entry
+// 0 at offset c * chunk (Resolved's local address), chunk c >= n0 covers entry 1 at local1 + (c - n0) * chunk, and the
+// remote side at len0 + (c - n0) * chunk.  One 16-byte load.
+struct alignas(16) SgSide {
+  uint64_t local1;            // entry 1, translated
+  uint32_t len0;              // entry 0's length
+  uint32_t n0;                // entry 0's chunks: ceil(len0 / chunk)
+};
+static_assert(sizeof(SgSide) == 16, "SgSide is one 16-byte load");
 
 // What a requester's engine needs to know about the connected responder QP.  All
 // pointers are already translated into the engine GPU's address space.
@@ -118,6 +132,7 @@ struct QpDev {
   RemoteView r;
   Resolved* resolved;         // one per SQ slot
   uint32_t* ready_flags;      // one per SQ slot: (index + 1) once the WQE bytes are complete (shared posters)
+  SgSide* sg;                 // one per SQ slot: the second entry of a two-entry WQE
   // ---- device poster state
   unsigned long long resv_head;    // next WQE index to hand out
   unsigned long long ready_head;   // every index below this has rung its doorbell

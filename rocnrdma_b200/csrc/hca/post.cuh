@@ -416,6 +416,28 @@ __device__ __forceinline__ unsigned long long rdma_send(QpDev* qp, uint64_t ladd
   });
 }
 
+// Two-entry scatter-gather verbs through the shared submit: the message is sg[0] then sg[1] (zero-length entries dropped;
+// with at most one left, the WQE is the one-entry verb's).  WRITE: gathered to [raddr, raddr + total).  READ: that range
+// scattered into sg[0] then sg[1].  SEND: the concatenation into the responder's next receive.
+__device__ __forceinline__ unsigned long long rdma_write_sg(QpDev* qp, const Sge (&sg)[MAX_SGE], uint64_t raddr, uint32_t rkey,
+                                                            bool signaled = true, bool fence = false) {
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_rdma_sg_wqe(w, OP_RDMA_WRITE, (uint16_t)idx, qp->qpn, sg, MAX_SGE, raddr, rkey, wr_flags(signaled, fence), 0);
+  });
+}
+__device__ __forceinline__ unsigned long long rdma_read_sg(QpDev* qp, const Sge (&sg)[MAX_SGE], uint64_t raddr, uint32_t rkey,
+                                                           bool signaled = true, bool fence = false) {
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_rdma_sg_wqe(w, OP_RDMA_READ, (uint16_t)idx, qp->qpn, sg, MAX_SGE, raddr, rkey, wr_flags(signaled, fence), 0);
+  });
+}
+__device__ __forceinline__ unsigned long long rdma_send_sg(QpDev* qp, const Sge (&sg)[MAX_SGE], bool signaled = true,
+                                                           uint32_t imm = 0, bool with_imm = false, bool fence = false) {
+  return post_one(qp, [&](Wqe64* w, unsigned long long idx) {
+    build_send_sg_wqe(w, with_imm ? OP_SEND_IMM : OP_SEND, (uint16_t)idx, qp->qpn, sg, MAX_SGE, wr_flags(signaled, fence), imm);
+  });
+}
+
 // Remote 8-byte atomics through the shared submit: any thread of any kernel may call them (a producer signalling
 // "data landed" after its RDMA WRITEs: the engine executes the atomic only after every earlier WQE of the QP).
 // The original remote value lands in the 8 local bytes at laddr.

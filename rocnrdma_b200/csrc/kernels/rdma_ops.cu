@@ -459,6 +459,95 @@ RN_API int rn_k_put_inline(uint64_t stream, const uint64_t* qps_host, uint32_t n
   return (int)cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- two-entry gathers and scatters
+// One warp per QP.  Message i of CTA c uses slot offset off = (i % nslots) * slot_stride and is cut at `split` bytes:
+// entry 0 is the first `split` bytes at laddr + c * stride + off, entry 1 the other bytes - split at
+// laddr1 + c * stride + off (the same slot of a second MR), and the remote side is [raddr + c * stride + off, + bytes).
+// WRITE and SEND gather the two entries into it (a SEND into the responder's next receive), READ scatters it into them.
+//   via 0: the windowed, bursted exclusive Poster of rdma_stream_kernel (stream_post)
+//   via 1: lane 0 posts each message with dev::rdma_write_sg / rdma_read_sg / rdma_send_sg (shared submit) and keeps at
+//          most `window` messages in flight with sq_wait
+struct GatherArgs {
+  QpDev* qps[kMaxStreamQps];
+  uint32_t opcode;
+  uint64_t laddr, laddr1, raddr, stride, slot_stride;
+  uint32_t lkey, lkey1, rkey;
+  uint32_t bytes, split, nslots;
+  uint32_t iters, window, signal_every, burst, via;
+  uint64_t timeout_ns;
+  unsigned long long* out;            // per CTA: [status, t_start, t_end, done, first_idx, last_idx, cons, 0]
+};
+
+__global__ void __launch_bounds__(32, 1) gather_stream_kernel(GatherArgs a) {
+  const uint64_t cta = (uint64_t)blockIdx.x * a.stride;
+  const uint64_t l0 = a.laddr + cta, l1 = a.laddr1 + cta, r = a.raddr + cta;
+  const uint8_t opc = (uint8_t)a.opcode;
+  auto entries = [&](uint32_t i, Sge (&sg)[MAX_SGE]) -> uint64_t {
+    const uint64_t off = (uint64_t)(i % a.nslots) * a.slot_stride;
+    sg[0] = Sge{l0 + off, a.lkey, a.split};
+    sg[1] = Sge{l1 + off, a.lkey1, a.bytes - a.split};
+    return r + off;
+  };
+  QpDev* qp = a.qps[blockIdx.x];
+  unsigned long long* out = a.out + (size_t)blockIdx.x * 8;
+  if (a.via == 0) {
+    stream_post(qp, 1, a.iters, a.window, a.burst, a.signal_every, false, a.timeout_ns, out,
+                [&](uint8_t* slot, uint16_t idx, uint32_t qpn, uint32_t i, uint32_t, uint8_t flags) {
+                  Sge sg[MAX_SGE];
+                  const uint64_t raddr = entries(i, sg);
+                  Wqe64 w;
+                  if (opc == OP_SEND) build_send_sg_wqe(&w, OP_SEND, idx, qpn, sg, MAX_SGE, flags, 0);
+                  else build_rdma_sg_wqe(&w, opc, idx, qpn, sg, MAX_SGE, raddr, a.rkey, flags, 0);
+                  store_wqe(slot, w);
+                });
+    return;
+  }
+  if (threadIdx.x != 0) return;
+  int status = qp->state == QPS_ERR ? WAIT_QP_ERROR : WAIT_OK;
+  unsigned long long first = ~0ull, last = 0;
+  uint32_t done = 0;
+  const unsigned long long t0 = globaltimer_ns();
+  for (; done < a.iters && status == WAIT_OK; ++done) {
+    const uint32_t i = done;
+    const bool sig = a.signal_every <= 1 || (i + 1) % a.signal_every == 0 || i + 1 == a.iters;
+    // at most `window` messages in flight: message i - window has completed (a signaled WQE lies within the window)
+    if (a.window && i >= a.window && (status = sq_wait(qp, first + i - a.window, a.timeout_ns)) != WAIT_OK) break;
+    Sge sg[MAX_SGE];
+    const uint64_t raddr = entries(i, sg);
+    const unsigned long long idx = opc == OP_SEND ? rdma_send_sg(qp, sg, sig)
+                                   : opc == OP_RDMA_READ ? rdma_read_sg(qp, sg, raddr, a.rkey, sig)
+                                                         : rdma_write_sg(qp, sg, raddr, a.rkey, sig);
+    if (idx == ~0ull) { status = WAIT_TIMEOUT; break; }
+    if (first == ~0ull) first = idx;
+    last = idx;
+  }
+  if (done && status == WAIT_OK) status = sq_wait(qp, last, a.timeout_ns);
+  out[0] = (unsigned long long)(long long)status;
+  out[1] = t0; out[2] = globaltimer_ns(); out[3] = done; out[4] = first; out[5] = last;
+  out[6] = ld_u64_volatile(&qp->sq_cons);
+  out[7] = 0;
+}
+
+RN_API int rn_k_gather_stream(uint64_t stream, const uint64_t* qps_host, uint32_t nqp, uint32_t opcode, uint64_t laddr,
+                              uint32_t lkey, uint64_t laddr1, uint32_t lkey1, uint64_t raddr, uint32_t rkey, uint64_t stride,
+                              uint32_t bytes, uint32_t split, uint64_t slot_stride, uint32_t nslots, uint32_t iters,
+                              uint32_t window, uint32_t signal_every, uint32_t burst, uint32_t via, uint64_t timeout_ms,
+                              uint64_t out_dev) {
+  GatherArgs a;
+  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps || split > bytes || via > 1) return -22;
+  if (opcode != OP_RDMA_WRITE && opcode != OP_RDMA_READ && opcode != OP_SEND) return -22;
+  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
+  a.opcode = opcode; a.laddr = laddr; a.laddr1 = laddr1; a.raddr = raddr; a.stride = stride; a.slot_stride = slot_stride;
+  a.lkey = lkey; a.lkey1 = lkey1; a.rkey = rkey; a.bytes = bytes; a.split = split; a.nslots = nslots ? nslots : 1;
+  a.iters = iters; a.window = window; a.via = via;
+  rn_stream_clamp(window, &burst, &signal_every);
+  a.signal_every = signal_every; a.burst = burst;
+  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.out = (unsigned long long*)out_dev;
+  gather_stream_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
 // ---------------------------------------------------------------- signal wait (receiver side)
 // Runs on the GPU that holds the signal word.  Thread 0 polls it with system-scope acquire loads until it reaches
 // `until`; every value 1..until is stamped (%globaltimer) when first seen.  Each wait for the next arrival is bounded
@@ -719,6 +808,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncGetAttributes(&a, atomic_stream_kernel);
   cudaFuncGetAttributes(&a, put_signal_kernel);
   cudaFuncGetAttributes(&a, put_inline_kernel);
+  cudaFuncGetAttributes(&a, gather_stream_kernel);
   cudaFuncGetAttributes(&a, signal_wait_kernel);
   cudaFuncGetAttributes(&a, cq_watch_kernel);
   cudaFuncGetAttributes(&a, fill_random_kernel);

@@ -32,8 +32,8 @@
 //     ibv_reg_dmabuf_mr() takes a dma-buf fd (CUDA-exported for HBM; a memfd is accepted as a host
 //     "dma-buf" so the path is testable without a GPU).
 //
-// Not modelled: UD/UC, SRQ, atomics, inline data, multi-SGE, events/completion channels, path MTU
-// segmentation, retransmission.
+// Send scatter-gather lists of up to two entries are modelled (one WQEBB per WQE); receive WQEs keep one.
+// Not modelled: UD/UC, SRQ, events/completion channels, path MTU segmentation, retransmission.
 #include <dlfcn.h>
 #include <errno.h>
 #include <fcntl.h>
@@ -201,6 +201,7 @@ struct MockQp {
   uint32_t* dbrec = nullptr;     // [0] rcv, [1] snd
   uint8_t* uar = nullptr;        // one page
   int sq_sig_all = 0;
+  uint32_t max_sge = 1;          // send scatter-gather entries granted at create (1..MAX_SGE)
   // host poster (ibv_post_send / ibv_post_recv) state
   std::mutex post_mu;
   uint64_t sq_head = 0, sq_tail = 0, rq_head = 0, rq_tail = 0;
@@ -409,6 +410,27 @@ MockQp* find_qp(uint16_t lid, uint32_t qpn) {
   return qpn < kMaxQps ? d.qps[qpn] : nullptr;
 }
 
+// A WQE's local entries: one, or the two of a gather / scatter list, each checked over its own range in list order.
+struct Local { uint64_t a[2]; MockMr* mr[2]; uint32_t len[2]; int n; };
+bool local_entries(MockDev* d, const rn::WqeView& v, unsigned need, uint8_t* syn, Local* L) {
+  L->n = v.nsge == 2 ? 2 : 1;
+  L->len[0] = L->n == 2 ? v.len0 : v.bytes;
+  L->len[1] = v.bytes - L->len[0];
+  L->mr[0] = L->mr[1] = nullptr;
+  L->a[0] = translate(d, v.lkey, v.laddr, L->len[0], need, false, syn, &L->mr[0]);
+  if (!L->a[0]) return false;
+  if (L->n == 2) L->a[1] = translate(d, v.lkey1, v.laddr1, L->len[1], need, false, syn, &L->mr[1]);
+  return L->n == 1 || L->a[1] != 0;
+}
+// The message is the entries in list order: gather them to [remote, remote + bytes), or scatter that range into them.
+bool dma_entries(const Local& L, uint64_t remote, MockMr* rmr, bool scatter) {
+  uint64_t off = 0;
+  for (int i = 0; i < L.n; off += L.len[i], ++i)
+    if (!(scatter ? dma_copy(L.a[i], L.mr[i], remote + off, rmr, L.len[i]) : dma_copy(remote + off, rmr, L.a[i], L.mr[i], L.len[i])))
+      return false;
+  return true;
+}
+
 // ------------------------------------------------------------------ the NIC: execute one WQE of `qp`
 // Returns false when it must be retried later (receiver not ready).
 bool nic_execute(MockQp* qp, uint64_t w) {
@@ -439,12 +461,12 @@ bool nic_execute(MockQp* qp, uint64_t w) {
       case rn::OP_RDMA_WRITE: case rn::OP_RDMA_WRITE_IMM: {
         // Zero length: no key is looked at and nothing moves (DESIGN.md 3.1).  Otherwise the keys are checked before the
         // receive wait, so a WRITE_IMM that fails them never takes a receive.  Inline: the payload is in the WQE (no
-        // local key); else it is gathered through the lkey.
-        uint64_t src = 0, dst = 0;
+        // local key); else it is gathered through the lkeys of its entries.
+        uint64_t dst = 0;
+        Local L;
         if (v.bytes) {
-          src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
-                          : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
-          dst = src ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_WRITE, true, &syn, &rmr) : 0;
+          const bool lok = v.inl_off || local_entries(ldev, v, 0, &syn, &L);
+          dst = lok ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_WRITE, true, &syn, &rmr) : 0;
         }
         if (syn == rn::SYN_OK && !(peer->access_flags & IBV_ACCESS_REMOTE_WRITE)) syn = rn::SYN_REMOTE_ACCESS_ERR;
         if (syn == rn::SYN_OK && v.opcode == rn::OP_RDMA_WRITE_IMM) {
@@ -452,7 +474,10 @@ bool nic_execute(MockQp* qp, uint64_t w) {
           if (r == 0) return false;
           if (r < 0) { syn = rn::SYN_RNR_RETRY_EXC_ERR; break; }
         }
-        if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, rmr, src, lmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
+        if (syn == rn::SYN_OK && v.bytes &&
+            !(v.inl_off ? dma_copy(dst, rmr, (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off), nullptr, v.bytes)
+                        : dma_entries(L, dst, rmr, false)))
+          syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) {
           moved = v.bytes;
           if (v.opcode == rn::OP_RDMA_WRITE_IMM) { consumed_rq = true; rq_index = (uint16_t)peer->hw_rq_cons++; }
@@ -460,22 +485,22 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         break;
       }
       case rn::OP_RDMA_READ: {
-        uint64_t dst = 0, src = 0;
-        if (v.bytes) {   // zero length: no key is looked at, as for WRITE
-          dst = translate(ldev, v.lkey, v.laddr, v.bytes, IBV_ACCESS_LOCAL_WRITE, false, &syn, &lmr);
-          src = dst ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_READ, true, &syn, &rmr) : 0;
+        uint64_t src = 0;
+        Local L;
+        if (v.bytes) {   // zero length: no key is looked at, as for WRITE; the fetched bytes scatter over the entries
+          const bool lok = local_entries(ldev, v, IBV_ACCESS_LOCAL_WRITE, &syn, &L);
+          src = lok ? translate(rdev, v.rkey, v.raddr, v.bytes, IBV_ACCESS_REMOTE_READ, true, &syn, &rmr) : 0;
         }
         if (syn == rn::SYN_OK && !(peer->access_flags & IBV_ACCESS_REMOTE_READ)) syn = rn::SYN_REMOTE_ACCESS_ERR;
-        if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, lmr, src, rmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
+        if (syn == rn::SYN_OK && v.bytes && !dma_entries(L, src, rmr, true)) syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) moved = v.bytes;
         break;
       }
       case rn::OP_SEND: case rn::OP_SEND_IMM: {
         // The requester's own check comes first: a SEND whose lkey fails never reaches the responder, so it neither
         // waits for nor consumes a receive.
-        uint64_t src = v.inl_off ? (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off)
-                                 : translate(ldev, v.lkey, v.laddr, v.bytes, 0, false, &syn, &lmr);
-        if (syn != rn::SYN_OK) break;
+        Local L;
+        if (!v.inl_off && !local_entries(ldev, v, 0, &syn, &L)) break;
         const int r = recv_wait(qp, peer);
         if (r == 0) return false;
         if (r < 0) { syn = rn::SYN_RNR_RETRY_EXC_ERR; break; }
@@ -487,7 +512,10 @@ bool nic_execute(MockQp* qp, uint64_t w) {
         if (rn::recv_wqe_bytes(rw) < v.bytes) syn = rn::SYN_REMOTE_INVAL_REQ_ERR;
         uint64_t dst = syn == rn::SYN_OK ? translate(rdev, rn::recv_wqe_lkey(rw), rn::recv_wqe_addr(rw), v.bytes, IBV_ACCESS_LOCAL_WRITE,
                                                      true, &syn, &rmr) : 0;
-        if (syn == rn::SYN_OK && v.bytes && !dma_copy(dst, rmr, src, lmr, v.bytes)) syn = rn::SYN_LOCAL_PROT_ERR;
+        if (syn == rn::SYN_OK && v.bytes &&
+            !(v.inl_off ? dma_copy(dst, rmr, (uint64_t)(uintptr_t)((const uint8_t*)&wqe + v.inl_off), nullptr, v.bytes)
+                        : dma_entries(L, dst, rmr, false)))
+          syn = rn::SYN_LOCAL_PROT_ERR;
         if (syn == rn::SYN_OK) moved = v.bytes;
         break;
       }
@@ -589,6 +617,19 @@ void nic_start() {
 }
 
 // ------------------------------------------------------------------ fast path: ops table
+// Publish the WQEs up to `head` (the caller holds post_mu): doorbell record, then the doorbell -- the first 8 bytes of the
+// last WQE's ctrl segment into the BlueFlame register, alternating between the two registers as libmlx5 does.
+void ring_sq(MockQp* qp, uint64_t head) {
+  std::atomic_thread_fence(std::memory_order_release);
+  *(volatile uint32_t*)&qp->dbrec[rn::DBR_SND] = rn::wq_dbr_word(head);
+  std::atomic_thread_fence(std::memory_order_release);
+  unsigned long long db;
+  memcpy(&db, qp->sq + (((head - 1) & (qp->sq_cnt - 1)) << 6), 8);
+  __atomic_store_n((unsigned long long*)(qp->uar + kBfOffset + qp->bf_off), db, __ATOMIC_RELEASE);
+  qp->bf_off ^= kBfSize;
+  qp->sq_head = head;
+}
+
 int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
   MockQp* qp = reinterpret_cast<MockQp*>(q);
   std::lock_guard<std::mutex> g(qp->post_mu);
@@ -597,7 +638,7 @@ int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
   const uint64_t first = head;
   for (; wr; wr = wr->next) {
     if (head - qp->sq_tail >= qp->sq_cnt) { if (bad) *bad = wr; errno = ENOMEM; break; }
-    if (wr->num_sge > 1 || wr->num_sge < 0) { if (bad) *bad = wr; errno = EINVAL; break; }
+    if (wr->num_sge > (int)qp->max_sge || wr->num_sge < 0) { if (bad) *bad = wr; errno = EINVAL; break; }
     uint8_t opc;
     switch (wr->opcode) {
       case IBV_WR_RDMA_WRITE: opc = rn::OP_RDMA_WRITE; break;
@@ -613,44 +654,47 @@ int mock_post_send(ibv_qp* q, ibv_send_wr* wr, ibv_send_wr** bad) {
     const uint8_t fm = (uint8_t)(((wr->send_flags & IBV_SEND_SIGNALED) || qp->sq_sig_all ? rn::CTRL_CQ_UPDATE : 0) |
                                  ((wr->send_flags & IBV_SEND_SOLICITED) ? rn::CTRL_SOLICITED : 0) |
                                  ((wr->send_flags & IBV_SEND_FENCE) ? rn::CTRL_FENCE : 0));
-    const uint64_t laddr = wr->num_sge ? wr->sg_list[0].addr : 0;
-    const uint32_t lkey = wr->num_sge ? wr->sg_list[0].lkey : 0, len = wr->num_sge ? wr->sg_list[0].length : 0;
+    if (rn::is_atomic(opc) && wr->num_sge != 1) { if (bad) *bad = wr; errno = EINVAL; break; }   // exactly one 8-byte SGE
+    rn::Sge sg[rn::MAX_SGE] = {};
+    for (int i = 0; i < wr->num_sge; ++i) sg[i] = rn::Sge{wr->sg_list[i].addr, wr->sg_list[i].lkey, wr->sg_list[i].length};
+    const int nsg = wr->num_sge;
+    const uint64_t laddr = sg[0].addr;
+    const uint32_t lkey = sg[0].lkey, len = sg[0].bytes;
     rn::Wqe64 w;
     memset(&w, 0, sizeof w);
     const uint32_t imm = be32(wr->imm_data);       // imm_data is already big-endian; build_* swaps it back onto the wire
     const bool inl = (wr->send_flags & IBV_SEND_INLINE) != 0;
-    if (inl && (opc == rn::OP_RDMA_READ || rn::is_atomic(opc) || len == 0 || len > rn::MAX_INLINE)) {
+    // Inline: the entries' bytes are concatenated into the WQE now, from their host addresses (libmlx5's set_data_inl_seg);
+    // the lkeys are not looked at.
+    uint8_t inl_buf[rn::MAX_INLINE];
+    uint64_t inl_len = 0;
+    bool inl_ok = inl && opc != rn::OP_RDMA_READ && !rn::is_atomic(opc);
+    for (int i = 0; inl_ok && i < nsg; ++i) {
+      if (inl_len + sg[i].bytes > rn::MAX_INLINE) { inl_ok = false; break; }
+      memcpy(inl_buf + inl_len, (const void*)(uintptr_t)sg[i].addr, sg[i].bytes);
+      inl_len += sg[i].bytes;
+    }
+    if (inl && (!inl_ok || inl_len == 0)) {
       if (bad) *bad = wr;
       errno = EINVAL;
       break;
     }
-    if (inl)   // the payload is copied into the WQE now, from the sge's host address; the lkey is not looked at
+    if (inl)
       rn::build_inline_wqe(&w, opc, (uint16_t)head, q->qp_num, wr->wr.rdma.remote_addr, wr->wr.rdma.rkey,
-                           (const void*)(uintptr_t)laddr, len, fm, imm);
-    else if (opc == rn::OP_SEND || opc == rn::OP_SEND_IMM)
-      rn::build_send_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, len, fm, imm);
+                           inl_buf, (uint32_t)inl_len, fm, imm);
+    else if (opc == rn::OP_SEND || opc == rn::OP_SEND_IMM)   // zero-length entries dropped, as libmlx5 does
+      rn::build_send_sg_wqe(&w, opc, (uint16_t)head, q->qp_num, sg, nsg, fm, imm);
     else if (rn::is_atomic(opc))   // libmlx5: FA carries compare_add as the addend, CS carries swap + compare
       rn::build_atomic_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, wr->wr.atomic.remote_addr, wr->wr.atomic.rkey,
                            opc == rn::OP_ATOMIC_FA ? wr->wr.atomic.compare_add : wr->wr.atomic.swap, wr->wr.atomic.compare_add, fm, len);
     else
-      rn::build_rdma_wqe(&w, opc, (uint16_t)head, q->qp_num, laddr, lkey, wr->wr.rdma.remote_addr, wr->wr.rdma.rkey, len, fm, imm);
+      rn::build_rdma_sg_wqe(&w, opc, (uint16_t)head, q->qp_num, sg, nsg, wr->wr.rdma.remote_addr, wr->wr.rdma.rkey, fm, imm);
     memcpy(qp->sq + ((head & (qp->sq_cnt - 1)) << 6), &w, 64);
     qp->sq_wrid[head & (qp->sq_cnt - 1)] = wr->wr_id;
     ++head;
   }
   int rc = wr ? errno : 0;
-  if (head != first) {
-    // doorbell record, then the doorbell: first 8 bytes of the last WQE's ctrl segment into the BlueFlame
-    // register, alternating between the two registers as libmlx5 does
-    std::atomic_thread_fence(std::memory_order_release);
-    *(volatile uint32_t*)&qp->dbrec[rn::DBR_SND] = rn::wq_dbr_word(head);
-    std::atomic_thread_fence(std::memory_order_release);
-    unsigned long long db;
-    memcpy(&db, qp->sq + (((head - 1) & (qp->sq_cnt - 1)) << 6), 8);
-    __atomic_store_n((unsigned long long*)(qp->uar + kBfOffset + qp->bf_off), db, __ATOMIC_RELEASE);
-    qp->bf_off ^= kBfSize;
-    qp->sq_head = head;
-  }
+  if (head != first) ring_sq(qp, head);
   return rc;
 }
 
@@ -959,7 +1003,7 @@ MOCK_API int ibv_destroy_cq(ibv_cq* c) {
 MOCK_API ibv_qp* ibv_create_qp(ibv_pd* pd, ibv_qp_init_attr* a) {
   if (!pd || !a || !a->send_cq || !a->recv_cq) { errno = EINVAL; return nullptr; }
   if (a->qp_type != IBV_QPT_RC) { errno = EOPNOTSUPP; return nullptr; }
-  if (a->cap.max_send_wr < 1 || a->cap.max_send_wr > 16384 || a->cap.max_recv_wr > 16384 || a->cap.max_send_sge > 1 || a->cap.max_recv_sge > 1 ||
+  if (a->cap.max_send_wr < 1 || a->cap.max_send_wr > 16384 || a->cap.max_recv_wr > 16384 || a->cap.max_send_sge > rn::MAX_SGE || a->cap.max_recv_sge > 1 ||
       a->cap.max_inline_data > rn::MAX_INLINE) {
     errno = EINVAL;
     return nullptr;
@@ -984,12 +1028,13 @@ MOCK_API ibv_qp* ibv_create_qp(ibv_pd* pd, ibv_qp_init_attr* a) {
   q->rq = q->buf; q->sq = q->buf + rq_bytes;
   q->sq_wrid.assign(q->sq_cnt, 0); q->rq_wrid.assign(q->rq_cnt, 0);
   q->sq_sig_all = a->sq_sig_all;
+  q->max_sge = a->cap.max_send_sge ? a->cap.max_send_sge : 1;   // what was asked for: ctrl + raddr + two data segments fit one WQEBB
   q->v.context = pd->context; q->v.qp_context = a->qp_context; q->v.pd = pd; q->v.send_cq = a->send_cq; q->v.recv_cq = a->recv_cq;
   q->v.handle = qpn; q->v.qp_num = qpn; q->v.state = IBV_QPS_RESET; q->v.qp_type = IBV_QPT_RC;
   pthread_mutex_init(&q->v.mutex, nullptr);
   pthread_cond_init(&q->v.cond, nullptr);
   a->cap.max_send_wr = q->sq_cnt; a->cap.max_recv_wr = q->rq_cnt; a->cap.max_inline_data = rn::MAX_INLINE;
-  a->cap.max_send_sge = 1; a->cap.max_recv_sge = 1;
+  a->cap.max_send_sge = q->max_sge; a->cap.max_recv_sge = 1;
   dev->qps[qpn] = q;
   return &q->v;
 }
@@ -1082,6 +1127,25 @@ MOCK_API int mock_qp_stats(ibv_qp* qq, MockQpStats* o) {
   std::lock_guard<std::recursive_mutex> g(g_mu);
   o->n_wqe = q->n_wqe; o->n_cqe = q->n_cqe; o->n_err = q->n_err; o->n_bytes = q->n_bytes; o->n_rnr = q->n_rnr;
   o->n_db_no_progress = q->n_db_no_progress; o->n_doorbells = q->n_doorbells; o->hw_sq_cons = q->hw_sq_cons; o->sq_cq_overruns = q->scq->overruns;
+  return 0;
+}
+// Test hook: post a caller-built WQE the way mock_post_send posts the ones it builds -- its 64 bytes as given, with this
+// QP's number and the next index written into the ctrl segment.  It hands the NIC WQEs no poster makes (a two-segment
+// list with a zero-length segment).
+MOCK_API int mock_post_wqe(ibv_qp* q, const uint8_t* wqe64, uint64_t wr_id) {
+  MockQp* qp = reinterpret_cast<MockQp*>(q);
+  std::lock_guard<std::mutex> g(qp->post_mu);
+  if (q->state != IBV_QPS_RTS && q->state != IBV_QPS_ERR && q->state != IBV_QPS_SQD) return EINVAL;   // as mock_post_send
+  const uint64_t head = qp->sq_head;
+  if (head - qp->sq_tail >= qp->sq_cnt) return ENOMEM;
+  rn::Wqe64 w;
+  memcpy(&w, wqe64, 64);
+  const uint32_t w0 = be32(w.ctrl.opmod_idx_opcode), w1 = be32(w.ctrl.qpn_ds);
+  w.ctrl.opmod_idx_opcode = rn::ctrl_word0((uint8_t)w0, (uint16_t)head, (uint8_t)(w0 >> 24));
+  w.ctrl.qpn_ds = rn::ctrl_word1(q->qp_num, (uint8_t)(w1 & 0x3f));
+  memcpy(qp->sq + ((head & (qp->sq_cnt - 1)) << 6), &w, 64);
+  qp->sq_wrid[head & (qp->sq_cnt - 1)] = wr_id;
+  ring_sq(qp, head + 1);
   return 0;
 }
 // CPU-only CI of the peer-memory path: declare a host range to be "GPU memory" (ib_core cannot pin it; a peer

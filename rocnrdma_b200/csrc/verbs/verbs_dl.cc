@@ -89,6 +89,7 @@ struct Api {
   int (*mock_declare_gpu_range)(uint64_t, uint64_t) = nullptr;
   int (*mock_gpu_free)(uint64_t) = nullptr;
   void (*mock_set_rnr_timeout_ms)(uint64_t) = nullptr;
+  int (*mock_post_wqe)(ibv_qp*, const uint8_t*, uint64_t) = nullptr;
   const char* (*mock_bridge_status)() = nullptr;
 };
 std::mutex g_api_mu;
@@ -118,7 +119,7 @@ Api& api() {
   SYM(destroy_cq, "ibv_destroy_cq"); SYM(create_qp, "ibv_create_qp"); SYM(destroy_qp, "ibv_destroy_qp");
   SYM(modify_qp, "ibv_modify_qp"); SYM(query_port, "ibv_query_port"); SYM(query_gid, "ibv_query_gid");
   SYM(mock_qp_stats, "mock_qp_stats"); SYM(mock_declare_gpu_range, "mock_declare_gpu_range"); SYM(mock_gpu_free, "mock_gpu_free");
-  SYM(mock_set_rnr_timeout_ms, "mock_set_rnr_timeout_ms"); SYM(mock_bridge_status, "mock_bridge_status");
+  SYM(mock_set_rnr_timeout_ms, "mock_set_rnr_timeout_ms"); SYM(mock_post_wqe, "mock_post_wqe"); SYM(mock_bridge_status, "mock_bridge_status");
 #undef SYM
   a.is_mock = dlsym(a.verbs, "mock_verbs_is_mock") != nullptr;
   if (a.mlx5) a.dv_init_obj = (decltype(a.dv_init_obj))dlsym(a.mlx5, "mlx5dv_init_obj");
@@ -145,6 +146,7 @@ struct QpH {
   ibv_qp* qp;
   uint32_t sq_depth, rq_depth;
   uint32_t max_inline = 0;    // what the provider granted (asked for: the 28 bytes one WQEBB holds)
+  uint32_t max_sge = 1;       // send SGEs the provider granted, capped at the two one WQEBB holds
   uint64_t next_wr_id = 1;
   bool raw_owned = false;     // queues handed to the GPU: host posting would fight over the producer index
   int proxy_slot = -1;
@@ -361,17 +363,19 @@ RN_API void* rn_verbs_create_qp(void* dev, void* scq, void* rcq, uint32_t sq_dep
   memset(&ia, 0, sizeof ia);
   ia.send_cq = ((CqH*)scq)->cq; ia.recv_cq = ((CqH*)(rcq ? rcq : scq))->cq;
   ia.qp_type = IBV_QPT_RC;
-  ia.cap.max_send_wr = sq_depth; ia.cap.max_recv_wr = rq_depth; ia.cap.max_send_sge = 1; ia.cap.max_recv_sge = 1;
-  // 28 inline bytes next to ctrl + raddr is still one WQEBB with one SGE, so libmlx5's send WQE size does not grow
+  // Two send SGEs (ctrl + raddr + two data segments) or 28 inline bytes next to ctrl + raddr: either is one 64-byte WQEBB.
+  ia.cap.max_send_wr = sq_depth; ia.cap.max_recv_wr = rq_depth; ia.cap.max_send_sge = rn::MAX_SGE; ia.cap.max_recv_sge = 1;
   ia.cap.max_inline_data = rn::MAX_INLINE;
   ibv_qp* qp = api().create_qp(d->pd, &ia);
   if (!qp) { why(0, "ibv_create_qp failed: errno %d", errno); return nullptr; }
   QpH* q = new QpH();
   q->dev = d; q->scq = (CqH*)scq; q->rcq = (CqH*)(rcq ? rcq : scq); q->qp = qp;
   q->sq_depth = ia.cap.max_send_wr; q->rq_depth = ia.cap.max_recv_wr; q->max_inline = ia.cap.max_inline_data;
+  q->max_sge = ia.cap.max_send_sge < rn::MAX_SGE ? ia.cap.max_send_sge : rn::MAX_SGE;
   return q;
 }
 RN_API uint32_t rn_verbs_qp_max_inline(void* qp) { return ((QpH*)qp)->max_inline; }
+RN_API uint32_t rn_verbs_qp_max_sge(void* qp) { return ((QpH*)qp)->max_sge; }
 // Host ranges rn_verbs_map_qp_to_gpu registered with CUDA, reference-counted: a CQ shared by two QPs is registered
 // once and stays mapped until the last QP that mapped it is destroyed.  Each range is unregistered before the provider
 // frees its memory.  A registration left behind on freed memory would make a later queue that lands on overlapping
@@ -535,6 +539,43 @@ RN_API int rn_verbs_post_inline(void* qp, uint32_t opcode, uint64_t raddr, uint3
   wr.wr.rdma.remote_addr = raddr; wr.wr.rdma.rkey = rkey;
   int rc = ibv_post_send(q->qp, &wr, &bad);
   if (rc) return why(-rc, "ibv_post_send failed: %d (%s)", rc, strerror(rc));
+  if (wr_id_out) *wr_id_out = wr.wr_id;
+  return 0;
+}
+// A work request with a scatter-gather list of n entries (opcode as in rn_verbs_post_send; the atomics are passed through
+// with zero operands): the message is the entries concatenated in list order.  flags as in rn_verbs_post_send, plus
+// RN_WR_INLINE: the entries are host bytes the provider concatenates into the WQE.  The provider judges the list (its
+// max_send_sge, the atomics' single SGE, the inline limit): its error comes back as -errno, and rn_verbs_why() says whether
+// it named this work request as the bad one.
+enum : int { RN_WR_INLINE = 4 };
+RN_API int rn_verbs_post_sg(void* qp, uint32_t opcode, const rn::Sge* sg, int n, uint64_t raddr, uint32_t rkey, int flags,
+                            uint32_t imm, uint64_t* wr_id_out) {
+  QpH* q = (QpH*)qp;
+  if (q->raw_owned) return why(-16, "this QP's queues are owned by the GPU poster; host posting would corrupt the producer index");
+  constexpr int kMax = 4;   // room to pass an over-long list to the provider, whose refusal is the one that counts
+  if (n < 0 || n > kMax) return why(-22, "rn_verbs_post_sg: %d entries (at most %d are passed on)", n, kMax);
+  ibv_sge sge[kMax];
+  for (int i = 0; i < n; ++i) sge[i] = ibv_sge{sg[i].addr, sg[i].bytes, sg[i].lkey};
+  ibv_send_wr wr, *bad = nullptr;
+  memset(&wr, 0, sizeof wr);
+  wr.wr_id = q->next_wr_id++;
+  wr.sg_list = sge; wr.num_sge = n;
+  switch (opcode) {
+    case 0x08: wr.opcode = IBV_WR_RDMA_WRITE; break;
+    case 0x09: wr.opcode = IBV_WR_RDMA_WRITE_WITH_IMM; break;
+    case 0x0a: wr.opcode = IBV_WR_SEND; break;
+    case 0x0b: wr.opcode = IBV_WR_SEND_WITH_IMM; break;
+    case 0x10: wr.opcode = IBV_WR_RDMA_READ; break;
+    case 0x11: wr.opcode = IBV_WR_ATOMIC_CMP_AND_SWP; break;
+    case 0x12: wr.opcode = IBV_WR_ATOMIC_FETCH_AND_ADD; break;
+    default: return why(-22, "unsupported opcode 0x%x for a host post", opcode);
+  }
+  wr.send_flags = send_flags(flags) | ((flags & RN_WR_INLINE) ? IBV_SEND_INLINE : 0u);
+  wr.imm_data = __builtin_bswap32(imm);
+  if (opcode == 0x11 || opcode == 0x12) { wr.wr.atomic.remote_addr = raddr; wr.wr.atomic.rkey = rkey; }
+  else { wr.wr.rdma.remote_addr = raddr; wr.wr.rdma.rkey = rkey; }
+  int rc = ibv_post_send(q->qp, &wr, &bad);
+  if (rc) return why(-rc, "ibv_post_send failed: %d (%s); bad_wr %s", rc, strerror(rc), bad == &wr ? "is this work request" : "not set");
   if (wr_id_out) *wr_id_out = wr.wr_id;
   return 0;
 }
@@ -758,4 +799,14 @@ RN_API int rn_verbs_mock_qp_stats(void* qp, RnMockQpStats* out) {
 RN_API int rn_verbs_mock_declare_gpu_range(uint64_t va, uint64_t len) { return api().mock_declare_gpu_range ? api().mock_declare_gpu_range(va, len) : -38; }
 RN_API int rn_verbs_mock_gpu_free(uint64_t va) { return api().mock_gpu_free ? api().mock_gpu_free(va) : -38; }
 RN_API int rn_verbs_mock_set_rnr_timeout_ms(uint64_t ms) { if (!api().mock_set_rnr_timeout_ms) return -38; api().mock_set_rnr_timeout_ms(ms); return 0; }
+// Test hook (mock provider only): post a caller-built WQE; its index and QP number are filled in.  Returns -errno.
+RN_API int rn_verbs_mock_post_wqe(void* qp, const uint8_t* wqe64, uint64_t* wr_id_out) {
+  QpH* q = (QpH*)qp;
+  if (!api().mock_post_wqe) return -38;
+  const uint64_t id = q->next_wr_id++;
+  const int rc = api().mock_post_wqe(q->qp, wqe64, id);
+  if (rc) return why(-rc, "mock_post_wqe failed: %d", rc);
+  if (wr_id_out) *wr_id_out = id;
+  return 0;
+}
 RN_API const char* rn_verbs_mock_bridge_status() { return api().mock_bridge_status ? api().mock_bridge_status() : "not a mock provider"; }

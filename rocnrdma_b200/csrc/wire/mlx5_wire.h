@@ -47,6 +47,7 @@ enum : uint32_t {
   INLINE_SEG = 0x80000000u,   // byte_count flag: the payload follows in the WQE itself
   MAX_BYTE_COUNT = 0x7fffffffu,   // largest byte count a gather data segment carries (bit 31 is INLINE_SEG)
   MAX_MSG = 1u << 30,         // longest message, inclusive (DESIGN.md 3.1); longer WRITE / READ / SEND: LOCAL_LENGTH_ERR
+  MAX_SGE = 2,                // scatter-gather entries per WRITE / READ / SEND: ctrl + raddr + two data segments fill one WQEBB
 };
 
 enum Opcode : uint8_t {  // ctrl.opmod_idx_opcode[7:0]
@@ -135,6 +136,9 @@ struct alignas(64) Wqe64 {
   union {
     struct { RaddrSeg raddr; DataSeg data; uint8_t pad[16]; } rdma;
     struct { DataSeg data; uint8_t pad[32]; } send;
+    // two-entry gather / scatter list: RDMA ds = 4 (exactly one WQEBB), SEND ds = 3
+    struct { RaddrSeg raddr; DataSeg data[2]; } rdma_sg;
+    struct { DataSeg data[2]; uint8_t pad[16]; } send_sg;
     struct { RaddrSeg raddr; AtomicSeg atomic; DataSeg data; } atom;
     // inline: the payload travels in the WQE (ds = 2 + ceil((4 + n) / 16) for RDMA, 1 + ... for SEND)
     struct { RaddrSeg raddr; InlineSeg inl; InlinePayload data; } rdma_inl;
@@ -290,6 +294,47 @@ RN_HD void build_inline_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t
   for (uint32_t i = 0; i < n; ++i) d.w[i / 4] |= (uint32_t)static_cast<const uint8_t*>(data)[i] << (8 * (i % 4));
   build_inline_wqe(w, opcode, wqe_idx, qpn, raddr, rkey, d, n, fm_ce_se, imm);
 }
+// One scatter-gather entry: `bytes` at `addr` under `lkey`.
+struct Sge { uint64_t addr; uint32_t lkey; uint32_t bytes; };
+// Drop zero-length entries, as libmlx5 does; returns how many remain (entries past MAX_SGE are the caller's to refuse).
+RN_HD int sg_compact(const Sge* in, int n, Sge* out) {
+  int k = 0;
+  for (int i = 0; i < n && i < (int)MAX_SGE; ++i)
+    if (in[i].bytes) out[k++] = in[i];
+  return k;
+}
+// Gather WRITE / WRITE_IMM or scatter READ of up to MAX_SGE entries: the message is the entries concatenated in list
+// order, at [raddr, raddr + sum).  Two non-empty entries: ctrl + raddr + two data segments (ds = 4, one WQEBB).  At most
+// one: exactly build_rdma_wqe's WQE, of that entry (of entry 0 with 0 bytes when every entry is empty).
+RN_HD void build_rdma_sg_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, const Sge* sg, int n,
+                             uint64_t raddr, uint32_t rkey, uint8_t fm_ce_se, uint32_t imm) {
+  Sge e[MAX_SGE];
+  const int k = sg_compact(sg, n, e);
+  if (k < 2) {
+    const Sge one = k ? e[0] : Sge{n ? sg[0].addr : 0, n ? sg[0].lkey : 0, 0};
+    build_rdma_wqe(w, opcode, wqe_idx, qpn, one.addr, one.lkey, raddr, rkey, one.bytes, fm_ce_se, imm);
+    return;
+  }
+  encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, 4, fm_ce_se, imm);
+  encode_raddr(&w->rdma_sg.raddr, raddr, rkey);
+  encode_data(&w->rdma_sg.data[0], e[0].addr, e[0].lkey, e[0].bytes);
+  encode_data(&w->rdma_sg.data[1], e[1].addr, e[1].lkey, e[1].bytes);
+}
+// Gather SEND / SEND_IMM: ctrl + two data segments (ds = 3); at most one non-empty entry: build_send_wqe's WQE.
+RN_HD void build_send_sg_wqe(Wqe64* w, uint8_t opcode, uint16_t wqe_idx, uint32_t qpn, const Sge* sg, int n,
+                             uint8_t fm_ce_se, uint32_t imm) {
+  Sge e[MAX_SGE];
+  const int k = sg_compact(sg, n, e);
+  if (k < 2) {
+    const Sge one = k ? e[0] : Sge{n ? sg[0].addr : 0, n ? sg[0].lkey : 0, 0};
+    build_send_wqe(w, opcode, wqe_idx, qpn, one.addr, one.lkey, one.bytes, fm_ce_se, imm);
+    return;
+  }
+  encode_ctrl(&w->ctrl, opcode, wqe_idx, qpn, 3, fm_ce_se, imm);
+  encode_data(&w->send_sg.data[0], e[0].addr, e[0].lkey, e[0].bytes);
+  encode_data(&w->send_sg.data[1], e[1].addr, e[1].lkey, e[1].bytes);
+  for (int i = 0; i < 16; ++i) w->send_sg.pad[i] = 0;
+}
 // NOP (ds = 1): a ctrl segment and nothing else.  Signaled, its CQE shows that every earlier WQE of the QP completed.
 RN_HD void build_nop_wqe(Wqe64* w, uint16_t wqe_idx, uint32_t qpn, uint8_t fm_ce_se) {
   encode_ctrl(&w->ctrl, OP_NOP, wqe_idx, qpn, 1, fm_ce_se, 0);
@@ -305,7 +350,22 @@ struct WqeView {
   uint32_t rkey, lkey, bytes;
   uint64_t swap_add, compare;    // atomics only (native byte order)
   uint8_t inl_off;               // inline WQE: offset of its `bytes` payload bytes in the WQEBB; 0: gather (laddr / lkey)
+  uint8_t nsge;                  // gather entries: 2 for a two-entry list (then bytes = len0 + the second entry's), else 1
+  uint32_t len0;                 // nsge == 2 only: entry 0's length, and entry 1 (bytes - len0 at laddr1 / lkey1)
+  uint64_t laddr1;
+  uint32_t lkey1;
 };
+// A data segment that names a second gather entry: its byte count without the inline flag, else false.
+RN_HD bool sg_second(const DataSeg& d, WqeView* v) {
+  const uint32_t bc = be32(d.byte_count);
+  if (bc & INLINE_SEG) return false;
+  v->nsge = 2;
+  v->len0 = v->bytes;
+  v->laddr1 = be64(d.addr);
+  v->lkey1 = be32(d.lkey);
+  v->bytes += bc;                // each count is below 2^31: the sum fits
+  return true;
+}
 RN_HD bool is_atomic(uint8_t opcode) { return opcode == OP_ATOMIC_CS || opcode == OP_ATOMIC_FA; }
 // An inline byte count is well formed when 1 <= n <= MAX_INLINE and ds counts exactly its segments.
 RN_HD bool inline_ok(uint32_t n, uint8_t ds, uint8_t head_segs) {
@@ -322,6 +382,7 @@ RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
   v->imm = be32(w->ctrl.imm);
   v->raddr = 0; v->rkey = 0; v->laddr = 0; v->lkey = 0; v->bytes = 0;
   v->swap_add = 0; v->compare = 0; v->inl_off = 0;
+  v->nsge = 1; v->len0 = 0; v->laddr1 = 0; v->lkey1 = 0;
   switch (v->opcode) {
     case OP_ATOMIC_CS: case OP_ATOMIC_FA:
       if (v->ds != 4 || (be32(w->atom.data.byte_count) & INLINE_SEG)) return false;
@@ -340,10 +401,12 @@ RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
         if (v->opcode == OP_RDMA_READ || !inline_ok(v->bytes, v->ds, 2)) return false;
         v->inl_off = INLINE_OFF_RDMA;
       } else {
-        if (v->ds != 3) return false;
+        // ds 3: one entry; ds 4: two (the inline flag above already told a 13-28-byte inline WRITE apart)
+        if (v->ds != 3 && v->ds != 4) return false;
         v->laddr = be64(w->rdma.data.addr);
         v->lkey = be32(w->rdma.data.lkey);
         v->bytes = bc;
+        if (v->ds == 4 && !sg_second(w->rdma_sg.data[1], v)) return false;
       }
       v->raddr = be64(w->rdma.raddr.raddr);
       v->rkey = be32(w->rdma.raddr.rkey);
@@ -357,11 +420,11 @@ RN_HD bool decode_wqe(const Wqe64* w, WqeView* v) {
         v->inl_off = INLINE_OFF_SEND;
         return true;
       }
-      if (v->ds != 2) return false;
+      if (v->ds != 2 && v->ds != 3) return false;
       v->laddr = be64(w->send.data.addr);
       v->lkey = be32(w->send.data.lkey);
       v->bytes = bc;
-      return true;
+      return v->ds == 2 || sg_second(w->send_sg.data[1], v);
     }
     case OP_NOP:
       return v->ds == 1;

@@ -328,6 +328,51 @@ def put_inline(qps, values, dst_mr, nbytes: int, iters: int = 1, window: int = 0
     return parse_stream_out(out_view, nq, nbytes)
 
 
+GATHER_VIA = {"poster": 0, "one_call": 1}
+_OP_WRITE, _OP_SEND, _OP_READ = 0x08, 0x0A, 0x10
+
+
+def gather_stream(qps, opcode: int, mr0, mr1, remote_mr, nbytes: int, split: int, iters: int = 1, window: int = 0,
+                  signal_every: int = 1, burst: int = 1, stride: int = 0, slot_stride: int = 0, nslots: int = 1,
+                  via: str = "poster", timeout_ms: int = 2000, stream=None, sync: bool = True,
+                  scratch_off: int = 36864) -> StreamResult:
+    """Device-posted two-entry work requests: one warp per QP posts ``iters`` messages of ``nbytes``, each one work
+    request whose scatter-gather list is cut at ``split`` bytes.  Message ``i`` of QP ``c`` uses slot offset
+    ``o = c * stride + (i % nslots) * slot_stride``: entry 0 is ``split`` bytes at ``mr0.addr + o``, entry 1 the other
+    ``nbytes - split`` at ``mr1.addr + o`` (the same slot of a second MR), and the remote side is ``nbytes`` at
+    ``remote_mr.addr + o``.  ``OP_RDMA_WRITE`` gathers the entries there, ``OP_SEND`` into the responder's next receive
+    (``remote_mr`` unused), ``OP_RDMA_READ`` scatters the remote bytes into the entries.  A zero-length entry is dropped,
+    so ``split`` 0 or ``nbytes`` posts one-entry work requests.
+    ``via="poster"`` uses the windowed, bursted exclusive poster of :func:`rdma_stream` (``window``, ``burst`` and
+    ``signal_every`` as there); ``via="one_call"`` posts every message with ``dev::rdma_write_sg`` / ``rdma_read_sg`` /
+    ``rdma_send_sg`` through the shared submit and keeps at most ``window`` in flight.  Returns a :class:`StreamResult`."""
+    nbytes, split = N.byte_count(nbytes), N.byte_count(split, "split")
+    if split > nbytes:
+        raise ValueError(f"split={split} exceeds nbytes={nbytes}")
+    if opcode not in (_OP_WRITE, _OP_READ, _OP_SEND):
+        raise ValueError(f"opcode 0x{opcode:x}: gather_stream posts RDMA_WRITE, RDMA_READ or SEND")
+    if via not in GATHER_VIA:
+        raise ValueError(f"via must be one of {sorted(GATHER_VIA)}")
+    lib = N.load()
+    if not isinstance(qps, (list, tuple)):
+        qps = [qps]
+    ctx = qps[0].ctx
+    nq = len(qps)
+    ws = work_stream(ctx, stream)
+    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
+    out_addr, out_view = ctx.scratch(nq * 64, offset=scratch_off)
+    rc = lib.rn_k_gather_stream(_stream_ptr(ws), qp_arr, nq, opcode, mr0.addr, mr0.lkey, mr1.addr, mr1.lkey,
+                                remote_mr.addr if remote_mr is not None else 0, remote_mr.rkey if remote_mr is not None else 0,
+                                stride, nbytes, split, slot_stride, nslots, iters, window, signal_every, burst, GATHER_VIA[via],
+                                timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"gather_stream launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_stream_out(out_view, nq, nbytes)
+
+
 def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, stream=None, sync: bool = True,
                 check=None, scratch_off: int = 20544):
     """Receiver side of :func:`put_signal`, on the GPU that holds the signal: waits until the u64 at ``signal`` (a

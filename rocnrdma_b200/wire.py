@@ -16,6 +16,7 @@ MAX_INLINE = 28            # largest inline payload: ctrl + raddr + a 4-byte inl
 INLINE_SEG = 0x80000000    # byte_count flag of an inline data segment
 MAX_BYTE_COUNT = 0x7FFFFFFF  # largest byte count a gather data segment carries
 MAX_MSG = 1 << 30          # longest message, inclusive; a longer WRITE / READ / SEND completes with LOCAL_LENGTH_ERR
+MAX_SGE = 2                # scatter-gather entries per WRITE / READ / SEND: ctrl + raddr + two data segments fill one WQEBB
 
 OP_NOP = 0x00
 OP_SEND_INVAL = 0x01
@@ -84,6 +85,32 @@ def send_wqe(opcode, wqe_idx, qpn, laddr, lkey, nbytes, fm_ce_se=CTRL_CQ_UPDATE,
     return b + bytes(WQEBB - len(b))
 
 
+def _nonempty(sges):
+    return [tuple(e) for e in sges if e[2]]
+
+
+def rdma_sg_wqe(opcode, wqe_idx, qpn, sges, raddr, rkey, fm_ce_se=CTRL_CQ_UPDATE, imm=0) -> bytes:
+    """Gather WRITE / WRITE_IMM or scatter READ of up to ``MAX_SGE`` ``(addr, lkey, nbytes)`` entries; the message is
+    their concatenation in list order.  Zero-length entries are dropped; two remaining: ctrl + raddr + two data segments
+    (ds = 4).  At most one: exactly :func:`rdma_wqe` of it (of entry 0 with 0 bytes when none remains)."""
+    e = _nonempty(sges)
+    if len(e) < 2:
+        a, k, n = e[0] if e else (sges[0][0], sges[0][1], 0)
+        return rdma_wqe(opcode, wqe_idx, qpn, a, k, raddr, rkey, n, fm_ce_se, imm)
+    return (ctrl_seg(opcode, wqe_idx, qpn, 4, fm_ce_se, imm) + raddr_seg(raddr, rkey)
+            + data_seg(e[0][0], e[0][1], e[0][2]) + data_seg(e[1][0], e[1][1], e[1][2]))
+
+
+def send_sg_wqe(opcode, wqe_idx, qpn, sges, fm_ce_se=CTRL_CQ_UPDATE, imm=0) -> bytes:
+    """Gather SEND / SEND_IMM: ctrl + two data segments (ds = 3); at most one non-empty entry: :func:`send_wqe` of it."""
+    e = _nonempty(sges)
+    if len(e) < 2:
+        a, k, n = e[0] if e else (sges[0][0], sges[0][1], 0)
+        return send_wqe(opcode, wqe_idx, qpn, a, k, n, fm_ce_se, imm)
+    b = ctrl_seg(opcode, wqe_idx, qpn, 3, fm_ce_se, imm) + data_seg(e[0][0], e[0][1], e[0][2]) + data_seg(e[1][0], e[1][1], e[1][2])
+    return b + bytes(WQEBB - len(b))
+
+
 def atomic_seg(swap_add: int, compare: int = 0) -> bytes:
     """The 16-byte atomic segment: big-endian ``swap_add`` (FA: the addend; CS: the swap value), then ``compare``."""
     return struct.pack(">QQ", swap_add & 0xFFFFFFFFFFFFFFFF, compare & 0xFFFFFFFFFFFFFFFF)
@@ -141,11 +168,21 @@ class WqeView:
     swap_add: int = 0
     compare: int = 0
     inline_data: Optional[bytes] = None    # the payload of an inline WQE (laddr / lkey are then 0)
+    sges: Optional[list] = None            # WRITE / READ / SEND: the (addr, lkey, nbytes) entries; nbytes above is their total
+
+
+def _second_seg(b: bytes, off: int, v: WqeView):
+    n, lkey, addr = struct.unpack_from(">IIQ", b, off)
+    if n & INLINE_SEG:
+        raise ValueError("the second data segment of a scatter-gather list cannot be inline")
+    v.sges.append((addr, lkey, n))
+    v.nbytes += n
 
 
 def decode_wqe(b: bytes) -> WqeView:
     """Decode one WQEBB.  An inline WQE (INLINE_SEG set on a WRITE, WRITE_IMM, SEND or SEND_IMM) fills ``inline_data``;
-    one whose length or ds is out of range raises ``ValueError``, as does the flag on a READ."""
+    one whose length or ds is out of range raises ``ValueError``, as does the flag on a READ.  A WRITE, READ or SEND fills
+    ``sges``: two entries for RDMA ds = 4 or SEND ds = 3, whose second segment must not carry the inline flag."""
     assert len(b) >= WQEBB
     w0, w1, _sig, _r0, _r1, fm, imm = struct.unpack_from(">IIBBBBI", b, 0)
     v = WqeView(opcode=w0 & 0xFF, opmod=w0 >> 24, wqe_idx=(w0 >> 8) & 0xFFFF, qpn=w1 >> 8, ds=w1 & 0x3F,
@@ -163,6 +200,9 @@ def decode_wqe(b: bytes) -> WqeView:
         v.raddr, v.rkey, _ = struct.unpack_from(">QII", b, 16)
         n, v.lkey, v.laddr = struct.unpack_from(">IIQ", b, 32)
         v.nbytes = n & 0x7FFFFFFF
+        v.sges = [(v.laddr, v.lkey, v.nbytes)]
+        if v.ds == 4:
+            _second_seg(b, 48, v)
     elif v.opcode in (OP_ATOMIC_CS, OP_ATOMIC_FA):
         v.raddr, v.rkey, _ = struct.unpack_from(">QII", b, 16)
         v.swap_add, v.compare = struct.unpack_from(">QQ", b, 32)
@@ -171,6 +211,9 @@ def decode_wqe(b: bytes) -> WqeView:
     elif v.opcode in (OP_SEND, OP_SEND_IMM):
         n, v.lkey, v.laddr = struct.unpack_from(">IIQ", b, 16)
         v.nbytes = n & 0x7FFFFFFF
+        v.sges = [(v.laddr, v.lkey, v.nbytes)]
+        if v.ds == 3:
+            _second_seg(b, 32, v)
     return v
 
 
