@@ -135,7 +135,7 @@ _SIGS = {
     "rn_k_shared_post_stress": (i32, [u64, u64, i32, u64, u32, u64, u32, u32, u64, u64, u64]),
     "rn_k_recv_consume": (i32, [u64, u64, u32, u32, u64, u64, u64, u64, u32, u32]),
     "rn_hca_enable_peer": (i32, [vp, i32]),
-    "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64]),
+    "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64, u64]),
     "rn_k_rdma_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u32, u32, u32, u32, u64, u32, u64, u64, u32]),
     "rn_k_write_read": (i32, [u64, u64, u64, u32, u64, u32, u64, u32, u32, u32, u32, u64, u64]),
     "rn_stream_clamp": (None, [u32, C.POINTER(u32), C.POINTER(u32)]),
@@ -156,6 +156,7 @@ _SIGS = {
                               u32, u32, u32, u64, u64]),
     "rn_k_gather_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u64, u32, u32, u64, u32, u32, u32,
                                  u32, u32, u32, u64, u64]),
+    "rn_k_read_records": (i32, [u64, u64, u64, u32, u64, u32, u64, u32, u32, u64, u64, u32, u32, u32, u64, u64]),
     "rn_gpu_page_size": (u64, []),
     "rn_dmabuf_export": (i32, [u64, u64, C.POINTER(i32)]),
     "rn_dmabuf_close": (i32, [i32]),

@@ -197,6 +197,8 @@ struct UnpackArgs {
   uint32_t n_chunks;
   QpDev* qp;                 // receiver QP whose recv CQ announces records (nullptr: data already there)
   unsigned int* arrived;     // [n_chunks] flags ; [n_chunks] CTAs done ; [n_chunks+1] records seen (self-cleaned)
+  const unsigned long long* ready;   // one arrival word per record, nonzero once it has landed (read_records, recv_consume);
+                                     // nullptr: no words.  Never together with qp.
   unsigned long long* out;   // [status, t_start, t_end, records_seen]
   uint64_t timeout_ns;
 };
@@ -210,7 +212,9 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
   // (The first version let every CTA poll the CQ for "its" record: hundreds of pollers contending for one consumer index made
   // the consumer, not the wire, the tail of the pack -> NVLink -> unpack chain.)  The other CTAs unpack, chunk-major, so that
   // every worker is on the oldest record not yet unpacked, and wait on the flag of the record they are about to read.
-  const bool polled = a.qp != nullptr;
+  // With arrival words there is no poller: every worker waits on the word of the record it is about to read, each wait
+  // bounded by timeout_ns, and a worker that times out stops the others through abort_flag.
+  const bool polled = a.qp != nullptr, gated = polled || a.ready != nullptr;
   unsigned int* abort_flag = a.arrived + a.n_chunks + 2;
   if (polled && blockIdx.x == 0) {
     if (threadIdx.x == 0) {
@@ -239,7 +243,7 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
     const uint64_t total = (uint64_t)a.n_chunks * tiles_per_chunk;
     constexpr int G = 4;
     for (uint64_t T0 = first; T0 < total; T0 += (uint64_t)stride * G) {
-      if (polled) {
+      if (gated) {
         if (threadIdx.x == 0) {                                  // the records this step reads have arrived
           ok = 1;
           uint32_t last = ~0u;
@@ -249,6 +253,21 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
             const uint32_t chunk = (uint32_t)(T / tiles_per_chunk);
             if (chunk == last) continue;
             last = chunk;
+            if (a.ready) {
+              unsigned long long v, t0 = 0;
+              for (unsigned n = 0;; ++n) {
+                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(a.ready + chunk) : "memory");
+                if (v) break;
+                if (*(volatile unsigned int*)abort_flag) { ok = 0; break; }
+                const unsigned long long now = globaltimer_ns();
+                if (!t0) t0 = now;
+                else if (now - t0 > a.timeout_ns) {
+                  a.out[0] = (unsigned long long)(long long)WAIT_TIMEOUT; atomicExch(abort_flag, 1u); ok = 0; break;
+                }
+                __nanosleep(n < 64 ? 50 : 400);
+              }
+              continue;
+            }
             for (unsigned n = 0; *(volatile unsigned int*)&a.arrived[chunk] == 0; ++n) {
               if (*(volatile unsigned int*)abort_flag) { ok = 0; break; }
               __nanosleep(n < 64 ? 50 : 400);
@@ -306,7 +325,10 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
       fence_gpu();
       a.out[1] = t_start;
       a.out[2] = globaltimer_ns();
-      a.out[3] = *(volatile unsigned int*)&a.arrived[a.n_chunks + 1];
+      uint32_t seen = *(volatile unsigned int*)&a.arrived[a.n_chunks + 1];
+      if (a.ready)                                                        // records whose word is set by now
+        for (uint32_t c = 0; c < a.n_chunks; ++c) seen += ld_u64_volatile(a.ready + c) != 0;
+      a.out[3] = seen;
       for (uint32_t c = 0; c <= a.n_chunks + 2; ++c) a.arrived[c] = 0;   // self-clean
     }
   }
@@ -345,7 +367,8 @@ RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t
 
 RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t dst, uint64_t n_elems,
                            uint32_t chunk_elems, uint64_t qp_dev, uint64_t arrived_dev, uint64_t out_dev,
-                           uint64_t timeout_ms) {
+                           uint64_t timeout_ms, uint64_t ready_dev) {
+  if (qp_dev && ready_dev) return -22;
   if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
     return -22;
   if ((staging | dst) & 31) return -22;                        // 256-bit loads / stores: records and output must be 32-byte aligned
@@ -353,10 +376,11 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
   a.staging = (const uint8_t*)staging; a.dst = (__nv_bfloat16*)dst; a.n_elems = n_elems; a.chunk_elems = chunk_elems;
   a.n_chunks = (uint32_t)(n_elems / chunk_elems); a.qp = (QpDev*)qp_dev; a.arrived = (unsigned int*)arrived_dev;
   a.out = (unsigned long long*)out_dev; a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.ready = (const unsigned long long*)ready_dev;
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
   // waiting for arrivals the kernel shares the GPU with whatever produces them (a pack kernel, an engine): one CTA per SM then
-  if (grid <= 0) grid = qp_dev ? device_sms() : device_sms() * 4;
+  if (grid <= 0) grid = (qp_dev || ready_dev) ? device_sms() : device_sms() * 4;
   {
     const uint64_t total_tiles = n_elems / kTileElems;
     if ((uint64_t)grid > total_tiles) grid = (int)total_tiles;

@@ -548,6 +548,131 @@ RN_API int rn_k_gather_stream(uint64_t stream, const uint64_t* qps_host, uint32_
   return (int)cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- pulled records with arrival words
+// One warp owns the QP and its send CQ (dev::Poster) and pulls n fixed-size records: record r is one RDMA READ of
+// rec_bytes from raddr + j * src_stride (j = indices[r], or r) into laddr + r * rec_bytes.  Record r is WQE base + r.
+// Word r of `ready` gets %globaltimer (st.release.gpu) once record r has landed, the same arrival word recv_consume writes
+// for pushed records, so unpack_fp8(ready=) and gemm_mxfp8(a_ready=) consume pulls and pushes alike.  RC completes in
+// order: a requester CQE covers its own WQE and every earlier one, a failed one only the earlier ones.  So one CQE stamps
+// up to signal_every records, all with one value, and after a failure nothing more is stamped.  The loop is stream_post's
+// (window, bursts, peek before the doorbell), but every completion is taken one at a time and stamped as it is taken,
+// the final drain included, so a record is stamped by the first CQ poll that sees its completion.
+struct ReadRecordsArgs {
+  QpDev* qp;
+  uint64_t laddr, raddr;             // dst_mr.addr + dst_off, src_mr.addr + src_off
+  uint64_t src_stride;
+  const int32_t* indices;            // nullptr: record r reads source record r
+  unsigned long long* ready;         // nullptr: no arrival words
+  uint32_t lkey, rkey, rec_bytes, n;
+  uint32_t window, burst, signal_every;
+  uint64_t timeout_ns;
+  unsigned long long* out;           // [status, t_start, t_end, records landed, first_idx, last_idx, cons, 0]
+};
+
+// Take the CQE whose tail poster_peek loaded, if it is ready and ours, and stamp the records it completes.  1 / 0 / WAIT_CQE_ERROR.
+__device__ __forceinline__ int read_records_take(Poster& p, const uint4 tail, unsigned long long base, uint32_t& landed,
+                                                 unsigned long long* ready) {
+  const int rc = poster_take(p, tail);   // its __threadfence is the acquire of everything the CQE announces
+  if (rc == 0) return 0;
+  const unsigned long long upto = p.cons - (rc < 0 ? 1 : 0);   // a failed WQE has not landed
+  if (upto > base + landed) {
+    const unsigned long long now = globaltimer_ns();
+    for (; base + landed < upto; ++landed)
+      if (ready) asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(ready + landed), "l"(now) : "memory");
+  }
+  return rc;
+}
+// Take completions one at a time until every WQE below `until` has completed.  WAIT_OK / WAIT_CQE_ERROR / WAIT_TIMEOUT.
+__device__ __forceinline__ int read_records_reap(Poster& p, unsigned long long base, uint32_t& landed, unsigned long long* ready,
+                                                 unsigned long long until, unsigned long long timeout_ns) {
+  unsigned long long t0 = 0;
+  for (unsigned it = 0; p.cons < until; ++it) {
+    const int rc = read_records_take(p, poster_peek(p), base, landed, ready);
+    if (rc < 0) return rc;
+    if (rc == 0) {
+      if (t0 == 0) t0 = globaltimer_ns();
+      else if ((it & 15) == 0 && globaltimer_ns() - t0 > timeout_ns) return WAIT_TIMEOUT;
+    }
+  }
+  return WAIT_OK;
+}
+
+__global__ void __launch_bounds__(32, 1) read_records_kernel(ReadRecordsArgs a) {
+  const uint32_t lane = threadIdx.x;
+  int status = WAIT_OK;
+  uint32_t posted = 0, landed = 0;
+  Poster p = poster_open(a.qp);
+  const unsigned long long base = p.head, depth = (unsigned long long)p.sq_mask + 1;
+  if (a.qp->state == QPS_ERR) status = WAIT_QP_ERROR;
+  const unsigned long long t0 = globaltimer_ns();
+  while (posted < a.n && status == WAIT_OK) {
+    const uint32_t m = min(a.burst, a.n - posted), r = posted + lane;
+    // this lane's record, worked out before the window wait so that it stays off the path from a completion to the doorbell
+    uint64_t src = 0;
+    bool sig = false;
+    if (lane < m) {
+      src = a.raddr + (uint64_t)(uint32_t)(a.indices ? __ldg(a.indices + r) : (int32_t)r) * a.src_stride;
+      sig = a.signal_every <= 1 || (r + 1) % a.signal_every == 0 || r + 1 == a.n;
+    }
+    int rc = WAIT_OK;
+    if (lane == 0) {
+      // at most window - m records outstanding, and room for m WQEs, before the burst is built: taken here, with stamps,
+      // so that poster_reserve never has to consume a completion itself
+      unsigned long long until = p.head + m > depth ? p.head + m - depth : 0;
+      if (a.window && posted + m > a.window && base + posted + m - a.window > until) until = base + posted + m - a.window;
+      rc = read_records_reap(p, base, landed, a.ready, until, a.timeout_ns);
+      if (rc == WAIT_OK && poster_reserve(p, m, a.timeout_ns) == ~0ull) rc = WAIT_TIMEOUT;
+    }
+    rc = __shfl_sync(0xffffffffu, rc, 0);
+    if (rc != WAIT_OK) { status = rc; break; }
+    if (lane < m) {
+      Wqe64 w;
+      build_rdma_wqe(&w, OP_RDMA_READ, (uint16_t)(base + r), p.qpn, a.laddr + (uint64_t)r * a.rec_bytes, a.lkey, src, a.rkey,
+                     a.rec_bytes, sig ? CTRL_CQ_UPDATE : 0, 0);
+      store_wqe(poster_slot(p, base + r), w);
+    }
+    if (m > 1) __syncwarp();                          // the burst's WQE bytes happen-before lane 0's release
+    if (lane == 0) {
+      const bool outstanding = p.head > p.cons;
+      uint4 tail = make_uint4(0, 0, 0, 0);
+      if (outstanding) tail = poster_peek(p);        // in flight while the doorbell's release waits for the WQE stores
+      poster_ring(p, base + posted + m);
+      if (outstanding && read_records_take(p, tail, base, landed, a.ready) < 0) status = WAIT_CQE_ERROR;
+    }
+    status = __shfl_sync(0xffffffffu, status, 0);
+    posted += m;
+  }
+  if (lane != 0) return;
+  if (status == WAIT_OK && posted) status = read_records_reap(p, base, landed, a.ready, base + posted, a.timeout_ns);
+  // after a failure the QP is in ERR and every later WQE completes flushed: take those completions (nothing is stamped)
+  // so that the queue state published below is whole
+  if (status == WAIT_CQE_ERROR && p.head > p.cons) poster_wait(p, p.head - 1, a.timeout_ns);
+  const unsigned long long t1 = globaltimer_ns();
+  poster_close(p);
+  a.out[0] = (unsigned long long)(long long)status;
+  a.out[1] = t0; a.out[2] = t1; a.out[3] = landed;
+  a.out[4] = posted ? base : ~0ull; a.out[5] = posted ? base + posted - 1 : 0;
+  a.out[6] = p.cons;
+  a.out[7] = 0;
+}
+
+RN_API int rn_k_read_records(uint64_t stream, uint64_t qp_dev, uint64_t laddr, uint32_t lkey, uint64_t raddr, uint32_t rkey,
+                             uint64_t src_stride, uint32_t rec_bytes, uint32_t n, uint64_t indices_dev, uint64_t ready_dev,
+                             uint32_t window, uint32_t burst, uint32_t signal_every, uint64_t timeout_ms, uint64_t out_dev) {
+  if (rec_bytes == 0) return -22;
+  ReadRecordsArgs a;
+  a.qp = (QpDev*)qp_dev;
+  a.laddr = laddr; a.raddr = raddr; a.src_stride = src_stride;
+  a.indices = (const int32_t*)indices_dev; a.ready = (unsigned long long*)ready_dev;
+  a.lkey = lkey; a.rkey = rkey; a.rec_bytes = rec_bytes; a.n = n;
+  rn_stream_clamp(window, &burst, &signal_every);
+  a.window = window; a.burst = burst; a.signal_every = signal_every;
+  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.out = (unsigned long long*)out_dev;
+  read_records_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
 // ---------------------------------------------------------------- signal wait (receiver side)
 // Runs on the GPU that holds the signal word.  Thread 0 polls it with system-scope acquire loads until it reaches
 // `until`; every value 1..until is stamped (%globaltimer) when first seen.  Each wait for the next arrival is bounded
@@ -809,6 +934,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncGetAttributes(&a, put_signal_kernel);
   cudaFuncGetAttributes(&a, put_inline_kernel);
   cudaFuncGetAttributes(&a, gather_stream_kernel);
+  cudaFuncGetAttributes(&a, read_records_kernel);
   cudaFuncGetAttributes(&a, signal_wait_kernel);
   cudaFuncGetAttributes(&a, cq_watch_kernel);
   cudaFuncGetAttributes(&a, fill_random_kernel);

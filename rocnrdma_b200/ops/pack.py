@@ -8,7 +8,7 @@ from dataclasses import dataclass
 import torch
 
 from .. import _native as N
-from .rdma import WAIT_STATUS, _stream_ptr, work_stream
+from .rdma import WAIT_STATUS, _stream_ptr, _device_words, work_stream
 
 TILE_ELEMS = 8192
 BLOCK = 32
@@ -94,20 +94,27 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
 
 
 def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int = 1 << 20, qp=None, grid: int = 0,
-               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_slot: int = 1):
+               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_slot: int = 1, ready=None):
     """fp8 chunk records -> bf16.  With ``qp`` the kernel waits for each record's receive
-    CQE (RDMA_WRITE_IMM, immediate = chunk id) before touching it."""
+    CQE (RDMA_WRITE_IMM, immediate = chunk id) before touching it.  With ``ready`` (int64 CUDA tensor, one arrival word
+    per record, as :func:`~rocnrdma_b200.ops.read_records` and ``recv_consume`` set them) every worker waits for the word of
+    the record it is about to read; a word still 0 after ``timeout_ms`` ends the kernel with ``TIMEOUT``.  ``qp`` and
+    ``ready`` exclude each other.  ``records_seen``: records announced on the CQ, or, with ``ready``, the words that are
+    nonzero when the kernel ends (after a ``TIMEOUT`` that can include records it never waited for or unpacked)."""
     assert dst.dtype == torch.bfloat16 and dst.is_contiguous()
     if (staging.data_ptr() | dst.data_ptr()) & 31:
         raise ValueError("unpack_fp8: records and output must be 32-byte aligned (256-bit loads / stores)")
     n = dst.numel()
+    n_chunks = n // chunk_elems
+    if qp is not None and ready is not None:
+        raise ValueError("unpack_fp8 waits on a receive CQ (qp) or on arrival words (ready), not both")
+    ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_chunks, ctx.device, "ready")
     lib = N.load()
     ws = work_stream(ctx, stream)
-    n_chunks = n // chunk_elems
     arrived = ctx.dev_scratch((n_chunks + 3) * 4, offset=scratch_slot * (256 << 10))
     out_addr, out_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
     rc = lib.rn_k_unpack_fp8(_stream_ptr(ws), grid, staging.data_ptr(), dst.data_ptr(), n, chunk_elems,
-                             qp.dev_ptr if qp is not None else 0, arrived, out_addr, timeout_ms)
+                             qp.dev_ptr if qp is not None else 0, arrived, out_addr, timeout_ms, ready_addr)
     if rc:
         raise N.NativeError(f"unpack_fp8 launch failed ({rc})")
     if not sync:

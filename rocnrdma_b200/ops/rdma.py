@@ -434,3 +434,72 @@ def parse_signal_wait(view) -> dict:
     w = (C.c_int64 * 8).from_buffer(view)
     return dict(status=WAIT_STATUS.get(w[0], str(w[0])), seen=w[3], mismatches=w[4], device_ns=w[2] - w[1],
                 t_start_ns=w[1], t_end_ns=w[2])
+
+
+def _device_words(t, dtype, n: int, device: int, what: str) -> int:
+    """Address of ``t``, a contiguous CUDA tensor of ``dtype`` with at least ``n`` entries on GPU ``device``; ``ValueError``
+    otherwise.  The values are never read on the host (that would synchronise)."""
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype:
+        raise ValueError(f"{what} must be a {dtype} tensor, not {getattr(t, 'dtype', type(t).__name__)}")
+    if not t.is_cuda or t.device.index != device:
+        raise ValueError(f"{what} must be on cuda:{device}, not {t.device}")
+    if not t.is_contiguous():
+        raise ValueError(f"{what} must be contiguous")
+    if t.numel() < n:
+        raise ValueError(f"{what} holds {t.numel()} entries; {n} are needed")
+    return t.data_ptr()
+
+
+def read_records(qp, src_mr, dst_mr, rec_bytes: int, n: int, *, indices=None, src_off: int = 0, src_stride=None,
+                 dst_off: int = 0, ready=None, window: int = 16, burst: int = 1, signal_every: int = 1, timeout_ms: int = 2000,
+                 stream=None, sync: bool = True, scratch_off: int = 40960):
+    """Pull ``n`` fixed-size records with device-posted RDMA READs and stamp an arrival word as each one lands.
+
+    Record ``r`` is one READ of ``rec_bytes`` from ``src_mr.addr + src_off + j * src_stride`` (the remote side) into
+    ``dst_mr.addr + dst_off + r * rec_bytes``, where ``j = indices[r]`` (an int32 CUDA tensor of ``n`` entries, read on
+    the device only: a permutation, a subset or repeats) or ``j = r``.  ``src_stride`` defaults to ``rec_bytes``, so K3
+    chunk records and K4 panel records can be pulled whole or gathered.  An index whose record does not fit the remote
+    region fails on the wire like any out-of-range READ (``REMOTE_ACCESS_ERR``, the QP goes to ERR).
+
+    ``ready`` (int64 CUDA tensor of at least ``n`` words, zeroed by the caller) gets word ``r`` set to a nonzero
+    %globaltimer value, with release semantics, once record ``r`` has landed: the arrival word that
+    ``unpack_fp8(ready=)`` and ``gemm_mxfp8(a_ready=)`` wait for.  One warp owns the QP and its send CQ; ``window``,
+    ``burst`` and ``signal_every`` are :func:`rdma_stream`'s knobs (one CQE stamps up to ``signal_every`` records with
+    one value).  ``window`` is at most the send queue's and the send CQ's depth.  When a READ fails the status is
+    ``CQE_ERROR``: every earlier record has landed and is stamped, the failing one and every later one are not.
+
+    Returns ``dict(status, done, device_ns, t_start_ns, t_end_ns, first_idx, last_idx, cons)`` (``done``: records landed),
+    or ``(result view, stream)`` with ``sync=False`` (decode with :func:`parse_read_records`)."""
+    ctx = qp.ctx
+    rec_bytes, n = N.byte_count(rec_bytes, "rec_bytes"), int(n)
+    if rec_bytes == 0 or rec_bytes > ctx.max_msg_bytes:
+        raise ValueError(f"rec_bytes={rec_bytes}: a record is one READ of 1..{ctx.max_msg_bytes} bytes")
+    if not 0 <= n < 1 << 32:
+        raise ValueError(f"n={n}: outside [0, 2**32)")
+    src_stride = rec_bytes if src_stride is None else int(src_stride)
+    if src_off < 0 or src_stride < 0 or dst_off < 0:
+        raise ValueError("src_off, src_stride and dst_off must be non-negative")
+    if dst_off + n * rec_bytes > dst_mr.length:
+        raise ValueError(f"{n} records of {rec_bytes} bytes at dst_off={dst_off} do not fit dst_mr ({dst_mr.length} bytes)")
+    idx_addr = 0 if indices is None else _device_words(indices, torch.int32, n, ctx.device, "indices")
+    ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n, ctx.device, "ready")
+    depth = min(qp.sq_depth, qp.scq.depth)
+    window = depth if window <= 0 else min(int(window), depth)
+    ws = work_stream(ctx, stream)
+    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    rc = N.load().rn_k_read_records(_stream_ptr(ws), qp.dev_ptr, dst_mr.addr + dst_off, dst_mr.lkey, src_mr.addr + src_off,
+                                    src_mr.rkey, src_stride, rec_bytes, n, idx_addr, ready_addr, window, burst, signal_every,
+                                    timeout_ms, out_addr)
+    if rc:
+        raise N.NativeError(f"read_records launch failed ({rc})")
+    if not sync:
+        return out_view, ws
+    ws.synchronize()
+    return parse_read_records(out_view)
+
+
+def parse_read_records(view) -> dict:
+    """Decode the record :func:`read_records` leaves in its scratch slot (for ``sync=False`` callers)."""
+    w = (C.c_int64 * 8).from_buffer(view)
+    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), done=w[3], device_ns=w[2] - w[1], t_start_ns=w[1], t_end_ns=w[2],
+                first_idx=w[4], last_idx=w[5], cons=w[6])
