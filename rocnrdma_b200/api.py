@@ -685,6 +685,13 @@ class Context:
             raise ValueError("device scratch request too large")
         return base + offset
 
+    @property
+    def dev_scratch_bytes(self) -> int:
+        """Size of the device scratch: ``ops`` kernels take 256 KiB slots of it (``scratch_slot``)."""
+        sz = C.c_uint64()
+        self._lib.rn_hca_dev_scratch(self._h, C.byref(sz))
+        return sz.value
+
     def scratch(self, nbytes: int, offset: int = 0):
         """(address, ctypes view) of the HCA's mapped pinned result area.  Kernels write
         their status/timing words here and the host reads them after a stream sync, so the

@@ -1,4 +1,4 @@
-// K3 / K5 (SURVEY.md section 2.3): payload pack fused with GPU-initiated networking.
+// K3 / K5 (SURVEY.md section 2.3): payload pack fused with GPU-initiated networking, and the reduce of several sources.
 //
 //  pack_fp8_write_kernel   bf16 -> fp8 e4m3 with one UE8M0 scale per 32 elements (MX-style
 //                          block scaling) written into a registered staging region as
@@ -10,16 +10,20 @@
 //                          pack+transfer pipeline.
 //  unpack_fp8_kernel       consumer: optionally waits for each record's arrival (receive
 //                          CQE carrying the chunk id as immediate), then fp8 -> bf16.
+//  reduce_fp8_kernel       the sum of P sources of records (plus a bf16 addend) as each record's sources land,
+//                          as bf16 and / or re-quantised records; the CTA that completes a record of the sum
+//                          posts its RDMA WRITE(_IMM), as K3 does.
 //
 // Record layout for a chunk of C elements (C % 8192 == 0):
 //     [ C bytes fp8 e4m3 ][ C/32 bytes UE8M0 scales ][ pad to 64 B ]
-// Quantisation (bit-exact reference: ops/pack.py, quantize_blocks / ref_pack_fp8 / ref_unpack_fp8):
+// Quantisation (bit-exact reference: ops/pack.py, quantize_blocks / ref_pack_fp8 / ref_unpack_fp8 / ref_reduce_fp8):
 //     v = amax * (1/448)  (fp32) ; e = exponent(v) + (mantissa(v) != 0), clamped to [-127, 127]
 //     q = cvt.rn.satfinite.e4m3(x * 2^-e) ; scale byte = e + 127
 // Non-finite input:
 //     NaN   amax is an fmaxf reduction, which drops NaN: a NaN stays in its own element, its neighbours quantise
 //           as if it were absent (an all-NaN block gets scale byte 0 and NaN codes)
 //     +-Inf e clamps to 127 (scale byte 254) and 2^-127 is 0.0 here: the Inf becomes NaN, its neighbours +-0
+//           (a finite sum that overflows fp32 in the reduce is such an Inf)
 // Decode: scale byte 0x00 is 2^-127 (the OCP MX value, fp32 0x00400000), as in the block-scaled GEMM; 0xFF is Inf.
 //
 // No counterpart in the reference (it moves no payload: SURVEY.md section 3.2).
@@ -76,6 +80,26 @@ __device__ __forceinline__ float bf16_bits_to_float(uint32_t hi16) { return __ui
 // UE8M0 scale byte -> 2^(e - 127); byte 0 is 2^-127, an fp32 denormal (the same decode as gemm_mxfp8.cu)
 __device__ __forceinline__ float ue8m0(uint32_t e) { return e ? __uint_as_float(e << 23) : __uint_as_float(0x00400000u); }
 
+// The quantiser of one MX block (K3's, and the reduce kernel's): 32 fp32 values in element order -> 32 e4m3 codes (q[i]
+// holds elements 4i..4i+3, lowest byte first) and the returned UE8M0 scale byte.  The rule is the header's.
+__device__ __forceinline__ uint32_t quantize_block32(const float (&x)[32], uint32_t (&q)[8]) {
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) amax = fmaxf(amax, fmaxf(fabsf(x[2 * i]), fabsf(x[2 * i + 1])));
+  // UE8M0 scale: smallest power of two 2^e with amax / 2^e <= 448
+  const uint32_t vb = __float_as_uint(amax * (1.0f / 448.0f));
+  int e = (int)((vb >> 23) & 0xff) - 127 + ((vb & 0x7fffffu) ? 1 : 0);
+  e = max(-127, min(127, e));
+  const float inv = __uint_as_float((uint32_t)(127 - e) << 23);   // 2^-e, exact (biased exponent 0..254)
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i] * inv, x[4 * i + 1] * inv), __NV_SATFINITE, __NV_E4M3);
+    uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i + 2] * inv, x[4 * i + 3] * inv), __NV_SATFINITE, __NV_E4M3);
+    q[i] = lo | (hi << 16);
+  }
+  return (uint32_t)(e + 127);
+}
+
 template <int G>
 __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_tile, uint32_t tiles_per_chunk, uint64_t rec) {
   // G tiles (G x 16 KiB of bf16) per step: all 4G 16-byte loads are issued before the first
@@ -94,29 +118,16 @@ __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_til
     const uint32_t tile_in_chunk = (uint32_t)(tile % tiles_per_chunk);
     const uint32_t w[16] = {v[g][0].x, v[g][0].y, v[g][0].z, v[g][0].w, v[g][1].x, v[g][1].y, v[g][1].z, v[g][1].w,
                             v[g][2].x, v[g][2].y, v[g][2].z, v[g][2].w, v[g][3].x, v[g][3].y, v[g][3].z, v[g][3].w};
-    float amax = 0.f;
+    float x[32];
 #pragma unroll
-    for (int i = 0; i < 16; ++i)
-      amax = fmaxf(amax, fmaxf(fabsf(bf16_bits_to_float(w[i] & 0xffffu)), fabsf(bf16_bits_to_float(w[i] >> 16))));
-    // UE8M0 scale: smallest power of two 2^e with amax / 2^e <= 448
-    const uint32_t vb = __float_as_uint(amax * (1.0f / 448.0f));
-    int e = (int)((vb >> 23) & 0xff) - 127 + ((vb & 0x7fffffu) ? 1 : 0);
-    e = max(-127, min(127, e));
-    const float inv = __uint_as_float((uint32_t)(127 - e) << 23);   // 2^-e, exact (biased exponent 0..254)
+    for (int i = 0; i < 16; ++i) { x[2 * i] = bf16_bits_to_float(w[i] & 0xffffu); x[2 * i + 1] = bf16_bits_to_float(w[i] >> 16); }
     uint32_t q[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      float s0 = bf16_bits_to_float(w[2 * i] & 0xffffu) * inv, s1 = bf16_bits_to_float(w[2 * i] >> 16) * inv;
-      float s2 = bf16_bits_to_float(w[2 * i + 1] & 0xffffu) * inv, s3 = bf16_bits_to_float(w[2 * i + 1] >> 16) * inv;
-      uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(s0, s1), __NV_SATFINITE, __NV_E4M3);
-      uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(s2, s3), __NV_SATFINITE, __NV_E4M3);
-      q[i] = lo | (hi << 16);
-    }
+    const uint32_t scale = quantize_block32(x, q);
     uint8_t* recp = a.staging + (uint64_t)chunk * rec;
     uint4* out = reinterpret_cast<uint4*>(recp + (uint64_t)tile_in_chunk * kTileElems + (uint64_t)threadIdx.x * kBlockElems);
     out[0] = make_uint4(q[0], q[1], q[2], q[3]);
     out[1] = make_uint4(q[4], q[5], q[6], q[7]);
-    recp[a.chunk_elems + (uint64_t)tile_in_chunk * kPackThreads + threadIdx.x] = (uint8_t)(e + 127);
+    recp[a.chunk_elems + (uint64_t)tile_in_chunk * kPackThreads + threadIdx.x] = (uint8_t)scale;
   }
 }
 
@@ -189,6 +200,24 @@ __device__ __forceinline__ void st256_cs(void* p, const uint32_t* r) {
                ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
 }
 
+// Wait for an arrival word (recv_consume, read_records): an acquire load until it is nonzero.  Returns false when the
+// abort flag is raised first, or when timeout_ns passes -- then this waiter writes TIMEOUT to out[0] and raises the flag.
+__device__ __forceinline__ bool wait_word(const unsigned long long* w, unsigned int* abort_flag, unsigned long long* out,
+                                          uint64_t timeout_ns) {
+  unsigned long long v, t0 = 0;
+  for (unsigned n = 0;; ++n) {
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(w) : "memory");
+    if (v) return true;
+    if (*(volatile unsigned int*)abort_flag) return false;
+    const unsigned long long now = globaltimer_ns();
+    if (!t0) t0 = now;
+    else if (now - t0 > timeout_ns) {
+      out[0] = (unsigned long long)(long long)WAIT_TIMEOUT; atomicExch(abort_flag, 1u); return false;
+    }
+    __nanosleep(n < 64 ? 50 : 400);
+  }
+}
+
 struct UnpackArgs {
   const uint8_t* staging;    // records, back to back
   __nv_bfloat16* dst;
@@ -254,18 +283,7 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
             if (chunk == last) continue;
             last = chunk;
             if (a.ready) {
-              unsigned long long v, t0 = 0;
-              for (unsigned n = 0;; ++n) {
-                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(a.ready + chunk) : "memory");
-                if (v) break;
-                if (*(volatile unsigned int*)abort_flag) { ok = 0; break; }
-                const unsigned long long now = globaltimer_ns();
-                if (!t0) t0 = now;
-                else if (now - t0 > a.timeout_ns) {
-                  a.out[0] = (unsigned long long)(long long)WAIT_TIMEOUT; atomicExch(abort_flag, 1u); ok = 0; break;
-                }
-                __nanosleep(n < 64 ? 50 : 400);
-              }
+              if (!wait_word(a.ready + chunk, abort_flag, a.out, a.timeout_ns)) ok = 0;
               continue;
             }
             for (unsigned n = 0; *(volatile unsigned int*)&a.arrived[chunk] == 0; ++n) {
@@ -334,6 +352,202 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
   }
 }
 
+// ---- reduce: the sum of P sources of K3 records (plus an optional bf16 addend) as bf16 and / or as K3 records, each
+// finished record posted as it completes.  One rule for the arithmetic: every decoded element is q * 2^(byte - 127) in
+// fp32 (exact, or +-Inf where it overflows), the sum starts from `local` (or from source 0) and adds the other sources in
+// source order, one __fadd_rn each.  __fmul_rn / __fadd_rn keep the compiler from contracting them into an FMA, which
+// would round once where the reference rounds twice.
+struct ReduceArgs {
+  const uint8_t* src;                // n_src x n_rec records, source-major
+  const __nv_bfloat16* local;        // optional addend of n_elems (nullptr: the sum starts from source 0)
+  __nv_bfloat16* out;                // optional bf16 sum
+  uint8_t* out_rec;                  // optional K3 records of the sum (registered when they are posted)
+  uint32_t chunk_elems, n_rec, n_src;
+  const unsigned long long* ready;   // optional: word s * n_rec + r is nonzero once record r of source s has landed
+  QpDev* qp;                         // nullptr: nothing is posted
+  uint64_t out_va;                   // VA of out_rec as registered
+  uint32_t lkey, rkey;
+  uint64_t remote_va;                // destination of record 0; records keep their stride remotely
+  uint32_t with_imm, post_only, signal_every;
+  unsigned int* counters;            // [0, n_rec) tiles done per record ; [n_rec] CTAs done ; [n_rec + 1] abort flag ;
+                                     // [n_rec + 2] records reduced (self-cleaned)
+  unsigned long long* acc;           // post_record's [max WQE index + 1, records posted, ~first post time]
+  unsigned long long* res;           // [status, t_start, t_end, records_reduced, records_posted, t_first_post, t_reduce_end, 0]
+  uint64_t timeout_ns;
+};
+
+// One step of G tiles, `stride` apart in the flattened record-major order, of up to PMAX sources: every load (PMAX x 32
+// bytes of fp8 and a scale byte per tile, and 64 bytes of the addend) is issued before the first use.
+template <int G, int PMAX, bool LOCAL>
+__device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, uint32_t stride, uint64_t total, uint32_t tpc,
+                                            uint64_t rec) {
+  uint32_t qv[G][PMAX][8];
+  uint32_t e[G][PMAX];
+  uint32_t lv[G][LOCAL ? 16 : 1];
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    const uint64_t T = T0 + (uint64_t)g * stride;
+    if (T < total) {
+      const uint32_t r = (uint32_t)(T / tpc), t = (uint32_t)(T % tpc);
+#pragma unroll
+      for (int s = 0; s < PMAX; ++s) {
+        if (s < (int)a.n_src) {
+          const uint8_t* recp = a.src + ((uint64_t)s * a.n_rec + r) * rec;
+          ld256_cs(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems, qv[g][s]);
+          e[g][s] = __ldcs(recp + a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x);
+        }
+      }
+      if (LOCAL) {
+        const __nv_bfloat16* lp = a.local + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems;
+        ld256_cs(lp, lv[g]);
+        ld256_cs(lp + 16, lv[g] + 8);
+      }
+    }
+  }
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    const uint64_t T = T0 + (uint64_t)g * stride;
+    if (T >= total) break;
+    float x[32];
+    if (LOCAL) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) { x[2 * i] = bf16_bits_to_float(lv[g][i] & 0xffffu); x[2 * i + 1] = bf16_bits_to_float(lv[g][i] >> 16); }
+    }
+#pragma unroll
+    for (int s = 0; s < PMAX; ++s) {
+      if (s < (int)a.n_src) {
+        const float sc = ue8m0(e[g][s]);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          __half2_raw h0 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(qv[g][s][i] & 0xffff), __NV_E4M3);
+          __half2_raw h1 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(qv[g][s][i] >> 16), __NV_E4M3);
+          const float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&h0));
+          const float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&h1));
+          const float d[4] = {__fmul_rn(f0.x, sc), __fmul_rn(f0.y, sc), __fmul_rn(f1.x, sc), __fmul_rn(f1.y, sc)};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) x[4 * i + k] = (!LOCAL && s == 0) ? d[k] : __fadd_rn(x[4 * i + k], d[k]);
+        }
+      }
+    }
+    if (a.out) {
+      uint32_t o[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        __nv_bfloat162 b = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+        o[i] = *reinterpret_cast<uint32_t*>(&b);
+      }
+      // record-major flattened tile T is also tile T of the output
+      __nv_bfloat16* dst = a.out + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems;
+      st256_cs(dst, o);
+      st256_cs(dst + 16, o + 8);
+    }
+    if (a.out_rec) {
+      uint32_t q[8];
+      const uint32_t scale = quantize_block32(x, q);
+      const uint32_t r = (uint32_t)(T / tpc), t = (uint32_t)(T % tpc);
+      uint8_t* recp = a.out_rec + (uint64_t)r * rec;
+      uint4* o = reinterpret_cast<uint4*>(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems);
+      o[0] = make_uint4(q[0], q[1], q[2], q[3]);
+      o[1] = make_uint4(q[4], q[5], q[6], q[7]);
+      recp[a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x] = (uint8_t)scale;
+    }
+  }
+}
+
+// Workers walk the tiles of all records in K5's flattened record-major order, G tiles per step, so the oldest records
+// finish (and are forwarded) first.  With arrival words there is no poller: before each step thread 0 waits for the
+// words of every source of every record the step reads.  The CTA whose tiles complete a record posts it, as in K3.
+template <int G, int PMAX, bool LOCAL>
+__global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) {
+  const unsigned long long t_start = globaltimer_ns();
+  const uint32_t tpc = a.chunk_elems / kTileElems;
+  const uint64_t rec = record_bytes(a.chunk_elems);
+  const uint64_t total = (uint64_t)a.n_rec * tpc;
+  unsigned int* abort_flag = a.counters + a.n_rec + 1;
+  const bool gated = a.ready != nullptr, counted = gated || a.qp != nullptr;
+  const bool sys = a.qp != nullptr && poster_sys(a.qp);
+  __shared__ int ok;
+  for (uint64_t T0 = blockIdx.x; T0 < total; T0 += (uint64_t)gridDim.x * G) {
+    if (gated) {
+      if (threadIdx.x == 0) {                                  // every source of every record this step reads has landed
+        ok = 1;
+        uint32_t last = ~0u;
+        for (int g = 0; g < G && ok; ++g) {
+          const uint64_t T = T0 + (uint64_t)g * gridDim.x;
+          if (T >= total) break;
+          const uint32_t r = (uint32_t)(T / tpc);
+          if (r == last) continue;
+          last = r;
+          for (uint32_t s = 0; s < a.n_src && ok; ++s)
+            if (!wait_word(a.ready + (uint64_t)s * a.n_rec + r, abort_flag, a.res, a.timeout_ns)) ok = 0;
+        }
+        fence_gpu();
+      }
+      __syncthreads();
+      const int good = ok;
+      __syncthreads();          // everybody has read `ok` before thread 0 re-arms it for the next step
+      if (!good) break;
+    }
+    reduce_step<G, PMAX, LOCAL>(a, T0, gridDim.x, total, tpc, rec);
+    if (!counted) continue;
+    // ---- count the step's tiles per record; the CTA that completes a record posts it
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      fence_gpu();   // release this step's stores (all threads, via the barrier) before the counts
+      for (int g = 0; g < G;) {
+        const uint64_t T = T0 + (uint64_t)g * gridDim.x;
+        if (T >= total) break;
+        const uint32_t r = (uint32_t)(T / tpc);
+        uint32_t n = 0;
+        while (g < G && T0 + (uint64_t)g * gridDim.x < total && (T0 + (uint64_t)g * gridDim.x) / tpc == r) { ++n; ++g; }
+        const unsigned int old = atomicAdd(&a.counters[r], n);
+        if (old + n == tpc) {
+          atomicAdd(&a.counters[a.n_rec + 2], 1u);
+          if (a.qp) {
+            // acquire every other CTA's bytes of the record; one cumulative system-scope fence on a NIC-facing QP
+            fence_scope(sys);
+            post_record(a.qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.out_va + (uint64_t)r * rec, a.lkey,
+                        a.remote_va + (uint64_t)r * rec, a.rkey, (uint32_t)rec, r, a.signal_every, a.acc, a.res, a.timeout_ns);
+          }
+          a.counters[r] = 0;
+        }
+      }
+    }
+  }
+  // ---- the CTA that finishes last posts the flush (a record not reduced is never posted; the posted ones still drain)
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    fence_gpu();
+    unsigned int old = atomicAdd(&a.counters[a.n_rec], 1u);
+    if (old + 1 == gridDim.x) {
+      const unsigned long long t_reduce_end = globaltimer_ns();
+      fence_gpu();
+      // with no words to wait on and nothing to post every tile is reduced: nothing counts them
+      const uint32_t reduced = counted ? ld_u32_volatile(&a.counters[a.n_rec + 2]) : a.n_rec;
+      unsigned long long posted = 0, first = 0;
+      if (a.qp) {
+        posted = ld_u64_volatile(&a.acc[1]);
+        first = posted ? ~ld_u64_volatile(&a.acc[2]) : 0;
+        int rc = post_flush(a.qp, a.post_only, a.timeout_ns);
+        if (posted != a.n_rec && rc == WAIT_OK) rc = WAIT_TIMEOUT;
+        if (rc != WAIT_OK) a.res[0] = (unsigned long long)(long long)rc;
+      }
+      a.res[1] = t_start;
+      a.res[2] = globaltimer_ns();
+      a.res[3] = reduced;
+      a.res[4] = posted;
+      a.res[5] = first;
+      a.res[6] = t_reduce_end;
+      for (uint32_t r = 0; r <= a.n_rec + 2; ++r) a.counters[r] = 0;   // self-clean, records left unfinished included
+      a.acc[0] = 0; a.acc[1] = 0; a.acc[2] = 0;
+    }
+  }
+}
+
+// Tiles per step and sources a variant holds, chosen from P and the addend so that every load of a step fits in
+// registers (about 72 per thread, as K3's four tiles of bf16) and P = 8 with an addend does not spill.
+#define RN_REDUCE_VARIANTS(X) X(4, 1, false) X(4, 2, false) X(2, 4, false) X(1, 8, false) X(2, 2, true) X(1, 8, true)
+
 }  // namespace
 
 RN_API uint64_t rn_pack_record_bytes(uint64_t chunk_elems) { return record_bytes(chunk_elems); }
@@ -390,8 +604,48 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
   return (int)cudaGetLastError();
 }
 
+// counters_dev: >= (n_rec + 3) * 4 bytes (rounded up to 8) + 24 of zero-initialised device memory, cleaned by the kernel.
+// flags: bit 0 RDMA_WRITE_IMM (immediate = record id), bit 1 post_only.
+RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_src, uint64_t local, uint64_t out,
+                           uint64_t out_rec, uint64_t n_elems, uint32_t chunk_elems, uint64_t ready_dev, uint64_t qp_dev,
+                           uint64_t out_va, uint32_t lkey, uint64_t remote_va, uint32_t rkey, uint32_t flags,
+                           uint32_t signal_every, uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms) {
+  if (n_src < 1 || n_src > 8) return -22;
+  if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
+    return -22;
+  if ((src | local | out | out_rec) & 31) return -22;          // 256-bit loads / stores
+  if (!out && !out_rec) return -22;
+  if (qp_dev && !out_rec) return -22;
+  ReduceArgs a;
+  a.src = (const uint8_t*)src; a.local = (const __nv_bfloat16*)local; a.out = (__nv_bfloat16*)out; a.out_rec = (uint8_t*)out_rec;
+  a.chunk_elems = chunk_elems; a.n_rec = (uint32_t)(n_elems / chunk_elems); a.n_src = n_src;
+  a.ready = (const unsigned long long*)ready_dev; a.qp = (QpDev*)qp_dev; a.out_va = out_va; a.lkey = lkey; a.rkey = rkey;
+  a.remote_va = remote_va; a.with_imm = flags & 1u; a.post_only = (flags >> 1) & 1u; a.signal_every = signal_every ? signal_every : 1;
+  a.counters = (unsigned int*)counters_dev;
+  a.acc = (unsigned long long*)(counters_dev + (((uint64_t)a.n_rec + 3) * 4 + 7) / 8 * 8);
+  a.res = (unsigned long long*)out_dev;
+  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  unsigned long long* o = (unsigned long long*)out_dev;
+  for (int i = 0; i < 8; ++i) o[i] = 0;
+  // waiting for arrivals the kernel shares the GPU with whatever produces them: one CTA per SM then (as K5)
+  if (grid <= 0) grid = ready_dev ? device_sms() : device_sms() * 4;
+  {
+    const uint64_t total_tiles = n_elems / kTileElems;
+    if ((uint64_t)grid > total_tiles) grid = (int)total_tiles;
+  }
+  const int pmax = local ? (n_src <= 2 ? 2 : 8) : (n_src == 1 ? 1 : n_src <= 2 ? 2 : n_src <= 4 ? 4 : 8);
+#define RN_LAUNCH(G, PMAX, LOCAL) \
+  if (pmax == PMAX && (local != 0) == LOCAL) reduce_fp8_kernel<G, PMAX, LOCAL><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  RN_REDUCE_VARIANTS(RN_LAUNCH)
+#undef RN_LAUNCH
+  return (int)cudaGetLastError();
+}
+
 extern "C" __attribute__((visibility("default"))) void rn_preload_pack() {
   cudaFuncAttributes at;
   cudaFuncGetAttributes(&at, pack_fp8_write_kernel);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel);
+#define RN_PRELOAD(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL>);
+  RN_REDUCE_VARIANTS(RN_PRELOAD)
+#undef RN_PRELOAD
 }

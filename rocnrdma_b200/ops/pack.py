@@ -1,5 +1,5 @@
 """K3 / K5 wrappers: bf16 -> fp8 block-scaled pack fused with GPU-initiated RDMA write,
-the receive-side unpack, and the bit-exact PyTorch reference of both."""
+the receive-side unpack, the reduction of several sources' records, and the bit-exact PyTorch references of all three."""
 from __future__ import annotations
 
 import ctypes as C
@@ -167,16 +167,20 @@ def quantize_blocks(x: torch.Tensor):
     return q, (e + 127).to(torch.uint8)
 
 
-def ref_pack_fp8(src: torch.Tensor, chunk_elems: int) -> torch.Tensor:
-    """Reference chunk records (uint8) for a bf16 tensor; runs on CPU or GPU."""
-    q, sc = quantize_blocks(src.float().reshape(-1, BLOCK))
-    n = src.numel()
-    n_chunks = n // chunk_elems
+def _quantized_records(x: torch.Tensor, chunk_elems: int) -> torch.Tensor:
+    """Chunk records (uint8) of the fp32 values ``x``, quantised by :func:`quantize_blocks`."""
+    q, sc = quantize_blocks(x.reshape(-1, BLOCK))
+    n_chunks = x.numel() // chunk_elems
     rec = record_bytes(chunk_elems)
-    out = torch.zeros(n_chunks, rec, dtype=torch.uint8, device=src.device)
+    out = torch.zeros(n_chunks, rec, dtype=torch.uint8, device=x.device)
     out[:, :chunk_elems] = q.reshape(n_chunks, chunk_elems)
     out[:, chunk_elems:chunk_elems + chunk_elems // BLOCK] = sc.reshape(n_chunks, -1)
     return out.reshape(-1)
+
+
+def ref_pack_fp8(src: torch.Tensor, chunk_elems: int) -> torch.Tensor:
+    """Reference chunk records (uint8) for a bf16 tensor; runs on CPU or GPU."""
+    return _quantized_records(src.float(), chunk_elems)
 
 
 def ref_unpack_fp8(records: torch.Tensor, n_elems: int, chunk_elems: int) -> torch.Tensor:
@@ -186,3 +190,157 @@ def ref_unpack_fp8(records: torch.Tensor, n_elems: int, chunk_elems: int) -> tor
     q = r[:, :chunk_elems].contiguous().view(torch.float8_e4m3fn).float().reshape(-1, BLOCK)
     s = ue8m0(r[:, chunk_elems:chunk_elems + chunk_elems // BLOCK].reshape(-1))
     return (q * s[:, None]).to(torch.bfloat16).reshape(-1)
+
+
+def _decode_records(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int) -> torch.Tensor:
+    """fp32 values [n_src, n_elems] of source-major records: q * 2^(byte - 127), exact (or +-Inf where it overflows)."""
+    n_chunks = n_elems // chunk_elems
+    rec = record_bytes(chunk_elems)
+    r = records.reshape(-1)[:n_src * n_chunks * rec].reshape(n_src * n_chunks, rec)
+    q = r[:, :chunk_elems].contiguous().view(torch.float8_e4m3fn).float().reshape(-1, BLOCK)
+    s = ue8m0(r[:, chunk_elems:chunk_elems + chunk_elems // BLOCK].reshape(-1))
+    return (q * s[:, None]).reshape(n_src, n_elems)
+
+
+def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int, local=None):
+    """Reference of :func:`reduce_fp8`; runs on CPU or GPU.  Returns (bf16 sum, K3 records of the sum).
+
+    The sum starts from ``local`` (bf16, exact in fp32) when given, else from source 0, and adds the other sources in
+    source order, one fp32 add each: only the adds round.  The records quantise that fp32 sum with the rule of every
+    producer (:func:`quantize_blocks`), so a block whose finite sum overflows to +-Inf gets scale byte 254, NaN where the
+    Inf is and +-0 beside it."""
+    d = _decode_records(records, n_src, n_elems, chunk_elems)
+    if local is not None:
+        acc, first = local.reshape(-1).float().to(d.device), 0
+    else:
+        acc, first = d[0], 1
+    for s in range(first, n_src):
+        acc = acc + d[s]
+    return acc.to(torch.bfloat16), _quantized_records(acc, chunk_elems)
+
+
+# ------------------------------------------------------------------ reduce
+MAX_SOURCES = 8
+_SLOT = 256 << 10
+
+
+@dataclass
+class ReduceResult:
+    status: str
+    t_start_ns: int
+    t_end_ns: int
+    records_reduced: int
+    records_posted: int
+    t_first_post_ns: int
+    t_reduce_end_ns: int
+    hbm_bytes: int = 0            # bytes the kernel reads and writes in HBM (sources, addend, outputs); 0 from parse_reduce
+
+    @property
+    def ok(self) -> bool:
+        return self.status == "OK"
+
+    @property
+    def device_ns(self) -> int:
+        return self.t_end_ns - self.t_start_ns
+
+    @property
+    def hbm_gbps(self) -> float:
+        """HBM bytes moved (read + written) per second of device time."""
+        return self.hbm_bytes / max(self.device_ns, 1)
+
+
+def parse_reduce(view, hbm_bytes: int = 0) -> ReduceResult:
+    """Decode the record :func:`reduce_fp8` leaves in its scratch slot (for ``sync=False`` callers)."""
+    w = (C.c_int64 * 8).from_buffer(view)
+    return ReduceResult(WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2], w[3], w[4], w[5], w[6], hbm_bytes)
+
+
+def _check_bf16(t, n, device, what):
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16:
+        raise ValueError(f"{what} must be a bfloat16 tensor, not {getattr(t, 'dtype', type(t).__name__)}")
+    if not t.is_cuda or t.device.index != device:
+        raise ValueError(f"{what} must be on cuda:{device}, not {t.device}")
+    if not t.is_contiguous() or t.data_ptr() & 31:
+        raise ValueError(f"{what} must be contiguous and 32-byte aligned (256-bit loads / stores)")
+    if t.numel() != n:
+        raise ValueError(f"{what} holds {t.numel()} elements; n_elems is {n}")
+    return t.data_ptr()
+
+
+def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int = 1 << 20, *, local=None, out=None,
+               out_mr=None, qp=None, dst_mr=None, dst_off: int = 0, with_imm: bool = False, signal_every: int = 1,
+               post_only: bool = False, ready=None, grid: int = 0, timeout_ms: int = 2000, stream=None, sync: bool = True,
+               scratch_slot: int = 4):
+    """Sum ``n_src`` sources of K3 chunk records, plus an optional bf16 addend, as the records land, and re-pack and forward
+    the sum: one hop of a reduce-scatter ring in one kernel.
+
+    ``records`` holds the sources back to back: record r of source s at ``(s * n_rec + r) * record_bytes(chunk_elems)``
+    (``n_rec = n_elems // chunk_elems``).  Every decoded element is q * 2^(byte - 127) in fp32; the sum starts from
+    ``local`` (bf16, ``n_elems``) or from source 0 and adds the other sources in source order, one fp32 add each
+    (:func:`ref_reduce_fp8` reproduces it bit for bit).  Outputs, at least one: ``out`` (bf16, ``n_elems``, round to
+    nearest even) and ``out_mr`` (a registered region that receives the K3 records of the fp32 sum).
+
+    With ``qp`` and ``dst_mr`` each record of ``out_mr`` is one RDMA WRITE (WRITE_IMM with immediate = record id when
+    ``with_imm``) to ``dst_mr`` at ``dst_off + r * record_bytes``, posted by the CTA that completes the record; the last
+    CTA posts a flush and waits for it unless ``post_only``, as :func:`pack_fp8_write` does.  With ``ready`` (int64 CUDA
+    tensor of ``n_src * n_rec`` arrival words, source s in ``ready[s * n_rec:(s + 1) * n_rec]``, as ``recv_consume`` and
+    :func:`~rocnrdma_b200.ops.read_records` set them) every step waits for the words of all sources of the records it
+    reads; a word still 0 after ``timeout_ms`` ends the kernel with ``TIMEOUT``, and a record not reduced is never posted.
+    Two reductions that run at once need different ``scratch_slot`` values (0..7; K3 uses 0, K5 1, the GEMMs 2 and 3).
+
+    Returns a :class:`ReduceResult`, or ``(result view, stream)`` with ``sync=False`` (decode with :func:`parse_reduce`)."""
+    n_src, n_elems, chunk_elems = int(n_src), int(n_elems), int(chunk_elems)
+    if not 1 <= n_src <= MAX_SOURCES:
+        raise ValueError(f"n_src={n_src}: 1..{MAX_SOURCES} sources")
+    if n_elems <= 0 or chunk_elems <= 0 or n_elems % TILE_ELEMS or chunk_elems % TILE_ELEMS or n_elems % chunk_elems:
+        raise ValueError(f"n_elems and chunk_elems must be multiples of {TILE_ELEMS}, n_elems of chunk_elems")
+    dev = ctx.device
+    n_rec = n_elems // chunk_elems
+    wire = staging_bytes(n_elems, chunk_elems)
+    if not isinstance(records, torch.Tensor) or not records.is_cuda or records.device.index != dev or not records.is_contiguous():
+        raise ValueError(f"records must be a contiguous tensor on cuda:{dev}")
+    if records.numel() * records.element_size() < n_src * wire:
+        raise ValueError(f"records hold {records.numel() * records.element_size()} bytes; {n_src} sources of {n_rec} "
+                         f"records need {n_src * wire}")
+    if records.data_ptr() & 31:
+        raise ValueError("records must be 32-byte aligned (256-bit loads)")
+    local_addr = 0 if local is None else _check_bf16(local, n_elems, dev, "local")
+    out_addr = 0 if out is None else _check_bf16(out, n_elems, dev, "out")
+    if out is None and out_mr is None:
+        raise ValueError("reduce_fp8 needs an output: out (bf16) and / or out_mr (records)")
+    if out_mr is not None:
+        if out_mr.length < wire:
+            raise ValueError(f"out_mr holds {out_mr.length} bytes; the records of the sum need {wire}")
+        if out_mr.addr & 31:
+            raise ValueError("out_mr must be 32-byte aligned")
+    if qp is not None and (out_mr is None or dst_mr is None):
+        raise ValueError("posting (qp) needs out_mr and dst_mr")
+    if dst_mr is not None and qp is None:
+        raise ValueError("dst_mr without qp: nothing would post to it")
+    if dst_mr is not None and (dst_off < 0 or dst_off + wire > dst_mr.length):
+        raise ValueError(f"{n_rec} records of {record_bytes(chunk_elems)} bytes at dst_off={dst_off} do not fit dst_mr "
+                         f"({dst_mr.length} bytes)")
+    ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_src * n_rec, dev, "ready")
+    counter_bytes = ((n_rec + 3) * 4 + 7) // 8 * 8 + 24
+    if counter_bytes > _SLOT:
+        raise ValueError(f"{n_rec} records need {counter_bytes} bytes of counters; a scratch slot holds {_SLOT}")
+    if not 0 <= scratch_slot < ctx.dev_scratch_bytes // _SLOT:
+        raise ValueError(f"scratch_slot={scratch_slot}: the device scratch has {ctx.dev_scratch_bytes // _SLOT} slots")
+    lib = N.load()
+    ws = work_stream(ctx, stream)
+    counters = ctx.dev_scratch(counter_bytes, offset=scratch_slot * _SLOT)
+    res_addr, res_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
+    hbm = n_src * wire + (2 * n_elems if local is not None else 0) + (2 * n_elems if out is not None else 0) + \
+        (wire if out_mr is not None else 0)
+    rc = lib.rn_k_reduce_fp8(_stream_ptr(ws), grid, records.data_ptr(), n_src, local_addr, out_addr,
+                             out_mr.addr if out_mr is not None else 0, n_elems, chunk_elems, ready_addr,
+                             qp.dev_ptr if qp is not None else 0, out_mr.addr if out_mr is not None else 0,
+                             out_mr.lkey if out_mr is not None else 0, dst_mr.addr + dst_off if dst_mr is not None else 0,
+                             dst_mr.rkey if dst_mr is not None else 0, int(with_imm) | (2 if post_only else 0), signal_every,
+                             counters, res_addr, timeout_ms)
+    if rc:
+        raise N.NativeError(f"reduce_fp8 launch failed ({rc})")
+    if not sync:
+        return res_view, ws
+    ws.synchronize()
+    return parse_reduce(res_view, hbm)
