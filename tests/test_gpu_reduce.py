@@ -69,11 +69,12 @@ def _poison(buf, chunk):
 
 # ------------------------------------------------------------------ 1. numerics, no waits
 CHUNKS = {8192: 5, 16384: 3, 1 << 20: 2}                # chunk -> records per source
+SOURCES = [1, 2, 3, 4, 5, 7, 8]                          # every variant at full and partial width (test_reduce_references.py)
 
 
 @pytest.mark.parametrize("outputs", ["bf16", "records", "both"])
 @pytest.mark.parametrize("local", [False, True], ids=["no_local", "local"])
-@pytest.mark.parametrize("n_src", [1, 2, 3, 8])
+@pytest.mark.parametrize("n_src", SOURCES)
 @pytest.mark.parametrize("chunk", list(CHUNKS), ids=[str(c) for c in CHUNKS])
 def test_reduce_matches_reference(ctx, chunk, n_src, local, outputs):
     """Every output at grids 1, 8 and the default, bit for bit (NaN up to its sign and payload), with canaries behind
