@@ -135,8 +135,9 @@ _SIGS = {
     "rn_k_shared_post_stress": (i32, [u64, u64, i32, u64, u32, u64, u32, u32, u64, u64, u64]),
     "rn_k_recv_consume": (i32, [u64, u64, u32, u32, u64, u64, u64, u64, u32, u32]),
     "rn_hca_enable_peer": (i32, [vp, i32]),
-    "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64, u64]),
-    "rn_k_reduce_fp8": (i32, [u64, i32, u64, u32, u64, u64, u64, u64, u32, u64, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64]),
+    "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64, u64, u64, u64, u32, u64, u32, u32, u32, u32]),
+    "rn_k_reduce_fp8": (i32, [u64, i32, u64, u32, u64, u64, u64, u64, u32, u64, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64,
+                              u32]),
     "rn_k_rdma_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u32, u32, u32, u32, u64, u32, u64, u64, u32]),
     "rn_k_write_read": (i32, [u64, u64, u64, u32, u64, u32, u64, u32, u32, u32, u32, u64, u64]),
     "rn_stream_clamp": (None, [u32, C.POINTER(u32), C.POINTER(u32)]),

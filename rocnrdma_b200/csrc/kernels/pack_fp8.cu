@@ -9,7 +9,8 @@
 //                          the last CQE has been seen: its device time is the whole
 //                          pack+transfer pipeline.
 //  unpack_fp8_kernel       consumer: optionally waits for each record's arrival (receive
-//                          CQE carrying the chunk id as immediate), then fp8 -> bf16.
+//                          CQE carrying the chunk id as immediate), then fp8 -> bf16; <true> also
+//                          forwards each record unchanged, from where it landed, as soon as it is seen.
 //  reduce_fp8_kernel       the sum of P sources of records (plus a bf16 addend) as each record's sources land,
 //                          as bf16 and / or re-quantised records; the CTA that completes a record of the sum
 //                          posts its RDMA WRITE(_IMM), as K3 does.
@@ -228,11 +229,24 @@ struct UnpackArgs {
   unsigned int* arrived;     // [n_chunks] flags ; [n_chunks] CTAs done ; [n_chunks+1] records seen (self-cleaned)
   const unsigned long long* ready;   // one arrival word per record, nonzero once it has landed (read_records, recv_consume);
                                      // nullptr: no words.  Never together with qp.
-  unsigned long long* out;   // [status, t_start, t_end, records_seen]
+  unsigned long long* out;   // [status, t_start, t_end, records_seen, records_forwarded, t_first_post, 0, 0]
   uint64_t timeout_ns;
+  // forwarding (unpack_fp8_kernel<true> only): record r is posted unchanged from the landing buffer, from fwd_src_va +
+  // r * rec to fwd_remote_va + r * rec, by the CTA that claims it first (arrived[r] is then the claim flag: forwarding
+  // never runs with the CQ poller, which owns those flags)
+  QpDev* fwd_qp;
+  uint64_t fwd_src_va;       // VA of `staging` as registered
+  uint64_t fwd_remote_va;
+  uint32_t fwd_lkey, fwd_rkey;
+  uint32_t with_imm, post_only, signal_every, imm_base;   // WRITE_IMM carries imm_base + r
+  unsigned long long* acc;   // post_record's [max WQE index + 1, records posted, ~first post time]
 };
 
-__global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) {
+// FWD = false is the plain consumer.  FWD = true also forwards each record, once, as soon as its word is seen (or at
+// the first step that reads it, with no words), before the record is unpacked; the last CTA posts the flush.  Its
+// minimum of 3 CTAs per SM lets ptxas take the 80 registers it needs instead of spilling at 64.
+template <bool FWD>
+__global__ void __launch_bounds__(kPackThreads, FWD ? 3 : 0) unpack_fp8_kernel(UnpackArgs a) {
   const unsigned long long t_start = globaltimer_ns();
   const uint32_t tiles_per_chunk = a.chunk_elems / kTileElems;
   const uint64_t rec = record_bytes(a.chunk_elems);
@@ -272,8 +286,29 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
     const uint64_t total = (uint64_t)a.n_chunks * tiles_per_chunk;
     constexpr int G = 4;
     for (uint64_t T0 = first; T0 < total; T0 += (uint64_t)stride * G) {
-      if (gated) {
-        if (threadIdx.x == 0) {                                  // the records this step reads have arrived
+      if (gated || FWD) {
+        if (FWD && threadIdx.x == 0) {                           // wait for, claim and forward the step's records
+          ok = 1;
+          uint32_t last = ~0u;
+#pragma unroll 1
+          for (int g = 0; g < G && ok; ++g) {
+            const uint64_t T = T0 + (uint64_t)g * stride;
+            if (T >= total) break;
+            const uint32_t chunk = (uint32_t)T / tiles_per_chunk;   // 32-bit: the host keeps total tiles below 2^32
+            if (chunk == last) continue;
+            last = chunk;
+            // the word's acquire (or, with no words, the stream order) makes the record visible to this thread; the CTA
+            // that claims it first releases it to the wire with one fence of the poster's scope and posts it
+            if (a.ready && !wait_word(a.ready + chunk, abort_flag, a.out, a.timeout_ns)) { ok = 0; break; }
+            if (atomicExch(&a.arrived[chunk], 1u) == 0u) {
+              fence_scope(poster_sys(a.fwd_qp));
+              post_record(a.fwd_qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.fwd_src_va + (uint64_t)chunk * rec,
+                          a.fwd_lkey, a.fwd_remote_va + (uint64_t)chunk * rec, a.fwd_rkey, (uint32_t)rec, a.imm_base + chunk,
+                          a.signal_every, a.acc, a.out, a.timeout_ns);
+            }
+          }
+          fence_gpu();
+        } else if (threadIdx.x == 0) {                           // the records this step reads have arrived
           ok = 1;
           uint32_t last = ~0u;
           for (int g = 0; g < G && ok; ++g) {
@@ -304,7 +339,9 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
       for (int g = 0; g < G; ++g) {
         const uint64_t T = T0 + (uint64_t)g * stride;
         if (T < total) {
-          const uint32_t chunk = (uint32_t)(T / tiles_per_chunk), t = (uint32_t)(T % tiles_per_chunk);
+          // <true> divides in 32 bits (the host keeps total tiles below 2^32): a 64-bit division is a call
+          const uint32_t chunk = FWD ? (uint32_t)T / tiles_per_chunk : (uint32_t)(T / tiles_per_chunk);
+          const uint32_t t = FWD ? (uint32_t)T % tiles_per_chunk : (uint32_t)(T % tiles_per_chunk);
           const uint8_t* recp = a.staging + (uint64_t)chunk * rec;
           ld256_cs(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems, qv[g]);
           e[g] = __ldcs(recp + a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x);
@@ -341,13 +378,23 @@ __global__ void __launch_bounds__(kPackThreads) unpack_fp8_kernel(UnpackArgs a) 
     unsigned int old = atomicAdd(&a.arrived[a.n_chunks], 1u);
     if (old + 1 == gridDim.x) {
       fence_gpu();
+      if (FWD) {
+        // the flush's CQE proves every forwarded record has landed; a record whose word never came was never posted
+        const unsigned long long posted = ld_u64_volatile(&a.acc[1]);
+        int rc = post_flush(a.fwd_qp, a.post_only, a.timeout_ns);
+        if (posted != a.n_chunks && rc == WAIT_OK) rc = WAIT_TIMEOUT;
+        if (rc != WAIT_OK) a.out[0] = (unsigned long long)(long long)rc;
+        a.out[4] = posted;
+        a.out[5] = posted ? ~ld_u64_volatile(&a.acc[2]) : 0;
+        a.acc[0] = 0; a.acc[1] = 0; a.acc[2] = 0;
+      }
       a.out[1] = t_start;
       a.out[2] = globaltimer_ns();
       uint32_t seen = *(volatile unsigned int*)&a.arrived[a.n_chunks + 1];
       if (a.ready)                                                        // records whose word is set by now
         for (uint32_t c = 0; c < a.n_chunks; ++c) seen += ld_u64_volatile(a.ready + c) != 0;
       a.out[3] = seen;
-      for (uint32_t c = 0; c <= a.n_chunks + 2; ++c) a.arrived[c] = 0;   // self-clean
+      for (uint32_t c = 0; c <= a.n_chunks + 2; ++c) a.arrived[c] = 0;   // self-clean (the claim flags included)
     }
   }
 }
@@ -374,6 +421,7 @@ struct ReduceArgs {
   unsigned long long* acc;           // post_record's [max WQE index + 1, records posted, ~first post time]
   unsigned long long* res;           // [status, t_start, t_end, records_reduced, records_posted, t_first_post, t_reduce_end, 0]
   uint64_t timeout_ns;
+  uint32_t imm_base;                 // WRITE_IMM carries imm_base + r (the record's id in a larger numbering: a ring's slots)
 };
 
 // One step of G tiles, `stride` apart in the flattened record-major order, of up to PMAX sources: every load (PMAX x 32
@@ -507,7 +555,8 @@ __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) 
             // acquire every other CTA's bytes of the record; one cumulative system-scope fence on a NIC-facing QP
             fence_scope(sys);
             post_record(a.qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.out_va + (uint64_t)r * rec, a.lkey,
-                        a.remote_va + (uint64_t)r * rec, a.rkey, (uint32_t)rec, r, a.signal_every, a.acc, a.res, a.timeout_ns);
+                        a.remote_va + (uint64_t)r * rec, a.rkey, (uint32_t)rec, a.imm_base + r, a.signal_every, a.acc, a.res,
+                        a.timeout_ns);
           }
           a.counters[r] = 0;
         }
@@ -579,28 +628,39 @@ RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t
   return (int)cudaGetLastError();
 }
 
+// arrived_dev: >= (n_chunks + 3) * 4 bytes of zeroed device memory, and with fwd_qp (rounded up to 8) + 24 more.
+// fwd_flags: bit 0 RDMA_WRITE_IMM (immediate = imm_base + record id), bit 1 post_only.
 RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t dst, uint64_t n_elems,
                            uint32_t chunk_elems, uint64_t qp_dev, uint64_t arrived_dev, uint64_t out_dev,
-                           uint64_t timeout_ms, uint64_t ready_dev) {
+                           uint64_t timeout_ms, uint64_t ready_dev, uint64_t fwd_qp, uint64_t fwd_src_va, uint32_t fwd_lkey,
+                           uint64_t fwd_remote_va, uint32_t fwd_rkey, uint32_t fwd_flags, uint32_t imm_base,
+                           uint32_t signal_every) {
   if (qp_dev && ready_dev) return -22;
+  if (qp_dev && fwd_qp) return -22;                            // the CQ poller owns the flags the forwarders claim
   if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
     return -22;
   if ((staging | dst) & 31) return -22;                        // 256-bit loads / stores: records and output must be 32-byte aligned
+  if (fwd_qp && n_elems / kTileElems >= (1ull << 32)) return -22;
   UnpackArgs a;
   a.staging = (const uint8_t*)staging; a.dst = (__nv_bfloat16*)dst; a.n_elems = n_elems; a.chunk_elems = chunk_elems;
   a.n_chunks = (uint32_t)(n_elems / chunk_elems); a.qp = (QpDev*)qp_dev; a.arrived = (unsigned int*)arrived_dev;
   a.out = (unsigned long long*)out_dev; a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
   a.ready = (const unsigned long long*)ready_dev;
+  a.fwd_qp = (QpDev*)fwd_qp; a.fwd_src_va = fwd_src_va; a.fwd_remote_va = fwd_remote_va; a.fwd_lkey = fwd_lkey;
+  a.fwd_rkey = fwd_rkey; a.with_imm = fwd_flags & 1u; a.post_only = (fwd_flags >> 1) & 1u;
+  a.signal_every = signal_every ? signal_every : 1; a.imm_base = imm_base;
+  a.acc = (unsigned long long*)(arrived_dev + (((uint64_t)a.n_chunks + 3) * 4 + 7) / 8 * 8);
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
   // waiting for arrivals the kernel shares the GPU with whatever produces them (a pack kernel, an engine): one CTA per SM then
-  if (grid <= 0) grid = (qp_dev || ready_dev) ? device_sms() : device_sms() * 4;
+  if (grid <= 0) grid = (qp_dev || ready_dev || fwd_qp) ? device_sms() : device_sms() * 4;
   {
     const uint64_t total_tiles = n_elems / kTileElems;
     if ((uint64_t)grid > total_tiles) grid = (int)total_tiles;
   }
   if (qp_dev) grid += 1;                                      // CTA 0 polls the receive CQ, the others unpack
-  unpack_fp8_kernel<<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  if (fwd_qp) unpack_fp8_kernel<true><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  else unpack_fp8_kernel<false><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
 }
 
@@ -609,7 +669,8 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
 RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_src, uint64_t local, uint64_t out,
                            uint64_t out_rec, uint64_t n_elems, uint32_t chunk_elems, uint64_t ready_dev, uint64_t qp_dev,
                            uint64_t out_va, uint32_t lkey, uint64_t remote_va, uint32_t rkey, uint32_t flags,
-                           uint32_t signal_every, uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms) {
+                           uint32_t signal_every, uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms,
+                           uint32_t imm_base) {
   if (n_src < 1 || n_src > 8) return -22;
   if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
     return -22;
@@ -625,6 +686,7 @@ RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_s
   a.acc = (unsigned long long*)(counters_dev + (((uint64_t)a.n_rec + 3) * 4 + 7) / 8 * 8);
   a.res = (unsigned long long*)out_dev;
   a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.imm_base = imm_base;
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
   // waiting for arrivals the kernel shares the GPU with whatever produces them: one CTA per SM then (as K5)
@@ -644,7 +706,8 @@ RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_s
 extern "C" __attribute__((visibility("default"))) void rn_preload_pack() {
   cudaFuncAttributes at;
   cudaFuncGetAttributes(&at, pack_fp8_write_kernel);
-  cudaFuncGetAttributes(&at, unpack_fp8_kernel);
+  cudaFuncGetAttributes(&at, unpack_fp8_kernel<false>);
+  cudaFuncGetAttributes(&at, unpack_fp8_kernel<true>);
 #define RN_PRELOAD(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL>);
   RN_REDUCE_VARIANTS(RN_PRELOAD)
 #undef RN_PRELOAD

@@ -60,9 +60,12 @@ def _parse(view, n_elems, wire) -> PackResult:
 
 def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chunk_elems: int = 1 << 20,
                    with_imm: bool = False, signal_every: int = 1, grid: int = 0, timeout_ms: int = 2000,
-                   stream=None, sync: bool = True, scratch_slot: int = 0, post_only: bool = False, direct: bool = False):
+                   stream=None, sync: bool = True, scratch_slot: int = 0, post_only: bool = False, direct: bool = False,
+                   result_off=None):
     """Pack ``src`` (bf16) into fp8 chunk records in ``staging_mr`` and, if ``qp`` is given,
     RDMA-write every record to the same offset of ``dst_mr`` from inside the kernel.
+    ``result_off``: where in the mapped scratch the kernel writes its result words (default ``4096 + scratch_slot * 64``,
+    see :func:`result_offset`).
     ``direct``: ``staging_mr`` is the *peer's* buffer registered with this context (NVLink-mapped, ``ctx.reg_mr(tensor_on_the_peer)``):
     the kernel's own stores deliver the records and each one is announced by a zero-length RDMA_WRITE_IMM (needs ``with_imm``)."""
     if direct and not (with_imm and qp is not None and dst_mr is not None):
@@ -78,7 +81,7 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     ws = work_stream(ctx, stream)
     n_chunks = n // chunk_elems
     counters = ctx.dev_scratch((n_chunks + 1) * 4 + 64, offset=scratch_slot * (256 << 10))
-    out_addr, out_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
+    out_addr, out_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     rc = lib.rn_k_pack_fp8_write(_stream_ptr(ws), grid, src.data_ptr(), staging_mr.addr, n, chunk_elems,
                                  qp.dev_ptr if qp is not None else 0, staging_mr.addr, staging_mr.lkey,
                                  dst_mr.addr if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
@@ -93,14 +96,37 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     return _parse(out_view, n, wire)
 
 
+def result_offset(scratch_slot: int, result_off=None) -> int:
+    """Offset in the mapped scratch of a launch's 64-byte result record: ``result_off``, else ``4096 + scratch_slot * 64``.
+    The host zeroes the record when it enqueues the launch, not when the launch runs, so launches queued on one stream
+    before the first of them has run need one record each."""
+    if result_off is None:
+        return 4096 + scratch_slot * 64
+    result_off = int(result_off)
+    if result_off < 0 or result_off % 64:
+        raise ValueError(f"result_off={result_off}: a non-negative multiple of 64")
+    return result_off
+
+
 def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int = 1 << 20, qp=None, grid: int = 0,
-               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_slot: int = 1, ready=None):
+               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_slot: int = 1, ready=None, *,
+               fwd_qp=None, fwd_src_mr=None, fwd_dst_mr=None, fwd_dst_off: int = 0, with_imm: bool = False,
+               imm_base: int = 0, signal_every: int = 1, post_only: bool = False, result_off=None):
     """fp8 chunk records -> bf16.  With ``qp`` the kernel waits for each record's receive
     CQE (RDMA_WRITE_IMM, immediate = chunk id) before touching it.  With ``ready`` (int64 CUDA tensor, one arrival word
     per record, as :func:`~rocnrdma_b200.ops.read_records` and ``recv_consume`` set them) every worker waits for the word of
     the record it is about to read; a word still 0 after ``timeout_ms`` ends the kernel with ``TIMEOUT``.  ``qp`` and
     ``ready`` exclude each other.  ``records_seen``: records announced on the CQ, or, with ``ready``, the words that are
-    nonzero when the kernel ends (after a ``TIMEOUT`` that can include records it never waited for or unpacked)."""
+    nonzero when the kernel ends (after a ``TIMEOUT`` that can include records it never waited for or unpacked).
+
+    Forwarding (``fwd_qp``, with ``fwd_src_mr`` -- the registered region that holds ``staging`` -- and ``fwd_dst_mr``):
+    each record is also posted unchanged, straight from where it landed, as one RDMA WRITE (WRITE_IMM with immediate
+    ``imm_base + r`` when ``with_imm``) from ``staging`` to ``fwd_dst_mr`` at ``fwd_dst_off + r * record_bytes``.  The
+    first CTA that sees record r's word (or, without ``ready``, the first that reads it) posts it, before unpacking it,
+    so each record is posted exactly once and a record whose word never comes is never posted.  The last CTA posts a
+    flush and waits for it unless ``post_only``; the status is ``TIMEOUT`` when fewer records were posted than exist.
+    Forwarding works with ``ready`` or with no wait at all, never with ``qp``.  ``records_forwarded`` and
+    ``t_first_post_ns`` are then set in the result."""
     assert dst.dtype == torch.bfloat16 and dst.is_contiguous()
     if (staging.data_ptr() | dst.data_ptr()) & 31:
         raise ValueError("unpack_fp8: records and output must be 32-byte aligned (256-bit loads / stores)")
@@ -108,25 +134,50 @@ def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int =
     n_chunks = n // chunk_elems
     if qp is not None and ready is not None:
         raise ValueError("unpack_fp8 waits on a receive CQ (qp) or on arrival words (ready), not both")
+    fwd = (fwd_qp, fwd_src_mr, fwd_dst_mr)
+    if any(f is not None for f in fwd) and any(f is None for f in fwd):
+        raise ValueError("forwarding needs fwd_qp, fwd_src_mr and fwd_dst_mr together")
+    if fwd_qp is not None:
+        if qp is not None:
+            raise ValueError("unpack_fp8 forwards with ready= or with no wait, not with the CQ poller (qp)")
+        if n <= 0 or chunk_elems <= 0 or n % TILE_ELEMS or chunk_elems % TILE_ELEMS or n % chunk_elems:
+            raise ValueError(f"n_elems and chunk_elems must be multiples of {TILE_ELEMS}, n_elems of chunk_elems")
+        wire = staging_bytes(n, chunk_elems)
+        src_off = staging.data_ptr() - fwd_src_mr.addr
+        if src_off < 0 or src_off + wire > fwd_src_mr.length:
+            raise ValueError(f"the {n_chunks} records in staging do not lie inside fwd_src_mr")
+        if fwd_dst_off < 0 or fwd_dst_off + wire > fwd_dst_mr.length:
+            raise ValueError(f"{n_chunks} records of {record_bytes(chunk_elems)} bytes at fwd_dst_off={fwd_dst_off} do not "
+                             f"fit fwd_dst_mr ({fwd_dst_mr.length} bytes)")
+        if not 0 <= imm_base or imm_base + n_chunks > 1 << 32:
+            raise ValueError(f"imm_base={imm_base}: the immediates imm_base + r of {n_chunks} records must fit 32 bits")
     ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_chunks, ctx.device, "ready")
     lib = N.load()
     ws = work_stream(ctx, stream)
-    arrived = ctx.dev_scratch((n_chunks + 3) * 4, offset=scratch_slot * (256 << 10))
-    out_addr, out_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
+    # [n_chunks] flags (claims when forwarding) ; CTAs done ; records seen ; abort flag ; then post_record's 3 words
+    arrived = ctx.dev_scratch(((n_chunks + 3) * 4 + 7) // 8 * 8 + 24, offset=scratch_slot * (256 << 10))
+    out_addr, out_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     rc = lib.rn_k_unpack_fp8(_stream_ptr(ws), grid, staging.data_ptr(), dst.data_ptr(), n, chunk_elems,
-                             qp.dev_ptr if qp is not None else 0, arrived, out_addr, timeout_ms, ready_addr)
+                             qp.dev_ptr if qp is not None else 0, arrived, out_addr, timeout_ms, ready_addr,
+                             fwd_qp.dev_ptr if fwd_qp is not None else 0,
+                             fwd_src_mr.addr + src_off if fwd_qp is not None else 0,
+                             fwd_src_mr.lkey if fwd_qp is not None else 0,
+                             fwd_dst_mr.addr + fwd_dst_off if fwd_qp is not None else 0,
+                             fwd_dst_mr.rkey if fwd_qp is not None else 0, int(with_imm) | (2 if post_only else 0),
+                             imm_base, signal_every)
     if rc:
         raise N.NativeError(f"unpack_fp8 launch failed ({rc})")
     if not sync:
         return out_view, ws
     ws.synchronize()
-    w = (C.c_int64 * 8).from_buffer(out_view)
     return parse_unpack(out_view)
 
 
 def parse_unpack(view) -> dict:
+    """Decode the record :func:`unpack_fp8` leaves in the mapped scratch (for ``sync=False`` callers)."""
     w = (C.c_int64 * 8).from_buffer(view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), device_ns=w[2] - w[1], records_seen=w[3])
+    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), device_ns=w[2] - w[1], records_seen=w[3], records_forwarded=w[4],
+                t_first_post_ns=w[5], t_start_ns=w[1], t_end_ns=w[2])
 
 
 # ------------------------------------------------------------------ bit-exact references
@@ -219,6 +270,27 @@ def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems:
     return acc.to(torch.bfloat16), _quantized_records(acc, chunk_elems)
 
 
+def ref_allreduce_fp8(xs, chunk_elems: int) -> torch.Tensor:
+    """Reference of the fp8 ring all-reduce (:class:`~rocnrdma_b200.parallel.ring_fp8.RingAllreduceFp8`), bit for bit;
+    runs on CPU or GPU.  ``xs``: the N ranks' bf16 tensors of n elements each.  Returns the bf16 result every rank holds.
+
+    Shard s (elements ``[s * n / N, (s + 1) * n / N)``) starts as ``ref_pack_fp8(xs[s])`` on rank s and is reduced with
+    ``xs[s + 1], ..., xs[s - 1]`` (indices mod N) in ring order, one :func:`ref_reduce_fp8` hop each (the addend first,
+    then the decoded records, one fp32 add, then re-quantised); the final records are unpacked.  The order is fixed, so
+    the result is deterministic, but it depends on which rank holds which tensor."""
+    N = len(xs)
+    n = xs[0].numel()
+    m = n // N
+    out = torch.empty(n, dtype=torch.bfloat16, device=xs[0].device)
+    for s in range(N):
+        part = slice(s * m, (s + 1) * m)
+        recs = ref_pack_fp8(xs[s].reshape(-1)[part], chunk_elems)
+        for h in range(1, N):
+            _, recs = ref_reduce_fp8(recs, 1, m, chunk_elems, local=xs[(s + h) % N].reshape(-1)[part])
+        out[part] = ref_unpack_fp8(recs, m, chunk_elems).to(out.device)
+    return out
+
+
 # ------------------------------------------------------------------ reduce
 MAX_SOURCES = 8
 _SLOT = 256 << 10
@@ -270,7 +342,7 @@ def _check_bf16(t, n, device, what):
 def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int = 1 << 20, *, local=None, out=None,
                out_mr=None, qp=None, dst_mr=None, dst_off: int = 0, with_imm: bool = False, signal_every: int = 1,
                post_only: bool = False, ready=None, grid: int = 0, timeout_ms: int = 2000, stream=None, sync: bool = True,
-               scratch_slot: int = 4):
+               scratch_slot: int = 4, imm_base: int = 0, result_off=None):
     """Sum ``n_src`` sources of K3 chunk records, plus an optional bf16 addend, as the records land, and re-pack and forward
     the sum: one hop of a reduce-scatter ring in one kernel.
 
@@ -287,6 +359,8 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     :func:`~rocnrdma_b200.ops.read_records` set them) every step waits for the words of all sources of the records it
     reads; a word still 0 after ``timeout_ms`` ends the kernel with ``TIMEOUT``, and a record not reduced is never posted.
     Two reductions that run at once need different ``scratch_slot`` values (0..7; K3 uses 0, K5 1, the GEMMs 2 and 3).
+    ``imm_base`` offsets the immediates (``imm_base + r``), so that the records of several hops that reach one QP stamp
+    different arrival words; ``result_off`` is :func:`result_offset`'s.
 
     Returns a :class:`ReduceResult`, or ``(result view, stream)`` with ``sync=False`` (decode with :func:`parse_reduce`)."""
     n_src, n_elems, chunk_elems = int(n_src), int(n_elems), int(chunk_elems)
@@ -320,6 +394,8 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     if dst_mr is not None and (dst_off < 0 or dst_off + wire > dst_mr.length):
         raise ValueError(f"{n_rec} records of {record_bytes(chunk_elems)} bytes at dst_off={dst_off} do not fit dst_mr "
                          f"({dst_mr.length} bytes)")
+    if not 0 <= imm_base or imm_base + n_rec > 1 << 32:
+        raise ValueError(f"imm_base={imm_base}: the immediates imm_base + r of {n_rec} records must fit 32 bits")
     ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_src * n_rec, dev, "ready")
     counter_bytes = ((n_rec + 3) * 4 + 7) // 8 * 8 + 24
     if counter_bytes > _SLOT:
@@ -329,7 +405,7 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     lib = N.load()
     ws = work_stream(ctx, stream)
     counters = ctx.dev_scratch(counter_bytes, offset=scratch_slot * _SLOT)
-    res_addr, res_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
+    res_addr, res_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     hbm = n_src * wire + (2 * n_elems if local is not None else 0) + (2 * n_elems if out is not None else 0) + \
         (wire if out_mr is not None else 0)
     rc = lib.rn_k_reduce_fp8(_stream_ptr(ws), grid, records.data_ptr(), n_src, local_addr, out_addr,
@@ -337,7 +413,7 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
                              qp.dev_ptr if qp is not None else 0, out_mr.addr if out_mr is not None else 0,
                              out_mr.lkey if out_mr is not None else 0, dst_mr.addr + dst_off if dst_mr is not None else 0,
                              dst_mr.rkey if dst_mr is not None else 0, int(with_imm) | (2 if post_only else 0), signal_every,
-                             counters, res_addr, timeout_ms)
+                             counters, res_addr, timeout_ms, imm_base)
     if rc:
         raise N.NativeError(f"reduce_fp8 launch failed ({rc})")
     if not sync:
