@@ -17,9 +17,13 @@
 //
 // Record layout for a chunk of C elements (C % 8192 == 0):
 //     [ C bytes fp8 e4m3 ][ C/32 bytes UE8M0 scales ][ pad to 64 B ]
-// Quantisation (bit-exact reference: ops/pack.py, quantize_blocks / ref_pack_fp8 / ref_unpack_fp8 / ref_reduce_fp8):
-//     v = amax * (1/448)  (fp32) ; e = exponent(v) + (mantissa(v) != 0), clamped to [-127, 127]
-//     q = cvt.rn.satfinite.e4m3(x * 2^-e) ; scale byte = e + 127
+// Quantisation (mx_scale.cuh; bit-exact reference: ops/pack.py, quantize_blocks / ref_pack_fp8 / ref_unpack_fp8 /
+// ref_reduce_fp8):
+//     e = the smallest integer with amax / 2^e <= 448, clamped to [-127, 127], from the fp32 bits of v = amax * (1/448):
+//         -127 when v <= 2^-127, else exponent(v) + (mantissa(v) != 0), at most 127
+//     y = x * 2^-e ; at e = 120 only, |y| > 240 becomes +-240 (codes 248 and 256 would decode to 2^128 = Inf in fp32)
+//     q = cvt.rn.satfinite.e4m3(y) ; scale byte = e + 127
+//     so every finite input decodes finite, and the saturation's relative error stays under 2^-4 (worst: 255.99 -> 240)
 // Non-finite input:
 //     NaN   amax is an fmaxf reduction, which drops NaN: a NaN stays in its own element, its neighbours quantise
 //           as if it were absent (an all-NaN block gets scale byte 0 and NaN codes)
@@ -34,6 +38,7 @@
 #include <stdint.h>
 
 #include "../hca/post.cuh"
+#include "mx_scale.cuh"
 
 using namespace rn;
 using namespace rn::dev;
@@ -87,16 +92,13 @@ __device__ __forceinline__ uint32_t quantize_block32(const float (&x)[32], uint3
   float amax = 0.f;
 #pragma unroll
   for (int i = 0; i < 16; ++i) amax = fmaxf(amax, fmaxf(fabsf(x[2 * i]), fabsf(x[2 * i + 1])));
-  // UE8M0 scale: smallest power of two 2^e with amax / 2^e <= 448
-  const uint32_t vb = __float_as_uint(amax * (1.0f / 448.0f));
-  int e = (int)((vb >> 23) & 0xff) - 127 + ((vb & 0x7fffffu) ? 1 : 0);
-  e = max(-127, min(127, e));
+  const int e = mx_scale_exponent(amax);
   const float inv = __uint_as_float((uint32_t)(127 - e) << 23);   // 2^-e, exact (biased exponent 0..254)
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i] * inv, x[4 * i + 1] * inv), __NV_SATFINITE, __NV_E4M3);
     uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(x[4 * i + 2] * inv, x[4 * i + 3] * inv), __NV_SATFINITE, __NV_E4M3);
-    q[i] = lo | (hi << 16);
+    q[i] = mx_saturate_codes(lo | (hi << 16), e);
   }
   return (uint32_t)(e + 127);
 }

@@ -187,13 +187,16 @@ def parse_unpack(view) -> dict:
 #   * a block holding +-Inf gets exponent 127 (scale byte 254) and multiplier 2^-127 == 0.0, so the Inf becomes
 #     NaN and every finite neighbour becomes +-0;
 #   * decoding, scale byte 0x00 is 2^-127 (the OCP MX value, an fp32 denormal) and 0xFF is 2^128 == Inf.
+#   * at e = 120, the one exponent whose codes 248 and 256 would decode past fp32 max (to 2^128 = Inf), a scaled value
+#     above 240 in magnitude saturates to +-240, so every finite input decodes finite (NaN is kept).
 def _scale_exponent(amax: torch.Tensor) -> torch.Tensor:
-    """e = smallest integer with amax / 2^e <= 448, computed on the fp32 bit pattern exactly
-    as the kernel does (no log2 rounding)."""
+    """e = smallest integer with amax / 2^e <= 448, clamped to [-127, 127], computed on the fp32 bit pattern of
+    amax * (1/448) exactly as the kernels do (no log2 rounding): a value at or below 2^-127 (fp32 0x00400000) gives
+    -127, any other exponent(v) + (mantissa(v) != 0)."""
     v = (amax.float() * (1.0 / 448.0)).contiguous()
     bits = v.view(torch.int32)
     e = ((bits >> 23) & 0xFF) - 127 + ((bits & 0x7FFFFF) != 0).to(torch.int32)
-    return e.clamp(-127, 127)
+    return torch.where(bits <= 0x00400000, torch.full_like(e, -127), e.clamp(max=127))
 
 
 def _pow2(e: torch.Tensor) -> torch.Tensor:
@@ -214,7 +217,10 @@ def quantize_blocks(x: torch.Tensor):
     a = x.abs()
     a = torch.where(torch.isnan(a), torch.zeros_like(a), a)       # fmaxf drops NaN; +Inf stays
     e = _scale_exponent(a.amax(dim=-1))
-    q = (x * _pow2(-e)[..., None]).to(torch.float8_e4m3fn).view(torch.uint8)
+    y = x * _pow2(-e)[..., None]
+    lim = torch.where(e == 120, 240.0, 448.0)[..., None]
+    y = torch.where(y.abs() > lim, torch.copysign(lim, y), y)     # NaN compares false and stays
+    q = y.to(torch.float8_e4m3fn).view(torch.uint8)
     return q, (e + 127).to(torch.uint8)
 
 

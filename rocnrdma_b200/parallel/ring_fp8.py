@@ -35,6 +35,13 @@ GUARD = 8                       # zero words behind the arrival words
 RESULT_BASE = 128 << 10         # mapped-scratch offset of the ring's result records: 4 KiB per device-scratch slot
 RESULT_SLOT_BYTES = 4096
 MAX_IN_PROCESS = 8              # one device-scratch slot per simulated rank
+MAX_QUEUE_DEPTH = 16384         # the deepest queue create_qp builds (a power of two; the doorbell index is 16 bits)
+
+
+def max_records(world: int) -> int:
+    """The most records per shard a plan of ``world`` ranks can have: its receive queue and CQ hold
+    ``_pow2(2 * 2(N-1)R)`` entries, at most ``MAX_QUEUE_DEPTH``."""
+    return MAX_QUEUE_DEPTH // (4 * (int(world) - 1))
 
 
 @dataclass(frozen=True)
@@ -133,6 +140,9 @@ class RingAllreduceFp8:
         counter_bytes = ((self.R + 3) * 4 + 7) // 8 * 8 + 24
         if counter_bytes > 256 << 10:
             raise ValueError(f"{self.R} records per shard need {counter_bytes} bytes of counters; a scratch slot holds 256 KiB")
+        if self.R > max_records(world):
+            raise ValueError(f"R={self.R} records per shard: the receive queue would need {_pow2(2 * self.n_ids)} entries, "
+                             f"above {MAX_QUEUE_DEPTH}; at world={world} R may be at most {max_records(world)}")
         dev = ctx.device
         self.staging = torch.zeros(self.R * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")
         self.landing = torch.zeros(self.n_ids * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")

@@ -141,3 +141,43 @@ def test_reference_error_against_the_exact_sum(N):
     err = np.abs(got - exact)
     assert np.all(err <= bound), f"max excess {np.max(err - bound)}"
     assert np.max(err / np.maximum(bound, 1e-300)) > 0.01, "the bound is never approached: the check is vacuous"
+
+
+# ------------------------------------------------------------------ the forwarding unpack's walk (test_gpu_ring_fp8_shapes.py)
+def test_unpack_schedule_hand_counted_walks():
+    from test_gpu_ring_fp8_shapes import UnpackSchedule
+    # tpc 3, R 5, grid 1: one CTA, four consecutive tiles per step; it visits records (0, 1), (1, 2), (2, 3), (4)
+    s = UnpackSchedule(3 * 8192, 5, 1)
+    assert s.steps == [[[0, 1, 2, 3], [4, 5, 6, 7], [8, 9, 10, 11], [12, 13, 14]]]
+    assert [s.visits(t) for t in s.steps[0]] == [[0, 1], [1, 2], [2, 3], [4]]
+    assert s.sure_claims() == {(0, 0): {0, 1}, (0, 1): {2}, (0, 2): {3}, (0, 3): {4}}
+    # tpc 5, R 4, grid 2: tiles two apart, so both CTAs hold every record and race to claim it
+    s = UnpackSchedule(5 * 8192, 4, 2)
+    assert s.steps[0] == [[0, 2, 4, 6], [8, 10, 12, 14], [16, 18]] and s.steps[1][0] == [1, 3, 5, 7]
+    assert [s.visits(t) for t in s.steps[0]] == [[0, 1], [1, 2], [3]]
+    assert all(c == {0, 1} for c in s.owners().values()) and s.sure_claims() == {}
+    # the grid clamps to one slot's tile count; the default is one CTA per SM
+    s = UnpackSchedule(8192, 2, 7)
+    assert (s.grid, s.steps) == (2, [[[0]], [[1]]]) and s.facts()["clamped_grid"]
+    assert UnpackSchedule(1 << 20, 2, sms=132).grid == 132 and not UnpackSchedule(1 << 20, 2, sms=132).facts()["clamped_grid"]
+    # tpc 1, R 7, grid 1: one step claims four records, the next three
+    s = UnpackSchedule(8192, 7, 1)
+    assert s.sure_claims() == {(0, 0): {0, 1, 2, 3}, (0, 1): {4, 5, 6}}
+
+
+def test_ring_geometry_cases_cover_every_fact_and_parameter():
+    """The GPU geometry cases: each asserts its facts at run time; together they exercise every fact of the forwarding
+    unpack, every N with a multi-tile R > 1 case, and every listed value of tiles per record, R, grid and signal_every."""
+    from test_gpu_ring_fp8_shapes import GEOMETRY_CASES, UNPACK_FACTS, case_facts, ring_grid
+    seen = set()
+    for (N, tpc, R, grid, sig), u, r in GEOMETRY_CASES:
+        assert case_facts(N, tpc, R, grid) == (u, r), (N, tpc, R, grid)
+        assert 16 + N * (ring_grid(N, grid) + 1) <= 132, "SM budget"
+        seen |= u
+    assert seen == set(UNPACK_FACTS)
+    cases = [c for c, _, _ in GEOMETRY_CASES]
+    assert {N for N, tpc, R, _, _ in cases if tpc > 1 and R > 1} == set(range(2, 9))
+    assert {c[1] for c in cases} == {1, 3, 5, 8, 128} and {c[2] for c in cases} == {1, 2, 4, 5, 7}
+    assert {1, 2, 3, 7, 0} <= {c[3] for c in cases}
+    assert any(grid > R * tpc for _, tpc, R, grid, _ in cases), "a grid larger than the slot's tile count"
+    assert {1, 3} <= {c[4] for c in cases} and any(sig > R for _, _, R, _, sig in cases)
