@@ -128,7 +128,7 @@ _SIGS = {
     "rn_hca_dev_scratch": (u64, [vp, C.POINTER(u64)]),
     "rn_pack_record_bytes": (u64, [u64]),
     "rn_pack_tile_elems": (u32, []),
-    "rn_k_pack_fp8_write": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64]),
+    "rn_k_pack_fp8_write": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64, u64]),
     "rn_gemm_timeline": (i32, [C.POINTER(C.c_uint64)]),
     "rn_k_gemm_send": (i32, [u64, i32, u64, u64, u64, u32, u32, u32, u64, u64, u32, u64, u32, u32, u32, u32, u32, u32, u32, u64, u64, u64]),
     "rn_k_gemm_mxfp8": (i32, [u64, i32, u64, u64, u32, u64, u64, u64, u32, u64, u64, u32, u32, u32, u64, u32, u64, u64, u64]),
@@ -137,7 +137,7 @@ _SIGS = {
     "rn_hca_enable_peer": (i32, [vp, i32]),
     "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64, u64, u64, u64, u32, u64, u32, u32, u32, u32]),
     "rn_k_reduce_fp8": (i32, [u64, i32, u64, u32, u64, u64, u64, u64, u32, u64, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64,
-                              u32]),
+                              u32, u64]),
     "rn_k_rdma_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u32, u32, u32, u32, u64, u32, u64, u64, u32]),
     "rn_k_write_read": (i32, [u64, u64, u64, u32, u64, u32, u64, u32, u32, u32, u32, u64, u64]),
     "rn_stream_clamp": (None, [u32, C.POINTER(u32), C.POINTER(u32)]),

@@ -30,6 +30,11 @@
 //     +-Inf e clamps to 127 (scale byte 254) and 2^-127 is 0.0 here: the Inf becomes NaN, its neighbours +-0
 //           (a finite sum that overflows fp32 in the reduce is such an Inf)
 // Decode: scale byte 0x00 is 2^-127 (the OCP MX value, fp32 0x00400000), as in the block-scaled GEMM; 0xFF is Inf.
+// Error feedback (K3 and the reduce with a residual, EF = true): an fp32 residual of n_elems, read and written in place
+// by the thread that quantises the element.  K3 quantises v = x + r_in, the reduce v = (its sum) + r_in, the residual
+// added last; then r_out = v - d, d = code * ue8m0(scale byte) as the decoders make it, exact in fp32 wherever v and d
+// are finite (|d| <= 2|v|, same sign: Sterbenz), and 0 wherever either is not (NaN, a block holding Inf, an overflowing
+// sum), so one bad step cannot poison the residual for good.
 //
 // No counterpart in the reference (it moves no payload: SURVEY.md section 3.2).
 #include <cuda_bf16.h>
@@ -80,6 +85,7 @@ struct PackArgs {
                              // (atomics stay in device memory; `out` is mapped host memory, plain stores only)
   unsigned long long* out;   // [status, t_start, t_end, wqes_posted, t_first_post, t_pack_end, 0, 0]
   uint64_t timeout_ns;
+  float* residual;           // pack_fp8_write_kernel<true> only: n_elems fp32, read and written in place
 };
 
 __device__ __forceinline__ float bf16_bits_to_float(uint32_t hi16) { return __uint_as_float(hi16 << 16); }
@@ -103,16 +109,59 @@ __device__ __forceinline__ uint32_t quantize_block32(const float (&x)[32], uint3
   return (uint32_t)(e + 127);
 }
 
-template <int G>
+// 32 contiguous bytes per thread, streaming (evict-first): a thread's 32 bytes of fp8 in, and its 64 bytes of bf16 out as two
+// whole 32-byte sectors.  Hopper's widest global access is 128 bits, so each is a pair of adjacent 16-byte accesses.
+__device__ __forceinline__ void ld256_cs(const void* p, uint32_t* r) {
+  asm volatile("ld.global.cs.v4.b32 {%0,%1,%2,%3}, [%8];\n\tld.global.cs.v4.b32 {%4,%5,%6,%7}, [%8+16];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p));
+}
+__device__ __forceinline__ void st256_cs(void* p, const uint32_t* r) {
+  asm volatile("st.global.cs.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.cs.v4.b32 [%0+16], {%5,%6,%7,%8};"
+               ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
+}
+
+// A thread's 32 fp32 residuals (128 contiguous bytes) in and out, as four 32-byte pairs of accesses.
+__device__ __forceinline__ void ld_residual(const float* p, uint32_t (&r)[32]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) ld256_cs(p + 8 * j, r + 8 * j);
+}
+__device__ __forceinline__ void st_residual(float* p, const float (&r)[32]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) st256_cs(p + 8 * j, reinterpret_cast<const uint32_t*>(r + 8 * j));
+}
+
+// Error feedback after quantize_block32: v[i] becomes r_out = v - d, d = code * ue8m0(scale) decoded as the decoders do
+// (e4m3 -> half -> fp32, one __fmul_rn).  The difference is exact where v and d are finite, and non-finite exactly where
+// one of them is not: then r_out = 0.
+__device__ __forceinline__ void ef_residual(float (&v)[32], const uint32_t (&q)[8], uint32_t scale) {
+  const float sc = ue8m0(scale);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    __half2_raw h0 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(q[i] & 0xffff), __NV_E4M3);
+    __half2_raw h1 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(q[i] >> 16), __NV_E4M3);
+    const float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&h0));
+    const float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&h1));
+    const float d[4] = {__fmul_rn(f0.x, sc), __fmul_rn(f0.y, sc), __fmul_rn(f1.x, sc), __fmul_rn(f1.y, sc)};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float r = __fsub_rn(v[4 * i + k], d[k]);
+      v[4 * i + k] = (__float_as_uint(r) & 0x7f800000u) != 0x7f800000u ? r : 0.f;
+    }
+  }
+}
+
+template <int G, bool EF>
 __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_tile, uint32_t tiles_per_chunk, uint64_t rec) {
   // G tiles (G x 16 KiB of bf16) per step: all 4G 16-byte loads are issued before the first
   // use, so each thread keeps G x 64 B in flight (the single-tile version left HBM idle:
-  // 16 KiB in flight per CTA measured ~2.7 TB/s aggregate at best).
+  // 16 KiB in flight per CTA measured ~2.7 TB/s aggregate at best).  With EF, G x 128 B of residual more.
   uint4 v[G][4];
+  uint32_t rv[G][EF ? 32 : 1];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     const uint4* p = reinterpret_cast<const uint4*>(a.src + (first_tile + g) * kTileElems + (uint64_t)threadIdx.x * kBlockElems);
     v[g][0] = __ldcs(p); v[g][1] = __ldcs(p + 1); v[g][2] = __ldcs(p + 2); v[g][3] = __ldcs(p + 3);
+    if constexpr (EF) ld_residual(a.residual + (first_tile + g) * kTileElems + (uint64_t)threadIdx.x * kBlockElems, rv[g]);
   }
 #pragma unroll
   for (int g = 0; g < G; ++g) {
@@ -124,6 +173,10 @@ __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_til
     float x[32];
 #pragma unroll
     for (int i = 0; i < 16; ++i) { x[2 * i] = bf16_bits_to_float(w[i] & 0xffffu); x[2 * i + 1] = bf16_bits_to_float(w[i] >> 16); }
+    if constexpr (EF) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) x[i] = __fadd_rn(x[i], __uint_as_float(rv[g][i]));
+    }
     uint32_t q[8];
     const uint32_t scale = quantize_block32(x, q);
     uint8_t* recp = a.staging + (uint64_t)chunk * rec;
@@ -131,25 +184,37 @@ __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_til
     out[0] = make_uint4(q[0], q[1], q[2], q[3]);
     out[1] = make_uint4(q[4], q[5], q[6], q[7]);
     recp[a.chunk_elems + (uint64_t)tile_in_chunk * kPackThreads + threadIdx.x] = (uint8_t)scale;
+    if constexpr (EF) {
+      ef_residual(x, q, scale);
+      st_residual(a.residual + tile * kTileElems + (uint64_t)threadIdx.x * kBlockElems, x);
+    }
   }
 }
 
+// EF = true quantises x + residual and writes the new residual back (pack_group's EF); everything else is the same.
+template <bool EF>
 __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a) {
   const unsigned long long t_start = globaltimer_ns();
   const uint64_t n_tiles = a.n_elems / kTileElems;
   const uint32_t tiles_per_chunk = a.chunk_elems / kTileElems;
   const uint64_t rec = record_bytes(a.chunk_elems);
-  // group = G consecutive tiles of one chunk; G is the largest of {4,2,1} dividing tiles_per_chunk
-  const uint32_t G = (tiles_per_chunk % 4 == 0) ? 4 : ((tiles_per_chunk % 2 == 0) ? 2 : 1);
+  // group = G consecutive tiles of one chunk; G is the largest of {4,2,1} dividing tiles_per_chunk ({2,1} with EF: its
+  // residual triples a tile's loads)
+  const uint32_t G = (!EF && tiles_per_chunk % 4 == 0) ? 4 : ((tiles_per_chunk % 2 == 0) ? 2 : 1);
   const uint64_t n_groups = n_tiles / G;
   const uint32_t groups_per_chunk = tiles_per_chunk / G;
   const bool sys = a.qp != nullptr && poster_sys(a.qp);
   for (uint64_t grp = blockIdx.x; grp < n_groups; grp += gridDim.x) {
     const uint64_t first_tile = grp * G;
     const uint32_t chunk = (uint32_t)(first_tile / tiles_per_chunk);
-    if (G == 4) pack_group<4>(a, first_tile, tiles_per_chunk, rec);
-    else if (G == 2) pack_group<2>(a, first_tile, tiles_per_chunk, rec);
-    else pack_group<1>(a, first_tile, tiles_per_chunk, rec);
+    if constexpr (EF) {
+      if (G == 2) pack_group<2, true>(a, first_tile, tiles_per_chunk, rec);
+      else pack_group<1, true>(a, first_tile, tiles_per_chunk, rec);
+    } else {
+      if (G == 4) pack_group<4, false>(a, first_tile, tiles_per_chunk, rec);
+      else if (G == 2) pack_group<2, false>(a, first_tile, tiles_per_chunk, rec);
+      else pack_group<1, false>(a, first_tile, tiles_per_chunk, rec);
+    }
     if (a.qp == nullptr) continue;
     // ---- last arriver of the chunk posts its record
     __syncthreads();
@@ -190,17 +255,6 @@ __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a
       a.acc[0] = 0; a.acc[1] = 0; a.acc[2] = 0;
     }
   }
-}
-
-// 32 contiguous bytes per thread, streaming (evict-first): a thread's 32 bytes of fp8 in, and its 64 bytes of bf16 out as two
-// whole 32-byte sectors.  Hopper's widest global access is 128 bits, so each is a pair of adjacent 16-byte accesses.
-__device__ __forceinline__ void ld256_cs(const void* p, uint32_t* r) {
-  asm volatile("ld.global.cs.v4.b32 {%0,%1,%2,%3}, [%8];\n\tld.global.cs.v4.b32 {%4,%5,%6,%7}, [%8+16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"(p));
-}
-__device__ __forceinline__ void st256_cs(void* p, const uint32_t* r) {
-  asm volatile("st.global.cs.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.cs.v4.b32 [%0+16], {%5,%6,%7,%8};"
-               ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
 }
 
 // Wait for an arrival word (recv_consume, read_records): an acquire load until it is nonzero.  Returns false when the
@@ -424,16 +478,19 @@ struct ReduceArgs {
   unsigned long long* res;           // [status, t_start, t_end, records_reduced, records_posted, t_first_post, t_reduce_end, 0]
   uint64_t timeout_ns;
   uint32_t imm_base;                 // WRITE_IMM carries imm_base + r (the record's id in a larger numbering: a ring's slots)
+  float* residual;                   // reduce_fp8_kernel<.., true> only: n_elems fp32, read and written in place
 };
 
 // One step of G tiles, `stride` apart in the flattened record-major order, of up to PMAX sources: every load (PMAX x 32
-// bytes of fp8 and a scale byte per tile, and 64 bytes of the addend) is issued before the first use.
-template <int G, int PMAX, bool LOCAL>
+// bytes of fp8 and a scale byte per tile, 64 bytes of the addend, and with EF 128 bytes of residual) is issued before the
+// first use.  EF adds the residual to the sum last, and `out` and the records then hold that value.
+template <int G, int PMAX, bool LOCAL, bool EF>
 __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, uint32_t stride, uint64_t total, uint32_t tpc,
                                             uint64_t rec) {
   uint32_t qv[G][PMAX][8];
   uint32_t e[G][PMAX];
   uint32_t lv[G][LOCAL ? 16 : 1];
+  uint32_t rv[G][EF ? 32 : 1];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     const uint64_t T = T0 + (uint64_t)g * stride;
@@ -452,6 +509,7 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
         ld256_cs(lp, lv[g]);
         ld256_cs(lp + 16, lv[g] + 8);
       }
+      if constexpr (EF) ld_residual(a.residual + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems, rv[g]);
     }
   }
 #pragma unroll
@@ -479,6 +537,10 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
         }
       }
     }
+    if constexpr (EF) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) x[i] = __fadd_rn(x[i], __uint_as_float(rv[g][i]));
+    }
     if (a.out) {
       uint32_t o[16];
 #pragma unroll
@@ -500,6 +562,10 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
       o[0] = make_uint4(q[0], q[1], q[2], q[3]);
       o[1] = make_uint4(q[4], q[5], q[6], q[7]);
       recp[a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x] = (uint8_t)scale;
+      if constexpr (EF) {                                      // EF always has out_rec (the host refuses it without)
+        ef_residual(x, q, scale);
+        st_residual(a.residual + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems, x);
+      }
     }
   }
 }
@@ -507,7 +573,7 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
 // Workers walk the tiles of all records in K5's flattened record-major order, G tiles per step, so the oldest records
 // finish (and are forwarded) first.  With arrival words there is no poller: before each step thread 0 waits for the
 // words of every source of every record the step reads.  The CTA whose tiles complete a record posts it, as in K3.
-template <int G, int PMAX, bool LOCAL>
+template <int G, int PMAX, bool LOCAL, bool EF>
 __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) {
   const unsigned long long t_start = globaltimer_ns();
   const uint32_t tpc = a.chunk_elems / kTileElems;
@@ -538,7 +604,7 @@ __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) 
       __syncthreads();          // everybody has read `ok` before thread 0 re-arms it for the next step
       if (!good) break;
     }
-    reduce_step<G, PMAX, LOCAL>(a, T0, gridDim.x, total, tpc, rec);
+    reduce_step<G, PMAX, LOCAL, EF>(a, T0, gridDim.x, total, tpc, rec);
     if (!counted) continue;
     // ---- count the step's tiles per record; the CTA that completes a record posts it
     __syncthreads();
@@ -598,6 +664,9 @@ __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) 
 // Tiles per step and sources a variant holds, chosen from P and the addend so that every load of a step fits in
 // registers (about 72 per thread, as K3's four tiles of bf16) and P = 8 with an addend does not spill.
 #define RN_REDUCE_VARIANTS(X) X(4, 1, false) X(4, 2, false) X(2, 4, false) X(1, 8, false) X(2, 2, true) X(1, 8, true)
+// With a residual (EF): P = 1 without the addend, and P <= 2 with it (the ring's hops), one tile per step: its 128
+// bytes per tile keep a step's loads near the others' (at two tiles P = 1 took 245 registers, one CTA per SM).
+#define RN_REDUCE_EF_VARIANTS(X) X(1, 1, false) X(1, 2, true)
 
 }  // namespace
 
@@ -609,9 +678,10 @@ RN_API uint32_t rn_pack_tile_elems() { return kTileElems; }
 RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t staging, uint64_t n_elems,
                                uint32_t chunk_elems, uint64_t qp_dev, uint64_t staging_va, uint32_t lkey,
                                uint64_t remote_va, uint32_t rkey, uint32_t with_imm, uint32_t signal_every,
-                               uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms) {
+                               uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms, uint64_t residual) {
   if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
     return -22;
+  if (residual & 31) return -22;                               // 256-bit loads / stores
   PackArgs a;
   a.src = (const __nv_bfloat16*)src; a.staging = (uint8_t*)staging; a.n_elems = n_elems; a.chunk_elems = chunk_elems;
   a.n_chunks = (uint32_t)(n_elems / chunk_elems); a.qp = (QpDev*)qp_dev; a.staging_va = staging_va; a.lkey = lkey;
@@ -620,13 +690,15 @@ RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t
   a.acc = (unsigned long long*)(counters_dev + (((uint64_t)a.n_chunks + 1) * 4 + 7) / 8 * 8);
   a.out = (unsigned long long*)out_dev;
   a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.residual = (float*)residual;
   // out[] lives in mapped pinned memory: the host zeroes it directly (no memset kernel)
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
   uint64_t n_tiles = n_elems / kTileElems;
   if (grid <= 0) grid = device_sms() * 4;
   if ((uint64_t)grid > n_tiles) grid = (int)n_tiles;
-  pack_fp8_write_kernel<<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  if (residual) pack_fp8_write_kernel<true><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  else pack_fp8_write_kernel<false><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
 }
 
@@ -667,18 +739,21 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
 }
 
 // counters_dev: >= (n_rec + 3) * 4 bytes (rounded up to 8) + 24 of zero-initialised device memory, cleaned by the kernel.
-// flags: bit 0 RDMA_WRITE_IMM (immediate = record id), bit 1 post_only.
+// flags: bit 0 RDMA_WRITE_IMM (immediate = record id), bit 1 post_only.  residual: n_elems fp32 of error feedback (0: none);
+// it needs out_rec, and P = 1, or P = 2 with the addend.
 RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_src, uint64_t local, uint64_t out,
                            uint64_t out_rec, uint64_t n_elems, uint32_t chunk_elems, uint64_t ready_dev, uint64_t qp_dev,
                            uint64_t out_va, uint32_t lkey, uint64_t remote_va, uint32_t rkey, uint32_t flags,
                            uint32_t signal_every, uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms,
-                           uint32_t imm_base) {
+                           uint32_t imm_base, uint64_t residual) {
   if (n_src < 1 || n_src > 8) return -22;
   if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
     return -22;
   if ((src | local | out | out_rec) & 31) return -22;          // 256-bit loads / stores
   if (!out && !out_rec) return -22;
   if (qp_dev && !out_rec) return -22;
+  if (residual & 31) return -22;
+  if (residual && (!out_rec || n_src > (local ? 2u : 1u))) return -22;
   ReduceArgs a;
   a.src = (const uint8_t*)src; a.local = (const __nv_bfloat16*)local; a.out = (__nv_bfloat16*)out; a.out_rec = (uint8_t*)out_rec;
   a.chunk_elems = chunk_elems; a.n_rec = (uint32_t)(n_elems / chunk_elems); a.n_src = n_src;
@@ -689,6 +764,7 @@ RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_s
   a.res = (unsigned long long*)out_dev;
   a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
   a.imm_base = imm_base;
+  a.residual = (float*)residual;
   unsigned long long* o = (unsigned long long*)out_dev;
   for (int i = 0; i < 8; ++i) o[i] = 0;
   // waiting for arrivals the kernel shares the GPU with whatever produces them: one CTA per SM then (as K5)
@@ -699,18 +775,26 @@ RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_s
   }
   const int pmax = local ? (n_src <= 2 ? 2 : 8) : (n_src == 1 ? 1 : n_src <= 2 ? 2 : n_src <= 4 ? 4 : 8);
 #define RN_LAUNCH(G, PMAX, LOCAL) \
-  if (pmax == PMAX && (local != 0) == LOCAL) reduce_fp8_kernel<G, PMAX, LOCAL><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
-  RN_REDUCE_VARIANTS(RN_LAUNCH)
+  if (pmax == PMAX && (local != 0) == LOCAL) reduce_fp8_kernel<G, PMAX, LOCAL, false><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+#define RN_LAUNCH_EF(G, PMAX, LOCAL) \
+  if (pmax == PMAX && (local != 0) == LOCAL) reduce_fp8_kernel<G, PMAX, LOCAL, true><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  if (!residual) { RN_REDUCE_VARIANTS(RN_LAUNCH) }
+  else { RN_REDUCE_EF_VARIANTS(RN_LAUNCH_EF) }
+#undef RN_LAUNCH_EF
 #undef RN_LAUNCH
   return (int)cudaGetLastError();
 }
 
 extern "C" __attribute__((visibility("default"))) void rn_preload_pack() {
   cudaFuncAttributes at;
-  cudaFuncGetAttributes(&at, pack_fp8_write_kernel);
+  cudaFuncGetAttributes(&at, pack_fp8_write_kernel<false>);
+  cudaFuncGetAttributes(&at, pack_fp8_write_kernel<true>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<false>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<true>);
-#define RN_PRELOAD(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL>);
+#define RN_PRELOAD(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL, false>);
+#define RN_PRELOAD_EF(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL, true>);
   RN_REDUCE_VARIANTS(RN_PRELOAD)
+  RN_REDUCE_EF_VARIANTS(RN_PRELOAD_EF)
+#undef RN_PRELOAD_EF
 #undef RN_PRELOAD
 }

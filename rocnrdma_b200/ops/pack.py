@@ -61,13 +61,16 @@ def _parse(view, n_elems, wire) -> PackResult:
 def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chunk_elems: int = 1 << 20,
                    with_imm: bool = False, signal_every: int = 1, grid: int = 0, timeout_ms: int = 2000,
                    stream=None, sync: bool = True, scratch_slot: int = 0, post_only: bool = False, direct: bool = False,
-                   result_off=None):
+                   result_off=None, residual=None):
     """Pack ``src`` (bf16) into fp8 chunk records in ``staging_mr`` and, if ``qp`` is given,
     RDMA-write every record to the same offset of ``dst_mr`` from inside the kernel.
     ``result_off``: where in the mapped scratch the kernel writes its result words (default ``4096 + scratch_slot * 64``,
     see :func:`result_offset`).
     ``direct``: ``staging_mr`` is the *peer's* buffer registered with this context (NVLink-mapped, ``ctx.reg_mr(tensor_on_the_peer)``):
-    the kernel's own stores deliver the records and each one is announced by a zero-length RDMA_WRITE_IMM (needs ``with_imm``)."""
+    the kernel's own stores deliver the records and each one is announced by a zero-length RDMA_WRITE_IMM (needs ``with_imm``).
+    ``residual``: error feedback, an fp32 CUDA tensor of ``src.numel()`` values (contiguous, 32-byte aligned) read and
+    written in place: the kernel quantises ``src + residual`` and leaves there what the records lost, ``v - decode``
+    (0 where either is not finite).  :func:`ref_pack_fp8` reproduces both bit for bit."""
     if direct and not (with_imm and qp is not None and dst_mr is not None):
         raise ValueError("direct mode announces records with RDMA_WRITE_IMM: pass qp, dst_mr and with_imm=True")
     assert src.dtype == torch.bfloat16 and src.is_contiguous()
@@ -77,6 +80,7 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     wire = staging_bytes(n, chunk_elems)
     if staging_mr.length < wire or (dst_mr is not None and dst_mr.length < wire):
         raise ValueError("staging / destination region too small for the records")
+    res_addr = 0 if residual is None else _check_residual(residual, n, ctx.device)
     lib = N.load()
     ws = work_stream(ctx, stream)
     n_chunks = n // chunk_elems
@@ -85,7 +89,8 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     rc = lib.rn_k_pack_fp8_write(_stream_ptr(ws), grid, src.data_ptr(), staging_mr.addr, n, chunk_elems,
                                  qp.dev_ptr if qp is not None else 0, staging_mr.addr, staging_mr.lkey,
                                  dst_mr.addr if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
-                                 int(with_imm) | (2 if post_only else 0) | (4 if direct else 0), signal_every, counters, out_addr, timeout_ms)
+                                 int(with_imm) | (2 if post_only else 0) | (4 if direct else 0), signal_every, counters, out_addr, timeout_ms,
+                                 res_addr)
     if rc:
         raise N.NativeError(f"pack_fp8_write launch failed ({rc})")
     if not sync:
@@ -235,9 +240,23 @@ def _quantized_records(x: torch.Tensor, chunk_elems: int) -> torch.Tensor:
     return out.reshape(-1)
 
 
-def ref_pack_fp8(src: torch.Tensor, chunk_elems: int) -> torch.Tensor:
-    """Reference chunk records (uint8) for a bf16 tensor; runs on CPU or GPU."""
-    return _quantized_records(src.float(), chunk_elems)
+def _ef_residual(v: torch.Tensor, records: torch.Tensor, chunk_elems: int) -> torch.Tensor:
+    """The residual error feedback keeps: ``v - d`` with ``d`` the decode of ``v``'s records, and 0 wherever that is
+    not finite (``v`` or ``d`` is not).  For finite ``v`` and ``d`` the difference is exact in fp32, so ``d + r == v``."""
+    d = _decode_records(records, 1, v.numel(), chunk_elems)[0]
+    r = v.reshape(-1) - d
+    return torch.where(torch.isfinite(r), r, torch.zeros_like(r))
+
+
+def ref_pack_fp8(src: torch.Tensor, chunk_elems: int, residual=None):
+    """Reference chunk records (uint8) for a bf16 tensor; runs on CPU or GPU.  With ``residual`` (fp32, ``src.numel()``)
+    it quantises ``src + residual`` (one fp32 add) and returns ``(records, new residual)``, as
+    :func:`pack_fp8_write` does with ``residual=``."""
+    if residual is None:
+        return _quantized_records(src.float(), chunk_elems)
+    v = src.reshape(-1).float() + residual.reshape(-1).float().to(src.device)
+    recs = _quantized_records(v, chunk_elems)
+    return recs, _ef_residual(v, recs, chunk_elems)
 
 
 def ref_unpack_fp8(records: torch.Tensor, n_elems: int, chunk_elems: int) -> torch.Tensor:
@@ -259,8 +278,10 @@ def _decode_records(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     return (q * s[:, None]).reshape(n_src, n_elems)
 
 
-def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int, local=None):
-    """Reference of :func:`reduce_fp8`; runs on CPU or GPU.  Returns (bf16 sum, K3 records of the sum).
+def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int, local=None, residual=None):
+    """Reference of :func:`reduce_fp8`; runs on CPU or GPU.  Returns (bf16 sum, K3 records of the sum), and with
+    ``residual`` (fp32, ``n_elems``) ``(bf16, records, new residual)``: the residual is added to the sum last, one fp32
+    add, and the bf16 output and the records both hold that value.
 
     The sum starts from ``local`` (bf16, exact in fp32) when given, else from source 0, and adds the other sources in
     source order, one fp32 add each: only the adds round.  The records quantise that fp32 sum with the rule of every
@@ -273,12 +294,21 @@ def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems:
         acc, first = d[0], 1
     for s in range(first, n_src):
         acc = acc + d[s]
-    return acc.to(torch.bfloat16), _quantized_records(acc, chunk_elems)
+    if residual is None:
+        return acc.to(torch.bfloat16), _quantized_records(acc, chunk_elems)
+    acc = acc + residual.reshape(-1).float().to(acc.device)
+    recs = _quantized_records(acc, chunk_elems)
+    return acc.to(torch.bfloat16), recs, _ef_residual(acc, recs, chunk_elems)
 
 
-def ref_allreduce_fp8(xs, chunk_elems: int) -> torch.Tensor:
+def ref_allreduce_fp8(xs, chunk_elems: int, residuals=None):
     """Reference of the fp8 ring all-reduce (:class:`~rocnrdma_b200.parallel.ring_fp8.RingAllreduceFp8`), bit for bit;
     runs on CPU or GPU.  ``xs``: the N ranks' bf16 tensors of n elements each.  Returns the bf16 result every rank holds.
+
+    ``residuals``: the N ranks' fp32 error-feedback residuals of n elements each (``error_feedback=True``); then returns
+    ``(out, new residuals)``.  Rank q quantises every shard once -- shard q in its pack, shard (q-1-k) mod N in reduce hop
+    k -- and shard s of its residual is the error it made there: the pack and each hop quantise ``value + residual`` and
+    keep what the records lost (:func:`ref_pack_fp8`, :func:`ref_reduce_fp8`).
 
     Shard s (elements ``[s * n / N, (s + 1) * n / N)``) starts as ``ref_pack_fp8(xs[s])`` on rank s and is reduced with
     ``xs[s + 1], ..., xs[s - 1]`` (indices mod N) in ring order, one :func:`ref_reduce_fp8` hop each (the addend first,
@@ -288,13 +318,24 @@ def ref_allreduce_fp8(xs, chunk_elems: int) -> torch.Tensor:
     n = xs[0].numel()
     m = n // N
     out = torch.empty(n, dtype=torch.bfloat16, device=xs[0].device)
+    ef = residuals is not None
+    if ef:
+        new = [r.reshape(-1).float().clone() for r in residuals]
     for s in range(N):
         part = slice(s * m, (s + 1) * m)
-        recs = ref_pack_fp8(xs[s].reshape(-1)[part], chunk_elems)
+        if ef:
+            recs, new[s][part] = ref_pack_fp8(xs[s].reshape(-1)[part], chunk_elems, residual=residuals[s].reshape(-1)[part])
+        else:
+            recs = ref_pack_fp8(xs[s].reshape(-1)[part], chunk_elems)
         for h in range(1, N):
-            _, recs = ref_reduce_fp8(recs, 1, m, chunk_elems, local=xs[(s + h) % N].reshape(-1)[part])
+            q = (s + h) % N
+            if ef:
+                _, recs, new[q][part] = ref_reduce_fp8(recs, 1, m, chunk_elems, local=xs[q].reshape(-1)[part],
+                                                       residual=residuals[q].reshape(-1)[part])
+            else:
+                _, recs = ref_reduce_fp8(recs, 1, m, chunk_elems, local=xs[q].reshape(-1)[part])
         out[part] = ref_unpack_fp8(recs, m, chunk_elems).to(out.device)
-    return out
+    return (out, new) if ef else out
 
 
 # ------------------------------------------------------------------ reduce
@@ -345,10 +386,23 @@ def _check_bf16(t, n, device, what):
     return t.data_ptr()
 
 
+def _check_residual(t, n, device):
+    """An error-feedback residual: fp32, on cuda:``device``, contiguous, 32-byte aligned, ``n`` values."""
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+        raise ValueError(f"residual must be a float32 tensor, not {getattr(t, 'dtype', type(t).__name__)}")
+    if not t.is_cuda or t.device.index != device:
+        raise ValueError(f"residual must be on cuda:{device}, not {t.device}")
+    if not t.is_contiguous() or t.data_ptr() & 31:
+        raise ValueError("residual must be contiguous and 32-byte aligned (256-bit loads / stores)")
+    if t.numel() != n:
+        raise ValueError(f"residual holds {t.numel()} elements; n_elems is {n}")
+    return t.data_ptr()
+
+
 def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int = 1 << 20, *, local=None, out=None,
                out_mr=None, qp=None, dst_mr=None, dst_off: int = 0, with_imm: bool = False, signal_every: int = 1,
                post_only: bool = False, ready=None, grid: int = 0, timeout_ms: int = 2000, stream=None, sync: bool = True,
-               scratch_slot: int = 4, imm_base: int = 0, result_off=None):
+               scratch_slot: int = 4, imm_base: int = 0, result_off=None, residual=None):
     """Sum ``n_src`` sources of K3 chunk records, plus an optional bf16 addend, as the records land, and re-pack and forward
     the sum: one hop of a reduce-scatter ring in one kernel.
 
@@ -367,6 +421,11 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     Two reductions that run at once need different ``scratch_slot`` values (0..7; K3 uses 0, K5 1, the GEMMs 2 and 3).
     ``imm_base`` offsets the immediates (``imm_base + r``), so that the records of several hops that reach one QP stamp
     different arrival words; ``result_off`` is :func:`result_offset`'s.
+
+    ``residual``: error feedback, an fp32 CUDA tensor of ``n_elems`` (contiguous, 32-byte aligned) read and written in
+    place.  It is added to the sum last, one fp32 add; ``out`` and the records hold that value, and the residual then
+    holds what the records lost (0 where the value or its decode is not finite), as :func:`ref_reduce_fp8` computes it.
+    It needs ``out_mr``, and P = 1, or P = 2 with ``local`` (the variants a ring hop uses).
 
     Returns a :class:`ReduceResult`, or ``(result view, stream)`` with ``sync=False`` (decode with :func:`parse_reduce`)."""
     n_src, n_elems, chunk_elems = int(n_src), int(n_elems), int(chunk_elems)
@@ -402,6 +461,13 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
                          f"({dst_mr.length} bytes)")
     if not 0 <= imm_base or imm_base + n_rec > 1 << 32:
         raise ValueError(f"imm_base={imm_base}: the immediates imm_base + r of {n_rec} records must fit 32 bits")
+    res_ptr = 0
+    if residual is not None:
+        if out_mr is None:
+            raise ValueError("residual= needs out_mr: the residual is what the records of the sum lose")
+        if n_src > (2 if local is not None else 1):
+            raise ValueError(f"residual= with n_src={n_src}: error feedback runs with P = 1, or P = 2 with local")
+        res_ptr = _check_residual(residual, n_elems, dev)
     ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_src * n_rec, dev, "ready")
     counter_bytes = ((n_rec + 3) * 4 + 7) // 8 * 8 + 24
     if counter_bytes > _SLOT:
@@ -413,13 +479,13 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     counters = ctx.dev_scratch(counter_bytes, offset=scratch_slot * _SLOT)
     res_addr, res_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     hbm = n_src * wire + (2 * n_elems if local is not None else 0) + (2 * n_elems if out is not None else 0) + \
-        (wire if out_mr is not None else 0)
+        (wire if out_mr is not None else 0) + (8 * n_elems if residual is not None else 0)
     rc = lib.rn_k_reduce_fp8(_stream_ptr(ws), grid, records.data_ptr(), n_src, local_addr, out_addr,
                              out_mr.addr if out_mr is not None else 0, n_elems, chunk_elems, ready_addr,
                              qp.dev_ptr if qp is not None else 0, out_mr.addr if out_mr is not None else 0,
                              out_mr.lkey if out_mr is not None else 0, dst_mr.addr + dst_off if dst_mr is not None else 0,
                              dst_mr.rkey if dst_mr is not None else 0, int(with_imm) | (2 if post_only else 0), signal_every,
-                             counters, res_addr, timeout_ms, imm_base)
+                             counters, res_addr, timeout_ms, imm_base, res_ptr)
     if rc:
         raise N.NativeError(f"reduce_fp8 launch failed ({rc})")
     if not sync:

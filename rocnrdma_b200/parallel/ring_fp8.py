@@ -19,6 +19,11 @@ so records of different hops that reach one queue pair never stamp the same word
 dequantisation of the same final records, so every rank holds the same bits (``ops.ref_allreduce_fp8``).  Every read of
 ``x`` precedes the first write of ``out`` on one stream, so ``out=None`` (in place) is safe; the send staging is reused
 from hop to hop because every posting launch waits for its flush.  DESIGN.md 3.4 has the details.
+
+Error feedback (``error_feedback=True``): rank q quantises every shard exactly once per run -- shard q in the pack and
+shard (q-1-k) mod N in reduce hop k -- so one fp32 residual of n elements holds, in shard s, the error rank q made on
+shard s.  The pack and each hop quantise ``value + residual`` and write back what the records lost, in the same pass;
+summed over runs the output then equals the exact sum up to the last residual.  Nothing on the wire changes.
 """
 from __future__ import annotations
 
@@ -115,10 +120,15 @@ class RingAllreduceFp8:
 
     ``grid`` is the CTAs of every launch (0: as many as the SM budget allows).  Every kernel that waits must be resident
     as a whole beside the engine and the other waiters, so ``engine_ctas + ranks on the GPU * (grid + 1)`` may not
-    exceed the device's SMs.  ``timeout_ms`` bounds every wait; a rank whose input never comes ends ``TIMEOUT``."""
+    exceed the device's SMs.  ``timeout_ms`` bounds every wait; a rank whose input never comes ends ``TIMEOUT``.
+
+    ``error_feedback``: carry this rank's quantisation error from run to run in ``residual`` (fp32, ``n_elems``, zero at
+    first), so that the bias of the fp8 rounding does not accumulate over the steps of a training loop.  ``residual`` is
+    a public tensor: copy it out and back in between runs to checkpoint it, and :meth:`reset_residual` zeroes it.  After
+    a run that did not end OK it is undefined, as ``out`` is; reset it before the next run."""
 
     def __init__(self, ctx, n_elems: int, chunk_elems: int, rank: int, world: int, *, grid: int = 0,
-                 timeout_ms: int = 2000, signal_every: int = 1, engine_ctas: int = 16):
+                 timeout_ms: int = 2000, signal_every: int = 1, engine_ctas: int = 16, error_feedback: bool = False):
         n_elems, chunk_elems, rank, world = int(n_elems), int(chunk_elems), int(rank), int(world)
         if world < 2:
             raise ValueError(f"world={world}: a ring needs at least 2 ranks")
@@ -148,6 +158,7 @@ class RingAllreduceFp8:
         self.landing = torch.zeros(self.n_ids * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")
         self.words_full = torch.zeros(self.n_ids + GUARD, dtype=torch.int64, device=f"cuda:{dev}")
         self.words = self.words_full[:self.n_ids]
+        self.residual = torch.zeros(n_elems, dtype=torch.float32, device=f"cuda:{dev}") if error_feedback else None
         self.staging_mr = ctx.reg_mr(self.staging)
         self.landing_mr = ctx.reg_mr(self.landing)
         self.consumer_stream = torch.cuda.Stream(device=dev)
@@ -155,6 +166,8 @@ class RingAllreduceFp8:
         self._cleared = torch.cuda.Event()
         with torch.cuda.stream(self.consumer_stream):
             self.words.zero_()              # loads the fill kernel now: a first load later would wait for the engine
+            if self.residual is not None:
+                self.residual.zero_()       # and reset_residual()'s
         self._cleared.record(self.consumer_stream)
         torch.cuda.synchronize(dev)
         self.send_qp = self.recv_qp = self.remote_landing = None
@@ -201,6 +214,17 @@ class RingAllreduceFp8:
         s %= self.world
         return t[s * self.shard:(s + 1) * self.shard]
 
+    @property
+    def error_feedback(self) -> bool:
+        return self.residual is not None
+
+    def reset_residual(self):
+        """Zero the error-feedback residual, on the main stream (ordered after the runs already enqueued)."""
+        if self.residual is None:
+            raise RuntimeError("this plan has no residual: build it with error_feedback=True")
+        with torch.cuda.stream(self.main_stream):
+            self.residual.zero_()
+
     def _slot(self, m):
         return self.landing[m * self.R * self.rec:(m + 1) * self.R * self.rec], self.words[m * self.R:(m + 1) * self.R]
 
@@ -245,6 +269,7 @@ class RingAllreduceFp8:
         common = dict(grid=self.grid, timeout_ms=self.timeout_ms, stream=ms, sync=False, scratch_slot=self.scratch_slot)
         post = dict(with_imm=True, signal_every=self.signal_every)
         views = self._views
+        ef = lambda s: {} if self.residual is None else dict(residual=self._shard(self.residual, s))  # noqa: E731
         for i, st in enumerate(schedule(q, N)):
             if steps is not None and i not in steps:
                 continue
@@ -252,13 +277,13 @@ class RingAllreduceFp8:
             dst = {} if st.send_slot is None else dict(qp=self.send_qp, dst_mr=self.remote_landing, **post)
             if st.kind == "pack":
                 v, _ = ops.pack_fp8_write(self.ctx, self._shard(x, st.shard), self.staging_mr, chunk_elems=self.chunk,
-                                          result_off=res, **dst, **common)
+                                          result_off=res, **ef(st.shard), **dst, **common)
                 views.append(("pack", v))
             elif st.kind == "reduce":
                 land, words = self._slot(st.read_slot)
                 v, _ = ops.reduce_fp8(self.ctx, land, 1, self.shard, self.chunk, local=self._shard(x, st.shard),
                                       out_mr=self.staging_mr, dst_off=st.send_slot * R * rec, ready=words,
-                                      imm_base=st.send_slot * R, result_off=res, **dst, **common)
+                                      imm_base=st.send_slot * R, result_off=res, **ef(st.shard), **dst, **common)
                 views.append((f"reduce hop {st.read_slot}", v))
             elif st.read_slot is not None:
                 land, words = self._slot(st.read_slot)
@@ -278,7 +303,7 @@ class RingAllreduceFp8:
         ``torch.distributed.all_reduce`` does.  Enqueues everything for this rank with no host step between hops; with
         ``sync`` waits and returns a :class:`RingResult`.  Ranks simulated in one process must all be enqueued before
         any is waited for: use :func:`run_in_process`.  After a run that did not end OK the contents of ``out`` are
-        undefined, as with NCCL."""
+        undefined, as with NCCL, and so is ``residual`` with error feedback."""
         self.start_consumer()
         self.enqueue_main(x, out)
         if not sync:
