@@ -25,6 +25,7 @@
 #include <stdint.h>
 
 #include "../hca/post.cuh"
+#include "mx_scale.cuh"
 #include "sm90.cuh"
 
 using namespace rn;
@@ -107,8 +108,6 @@ __device__ __forceinline__ uint32_t load_scales(const uint8_t* base, uint64_t re
   for (uint32_t i = 0; i < 4; ++i) v |= (uint32_t)(kb * 4 + i < ks ? p[i] : 0x7f) << (8 * i);
   return v;
 }
-
-__device__ __forceinline__ float ue8m0(uint32_t e) { return e ? __uint_as_float(e << 23) : __uint_as_float(0x00400000u); }   // 2^(e - 127)
 
 template <int CTAS>
 __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const MxArgs& g) {

@@ -80,17 +80,13 @@ struct PackArgs {
                              //    transfer; each finished record is announced by a zero-length RDMA_WRITE_IMM posted after a cumulative
                              //    system-scope fence (as gemm_send.cu's direct mode; no engine / NIC moves the payload)
   uint32_t signal_every;     // CQE every k-th chunk (the last one is always signaled)
-  unsigned int* counters;    // [0..n_chunks): tiles done per chunk ; [n_chunks]: CTAs done
+  unsigned int* counters;    // [0..n_chunks): groups done per chunk ; [n_chunks]: CTAs done
   unsigned long long* acc;   // device accumulators: [0] max WQE index+1, [1] WQEs posted, [2] ~first post time
                              // (atomics stay in device memory; `out` is mapped host memory, plain stores only)
   unsigned long long* out;   // [status, t_start, t_end, wqes_posted, t_first_post, t_pack_end, 0, 0]
   uint64_t timeout_ns;
   float* residual;           // pack_fp8_write_kernel<true> only: n_elems fp32, read and written in place
 };
-
-__device__ __forceinline__ float bf16_bits_to_float(uint32_t hi16) { return __uint_as_float(hi16 << 16); }
-// UE8M0 scale byte -> 2^(e - 127); byte 0 is 2^-127, an fp32 denormal (the same decode as gemm_mxfp8.cu)
-__device__ __forceinline__ float ue8m0(uint32_t e) { return e ? __uint_as_float(e << 23) : __uint_as_float(0x00400000u); }
 
 // The quantiser of one MX block (K3's, and the reduce kernel's): 32 fp32 values in element order -> 32 e4m3 codes (q[i]
 // holds elements 4i..4i+3, lowest byte first) and the returned UE8M0 scale byte.  The rule is the header's.
@@ -130,24 +126,50 @@ __device__ __forceinline__ void st_residual(float* p, const float (&r)[32]) {
   for (int j = 0; j < 4; ++j) st256_cs(p + 8 * j, reinterpret_cast<const uint32_t*>(r + 8 * j));
 }
 
-// Error feedback after quantize_block32: v[i] becomes r_out = v - d, d = code * ue8m0(scale) decoded as the decoders do
-// (e4m3 -> half -> fp32, one __fmul_rn).  The difference is exact where v and d are finite, and non-finite exactly where
-// one of them is not: then r_out = 0.
-__device__ __forceinline__ void ef_residual(float (&v)[32], const uint32_t (&q)[8], uint32_t scale) {
-  const float sc = ue8m0(scale);
+// A thread's block of tile t: the offset of its first element in a tensor (bf16 data, an fp32 residual), and of its
+// first code byte in a record (one byte per element).  Record-major flattened tile T of a launch's records is also tile
+// T of its tensors.
+__device__ __forceinline__ uint64_t block_off(uint64_t t) { return t * kTileElems + (uint64_t)threadIdx.x * kBlockElems; }
+// ... and of its scale byte in a record, after the record's chunk_elems codes.
+__device__ __forceinline__ uint64_t scale_off(uint32_t chunk_elems, uint32_t t) {
+  return chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x;
+}
+
+// Store one quantised block (quantize_block32's codes and scale byte) as tile t of the record at recp.
+__device__ __forceinline__ void store_block(uint8_t* recp, uint32_t chunk_elems, uint32_t t, const uint32_t (&q)[8],
+                                            uint32_t scale) {
+  uint4* o = reinterpret_cast<uint4*>(recp + block_off(t));
+  o[0] = make_uint4(q[0], q[1], q[2], q[3]);
+  o[1] = make_uint4(q[4], q[5], q[6], q[7]);
+  recp[scale_off(chunk_elems, t)] = (uint8_t)scale;
+}
+
+// 32 bf16 (w[i] holds elements 2i and 2i+1, lowest half first) -> fp32, exact.
+__device__ __forceinline__ void widen_bf16x32(const uint32_t (&w)[16], float (&x)[32]) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    __half2_raw h0 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(q[i] & 0xffff), __NV_E4M3);
-    __half2_raw h1 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(q[i] >> 16), __NV_E4M3);
-    const float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&h0));
-    const float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&h1));
-    const float d[4] = {__fmul_rn(f0.x, sc), __fmul_rn(f0.y, sc), __fmul_rn(f1.x, sc), __fmul_rn(f1.y, sc)};
+  for (int i = 0; i < 16; ++i) { x[2 * i] = __uint_as_float(w[i] << 16); x[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u); }
+}
+
+// 32 fp32 -> bf16 (round to nearest even), stored at dst as two whole 32-byte sectors.
+__device__ __forceinline__ void st_bf16x32(__nv_bfloat16* dst, const float (&x)[32]) {
+  uint32_t o[16];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float r = __fsub_rn(v[4 * i + k], d[k]);
-      v[4 * i + k] = (__float_as_uint(r) & 0x7f800000u) != 0x7f800000u ? r : 0.f;
-    }
+  for (int i = 0; i < 16; ++i) {
+    __nv_bfloat162 b = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+    o[i] = *reinterpret_cast<uint32_t*>(&b);
   }
+  st256_cs(dst, o);
+  st256_cs(dst + 16, o + 8);
+}
+
+// Error feedback after quantize_block32: v[i] becomes r_out = v - d, d = the block's decode as every decoder makes it
+// (mx_decode_block32).  The difference is exact where v and d are finite, and non-finite exactly where one of them is
+// not: then r_out = 0.
+__device__ __forceinline__ void ef_residual(float (&v)[32], const uint32_t (&q)[8], uint32_t scale) {
+  mx_decode_block32(q, scale, [&](int i, float d) {
+    const float r = __fsub_rn(v[i], d);
+    v[i] = (__float_as_uint(r) & 0x7f800000u) != 0x7f800000u ? r : 0.f;
+  });
 }
 
 template <int G, bool EF>
@@ -159,9 +181,9 @@ __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_til
   uint32_t rv[G][EF ? 32 : 1];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
-    const uint4* p = reinterpret_cast<const uint4*>(a.src + (first_tile + g) * kTileElems + (uint64_t)threadIdx.x * kBlockElems);
+    const uint4* p = reinterpret_cast<const uint4*>(a.src + block_off(first_tile + g));
     v[g][0] = __ldcs(p); v[g][1] = __ldcs(p + 1); v[g][2] = __ldcs(p + 2); v[g][3] = __ldcs(p + 3);
-    if constexpr (EF) ld_residual(a.residual + (first_tile + g) * kTileElems + (uint64_t)threadIdx.x * kBlockElems, rv[g]);
+    if constexpr (EF) ld_residual(a.residual + block_off(first_tile + g), rv[g]);
   }
 #pragma unroll
   for (int g = 0; g < G; ++g) {
@@ -171,24 +193,62 @@ __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_til
     const uint32_t w[16] = {v[g][0].x, v[g][0].y, v[g][0].z, v[g][0].w, v[g][1].x, v[g][1].y, v[g][1].z, v[g][1].w,
                             v[g][2].x, v[g][2].y, v[g][2].z, v[g][2].w, v[g][3].x, v[g][3].y, v[g][3].z, v[g][3].w};
     float x[32];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) { x[2 * i] = bf16_bits_to_float(w[i] & 0xffffu); x[2 * i + 1] = bf16_bits_to_float(w[i] >> 16); }
+    widen_bf16x32(w, x);
     if constexpr (EF) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) x[i] = __fadd_rn(x[i], __uint_as_float(rv[g][i]));
     }
     uint32_t q[8];
     const uint32_t scale = quantize_block32(x, q);
-    uint8_t* recp = a.staging + (uint64_t)chunk * rec;
-    uint4* out = reinterpret_cast<uint4*>(recp + (uint64_t)tile_in_chunk * kTileElems + (uint64_t)threadIdx.x * kBlockElems);
-    out[0] = make_uint4(q[0], q[1], q[2], q[3]);
-    out[1] = make_uint4(q[4], q[5], q[6], q[7]);
-    recp[a.chunk_elems + (uint64_t)tile_in_chunk * kPackThreads + threadIdx.x] = (uint8_t)scale;
+    store_block(a.staging + (uint64_t)chunk * rec, a.chunk_elems, tile_in_chunk, q, scale);
     if constexpr (EF) {
       ef_residual(x, q, scale);
-      st_residual(a.residual + tile * kTileElems + (uint64_t)threadIdx.x * kBlockElems, x);
+      st_residual(a.residual + block_off(tile), x);
     }
   }
+}
+
+// Thread 0, once this CTA's stores of n units (tiles, or K3's groups of tiles) of a record are released (a barrier, then
+// fence_gpu): add them to the record's count.  The arriver that brings it to all `units` counts the record in `done`
+// (when given), acquires every other CTA's part of it with one fence -- fences are cumulative, so on a NIC-facing QP
+// (`sys`) one system-scope fence here covers the whole record without a sys fence per step -- posts it through post()
+// when there is a qp, and re-arms the count for the next launch.
+template <class Post>
+__device__ __forceinline__ void complete_run(unsigned int* count, uint32_t n, uint32_t units, unsigned int* done,
+                                             const QpDev* qp, bool sys, Post post) {
+  if (atomicAdd(count, n) + n != units) return;
+  if (done) atomicAdd(done, 1u);
+  if (qp) {
+    fence_scope(sys);
+    post();
+  }
+  *count = 0;
+}
+
+// After a CTA's last step: true in thread 0 of the CTA that arrives last, false everywhere else.  The barrier and the
+// fence release all of this CTA's work before its arrival.
+__device__ __forceinline__ bool last_cta(unsigned int* ctas_done) {
+  __syncthreads();
+  if (threadIdx.x != 0) return false;
+  fence_gpu();
+  return atomicAdd(ctas_done, 1u) + 1 == gridDim.x;
+}
+
+// The last CTA of a launch that posts records: one flush behind them, whose CQE proves that every record the launch
+// posted has landed (waited for unless post_only).  Fewer than `expected` records posted ends the launch TIMEOUT: a
+// record whose inputs never came is never posted, and the posted ones still drain.  Re-arms post_record's accumulators
+// for the next launch.  Returns the records posted, and in `first` ~acc[2], the time of the first post (all ones when
+// nothing was posted).
+__device__ __forceinline__ unsigned long long flush_records(QpDev* qp, uint32_t post_only, uint64_t timeout_ns, uint32_t expected,
+                                                            unsigned long long* acc, unsigned long long* out,
+                                                            unsigned long long& first) {
+  const unsigned long long posted = ld_u64_volatile(&acc[1]);
+  first = ~ld_u64_volatile(&acc[2]);
+  int rc = post_flush(qp, post_only, timeout_ns);
+  if (posted != expected && rc == WAIT_OK) rc = WAIT_TIMEOUT;
+  if (rc != WAIT_OK) out[0] = (unsigned long long)(long long)rc;
+  acc[0] = 0; acc[1] = 0; acc[2] = 0;
+  return posted;
 }
 
 // EF = true quantises x + residual and writes the new residual back (pack_group's EF); everything else is the same.
@@ -216,44 +276,31 @@ __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a
       else pack_group<1, false>(a, first_tile, tiles_per_chunk, rec);
     }
     if (a.qp == nullptr) continue;
-    // ---- last arriver of the chunk posts its record
+    // ---- the last arriver of the chunk posts its record.  Counted in groups: counted in tiles (G per group, the same
+    // protocol) the <true> kernel takes 130 registers instead of 128, which halves its residency.
     __syncthreads();
     if (threadIdx.x == 0) {
       fence_gpu();   // release this group's record bytes (all threads, via the barrier) before the count
-      unsigned int old = atomicAdd(&a.counters[chunk], 1u);
-      if (old + 1 == groups_per_chunk) {
-        // acquire every other group's bytes; fences are cumulative, so on a NIC-facing QP one
-        // system-scope fence here covers the whole record without a sys fence per group
-        fence_scope(sys || a.direct);
+      complete_run(&a.counters[chunk], 1, groups_per_chunk, nullptr, a.qp, sys || a.direct, [&] {
         post_record(a.qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.staging_va + (uint64_t)chunk * rec, a.lkey,
                     a.remote_va + (uint64_t)chunk * rec, a.rkey, a.direct ? 0u : (uint32_t)rec, chunk, a.signal_every, a.acc,
                     a.out, a.timeout_ns);
-        a.counters[chunk] = 0;   // self-clean for the next launch
-      }
+      });
     }
   }
   if (a.qp == nullptr) return;
   // ---- the CTA that finishes last waits for the wire to drain
-  __syncthreads();
-  if (threadIdx.x == 0) {
+  if (last_cta(&a.counters[a.n_chunks])) {
+    const unsigned long long t_pack_end = globaltimer_ns();
     fence_gpu();
-    unsigned int old = atomicAdd(&a.counters[a.n_chunks], 1u);
-    if (old + 1 == gridDim.x) {
-      const unsigned long long t_pack_end = globaltimer_ns();
-      fence_gpu();
-      unsigned long long posted = ld_u64_volatile(&a.acc[1]);
-      // the flush's CQE proves every record this launch posted has landed
-      int rc = post_flush(a.qp, a.post_only, a.timeout_ns);
-      if (posted != a.n_chunks && rc == WAIT_OK) rc = WAIT_TIMEOUT;
-      if (rc != WAIT_OK) a.out[0] = (unsigned long long)(long long)rc;
-      a.out[1] = t_start;                 // this CTA's start: within a launch skew of the grid's
-      a.out[2] = globaltimer_ns();
-      a.out[3] = posted;
-      a.out[4] = ~ld_u64_volatile(&a.acc[2]);
-      a.out[5] = t_pack_end;
-      a.counters[a.n_chunks] = 0;
-      a.acc[0] = 0; a.acc[1] = 0; a.acc[2] = 0;
-    }
+    unsigned long long first;
+    const unsigned long long posted = flush_records(a.qp, a.post_only, a.timeout_ns, a.n_chunks, a.acc, a.out, first);
+    a.out[1] = t_start;                 // this CTA's start: within a launch skew of the grid's
+    a.out[2] = globaltimer_ns();
+    a.out[3] = posted;
+    a.out[4] = first;
+    a.out[5] = t_pack_end;
+    a.counters[a.n_chunks] = 0;
   }
 }
 
@@ -273,6 +320,34 @@ __device__ __forceinline__ bool wait_word(const unsigned long long* w, unsigned 
     }
     __nanosleep(n < 64 ? 50 : 400);
   }
+}
+
+// Before a step reads its records: thread 0 runs wait(r) once for each distinct record r of the step's G tiles (`stride`
+// apart from T0 in the flattened record-major order, below `total`), stops at the first that returns false, and fences;
+// then every thread gets the outcome.  DIV32 divides in 32 bits, for a caller whose total is below 2^32: a 64-bit
+// division is a call.
+template <int G, bool DIV32, class Wait>
+__device__ __forceinline__ bool step_gate(uint64_t T0, uint32_t stride, uint64_t total, uint32_t tpc, Wait wait) {
+  __shared__ int ok;
+  if (threadIdx.x == 0) {
+    int good = 1;
+    uint32_t last = ~0u;
+#pragma unroll 1
+    for (int g = 0; g < G; ++g) {
+      const uint64_t T = T0 + (uint64_t)g * stride;
+      if (T >= total) break;
+      const uint32_t r = DIV32 ? (uint32_t)T / tpc : (uint32_t)(T / tpc);
+      if (r == last) continue;
+      last = r;
+      if (!wait(r)) { good = 0; break; }
+    }
+    fence_gpu();
+    ok = good;
+  }
+  __syncthreads();
+  const int good = ok;
+  __syncthreads();          // everybody has read `ok` before thread 0 re-arms it for the next step
+  return good;
 }
 
 struct UnpackArgs {
@@ -306,7 +381,6 @@ __global__ void __launch_bounds__(kPackThreads, FWD ? 3 : 0) unpack_fp8_kernel(U
   const unsigned long long t_start = globaltimer_ns();
   const uint32_t tiles_per_chunk = a.chunk_elems / kTileElems;
   const uint64_t rec = record_bytes(a.chunk_elems);
-  __shared__ int ok;
   // With a QP, CTA 0 is the receive-CQ poller and nothing else: it turns every RDMA_WRITE_IMM completion into an arrival flag.
   // (The first version let every CTA poll the CQ for "its" record: hundreds of pollers contending for one consumer index made
   // the consumer, not the wire, the tail of the pack -> NVLink -> unpack chain.)  The other CTAs unpack, chunk-major, so that
@@ -342,52 +416,32 @@ __global__ void __launch_bounds__(kPackThreads, FWD ? 3 : 0) unpack_fp8_kernel(U
     const uint64_t total = (uint64_t)a.n_chunks * tiles_per_chunk;
     constexpr int G = 4;
     for (uint64_t T0 = first; T0 < total; T0 += (uint64_t)stride * G) {
-      if (gated || FWD) {
-        if (FWD && threadIdx.x == 0) {                           // wait for, claim and forward the step's records
-          ok = 1;
-          uint32_t last = ~0u;
-#pragma unroll 1
-          for (int g = 0; g < G && ok; ++g) {
-            const uint64_t T = T0 + (uint64_t)g * stride;
-            if (T >= total) break;
-            const uint32_t chunk = (uint32_t)T / tiles_per_chunk;   // 32-bit: the host keeps total tiles below 2^32
-            if (chunk == last) continue;
-            last = chunk;
-            // the word's acquire (or, with no words, the stream order) makes the record visible to this thread; the CTA
-            // that claims it first releases it to the wire with one fence of the poster's scope and posts it
-            if (a.ready && !wait_word(a.ready + chunk, abort_flag, a.out, a.timeout_ns)) { ok = 0; break; }
-            if (atomicExch(&a.arrived[chunk], 1u) == 0u) {
-              fence_scope(poster_sys(a.fwd_qp));
-              post_record(a.fwd_qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.fwd_src_va + (uint64_t)chunk * rec,
-                          a.fwd_lkey, a.fwd_remote_va + (uint64_t)chunk * rec, a.fwd_rkey, (uint32_t)rec, a.imm_base + chunk,
-                          a.signal_every, a.acc, a.out, a.timeout_ns);
-            }
-          }
-          fence_gpu();
-        } else if (threadIdx.x == 0) {                           // the records this step reads have arrived
-          ok = 1;
-          uint32_t last = ~0u;
-          for (int g = 0; g < G && ok; ++g) {
-            const uint64_t T = T0 + (uint64_t)g * stride;
-            if (T >= total) break;
-            const uint32_t chunk = (uint32_t)(T / tiles_per_chunk);
-            if (chunk == last) continue;
-            last = chunk;
-            if (a.ready) {
-              if (!wait_word(a.ready + chunk, abort_flag, a.out, a.timeout_ns)) ok = 0;
-              continue;
-            }
-            for (unsigned n = 0; *(volatile unsigned int*)&a.arrived[chunk] == 0; ++n) {
-              if (*(volatile unsigned int*)abort_flag) { ok = 0; break; }
-              __nanosleep(n < 64 ? 50 : 400);
-            }
-          }
-          fence_gpu();
-        }
-        __syncthreads();
-        const int good = ok;
-        __syncthreads();          // everybody has read `ok` before thread 0 re-arms it for the next step
-        if (!good) break;
+      if constexpr (FWD) {
+        // wait for, claim and forward the step's records: the word's acquire (or, with no words, the stream order) makes
+        // the record visible to thread 0; the CTA that claims it first releases it to the wire with one fence of the
+        // poster's scope and posts it.  32-bit divisions: the host keeps total tiles below 2^32.
+        if (!step_gate<G, true>(T0, stride, total, tiles_per_chunk, [&](uint32_t r) {
+              if (a.ready && !wait_word(a.ready + r, abort_flag, a.out, a.timeout_ns)) return false;
+              if (atomicExch(&a.arrived[r], 1u) == 0u) {
+                fence_scope(poster_sys(a.fwd_qp));
+                post_record(a.fwd_qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.fwd_src_va + (uint64_t)r * rec,
+                            a.fwd_lkey, a.fwd_remote_va + (uint64_t)r * rec, a.fwd_rkey, (uint32_t)rec, a.imm_base + r,
+                            a.signal_every, a.acc, a.out, a.timeout_ns);
+              }
+              return true;
+            }))
+          break;
+      } else if (gated) {
+        // the records this step reads have arrived: their words, or the poller's flags
+        if (!step_gate<G, false>(T0, stride, total, tiles_per_chunk, [&](uint32_t r) {
+              if (a.ready) return wait_word(a.ready + r, abort_flag, a.out, a.timeout_ns);
+              for (unsigned n = 0; *(volatile unsigned int*)&a.arrived[r] == 0; ++n) {
+                if (*(volatile unsigned int*)abort_flag) return false;
+                __nanosleep(n < 64 ? 50 : 400);
+              }
+              return true;
+            }))
+          break;
       }
       uint32_t qv[G][8];
       uint32_t e[G];
@@ -399,59 +453,36 @@ __global__ void __launch_bounds__(kPackThreads, FWD ? 3 : 0) unpack_fp8_kernel(U
           const uint32_t chunk = FWD ? (uint32_t)T / tiles_per_chunk : (uint32_t)(T / tiles_per_chunk);
           const uint32_t t = FWD ? (uint32_t)T % tiles_per_chunk : (uint32_t)(T % tiles_per_chunk);
           const uint8_t* recp = a.staging + (uint64_t)chunk * rec;
-          ld256_cs(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems, qv[g]);
-          e[g] = __ldcs(recp + a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x);
+          ld256_cs(recp + block_off(t), qv[g]);
+          e[g] = __ldcs(recp + scale_off(a.chunk_elems, t));
         }
       }
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         const uint64_t T = T0 + (uint64_t)g * stride;
         if (T >= total) break;
-        const float s = ue8m0(e[g]);
-        const uint32_t* q = qv[g];
-        uint32_t o[16];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          __half2_raw h0 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(q[i] & 0xffff), __NV_E4M3);
-          __half2_raw h1 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(q[i] >> 16), __NV_E4M3);
-          float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&h0));
-          float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&h1));
-          __nv_bfloat162 b0 = __floats2bfloat162_rn(f0.x * s, f0.y * s);
-          __nv_bfloat162 b1 = __floats2bfloat162_rn(f1.x * s, f1.y * s);
-          o[2 * i] = *reinterpret_cast<uint32_t*>(&b0);
-          o[2 * i + 1] = *reinterpret_cast<uint32_t*>(&b1);
-        }
-        // record-major flattened tile T is also tile T of the output: chunk * chunk_elems + t * kTileElems
-        __nv_bfloat16* dst = a.dst + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems;
-        st256_cs(dst, o);
-        st256_cs(dst + 16, o + 8);
+        float x[32];
+        mx_decode_block32(qv[g], e[g], [&](int i, float d) { x[i] = d; });
+        st_bf16x32(a.dst + block_off(T), x);
       }
     }
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
+  if (last_cta(&a.arrived[a.n_chunks])) {
     fence_gpu();
-    unsigned int old = atomicAdd(&a.arrived[a.n_chunks], 1u);
-    if (old + 1 == gridDim.x) {
-      fence_gpu();
-      if (FWD) {
-        // the flush's CQE proves every forwarded record has landed; a record whose word never came was never posted
-        const unsigned long long posted = ld_u64_volatile(&a.acc[1]);
-        int rc = post_flush(a.fwd_qp, a.post_only, a.timeout_ns);
-        if (posted != a.n_chunks && rc == WAIT_OK) rc = WAIT_TIMEOUT;
-        if (rc != WAIT_OK) a.out[0] = (unsigned long long)(long long)rc;
-        a.out[4] = posted;
-        a.out[5] = posted ? ~ld_u64_volatile(&a.acc[2]) : 0;
-        a.acc[0] = 0; a.acc[1] = 0; a.acc[2] = 0;
-      }
-      a.out[1] = t_start;
-      a.out[2] = globaltimer_ns();
-      uint32_t seen = *(volatile unsigned int*)&a.arrived[a.n_chunks + 1];
-      if (a.ready)                                                        // records whose word is set by now
-        for (uint32_t c = 0; c < a.n_chunks; ++c) seen += ld_u64_volatile(a.ready + c) != 0;
-      a.out[3] = seen;
-      for (uint32_t c = 0; c <= a.n_chunks + 2; ++c) a.arrived[c] = 0;   // self-clean (the claim flags included)
+    if (FWD) {
+      // a record whose word never came was never posted
+      unsigned long long first;
+      const unsigned long long posted = flush_records(a.fwd_qp, a.post_only, a.timeout_ns, a.n_chunks, a.acc, a.out, first);
+      a.out[4] = posted;
+      a.out[5] = posted ? first : 0;
     }
+    a.out[1] = t_start;
+    a.out[2] = globaltimer_ns();
+    uint32_t seen = *(volatile unsigned int*)&a.arrived[a.n_chunks + 1];
+    if (a.ready)                                                        // records whose word is set by now
+      for (uint32_t c = 0; c < a.n_chunks; ++c) seen += ld_u64_volatile(a.ready + c) != 0;
+    a.out[3] = seen;
+    for (uint32_t c = 0; c <= a.n_chunks + 2; ++c) a.arrived[c] = 0;   // self-clean (the claim flags included)
   }
 }
 
@@ -500,16 +531,16 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
       for (int s = 0; s < PMAX; ++s) {
         if (s < (int)a.n_src) {
           const uint8_t* recp = a.src + ((uint64_t)s * a.n_rec + r) * rec;
-          ld256_cs(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems, qv[g][s]);
-          e[g][s] = __ldcs(recp + a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x);
+          ld256_cs(recp + block_off(t), qv[g][s]);
+          e[g][s] = __ldcs(recp + scale_off(a.chunk_elems, t));
         }
       }
-      if (LOCAL) {
-        const __nv_bfloat16* lp = a.local + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems;
+      if constexpr (LOCAL) {
+        const __nv_bfloat16* lp = a.local + block_off(T);
         ld256_cs(lp, lv[g]);
         ld256_cs(lp + 16, lv[g] + 8);
       }
-      if constexpr (EF) ld_residual(a.residual + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems, rv[g]);
+      if constexpr (EF) ld_residual(a.residual + block_off(T), rv[g]);
     }
   }
 #pragma unroll
@@ -517,54 +548,26 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
     const uint64_t T = T0 + (uint64_t)g * stride;
     if (T >= total) break;
     float x[32];
-    if (LOCAL) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) { x[2 * i] = bf16_bits_to_float(lv[g][i] & 0xffffu); x[2 * i + 1] = bf16_bits_to_float(lv[g][i] >> 16); }
-    }
+    if constexpr (LOCAL) widen_bf16x32(lv[g], x);
 #pragma unroll
     for (int s = 0; s < PMAX; ++s) {
       if (s < (int)a.n_src) {
-        const float sc = ue8m0(e[g][s]);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          __half2_raw h0 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(qv[g][s][i] & 0xffff), __NV_E4M3);
-          __half2_raw h1 = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(qv[g][s][i] >> 16), __NV_E4M3);
-          const float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&h0));
-          const float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&h1));
-          const float d[4] = {__fmul_rn(f0.x, sc), __fmul_rn(f0.y, sc), __fmul_rn(f1.x, sc), __fmul_rn(f1.y, sc)};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) x[4 * i + k] = (!LOCAL && s == 0) ? d[k] : __fadd_rn(x[4 * i + k], d[k]);
-        }
+        mx_decode_block32(qv[g][s], e[g][s], [&](int i, float d) { x[i] = (!LOCAL && s == 0) ? d : __fadd_rn(x[i], d); });
       }
     }
     if constexpr (EF) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) x[i] = __fadd_rn(x[i], __uint_as_float(rv[g][i]));
     }
-    if (a.out) {
-      uint32_t o[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        __nv_bfloat162 b = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
-        o[i] = *reinterpret_cast<uint32_t*>(&b);
-      }
-      // record-major flattened tile T is also tile T of the output
-      __nv_bfloat16* dst = a.out + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems;
-      st256_cs(dst, o);
-      st256_cs(dst + 16, o + 8);
-    }
+    if (a.out) st_bf16x32(a.out + block_off(T), x);
     if (a.out_rec) {
       uint32_t q[8];
       const uint32_t scale = quantize_block32(x, q);
       const uint32_t r = (uint32_t)(T / tpc), t = (uint32_t)(T % tpc);
-      uint8_t* recp = a.out_rec + (uint64_t)r * rec;
-      uint4* o = reinterpret_cast<uint4*>(recp + (uint64_t)t * kTileElems + (uint64_t)threadIdx.x * kBlockElems);
-      o[0] = make_uint4(q[0], q[1], q[2], q[3]);
-      o[1] = make_uint4(q[4], q[5], q[6], q[7]);
-      recp[a.chunk_elems + (uint64_t)t * kPackThreads + threadIdx.x] = (uint8_t)scale;
+      store_block(a.out_rec + (uint64_t)r * rec, a.chunk_elems, t, q, scale);
       if constexpr (EF) {                                      // EF always has out_rec (the host refuses it without)
         ef_residual(x, q, scale);
-        st_residual(a.residual + T * kTileElems + (uint64_t)threadIdx.x * kBlockElems, x);
+        st_residual(a.residual + block_off(T), x);
       }
     }
   }
@@ -582,31 +585,17 @@ __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) 
   unsigned int* abort_flag = a.counters + a.n_rec + 1;
   const bool gated = a.ready != nullptr, counted = gated || a.qp != nullptr;
   const bool sys = a.qp != nullptr && poster_sys(a.qp);
-  __shared__ int ok;
   for (uint64_t T0 = blockIdx.x; T0 < total; T0 += (uint64_t)gridDim.x * G) {
-    if (gated) {
-      if (threadIdx.x == 0) {                                  // every source of every record this step reads has landed
-        ok = 1;
-        uint32_t last = ~0u;
-        for (int g = 0; g < G && ok; ++g) {
-          const uint64_t T = T0 + (uint64_t)g * gridDim.x;
-          if (T >= total) break;
-          const uint32_t r = (uint32_t)(T / tpc);
-          if (r == last) continue;
-          last = r;
-          for (uint32_t s = 0; s < a.n_src && ok; ++s)
-            if (!wait_word(a.ready + (uint64_t)s * a.n_rec + r, abort_flag, a.res, a.timeout_ns)) ok = 0;
-        }
-        fence_gpu();
-      }
-      __syncthreads();
-      const int good = ok;
-      __syncthreads();          // everybody has read `ok` before thread 0 re-arms it for the next step
-      if (!good) break;
-    }
+    // every source of every record this step reads has landed
+    if (gated && !step_gate<G, false>(T0, gridDim.x, total, tpc, [&](uint32_t r) {
+          for (uint32_t s = 0; s < a.n_src; ++s)
+            if (!wait_word(a.ready + (uint64_t)s * a.n_rec + r, abort_flag, a.res, a.timeout_ns)) return false;
+          return true;
+        }))
+      break;
     reduce_step<G, PMAX, LOCAL, EF>(a, T0, gridDim.x, total, tpc, rec);
     if (!counted) continue;
-    // ---- count the step's tiles per record; the CTA that completes a record posts it
+    // ---- count the step's tiles per record, one run of consecutive tiles of a record at a time
     __syncthreads();
     if (threadIdx.x == 0) {
       fence_gpu();   // release this step's stores (all threads, via the barrier) before the counts
@@ -616,87 +605,84 @@ __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) 
         const uint32_t r = (uint32_t)(T / tpc);
         uint32_t n = 0;
         while (g < G && T0 + (uint64_t)g * gridDim.x < total && (T0 + (uint64_t)g * gridDim.x) / tpc == r) { ++n; ++g; }
-        const unsigned int old = atomicAdd(&a.counters[r], n);
-        if (old + n == tpc) {
-          atomicAdd(&a.counters[a.n_rec + 2], 1u);
-          if (a.qp) {
-            // acquire every other CTA's bytes of the record; one cumulative system-scope fence on a NIC-facing QP
-            fence_scope(sys);
-            post_record(a.qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.out_va + (uint64_t)r * rec, a.lkey,
-                        a.remote_va + (uint64_t)r * rec, a.rkey, (uint32_t)rec, a.imm_base + r, a.signal_every, a.acc, a.res,
-                        a.timeout_ns);
-          }
-          a.counters[r] = 0;
-        }
+        complete_run(&a.counters[r], n, tpc, &a.counters[a.n_rec + 2], a.qp, sys, [&] {
+          post_record(a.qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.out_va + (uint64_t)r * rec, a.lkey,
+                      a.remote_va + (uint64_t)r * rec, a.rkey, (uint32_t)rec, a.imm_base + r, a.signal_every, a.acc, a.res,
+                      a.timeout_ns);
+        });
       }
     }
   }
-  // ---- the CTA that finishes last posts the flush (a record not reduced is never posted; the posted ones still drain)
-  __syncthreads();
-  if (threadIdx.x == 0) {
+  // ---- the CTA that finishes last posts the flush
+  if (last_cta(&a.counters[a.n_rec])) {
+    const unsigned long long t_reduce_end = globaltimer_ns();
     fence_gpu();
-    unsigned int old = atomicAdd(&a.counters[a.n_rec], 1u);
-    if (old + 1 == gridDim.x) {
-      const unsigned long long t_reduce_end = globaltimer_ns();
-      fence_gpu();
-      // with no words to wait on and nothing to post every tile is reduced: nothing counts them
-      const uint32_t reduced = counted ? ld_u32_volatile(&a.counters[a.n_rec + 2]) : a.n_rec;
-      unsigned long long posted = 0, first = 0;
-      if (a.qp) {
-        posted = ld_u64_volatile(&a.acc[1]);
-        first = posted ? ~ld_u64_volatile(&a.acc[2]) : 0;
-        int rc = post_flush(a.qp, a.post_only, a.timeout_ns);
-        if (posted != a.n_rec && rc == WAIT_OK) rc = WAIT_TIMEOUT;
-        if (rc != WAIT_OK) a.res[0] = (unsigned long long)(long long)rc;
-      }
-      a.res[1] = t_start;
-      a.res[2] = globaltimer_ns();
-      a.res[3] = reduced;
-      a.res[4] = posted;
-      a.res[5] = first;
-      a.res[6] = t_reduce_end;
-      for (uint32_t r = 0; r <= a.n_rec + 2; ++r) a.counters[r] = 0;   // self-clean, records left unfinished included
-      a.acc[0] = 0; a.acc[1] = 0; a.acc[2] = 0;
+    // with no words to wait on and nothing to post every tile is reduced: nothing counts them
+    const uint32_t reduced = counted ? ld_u32_volatile(&a.counters[a.n_rec + 2]) : a.n_rec;
+    unsigned long long posted = 0, first = 0;
+    if (a.qp) {
+      posted = flush_records(a.qp, a.post_only, a.timeout_ns, a.n_rec, a.acc, a.res, first);
+      if (!posted) first = 0;
     }
+    a.res[1] = t_start;
+    a.res[2] = globaltimer_ns();
+    a.res[3] = reduced;
+    a.res[4] = posted;
+    a.res[5] = first;
+    a.res[6] = t_reduce_end;
+    for (uint32_t r = 0; r <= a.n_rec + 2; ++r) a.counters[r] = 0;   // self-clean, records left unfinished included
   }
 }
 
-// Tiles per step and sources a variant holds, chosen from P and the addend so that every load of a step fits in
-// registers (about 72 per thread, as K3's four tiles of bf16) and P = 8 with an addend does not spill.
-#define RN_REDUCE_VARIANTS(X) X(4, 1, false) X(4, 2, false) X(2, 4, false) X(1, 8, false) X(2, 2, true) X(1, 8, true)
+// (G, PMAX, LOCAL, EF): tiles per step and sources a variant holds, chosen from P and the addend so that every load of a
+// step fits in registers (about 72 per thread, as K3's four tiles of bf16) and P = 8 with an addend does not spill.
 // With a residual (EF): P = 1 without the addend, and P <= 2 with it (the ring's hops), one tile per step: its 128
 // bytes per tile keep a step's loads near the others' (at two tiles P = 1 took 245 registers, one CTA per SM).
-#define RN_REDUCE_EF_VARIANTS(X) X(1, 1, false) X(1, 2, true)
+#define RN_REDUCE_VARIANTS(X)                                                                                           \
+  X(4, 1, false, false) X(4, 2, false, false) X(2, 4, false, false) X(1, 8, false, false) X(2, 2, true, false)          \
+  X(1, 8, true, false) X(1, 1, false, true) X(1, 2, true, true)
+
+// What every entry point does once its own checks pass: refuse (-22) a geometry the kernels cannot walk, zero the result
+// words (mapped pinned memory: the host writes them directly, no memset kernel), turn the timeout into ns (0: 2 s), and
+// pick the grid: `ctas_per_sm` per SM when grid <= 0, at most one CTA per tile.
+int launch_setup(uint64_t n_elems, uint32_t chunk_elems, uint64_t out_dev, uint64_t timeout_ms, int ctas_per_sm, int& grid,
+                 uint64_t& timeout_ns) {
+  if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
+    return -22;
+  unsigned long long* o = (unsigned long long*)out_dev;
+  for (int i = 0; i < 8; ++i) o[i] = 0;
+  timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  if (grid <= 0) grid = device_sms() * ctas_per_sm;
+  if ((uint64_t)grid > n_elems / kTileElems) grid = (int)(n_elems / kTileElems);
+  return 0;
+}
+
+// post_record's three accumulators, after a launch's n_words 32-bit counters rounded up to 8 bytes.
+unsigned long long* acc_after(uint64_t counters_dev, uint64_t n_words) {
+  return (unsigned long long*)(counters_dev + (n_words * 4 + 7) / 8 * 8);
+}
 
 }  // namespace
 
 RN_API uint64_t rn_pack_record_bytes(uint64_t chunk_elems) { return record_bytes(chunk_elems); }
 RN_API uint32_t rn_pack_tile_elems() { return kTileElems; }
 
-// counters_dev: >= (n_chunks + 1) * 4 + 8 bytes of zero-initialised device memory that the
+// counters_dev: >= (n_chunks + 1) * 4 bytes (rounded up to 8) + 24 of zero-initialised device memory that the
 // kernel cleans up after itself (no memset on the hot path: see Context.stream docs).
 RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t staging, uint64_t n_elems,
                                uint32_t chunk_elems, uint64_t qp_dev, uint64_t staging_va, uint32_t lkey,
                                uint64_t remote_va, uint32_t rkey, uint32_t with_imm, uint32_t signal_every,
                                uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms, uint64_t residual) {
-  if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
-    return -22;
   if (residual & 31) return -22;                               // 256-bit loads / stores
   PackArgs a;
+  if (int rc = launch_setup(n_elems, chunk_elems, out_dev, timeout_ms, 4, grid, a.timeout_ns)) return rc;
   a.src = (const __nv_bfloat16*)src; a.staging = (uint8_t*)staging; a.n_elems = n_elems; a.chunk_elems = chunk_elems;
   a.n_chunks = (uint32_t)(n_elems / chunk_elems); a.qp = (QpDev*)qp_dev; a.staging_va = staging_va; a.lkey = lkey;
   a.rkey = rkey; a.remote_va = remote_va; a.with_imm = with_imm & 1u; a.post_only = (with_imm >> 1) & 1u; a.direct = (with_imm >> 2) & 1u; a.signal_every = signal_every ? signal_every : 1;
   a.counters = (unsigned int*)counters_dev;
-  a.acc = (unsigned long long*)(counters_dev + (((uint64_t)a.n_chunks + 1) * 4 + 7) / 8 * 8);
+  a.acc = acc_after(counters_dev, (uint64_t)a.n_chunks + 1);
   a.out = (unsigned long long*)out_dev;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
   a.residual = (float*)residual;
-  // out[] lives in mapped pinned memory: the host zeroes it directly (no memset kernel)
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
-  uint64_t n_tiles = n_elems / kTileElems;
-  if (grid <= 0) grid = device_sms() * 4;
-  if ((uint64_t)grid > n_tiles) grid = (int)n_tiles;
   if (residual) pack_fp8_write_kernel<true><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
   else pack_fp8_write_kernel<false><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -711,27 +697,21 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
                            uint32_t signal_every) {
   if (qp_dev && ready_dev) return -22;
   if (qp_dev && fwd_qp) return -22;                            // the CQ poller owns the flags the forwarders claim
-  if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
-    return -22;
   if ((staging | dst) & 31) return -22;                        // 256-bit loads / stores: records and output must be 32-byte aligned
   if (fwd_qp && n_elems / kTileElems >= (1ull << 32)) return -22;
   UnpackArgs a;
+  // waiting for arrivals the kernel shares the GPU with whatever produces them (a pack kernel, an engine): one CTA per SM then
+  if (int rc = launch_setup(n_elems, chunk_elems, out_dev, timeout_ms, (qp_dev || ready_dev || fwd_qp) ? 1 : 4, grid,
+                            a.timeout_ns))
+    return rc;
   a.staging = (const uint8_t*)staging; a.dst = (__nv_bfloat16*)dst; a.n_elems = n_elems; a.chunk_elems = chunk_elems;
   a.n_chunks = (uint32_t)(n_elems / chunk_elems); a.qp = (QpDev*)qp_dev; a.arrived = (unsigned int*)arrived_dev;
-  a.out = (unsigned long long*)out_dev; a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.out = (unsigned long long*)out_dev;
   a.ready = (const unsigned long long*)ready_dev;
   a.fwd_qp = (QpDev*)fwd_qp; a.fwd_src_va = fwd_src_va; a.fwd_remote_va = fwd_remote_va; a.fwd_lkey = fwd_lkey;
   a.fwd_rkey = fwd_rkey; a.with_imm = fwd_flags & 1u; a.post_only = (fwd_flags >> 1) & 1u;
   a.signal_every = signal_every ? signal_every : 1; a.imm_base = imm_base;
-  a.acc = (unsigned long long*)(arrived_dev + (((uint64_t)a.n_chunks + 3) * 4 + 7) / 8 * 8);
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
-  // waiting for arrivals the kernel shares the GPU with whatever produces them (a pack kernel, an engine): one CTA per SM then
-  if (grid <= 0) grid = (qp_dev || ready_dev || fwd_qp) ? device_sms() : device_sms() * 4;
-  {
-    const uint64_t total_tiles = n_elems / kTileElems;
-    if ((uint64_t)grid > total_tiles) grid = (int)total_tiles;
-  }
+  a.acc = acc_after(arrived_dev, (uint64_t)a.n_chunks + 3);
   if (qp_dev) grid += 1;                                      // CTA 0 polls the receive CQ, the others unpack
   if (fwd_qp) unpack_fp8_kernel<true><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
   else unpack_fp8_kernel<false><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
@@ -747,40 +727,28 @@ RN_API int rn_k_reduce_fp8(uint64_t stream, int grid, uint64_t src, uint32_t n_s
                            uint32_t signal_every, uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms,
                            uint32_t imm_base, uint64_t residual) {
   if (n_src < 1 || n_src > 8) return -22;
-  if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
-    return -22;
   if ((src | local | out | out_rec) & 31) return -22;          // 256-bit loads / stores
   if (!out && !out_rec) return -22;
   if (qp_dev && !out_rec) return -22;
   if (residual & 31) return -22;
   if (residual && (!out_rec || n_src > (local ? 2u : 1u))) return -22;
   ReduceArgs a;
+  // waiting for arrivals the kernel shares the GPU with whatever produces them: one CTA per SM then (as K5)
+  if (int rc = launch_setup(n_elems, chunk_elems, out_dev, timeout_ms, ready_dev ? 1 : 4, grid, a.timeout_ns)) return rc;
   a.src = (const uint8_t*)src; a.local = (const __nv_bfloat16*)local; a.out = (__nv_bfloat16*)out; a.out_rec = (uint8_t*)out_rec;
   a.chunk_elems = chunk_elems; a.n_rec = (uint32_t)(n_elems / chunk_elems); a.n_src = n_src;
   a.ready = (const unsigned long long*)ready_dev; a.qp = (QpDev*)qp_dev; a.out_va = out_va; a.lkey = lkey; a.rkey = rkey;
   a.remote_va = remote_va; a.with_imm = flags & 1u; a.post_only = (flags >> 1) & 1u; a.signal_every = signal_every ? signal_every : 1;
   a.counters = (unsigned int*)counters_dev;
-  a.acc = (unsigned long long*)(counters_dev + (((uint64_t)a.n_rec + 3) * 4 + 7) / 8 * 8);
+  a.acc = acc_after(counters_dev, (uint64_t)a.n_rec + 3);
   a.res = (unsigned long long*)out_dev;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
   a.imm_base = imm_base;
   a.residual = (float*)residual;
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
-  // waiting for arrivals the kernel shares the GPU with whatever produces them: one CTA per SM then (as K5)
-  if (grid <= 0) grid = ready_dev ? device_sms() : device_sms() * 4;
-  {
-    const uint64_t total_tiles = n_elems / kTileElems;
-    if ((uint64_t)grid > total_tiles) grid = (int)total_tiles;
-  }
   const int pmax = local ? (n_src <= 2 ? 2 : 8) : (n_src == 1 ? 1 : n_src <= 2 ? 2 : n_src <= 4 ? 4 : 8);
-#define RN_LAUNCH(G, PMAX, LOCAL) \
-  if (pmax == PMAX && (local != 0) == LOCAL) reduce_fp8_kernel<G, PMAX, LOCAL, false><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
-#define RN_LAUNCH_EF(G, PMAX, LOCAL) \
-  if (pmax == PMAX && (local != 0) == LOCAL) reduce_fp8_kernel<G, PMAX, LOCAL, true><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
-  if (!residual) { RN_REDUCE_VARIANTS(RN_LAUNCH) }
-  else { RN_REDUCE_EF_VARIANTS(RN_LAUNCH_EF) }
-#undef RN_LAUNCH_EF
+#define RN_LAUNCH(G, PMAX, LOCAL, EF)                                                   \
+  if (pmax == PMAX && (local != 0) == LOCAL && (residual != 0) == EF)                 \
+    reduce_fp8_kernel<G, PMAX, LOCAL, EF><<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  RN_REDUCE_VARIANTS(RN_LAUNCH)
 #undef RN_LAUNCH
   return (int)cudaGetLastError();
 }
@@ -791,10 +759,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_pack() {
   cudaFuncGetAttributes(&at, pack_fp8_write_kernel<true>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<false>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<true>);
-#define RN_PRELOAD(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL, false>);
-#define RN_PRELOAD_EF(G, PMAX, LOCAL) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL, true>);
+#define RN_PRELOAD(G, PMAX, LOCAL, EF) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL, EF>);
   RN_REDUCE_VARIANTS(RN_PRELOAD)
-  RN_REDUCE_EF_VARIANTS(RN_PRELOAD_EF)
-#undef RN_PRELOAD_EF
 #undef RN_PRELOAD
 }

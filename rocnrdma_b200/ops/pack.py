@@ -80,11 +80,11 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     wire = staging_bytes(n, chunk_elems)
     if staging_mr.length < wire or (dst_mr is not None and dst_mr.length < wire):
         raise ValueError("staging / destination region too small for the records")
-    res_addr = 0 if residual is None else _check_residual(residual, n, ctx.device)
+    res_addr = 0 if residual is None else _check_tensor(residual, torch.float32, n, ctx.device, "residual")
     lib = N.load()
     ws = work_stream(ctx, stream)
-    n_chunks = n // chunk_elems
-    counters = ctx.dev_scratch((n_chunks + 1) * 4 + 64, offset=scratch_slot * (256 << 10))
+    # [n_chunks] groups packed per record ; CTAs done
+    counters = _counters(ctx, n // chunk_elems + 1, scratch_slot)
     out_addr, out_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     rc = lib.rn_k_pack_fp8_write(_stream_ptr(ws), grid, src.data_ptr(), staging_mr.addr, n, chunk_elems,
                                  qp.dev_ptr if qp is not None else 0, staging_mr.addr, staging_mr.lkey,
@@ -99,6 +99,25 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     if qp is None:
         return None
     return _parse(out_view, n, wire)
+
+
+SLOT_BYTES = 256 << 10          # one launch's share of the device scratch (``scratch_slot``)
+
+
+def counter_bytes(n_words: int) -> int:
+    """Device scratch a launch with ``n_words`` 32-bit counters takes: the counters, rounded up to 8 bytes, then the
+    three 64-bit words the kernels post records through."""
+    return (int(n_words) * 4 + 7) // 8 * 8 + 24
+
+
+def _counters(ctx, n_words: int, scratch_slot: int) -> int:
+    """Address of a launch's zeroed counters in device-scratch slot ``scratch_slot``."""
+    nb = counter_bytes(n_words)
+    if nb > SLOT_BYTES:
+        raise ValueError(f"{n_words} counters need {nb} bytes; a scratch slot holds {SLOT_BYTES}")
+    if not 0 <= scratch_slot < ctx.dev_scratch_bytes // SLOT_BYTES:
+        raise ValueError(f"scratch_slot={scratch_slot}: the device scratch has {ctx.dev_scratch_bytes // SLOT_BYTES} slots")
+    return ctx.dev_scratch(nb, offset=scratch_slot * SLOT_BYTES)
 
 
 def result_offset(scratch_slot: int, result_off=None) -> int:
@@ -159,8 +178,8 @@ def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int =
     ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_chunks, ctx.device, "ready")
     lib = N.load()
     ws = work_stream(ctx, stream)
-    # [n_chunks] flags (claims when forwarding) ; CTAs done ; records seen ; abort flag ; then post_record's 3 words
-    arrived = ctx.dev_scratch(((n_chunks + 3) * 4 + 7) // 8 * 8 + 24, offset=scratch_slot * (256 << 10))
+    # [n_chunks] flags (claims when forwarding) ; CTAs done ; records seen ; abort flag
+    arrived = _counters(ctx, n_chunks + 3, scratch_slot)
     out_addr, out_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     rc = lib.rn_k_unpack_fp8(_stream_ptr(ws), grid, staging.data_ptr(), dst.data_ptr(), n, chunk_elems,
                              qp.dev_ptr if qp is not None else 0, arrived, out_addr, timeout_ms, ready_addr,
@@ -260,12 +279,7 @@ def ref_pack_fp8(src: torch.Tensor, chunk_elems: int, residual=None):
 
 
 def ref_unpack_fp8(records: torch.Tensor, n_elems: int, chunk_elems: int) -> torch.Tensor:
-    n_chunks = n_elems // chunk_elems
-    rec = record_bytes(chunk_elems)
-    r = records.reshape(n_chunks, rec)
-    q = r[:, :chunk_elems].contiguous().view(torch.float8_e4m3fn).float().reshape(-1, BLOCK)
-    s = ue8m0(r[:, chunk_elems:chunk_elems + chunk_elems // BLOCK].reshape(-1))
-    return (q * s[:, None]).to(torch.bfloat16).reshape(-1)
+    return _decode_records(records, 1, n_elems, chunk_elems)[0].to(torch.bfloat16)
 
 
 def _decode_records(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int) -> torch.Tensor:
@@ -340,7 +354,6 @@ def ref_allreduce_fp8(xs, chunk_elems: int, residuals=None):
 
 # ------------------------------------------------------------------ reduce
 MAX_SOURCES = 8
-_SLOT = 256 << 10
 
 
 @dataclass
@@ -374,9 +387,10 @@ def parse_reduce(view, hbm_bytes: int = 0) -> ReduceResult:
     return ReduceResult(WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2], w[3], w[4], w[5], w[6], hbm_bytes)
 
 
-def _check_bf16(t, n, device, what):
-    if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16:
-        raise ValueError(f"{what} must be a bfloat16 tensor, not {getattr(t, 'dtype', type(t).__name__)}")
+def _check_tensor(t, dtype, n, device, what):
+    """Address of ``t``: a ``dtype`` tensor on cuda:``device``, contiguous, 32-byte aligned, of ``n`` elements."""
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype:
+        raise ValueError(f"{what} must be a {str(dtype).removeprefix('torch.')} tensor, not {getattr(t, 'dtype', type(t).__name__)}")
     if not t.is_cuda or t.device.index != device:
         raise ValueError(f"{what} must be on cuda:{device}, not {t.device}")
     if not t.is_contiguous() or t.data_ptr() & 31:
@@ -386,17 +400,8 @@ def _check_bf16(t, n, device, what):
     return t.data_ptr()
 
 
-def _check_residual(t, n, device):
-    """An error-feedback residual: fp32, on cuda:``device``, contiguous, 32-byte aligned, ``n`` values."""
-    if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
-        raise ValueError(f"residual must be a float32 tensor, not {getattr(t, 'dtype', type(t).__name__)}")
-    if not t.is_cuda or t.device.index != device:
-        raise ValueError(f"residual must be on cuda:{device}, not {t.device}")
-    if not t.is_contiguous() or t.data_ptr() & 31:
-        raise ValueError("residual must be contiguous and 32-byte aligned (256-bit loads / stores)")
-    if t.numel() != n:
-        raise ValueError(f"residual holds {t.numel()} elements; n_elems is {n}")
-    return t.data_ptr()
+def _check_bf16(t, n, device, what):
+    return _check_tensor(t, torch.bfloat16, n, device, what)
 
 
 def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int = 1 << 20, *, local=None, out=None,
@@ -467,16 +472,12 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
             raise ValueError("residual= needs out_mr: the residual is what the records of the sum lose")
         if n_src > (2 if local is not None else 1):
             raise ValueError(f"residual= with n_src={n_src}: error feedback runs with P = 1, or P = 2 with local")
-        res_ptr = _check_residual(residual, n_elems, dev)
+        res_ptr = _check_tensor(residual, torch.float32, n_elems, dev, "residual")
     ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_src * n_rec, dev, "ready")
-    counter_bytes = ((n_rec + 3) * 4 + 7) // 8 * 8 + 24
-    if counter_bytes > _SLOT:
-        raise ValueError(f"{n_rec} records need {counter_bytes} bytes of counters; a scratch slot holds {_SLOT}")
-    if not 0 <= scratch_slot < ctx.dev_scratch_bytes // _SLOT:
-        raise ValueError(f"scratch_slot={scratch_slot}: the device scratch has {ctx.dev_scratch_bytes // _SLOT} slots")
+    # [n_rec] tiles done per record ; CTAs done ; abort flag ; records reduced
+    counters = _counters(ctx, n_rec + 3, scratch_slot)
     lib = N.load()
     ws = work_stream(ctx, stream)
-    counters = ctx.dev_scratch(counter_bytes, offset=scratch_slot * _SLOT)
     res_addr, res_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
     hbm = n_src * wire + (2 * n_elems if local is not None else 0) + (2 * n_elems if out is not None else 0) + \
         (wire if out_mr is not None else 0) + (8 * n_elems if residual is not None else 0)

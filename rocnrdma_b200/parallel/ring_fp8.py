@@ -34,7 +34,7 @@ import torch
 
 from .. import ops
 from ..ops import pack as P
-from ..ops.rdma import WAIT_STATUS
+from ..ops.rdma import parse_recv
 
 GUARD = 8                       # zero words behind the arrival words
 RESULT_BASE = 128 << 10         # mapped-scratch offset of the ring's result records: 4 KiB per device-scratch slot
@@ -69,6 +69,11 @@ def schedule(rank: int, world: int) -> List[Step]:
     steps += [Step("unpack", N - 1 + j, (q - j) % N, N + j if j <= N - 3 else None) for j in range(N - 1)]
     steps.append(Step("unpack", None, (q + 1) % N, None))
     return steps
+
+
+# a launch's result words, by kind, decoded by the parser that owns their layout
+_PARSERS = {"pack": lambda v: vars(P._parse(v, 0, 0)), "reduce": lambda v: vars(P.parse_reduce(v)),
+            "unpack": P.parse_unpack, "recv": parse_recv}
 
 
 def _pow2(n: int) -> int:
@@ -147,8 +152,8 @@ class RingAllreduceFp8:
         self.R = self.shard // chunk_elems
         self.rec = P.record_bytes(chunk_elems)
         self.n_ids = 2 * (world - 1) * self.R
-        counter_bytes = ((self.R + 3) * 4 + 7) // 8 * 8 + 24
-        if counter_bytes > 256 << 10:
+        counter_bytes = P.counter_bytes(self.R + 3)       # the reduce's and the unpack's: R records and 3 words
+        if counter_bytes > P.SLOT_BYTES:
             raise ValueError(f"{self.R} records per shard need {counter_bytes} bytes of counters; a scratch slot holds 256 KiB")
         if self.R > max_records(world):
             raise ValueError(f"R={self.R} records per shard: the receive queue would need {_pow2(2 * self.n_ids)} entries, "
@@ -242,16 +247,16 @@ class RingAllreduceFp8:
         views = []
         if self._stale_cqes:
             # completions of a failed run's late records: reap them before this run's words are cleared
-            views.append(("drain", ops.recv_consume(self.recv_qp, self._stale_cqes, 0, None, scratch_off=self._res(2 * self.world + 1), **kw)[0]))
+            views.append(("drain", "recv", ops.recv_consume(self.recv_qp, self._stale_cqes, 0, None, scratch_off=self._res(2 * self.world + 1), **kw)[0]))
         with torch.cuda.stream(cs):
             self.words.zero_()
         self._cleared.record(cs)
         fresh = self.n_ids - self._rq_backlog
-        views.append(("receive", ops.recv_consume(self.recv_qp, fresh, self.n_ids, self.words, scratch_off=self._res(0),
+        views.append(("receive", "recv", ops.recv_consume(self.recv_qp, fresh, self.n_ids, self.words, scratch_off=self._res(0),
                                                   prepost_mr=self.landing_mr, prepost_bytes=0, **kw)[0]))
         if self._rq_backlog:
             # the receive WQEs a failed run left posted take the rest of this run's records
-            views.append(("receive", ops.recv_consume(self.recv_qp, self._rq_backlog, self.n_ids, self.words,
+            views.append(("receive", "recv", ops.recv_consume(self.recv_qp, self._rq_backlog, self.n_ids, self.words,
                                                       scratch_off=self._res(2 * self.world + 2), **kw)[0]))
         self._stale_cqes = self._rq_backlog = 0
         self._views = views
@@ -278,13 +283,13 @@ class RingAllreduceFp8:
             if st.kind == "pack":
                 v, _ = ops.pack_fp8_write(self.ctx, self._shard(x, st.shard), self.staging_mr, chunk_elems=self.chunk,
                                           result_off=res, **ef(st.shard), **dst, **common)
-                views.append(("pack", v))
+                views.append(("pack", "pack", v))
             elif st.kind == "reduce":
                 land, words = self._slot(st.read_slot)
                 v, _ = ops.reduce_fp8(self.ctx, land, 1, self.shard, self.chunk, local=self._shard(x, st.shard),
                                       out_mr=self.staging_mr, dst_off=st.send_slot * R * rec, ready=words,
                                       imm_base=st.send_slot * R, result_off=res, **ef(st.shard), **dst, **common)
-                views.append((f"reduce hop {st.read_slot}", v))
+                views.append((f"reduce hop {st.read_slot}", "reduce", v))
             elif st.read_slot is not None:
                 land, words = self._slot(st.read_slot)
                 fwd = {} if st.send_slot is None else dict(
@@ -292,11 +297,11 @@ class RingAllreduceFp8:
                     fwd_dst_off=st.send_slot * R * rec, imm_base=st.send_slot * R, **post)
                 v, _ = ops.unpack_fp8(self.ctx, land, self._shard(out, st.shard), self.chunk, ready=words, result_off=res,
                                       **fwd, **common)
-                views.append((f"unpack slot {st.read_slot}" + (" + forward" if fwd else ""), v))
+                views.append((f"unpack slot {st.read_slot}" + (" + forward" if fwd else ""), "unpack", v))
             else:
                 v, _ = ops.unpack_fp8(self.ctx, self.staging, self._shard(out, st.shard), self.chunk, result_off=res,
                                       **common)
-                views.append(("unpack own", v))
+                views.append(("unpack own", "unpack", v))
 
     def run(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, sync: bool = True):
         """All-reduce ``x`` (bf16, ``n_elems``) over the ring into ``out``, or in place when ``out`` is None, as
@@ -317,19 +322,12 @@ class RingAllreduceFp8:
 
     def result(self) -> RingResult:
         """Decode the last run's result records (after :meth:`synchronize`)."""
-        import ctypes as C
         launches, received, posted = [], 0, 0
-        for name, view in self._views:
-            w = (C.c_int64 * 8).from_buffer(view)
-            launches.append(LaunchResult(name, WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2]))
-            if name == "receive":
-                received += w[3]
-            elif name == "pack":
-                posted += w[3]
-            elif name.startswith("reduce"):
-                posted += w[4]
-            elif name.endswith("forward"):
-                posted += w[4]
+        for name, kind, view in self._views:
+            w = _PARSERS[kind](view)
+            launches.append(LaunchResult(name, w["status"], w["t_start_ns"], w["t_end_ns"]))
+            posted += w.get("wqes", 0) + w.get("records_posted", 0) + w.get("records_forwarded", 0)
+            received += w["seen"] if name == "receive" else 0
         bad = next((l for l in launches if l.status != "OK"), None)
         starts = [l.t_start_ns for l in launches if l.t_start_ns > 0]
         ends = [l.t_end_ns for l in launches if l.t_end_ns > 0]

@@ -34,7 +34,7 @@ from test_gpu_reduce import CANARY, POISON_Q, POISON_S, WAIT_MS, _bf16_equal_up_
 pytestmark = pytest.mark.gpu
 
 TILE = P.TILE_ELEMS
-# (G tiles per step, PMAX sources, addend): pack_fp8.cu RN_REDUCE_VARIANTS
+# (G tiles per step, PMAX sources, addend): pack_fp8.cu RN_REDUCE_VARIANTS, the entries with EF = false
 VARIANTS = ((4, 1, False), (4, 2, False), (2, 4, False), (1, 8, False), (2, 2, True), (1, 8, True))
 
 

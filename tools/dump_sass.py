@@ -11,9 +11,20 @@ summary = {}
 for m in re.finditer(r"\t\tFunction : (\S+)\n(.*?)(?=\n\t\tFunction : |\Z)", txt, re.S):
     mangled, body = m.group(1), m.group(2)
     name = next((w for w in want if re.search(r"\d+" + w + r"(?![a-z_])", mangled) or mangled == w), None)
-    if not name or name in summary:
+    if not name:
         continue
-    open(os.path.join(out, name + ".sass"), "w").write("Function : " + mangled + "\n" + body + "\n")
+    # the first instance of a kernel keeps its plain key; every instance of a template is also keyed by its arguments,
+    # e.g. reduce_fp8_kernel<4,1,false,false>, so that each one is listed
+    base = re.match(r"[a-z0-9_]+", name).group(0)
+    targs = re.search(r"\d+" + base + r"I((?:L[ib]\d+E)+)E", mangled)
+    keys = [] if name in summary else [name]
+    if targs:
+        args = [v if t == "i" else ("true" if v == "1" else "false") for t, v in re.findall(r"L([ib])(\d+)E", targs.group(1))]
+        keys.append(base + "<" + ",".join(args) + ">")
+    if not keys:
+        continue
+    for key in keys:
+        open(os.path.join(out, re.sub(r"[<>,]", "_", key).rstrip("_") + ".sass"), "w").write("Function : " + mangled + "\n" + body + "\n")
     ops = collections.Counter()
     full = collections.Counter()
     for line in body.splitlines():
@@ -22,7 +33,8 @@ for m in re.finditer(r"\t\tFunction : (\S+)\n(.*?)(?=\n\t\tFunction : |\Z)", txt
             ops[mm.group(1)] += 1
             full[mm.group(1) + mm.group(2)] += 1
     hopper = {k: v for k, v in full.items() if k.split(".")[0] in ("HGMMA", "QGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "UTMACMDFLUSH", "F2FP")}
-    summary[name] = {"mangled": mangled, "instructions": sum(ops.values()), "hopper": dict(sorted(hopper.items())), "mnemonics": dict(ops.most_common())}
+    for key in keys:
+        summary[key] = {"mangled": mangled, "instructions": sum(ops.values()), "hopper": dict(sorted(hopper.items())), "mnemonics": dict(ops.most_common())}
 json.dump(summary, open(os.path.join(out, "summary.json"), "w"), indent=1)
 for k, v in summary.items():
     print(k, v["instructions"], v["hopper"])
