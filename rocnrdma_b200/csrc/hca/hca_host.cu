@@ -217,7 +217,7 @@ RN_API int rn_hca_open(int dev, uint32_t max_mkeys, uint32_t max_qps, uint64_t a
   h->h_stop = (volatile uint32_t*)arena_alloc(h, 64, true);
   h->scratch_size = 256 << 10;
   h->scratch = (uint8_t*)arena_alloc(h, h->scratch_size, true);
-  h->dscratch_size = 2 << 20;           // eight 256 KiB slots of kernel counters (ops: scratch_slot)
+  h->dscratch_size = 2 << 20;           // eight 256 KiB slots of kernel counters (ops/launch.py maps both scratches)
   h->dscratch = (uint8_t*)arena_alloc(h, h->dscratch_size, false);
   h->mrs.resize(h->max_mkeys);
   if (rn_gemm_workspace_bytes && rn_gemm_set_workspace) {

@@ -559,4 +559,23 @@ static inline int device_sms() {
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
   return n;
 }
+
+// What the ops launchers share on the host.
+// A wait bound in ns from the timeout_ms every entry point takes (0: 2 s).
+static inline unsigned long long timeout_ns(uint64_t timeout_ms) { return (timeout_ms ? timeout_ms : 2000) * 1000000ull; }
+
+// Zero a launch's 8-word result record: mapped pinned memory, so the host writes it directly (no memset kernel).
+static inline unsigned long long* clear_record(uint64_t out_dev) {
+  unsigned long long* o = (unsigned long long*)out_dev;
+  for (int i = 0; i < 8; ++i) o[i] = 0;
+  return o;
+}
+
+// Copy a multi-QP launch's queue pairs, one per CTA, into its by-value argument array; false unless 1 <= nqp <= kMax.
+template <int kMax>
+static inline bool copy_qps(QpDev* (&qps)[kMax], const uint64_t* qps_host, uint32_t nqp) {
+  if (nqp == 0 || nqp > (uint32_t)kMax) return false;
+  for (uint32_t i = 0; i < nqp; ++i) qps[i] = (QpDev*)qps_host[i];
+  return true;
+}
 }  // namespace rn

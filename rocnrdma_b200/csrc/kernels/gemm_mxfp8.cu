@@ -301,12 +301,11 @@ RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s
   g.a_s = (const uint8_t*)a_s; g.b_s = (const uint8_t*)b_s;
   g.a_rec_stride = a_rec_stride; g.b_rec_stride = b_rec_stride; g.a_rows_per_rec = a_rows_per_rec; g.b_rows_per_rec = b_rows_per_rec;
   g.c = (__nv_bfloat16*)c; g.M = M; g.N = N; g.K = K;
-  g.a_ready = (const unsigned long long*)a_ready_dev; g.ready_timeout_ns = (ready_timeout_ms ? ready_timeout_ms : 2000) * 1000000ull;
+  g.a_ready = (const unsigned long long*)a_ready_dev; g.ready_timeout_ns = timeout_ns(ready_timeout_ms);
   g.out = (unsigned long long*)out_dev;
   g.done = (unsigned int*)done_dev;
   if (!done_dev) return -22;
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
+  clear_record(out_dev);
   // persistent kernels, one CTA per SM
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);

@@ -643,15 +643,13 @@ __global__ void __launch_bounds__(kPackThreads) reduce_fp8_kernel(ReduceArgs a) 
   X(1, 8, true, false) X(1, 1, false, true) X(1, 2, true, true)
 
 // What every entry point does once its own checks pass: refuse (-22) a geometry the kernels cannot walk, zero the result
-// words (mapped pinned memory: the host writes them directly, no memset kernel), turn the timeout into ns (0: 2 s), and
-// pick the grid: `ctas_per_sm` per SM when grid <= 0, at most one CTA per tile.
+// record, turn the timeout into ns, and pick the grid: `ctas_per_sm` per SM when grid <= 0, at most one CTA per tile.
 int launch_setup(uint64_t n_elems, uint32_t chunk_elems, uint64_t out_dev, uint64_t timeout_ms, int ctas_per_sm, int& grid,
-                 uint64_t& timeout_ns) {
+                 uint64_t& wait_ns) {
   if (n_elems == 0 || chunk_elems == 0 || n_elems % kTileElems || chunk_elems % kTileElems || n_elems % chunk_elems)
     return -22;
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
-  timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  clear_record(out_dev);
+  wait_ns = timeout_ns(timeout_ms);
   if (grid <= 0) grid = device_sms() * ctas_per_sm;
   if ((uint64_t)grid > n_elems / kTileElems) grid = (int)(n_elems / kTileElems);
   return 0;

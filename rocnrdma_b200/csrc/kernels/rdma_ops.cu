@@ -145,8 +145,7 @@ RN_API int rn_k_rdma_stream(uint64_t stream, const uint64_t* qps_host, uint32_t 
                             uint32_t iters, uint32_t window, uint32_t signal_every, uint32_t burst, uint64_t slot_stride,
                             uint32_t nslots, uint64_t timeout_ms, uint64_t out_dev, uint32_t fence_every) {
   StreamArgs a;
-  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps) return -22;
-  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
+  if (!copy_qps(a.qps, qps_host, nqp)) return -22;
   a.post_only = (opcode >> 31) & 1u; opcode &= 0x7fffffffu;
   a.opcode = opcode; a.laddr = laddr; a.raddr = raddr; a.stride = stride;
   a.lkey = lkey; a.rkey = rkey; a.bytes = bytes; a.iters = iters; a.window = window;
@@ -154,7 +153,7 @@ RN_API int rn_k_rdma_stream(uint64_t stream, const uint64_t* qps_host, uint32_t 
   a.signal_every = signal_every; a.burst = burst;
   a.slot_stride = slot_stride; a.nslots = nslots ? nslots : 1;
   a.fence_every = fence_every;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.timeout_ns = timeout_ns(timeout_ms);
   a.out = (unsigned long long*)out_dev;
   rdma_stream_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -216,7 +215,7 @@ RN_API int rn_k_write_read(uint64_t stream, uint64_t qp_dev, uint64_t laddr, uin
                            uint64_t out_dev) {
   if (mode > 2) return -22;
   write_read_kernel<<<1, 32, 0, (cudaStream_t)stream>>>((QpDev*)qp_dev, laddr, lkey, raddr, rkey, back, back_lkey, bytes, iters, mode,
-                                                        (timeout_ms ? timeout_ms : 2000) * 1000000ull, (unsigned long long*)out_dev);
+                                                        timeout_ns(timeout_ms), (unsigned long long*)out_dev);
   return (int)cudaGetLastError();
 }
 
@@ -249,11 +248,9 @@ __global__ void __launch_bounds__(32) shared_post_stress_kernel(QpDev* qp, uint6
 }
 RN_API int rn_k_shared_post_stress(uint64_t stream, uint64_t qp_dev, int ctas, uint64_t laddr, uint32_t lkey, uint64_t raddr,
                                    uint32_t rkey, uint32_t per_cta, uint64_t counter_dev, uint64_t out_dev, uint64_t timeout_ms) {
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
+  unsigned long long* o = clear_record(out_dev);
   shared_post_stress_kernel<<<ctas, 32, 0, (cudaStream_t)stream>>>((QpDev*)qp_dev, laddr, lkey, raddr, rkey, per_cta,
-                                                                   (unsigned int*)counter_dev, (unsigned long long*)out_dev,
-                                                                   (timeout_ms ? timeout_ms : 2000) * 1000000ull);
+                                                                   (unsigned int*)counter_dev, o, timeout_ns(timeout_ms));
   return (int)cudaGetLastError();
 }
 
@@ -288,7 +285,7 @@ RN_API int rn_k_recv_consume(uint64_t stream, uint64_t qp_dev, uint32_t n, uint3
                              uint64_t out_dev, uint64_t timeout_ms, uint64_t prepost_addr, uint32_t prepost_lkey,
                              uint32_t prepost_bytes) {
   recv_consume_kernel<<<1, 32, 0, (cudaStream_t)stream>>>((QpDev*)qp_dev, n, max_imm, (unsigned long long*)stamps_dev,
-                                                          (unsigned long long*)out_dev, (timeout_ms ? timeout_ms : 2000) * 1000000ull,
+                                                          (unsigned long long*)out_dev, timeout_ns(timeout_ms),
                                                           prepost_addr, prepost_lkey, prepost_bytes);
   return (int)cudaGetLastError();
 }
@@ -329,16 +326,15 @@ RN_API int rn_k_atomic_stream(uint64_t stream, const uint64_t* qps_host, uint32_
                               uint64_t add, uint64_t compare, uint64_t swap, uint32_t iters, uint32_t window,
                               uint32_t signal_every, uint32_t burst, uint64_t timeout_ms, uint64_t out_dev) {
   AtomicArgs a;
-  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps) return -22;
+  if (!copy_qps(a.qps, qps_host, nqp)) return -22;
   if (opcode != OP_ATOMIC_FA && opcode != OP_ATOMIC_CS) return -22;
-  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
   a.opcode = opcode; a.chain = chain && opcode == OP_ATOMIC_CS;
   a.target = target; a.target_stride = target_stride; a.fetch = fetch; a.rkey = rkey; a.lkey = lkey;
   a.add = add; a.compare = compare; a.swap = swap;
   a.iters = iters; a.window = window;
   rn_stream_clamp(window, &burst, &signal_every);
   a.signal_every = signal_every; a.burst = burst;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.timeout_ns = timeout_ns(timeout_ms);
   a.out = (unsigned long long*)out_dev;
   atomic_stream_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -389,7 +385,7 @@ RN_API int rn_k_put_signal(uint64_t stream, uint64_t qp_dev, uint64_t src, uint3
   a.nslots = nslots ? nslots : 1; a.slot_stride = slot_stride;
   a.sig = sig; a.sig_rkey = sig_rkey; a.fetch = fetch; a.fetch_lkey = fetch_lkey; a.fetch_slots = fetch_slots ? fetch_slots : 1;
   a.iters = iters; a.window = window; a.pad = 0; a.add = add;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.timeout_ns = timeout_ns(timeout_ms);
   a.out = (unsigned long long*)out_dev;
   put_signal_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -442,9 +438,8 @@ RN_API int rn_k_put_inline(uint64_t stream, const uint64_t* qps_host, uint32_t n
                            uint64_t add, uint32_t iters, uint32_t window, uint32_t signal_every, uint32_t burst,
                            uint64_t timeout_ms, uint64_t out_dev) {
   PutInlineArgs a;
-  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps) return -22;
+  if (!copy_qps(a.qps, qps_host, nqp)) return -22;
   if (nbytes == 0 || nbytes > MAX_INLINE || rows == 0 || (uint64_t)nqp * iters > 0xffffffffull) return -22;
-  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
   a.values = (const uint8_t*)values; a.row_bytes = row_bytes; a.rows = rows; a.nbytes = nbytes;
   a.dst = dst; a.slot_stride = slot_stride; a.rkey = rkey; a.nslots = nslots ? nslots : 1;
   a.sig = sig; a.fetch = fetch; a.add = add;
@@ -453,7 +448,7 @@ RN_API int rn_k_put_inline(uint64_t stream, const uint64_t* qps_host, uint32_t n
   if (sig && burst > 16) burst = 16;                  // two WQEs per message, one lane each
   rn_stream_clamp(window, &burst, &signal_every);
   a.signal_every = signal_every; a.burst = burst;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.timeout_ns = timeout_ns(timeout_ms);
   a.out = (unsigned long long*)out_dev;
   put_inline_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -534,15 +529,14 @@ RN_API int rn_k_gather_stream(uint64_t stream, const uint64_t* qps_host, uint32_
                               uint32_t window, uint32_t signal_every, uint32_t burst, uint32_t via, uint64_t timeout_ms,
                               uint64_t out_dev) {
   GatherArgs a;
-  if (nqp == 0 || nqp > (uint32_t)kMaxStreamQps || split > bytes || via > 1) return -22;
+  if (!copy_qps(a.qps, qps_host, nqp) || split > bytes || via > 1) return -22;
   if (opcode != OP_RDMA_WRITE && opcode != OP_RDMA_READ && opcode != OP_SEND) return -22;
-  for (uint32_t i = 0; i < nqp; ++i) a.qps[i] = (QpDev*)qps_host[i];
   a.opcode = opcode; a.laddr = laddr; a.laddr1 = laddr1; a.raddr = raddr; a.stride = stride; a.slot_stride = slot_stride;
   a.lkey = lkey; a.lkey1 = lkey1; a.rkey = rkey; a.bytes = bytes; a.split = split; a.nslots = nslots ? nslots : 1;
   a.iters = iters; a.window = window; a.via = via;
   rn_stream_clamp(window, &burst, &signal_every);
   a.signal_every = signal_every; a.burst = burst;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.timeout_ns = timeout_ns(timeout_ms);
   a.out = (unsigned long long*)out_dev;
   gather_stream_kernel<<<nqp, 32, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -667,7 +661,7 @@ RN_API int rn_k_read_records(uint64_t stream, uint64_t qp_dev, uint64_t laddr, u
   a.lkey = lkey; a.rkey = rkey; a.rec_bytes = rec_bytes; a.n = n;
   rn_stream_clamp(window, &burst, &signal_every);
   a.window = window; a.burst = burst; a.signal_every = signal_every;
-  a.timeout_ns = (timeout_ms ? timeout_ms : 2000) * 1000000ull;
+  a.timeout_ns = timeout_ns(timeout_ms);
   a.out = (unsigned long long*)out_dev;
   read_records_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
   return (int)cudaGetLastError();
@@ -738,10 +732,9 @@ RN_API int rn_k_signal_wait(uint64_t stream, uint64_t signal, uint64_t until, ui
                             uint64_t timeout_ms, uint64_t check_dst, uint64_t check_src, uint64_t check_bytes,
                             uint64_t check_stride) {
   if (check_bytes & 15) return -22;
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
+  unsigned long long* o = clear_record(out_dev);
   signal_wait_kernel<<<1, kSignalWaitThreads, 0, (cudaStream_t)stream>>>(
-      (const unsigned long long*)signal, until, (unsigned long long*)stamps_dev, o, (timeout_ms ? timeout_ms : 2000) * 1000000ull,
+      (const unsigned long long*)signal, until, (unsigned long long*)stamps_dev, o, timeout_ns(timeout_ms),
       (const uint8_t*)check_dst, (const uint8_t*)check_src, check_bytes, check_stride);
   return (int)cudaGetLastError();
 }
@@ -807,11 +800,10 @@ RN_API int rn_k_cq_watch(uint64_t stream, uint64_t cq_dev, uint32_t n, uint64_t 
                          uint32_t nslots, uint64_t msg_bytes, uint64_t piece, uint64_t tail, uint64_t timeout_ms,
                          uint64_t out_dev) {
   if (!nslots || !piece || !tail || ((dst | src | stride | piece | tail) & 15)) return -22;
-  unsigned long long* o = (unsigned long long*)out_dev;
-  for (int i = 0; i < 8; ++i) o[i] = 0;
+  unsigned long long* o = clear_record(out_dev);
   cq_watch_kernel<<<1, kCqWatchThreads, 0, (cudaStream_t)stream>>>(
       (const CqDev*)cq_dev, n, (const uint8_t*)dst, (const uint8_t*)src, stride, nslots, msg_bytes, piece, tail,
-      (timeout_ms ? timeout_ms : 2000) * 1000000ull, o);
+      timeout_ns(timeout_ms), o);
   return (int)cudaGetLastError();
 }
 

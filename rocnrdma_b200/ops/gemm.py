@@ -3,13 +3,13 @@ from __future__ import annotations
 
 import os
 
-import ctypes as C
 from dataclasses import dataclass
 
 import torch
 
 from .. import _native as N
-from .rdma import WAIT_STATUS, _stream_ptr, work_stream
+from . import launch as L
+from .rdma import _stream_ptr, work_stream
 
 BM, BN, BK = 128, 256, 64
 
@@ -76,7 +76,7 @@ def dequant_fp8_panels(rec: torch.Tensor, M: int, Nn: int) -> torch.Tensor:
 
 def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None, qp=None, dst_mr=None,
               signal_every: int = 1, with_imm: bool = False, out_fp8: bool = False, cta_group: int = 0, group_m: int = 0, direct: bool = False, plain_stores: bool = False, grid: int = 0, timeout_ms: int = 2000, stream=None, sync: bool = True, post_only: bool = False, stream_k: bool = False,
-              scratch_slot: int = 2):
+              scratch_slot: int = L.SLOT["gemm_send"]):
     """``c[M,N] = a[M,K] @ b[N,K].T`` (bf16 in/out, fp32 accumulate: wgmma on the H100 tensor cores).
 
     With ``qp``/``c_mr``/``dst_mr`` every finished 128-row panel of ``c`` is RDMA-written to the same
@@ -122,23 +122,17 @@ def gemm_send(ctx, a: torch.Tensor, b: torch.Tensor, c: torch.Tensor, c_mr=None,
     lib = N.load()
     ws = work_stream(ctx, stream)
     m_blks = -(-M // BM)
-    counters = ctx.dev_scratch((m_blks + 1) * 4 + 64, offset=scratch_slot * (256 << 10))
-    out_addr, out_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
+    counters = L.counters(ctx, m_blks + 1, scratch_slot)
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot))
     rc = lib.rn_k_gemm_send(_stream_ptr(ws), grid, a.data_ptr(), b.data_ptr(), c.data_ptr(), M, Nn, K,
                             qp.dev_ptr if qp is not None else 0, c_mr.addr if c_mr is not None else 0,
                             c_mr.lkey if c_mr is not None else 0, dst_mr.addr if dst_mr is not None else 0,
                             dst_mr.rkey if dst_mr is not None else 0, signal_every, int(with_imm) | (2 if post_only else 0), int(out_fp8), cta_group, group_m, int(direct) | (2 if plain_stores else 0) | (4 if os.environ.get("RN_GEMM_DENSE_PROBE") else 0) | (8 if (not stream_k or os.environ.get("RN_GEMM_NO_STREAMK")) else 0), counters, out_addr, timeout_ms)
-    if rc:
-        raise N.NativeError(f"gemm_send launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse(out_view, M, Nn, K)
+    return L.finish(rc, "gemm_send", out_view, ws, sync, parse, M, Nn, K)
 
 
 def parse(view, M, Nn, K) -> GemmResult:
-    w = (C.c_int64 * 8).from_buffer(view)
-    r = GemmResult(WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2], w[3], w[4], w[5], M, Nn, K)
-    r.variant = int(w[6])
-    r.stream_k = bool(w[7])
+    r = L.decode_as(GemmResult, view, ("panels_posted", "t_first_post_ns", "t_compute_end_ns", "variant", "stream_k"),
+                    M=M, N=Nn, K=K)
+    r.stream_k = bool(r.stream_k)
     return r

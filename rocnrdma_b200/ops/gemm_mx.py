@@ -2,14 +2,14 @@
 the send side produces -- so a receiver multiplies straight out of its receive buffer."""
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
 
 import torch
 
 from .. import _native as N
+from . import launch as L
 from .pack import BLOCK, quantize_blocks, record_bytes, ue8m0
-from .rdma import WAIT_STATUS, _stream_ptr, work_stream
+from .rdma import _stream_ptr, work_stream
 
 PANEL_ROWS = 128
 
@@ -68,7 +68,7 @@ class MxResult:
         return 2.0 * self.M * self.N * self.K / max(self.device_ns, 1) / 1e3
 
 
-def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, stream=None, sync: bool = True, scratch_slot: int = 3,
+def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, stream=None, sync: bool = True, scratch_slot: int = L.SLOT["gemm_mxfp8"],
                cta_group: int = 0, a_ready=None, timeout_ms: int = 2000):
     """``c[M,N] (bf16) = dequant(a)[M,K] @ dequant(b)[N,K].T`` with the block scales applied by the tensor core.
     Any M and N; K a multiple of 32 (one MX block) and of 16 bytes.
@@ -85,26 +85,19 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
         cta_group = int(os.environ["RN_MX_CTA_GROUP"])
     M, Nn, K = a.rows, b.rows, a.K
     assert b.K == K and c.dtype == torch.bfloat16 and tuple(c.shape) == (M, Nn) and c.is_contiguous()
-    if a_ready is not None:
-        n_rec = -(-M // (a.rows_per_rec or M))
-        if a_ready.dtype != torch.int64 or not a_ready.is_cuda or a_ready.numel() < n_rec:
-            raise ValueError(f"a_ready must be an int64 CUDA tensor with one word per record of a ({n_rec}), "
-                             f"got {a_ready.dtype} x {a_ready.numel()} on {a_ready.device}")
+    ready_addr = 0 if a_ready is None else L.tensor_ptr(a_ready, torch.int64, ctx.device,
+                                                        "a_ready (one word per record of a)", -(-M // (a.rows_per_rec or M)))
     lib = N.load()
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=4096 + scratch_slot * 64)
-    done = ctx.dev_scratch(64, offset=scratch_slot * (256 << 10))          # zeroed device counter, cleaned by the kernel
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot))
+    done = L.counters(ctx, 1, scratch_slot)          # zeroed device counter, cleaned by the kernel
     rc = lib.rn_k_gemm_mxfp8(_stream_ptr(ws), grid, a.q_ptr, a.s_ptr, a.rows_per_rec, a.rec_stride, b.q_ptr, b.s_ptr, b.rows_per_rec,
-                             b.rec_stride, c.data_ptr(), M, Nn, K, out_addr, cta_group, done,
-                             a_ready.data_ptr() if a_ready is not None else 0, timeout_ms)
-    if rc:
-        raise N.NativeError(f"gemm_mxfp8 launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    w = (C.c_int64 * 8).from_buffer(out_view)
-    r = MxResult(WAIT_STATUS.get(w[0], str(w[0])), w[2] - w[1], M, Nn, K, variant=int(w[6]))
-    return r
+                             b.rec_stride, c.data_ptr(), M, Nn, K, out_addr, cta_group, done, ready_addr, timeout_ms)
+    return L.finish(rc, "gemm_mxfp8", out_view, ws, sync, _parse, M, Nn, K)
+
+
+def _parse(view, M, Nn, K) -> MxResult:
+    return L.decode_as(MxResult, view, (None, None, None, "variant"), M=M, N=Nn, K=K)
 
 
 # ------------------------------------------------------------------ PyTorch references

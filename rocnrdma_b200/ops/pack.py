@@ -2,13 +2,14 @@
 the receive-side unpack, the reduction of several sources' records, and the bit-exact PyTorch references of all three."""
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
 
 import torch
 
 from .. import _native as N
-from .rdma import WAIT_STATUS, _stream_ptr, _device_words, work_stream
+from . import launch as L
+from .launch import SLOT
+from .rdma import _stream_ptr, work_stream
 
 TILE_ELEMS = 8192
 BLOCK = 32
@@ -53,19 +54,23 @@ class PackResult:
         return 2 * self.n_elems / max(self.device_ns, 1)
 
 
+PACK_WORDS = ("wqes", "t_first_post_ns", "t_pack_end_ns")
+UNPACK_WORDS = ("records_seen", "records_forwarded", "t_first_post_ns")
+REDUCE_WORDS = ("records_reduced", "records_posted", "t_first_post_ns", "t_reduce_end_ns")
+
+
 def _parse(view, n_elems, wire) -> PackResult:
-    w = (C.c_int64 * 8).from_buffer(view)
-    return PackResult(WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2], w[3], w[4], w[5], n_elems, wire)
+    return L.decode_as(PackResult, view, PACK_WORDS, n_elems=n_elems, wire_bytes=wire)
 
 
 def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chunk_elems: int = 1 << 20,
                    with_imm: bool = False, signal_every: int = 1, grid: int = 0, timeout_ms: int = 2000,
-                   stream=None, sync: bool = True, scratch_slot: int = 0, post_only: bool = False, direct: bool = False,
+                   stream=None, sync: bool = True, scratch_slot: int = SLOT["pack"], post_only: bool = False, direct: bool = False,
                    result_off=None, residual=None):
     """Pack ``src`` (bf16) into fp8 chunk records in ``staging_mr`` and, if ``qp`` is given,
     RDMA-write every record to the same offset of ``dst_mr`` from inside the kernel.
-    ``result_off``: where in the mapped scratch the kernel writes its result words (default ``4096 + scratch_slot * 64``,
-    see :func:`result_offset`).
+    ``result_off``: where in the mapped scratch the kernel writes its result words (default: the record of
+    ``scratch_slot``, see :func:`~rocnrdma_b200.ops.launch.result_offset`).
     ``direct``: ``staging_mr`` is the *peer's* buffer registered with this context (NVLink-mapped, ``ctx.reg_mr(tensor_on_the_peer)``):
     the kernel's own stores deliver the records and each one is announced by a zero-length RDMA_WRITE_IMM (needs ``with_imm``).
     ``residual``: error feedback, an fp32 CUDA tensor of ``src.numel()`` values (contiguous, 32-byte aligned) read and
@@ -80,60 +85,22 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     wire = staging_bytes(n, chunk_elems)
     if staging_mr.length < wire or (dst_mr is not None and dst_mr.length < wire):
         raise ValueError("staging / destination region too small for the records")
-    res_addr = 0 if residual is None else _check_tensor(residual, torch.float32, n, ctx.device, "residual")
+    res_addr = 0 if residual is None else L.tensor_ptr(residual, torch.float32, ctx.device, "residual", n, exact=True, align=32)
     lib = N.load()
     ws = work_stream(ctx, stream)
     # [n_chunks] groups packed per record ; CTAs done
-    counters = _counters(ctx, n // chunk_elems + 1, scratch_slot)
-    out_addr, out_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
+    counters = L.counters(ctx, n // chunk_elems + 1, scratch_slot)
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
     rc = lib.rn_k_pack_fp8_write(_stream_ptr(ws), grid, src.data_ptr(), staging_mr.addr, n, chunk_elems,
                                  qp.dev_ptr if qp is not None else 0, staging_mr.addr, staging_mr.lkey,
                                  dst_mr.addr if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
                                  int(with_imm) | (2 if post_only else 0) | (4 if direct else 0), signal_every, counters, out_addr, timeout_ms,
                                  res_addr)
-    if rc:
-        raise N.NativeError(f"pack_fp8_write launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    if qp is None:
-        return None
-    return _parse(out_view, n, wire)
-
-
-SLOT_BYTES = 256 << 10          # one launch's share of the device scratch (``scratch_slot``)
-
-
-def counter_bytes(n_words: int) -> int:
-    """Device scratch a launch with ``n_words`` 32-bit counters takes: the counters, rounded up to 8 bytes, then the
-    three 64-bit words the kernels post records through."""
-    return (int(n_words) * 4 + 7) // 8 * 8 + 24
-
-
-def _counters(ctx, n_words: int, scratch_slot: int) -> int:
-    """Address of a launch's zeroed counters in device-scratch slot ``scratch_slot``."""
-    nb = counter_bytes(n_words)
-    if nb > SLOT_BYTES:
-        raise ValueError(f"{n_words} counters need {nb} bytes; a scratch slot holds {SLOT_BYTES}")
-    if not 0 <= scratch_slot < ctx.dev_scratch_bytes // SLOT_BYTES:
-        raise ValueError(f"scratch_slot={scratch_slot}: the device scratch has {ctx.dev_scratch_bytes // SLOT_BYTES} slots")
-    return ctx.dev_scratch(nb, offset=scratch_slot * SLOT_BYTES)
-
-
-def result_offset(scratch_slot: int, result_off=None) -> int:
-    """Offset in the mapped scratch of a launch's 64-byte result record: ``result_off``, else ``4096 + scratch_slot * 64``.
-    The host zeroes the record when it enqueues the launch, not when the launch runs, so launches queued on one stream
-    before the first of them has run need one record each."""
-    if result_off is None:
-        return 4096 + scratch_slot * 64
-    result_off = int(result_off)
-    if result_off < 0 or result_off % 64:
-        raise ValueError(f"result_off={result_off}: a non-negative multiple of 64")
-    return result_off
+    return L.finish(rc, "pack_fp8_write", out_view, ws, sync, None if qp is None else _parse, n, wire)
 
 
 def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int = 1 << 20, qp=None, grid: int = 0,
-               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_slot: int = 1, ready=None, *,
+               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_slot: int = SLOT["unpack"], ready=None, *,
                fwd_qp=None, fwd_src_mr=None, fwd_dst_mr=None, fwd_dst_off: int = 0, with_imm: bool = False,
                imm_base: int = 0, signal_every: int = 1, post_only: bool = False, result_off=None):
     """fp8 chunk records -> bf16.  With ``qp`` the kernel waits for each record's receive
@@ -175,12 +142,12 @@ def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int =
                              f"fit fwd_dst_mr ({fwd_dst_mr.length} bytes)")
         if not 0 <= imm_base or imm_base + n_chunks > 1 << 32:
             raise ValueError(f"imm_base={imm_base}: the immediates imm_base + r of {n_chunks} records must fit 32 bits")
-    ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_chunks, ctx.device, "ready")
+    ready_addr = 0 if ready is None else L.tensor_ptr(ready, torch.int64, ctx.device, "ready", n_chunks)
     lib = N.load()
     ws = work_stream(ctx, stream)
     # [n_chunks] flags (claims when forwarding) ; CTAs done ; records seen ; abort flag
-    arrived = _counters(ctx, n_chunks + 3, scratch_slot)
-    out_addr, out_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
+    arrived = L.counters(ctx, n_chunks + 3, scratch_slot)
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
     rc = lib.rn_k_unpack_fp8(_stream_ptr(ws), grid, staging.data_ptr(), dst.data_ptr(), n, chunk_elems,
                              qp.dev_ptr if qp is not None else 0, arrived, out_addr, timeout_ms, ready_addr,
                              fwd_qp.dev_ptr if fwd_qp is not None else 0,
@@ -189,19 +156,12 @@ def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int =
                              fwd_dst_mr.addr + fwd_dst_off if fwd_qp is not None else 0,
                              fwd_dst_mr.rkey if fwd_qp is not None else 0, int(with_imm) | (2 if post_only else 0),
                              imm_base, signal_every)
-    if rc:
-        raise N.NativeError(f"unpack_fp8 launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_unpack(out_view)
+    return L.finish(rc, "unpack_fp8", out_view, ws, sync, parse_unpack)
 
 
 def parse_unpack(view) -> dict:
     """Decode the record :func:`unpack_fp8` leaves in the mapped scratch (for ``sync=False`` callers)."""
-    w = (C.c_int64 * 8).from_buffer(view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), device_ns=w[2] - w[1], records_seen=w[3], records_forwarded=w[4],
-                t_first_post_ns=w[5], t_start_ns=w[1], t_end_ns=w[2])
+    return L.decode(view, UNPACK_WORDS)
 
 
 # ------------------------------------------------------------------ bit-exact references
@@ -383,31 +343,13 @@ class ReduceResult:
 
 def parse_reduce(view, hbm_bytes: int = 0) -> ReduceResult:
     """Decode the record :func:`reduce_fp8` leaves in its scratch slot (for ``sync=False`` callers)."""
-    w = (C.c_int64 * 8).from_buffer(view)
-    return ReduceResult(WAIT_STATUS.get(w[0], str(w[0])), w[1], w[2], w[3], w[4], w[5], w[6], hbm_bytes)
-
-
-def _check_tensor(t, dtype, n, device, what):
-    """Address of ``t``: a ``dtype`` tensor on cuda:``device``, contiguous, 32-byte aligned, of ``n`` elements."""
-    if not isinstance(t, torch.Tensor) or t.dtype != dtype:
-        raise ValueError(f"{what} must be a {str(dtype).removeprefix('torch.')} tensor, not {getattr(t, 'dtype', type(t).__name__)}")
-    if not t.is_cuda or t.device.index != device:
-        raise ValueError(f"{what} must be on cuda:{device}, not {t.device}")
-    if not t.is_contiguous() or t.data_ptr() & 31:
-        raise ValueError(f"{what} must be contiguous and 32-byte aligned (256-bit loads / stores)")
-    if t.numel() != n:
-        raise ValueError(f"{what} holds {t.numel()} elements; n_elems is {n}")
-    return t.data_ptr()
-
-
-def _check_bf16(t, n, device, what):
-    return _check_tensor(t, torch.bfloat16, n, device, what)
+    return L.decode_as(ReduceResult, view, REDUCE_WORDS, hbm_bytes=hbm_bytes)
 
 
 def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int = 1 << 20, *, local=None, out=None,
                out_mr=None, qp=None, dst_mr=None, dst_off: int = 0, with_imm: bool = False, signal_every: int = 1,
                post_only: bool = False, ready=None, grid: int = 0, timeout_ms: int = 2000, stream=None, sync: bool = True,
-               scratch_slot: int = 4, imm_base: int = 0, result_off=None, residual=None):
+               scratch_slot: int = SLOT["reduce"], imm_base: int = 0, result_off=None, residual=None):
     """Sum ``n_src`` sources of K3 chunk records, plus an optional bf16 addend, as the records land, and re-pack and forward
     the sum: one hop of a reduce-scatter ring in one kernel.
 
@@ -423,9 +365,9 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     tensor of ``n_src * n_rec`` arrival words, source s in ``ready[s * n_rec:(s + 1) * n_rec]``, as ``recv_consume`` and
     :func:`~rocnrdma_b200.ops.read_records` set them) every step waits for the words of all sources of the records it
     reads; a word still 0 after ``timeout_ms`` ends the kernel with ``TIMEOUT``, and a record not reduced is never posted.
-    Two reductions that run at once need different ``scratch_slot`` values (0..7; K3 uses 0, K5 1, the GEMMs 2 and 3).
+    Two reductions that run at once need different ``scratch_slot`` values (0..7; the defaults are ``ops.launch.SLOT``).
     ``imm_base`` offsets the immediates (``imm_base + r``), so that the records of several hops that reach one QP stamp
-    different arrival words; ``result_off`` is :func:`result_offset`'s.
+    different arrival words; ``result_off`` is :func:`~rocnrdma_b200.ops.launch.result_offset`'s.
 
     ``residual``: error feedback, an fp32 CUDA tensor of ``n_elems`` (contiguous, 32-byte aligned) read and written in
     place.  It is added to the sum last, one fp32 add; ``out`` and the records hold that value, and the residual then
@@ -448,8 +390,8 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
                          f"records need {n_src * wire}")
     if records.data_ptr() & 31:
         raise ValueError("records must be 32-byte aligned (256-bit loads)")
-    local_addr = 0 if local is None else _check_bf16(local, n_elems, dev, "local")
-    out_addr = 0 if out is None else _check_bf16(out, n_elems, dev, "out")
+    local_addr = 0 if local is None else L.tensor_ptr(local, torch.bfloat16, dev, "local", n_elems, exact=True, align=32)
+    out_addr = 0 if out is None else L.tensor_ptr(out, torch.bfloat16, dev, "out", n_elems, exact=True, align=32)
     if out is None and out_mr is None:
         raise ValueError("reduce_fp8 needs an output: out (bf16) and / or out_mr (records)")
     if out_mr is not None:
@@ -472,13 +414,13 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
             raise ValueError("residual= needs out_mr: the residual is what the records of the sum lose")
         if n_src > (2 if local is not None else 1):
             raise ValueError(f"residual= with n_src={n_src}: error feedback runs with P = 1, or P = 2 with local")
-        res_ptr = _check_tensor(residual, torch.float32, n_elems, dev, "residual")
-    ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n_src * n_rec, dev, "ready")
+        res_ptr = L.tensor_ptr(residual, torch.float32, dev, "residual", n_elems, exact=True, align=32)
+    ready_addr = 0 if ready is None else L.tensor_ptr(ready, torch.int64, dev, "ready", n_src * n_rec)
     # [n_rec] tiles done per record ; CTAs done ; abort flag ; records reduced
-    counters = _counters(ctx, n_rec + 3, scratch_slot)
+    counters = L.counters(ctx, n_rec + 3, scratch_slot)
     lib = N.load()
     ws = work_stream(ctx, stream)
-    res_addr, res_view = ctx.scratch(64, offset=result_offset(scratch_slot, result_off))
+    res_addr, res_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
     hbm = n_src * wire + (2 * n_elems if local is not None else 0) + (2 * n_elems if out is not None else 0) + \
         (wire if out_mr is not None else 0) + (8 * n_elems if residual is not None else 0)
     rc = lib.rn_k_reduce_fp8(_stream_ptr(ws), grid, records.data_ptr(), n_src, local_addr, out_addr,
@@ -487,9 +429,4 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
                              out_mr.lkey if out_mr is not None else 0, dst_mr.addr + dst_off if dst_mr is not None else 0,
                              dst_mr.rkey if dst_mr is not None else 0, int(with_imm) | (2 if post_only else 0), signal_every,
                              counters, res_addr, timeout_ms, imm_base, res_ptr)
-    if rc:
-        raise N.NativeError(f"reduce_fp8 launch failed ({rc})")
-    if not sync:
-        return res_view, ws
-    ws.synchronize()
-    return parse_reduce(res_view, hbm)
+    return L.finish(rc, "reduce_fp8", res_view, ws, sync, parse_reduce, hbm)

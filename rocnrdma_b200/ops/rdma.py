@@ -1,15 +1,14 @@
 """K1 / K2 / K6 wrappers: GPU-initiated RDMA streams and verification helpers."""
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
 from typing import List
 
 import torch
 
 from .. import _native as N
-
-WAIT_STATUS = {0: "OK", -1: "TIMEOUT", -2: "CQE_ERROR", -3: "QP_ERROR"}
+from . import launch as L
+from .launch import MAPPED, WAIT_STATUS  # noqa: F401  (WAIT_STATUS: ops.rdma.WAIT_STATUS is public)
 
 
 def _stream_ptr(stream=None) -> int:
@@ -85,37 +84,29 @@ def rdma_stream(qps, opcode: int, src_mr, dst_mr, nbytes: int, iters: int = 1, w
     """
     nbytes = N.byte_count(nbytes)
     lib = N.load()
-    if not isinstance(qps, (list, tuple)):
-        qps = [qps]
+    qps, qp_arr = L.qp_array(qps)
     ctx = qps[0].ctx
     ws = work_stream(ctx, stream)
     nq = len(qps)
-    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
-    out_addr, out_view = ctx.scratch(nq * 64) if out is None else out
+    out_addr, out_view = L.result(ctx, MAPPED["rdma_stream"].offset, nq) if out is None else out
     rc = lib.rn_k_rdma_stream(_stream_ptr(ws), qp_arr, nq, opcode | (0x80000000 if post_only else 0), src_mr.addr, src_mr.lkey,
                               dst_mr.addr if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
                               stride, nbytes, iters, window, signal_every, burst, slot_stride, nslots, timeout_ms, out_addr,
                               fence_every)
-    if rc:
-        raise N.NativeError(f"rdma_stream launch failed: cuda error {rc}")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_stream_out(out_view, nq, nbytes)
+    return L.finish(rc, "rdma_stream", out_view, ws, sync, parse_stream_out, nq, nbytes)
 
 
 def parse_stream_out(out, nqp: int, nbytes: int) -> StreamResult:
-    words = (C.c_int64 * (nqp * 8)).from_buffer(out)
-    o = [list(words[i * 8:(i + 1) * 8]) for i in range(nqp)]
-    return StreamResult(status=[WAIT_STATUS.get(r[0], str(r[0])) for r in o], t_start_ns=[r[1] for r in o],
-                        t_end_ns=[r[2] for r in o], done=[r[3] for r in o], bytes_per_msg=nbytes)
+    o = [L.decode(out, ("done",), i) for i in range(nqp)]
+    return StreamResult(status=[r["status"] for r in o], t_start_ns=[r["t_start_ns"] for r in o],
+                        t_end_ns=[r["t_end_ns"] for r in o], done=[r["done"] for r in o], bytes_per_msg=nbytes)
 
 
 WRITE_READ_MODES = {"fenced": 0, "wait": 1, "one_call": 2}
 
 
 def write_read(qp, src_mr, dst_mr, back_mr, nbytes: int, iters: int = 1, mode: str = "fenced", timeout_ms: int = 2000,
-               stream=None, scratch_off: int = 32768) -> dict:
+               stream=None, scratch_off: int = MAPPED["write_read"].offset) -> dict:
     """A WRITE followed by a READ of the same bytes, posted from one GPU thread ``iters`` times: ``nbytes`` from
     ``src_mr`` to ``dst_mr``, then back from ``dst_mr`` into ``back_mr`` (all at offset 0), waiting for the READ's
     completion each time.  ``mode`` says how the READ is kept behind the WRITE: ``"fenced"`` posts both under one doorbell
@@ -126,15 +117,16 @@ def write_read(qp, src_mr, dst_mr, back_mr, nbytes: int, iters: int = 1, mode: s
     nbytes = N.byte_count(nbytes)
     ctx = qp.ctx
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off)
     rc = N.load().rn_k_write_read(_stream_ptr(ws), qp.dev_ptr, src_mr.addr, src_mr.lkey, dst_mr.addr, dst_mr.rkey, back_mr.addr,
                                   back_mr.lkey, nbytes, iters, WRITE_READ_MODES[mode], timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"write_read launch failed ({rc})")
-    ws.synchronize()
-    w = (C.c_int64 * 8).from_buffer(out_view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), done=w[3], device_ns=w[2] - w[1], mean_ns=w[4] / max(w[3], 1),
-                min_ns=w[5] if w[3] else 0)
+    return L.finish(rc, "write_read", out_view, ws, True, _parse_write_read)
+
+
+def _parse_write_read(view) -> dict:
+    d = L.decode(view, ("done", "sum_ns", "min_ns"))
+    return dict(status=d["status"], done=d["done"], device_ns=d["device_ns"], mean_ns=d["sum_ns"] / max(d["done"], 1),
+                min_ns=d["min_ns"] if d["done"] else 0)
 
 
 def fill_random(t: torch.Tensor, seed: int = 1, stream=None):
@@ -167,43 +159,36 @@ def l2_flush(scratch: torch.Tensor, value: int = 0, stream=None):
 
 
 def recv_consume(qp, n: int, max_imm: int = 0, stamps=None, timeout_ms: int = 2000, stream=None, sync: bool = True,
-                 scratch_off: int = 8192, prepost_mr=None, prepost_bytes: int = 0):
+                 scratch_off: int = MAPPED["recv_consume"].offset, prepost_mr=None, prepost_bytes: int = 0):
     """Receive-side consumer kernel on ``qp``'s GPU: waits for ``n`` arrivals (SEND / RDMA_WRITE_IMM) on the
     receive CQ and, if ``stamps`` (int64 tensor on that GPU) is given, stamps %globaltimer per immediate."""
     ctx = qp.ctx
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off)
     # prepost_mr: the kernel posts its own n receive WQEs from the device before polling (buffer i at offset i * prepost_bytes)
     rc = N.load().rn_k_recv_consume(_stream_ptr(ws), qp.dev_ptr, n, max_imm, stamps.data_ptr() if stamps is not None else 0,
                                     out_addr, timeout_ms, prepost_mr.addr if prepost_mr is not None else 0,
                                     prepost_mr.lkey if prepost_mr is not None else 0,
                                     prepost_bytes if prepost_mr is not None else 0xFFFFFFFF)
-    if rc:
-        raise N.NativeError(f"recv_consume launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_recv(out_view)
+    return L.finish(rc, "recv_consume", out_view, ws, sync, parse_recv)
+
+
+RECV_WORDS = ("seen", "bytes")
 
 
 def parse_recv(view) -> dict:
-    w = (C.c_int64 * 8).from_buffer(view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), device_ns=w[2] - w[1], t_start_ns=w[1], t_end_ns=w[2], seen=w[3], bytes=w[4])
+    return L.decode(view, RECV_WORDS)
 
 
 def shared_post_stress(qp, src_mr, dst_mr, ctas: int = 64, per_cta: int = 64, timeout_ms: int = 3000, stream=None):
     """``ctas`` CTAs hammer one QP with ``per_cta`` 64-byte writes each through the shared submit."""
     ctx = qp.ctx
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=12288)
-    counter = ctx.dev_scratch(64, offset=900 << 10)
+    out_addr, out_view = L.result(ctx, MAPPED["shared_post_stress"].offset)
+    counter = ctx.dev_scratch(L.SHARED_POST_STRESS_COUNTER.nbytes, offset=L.SHARED_POST_STRESS_COUNTER.offset)
     rc = N.load().rn_k_shared_post_stress(_stream_ptr(ws), qp.dev_ptr, ctas, src_mr.addr, src_mr.lkey, dst_mr.addr, dst_mr.rkey,
                                           per_cta, counter, out_addr, timeout_ms)
-    if rc:
-        raise N.NativeError(f"shared_post_stress launch failed ({rc})")
-    ws.synchronize()
-    w = (C.c_int64 * 8).from_buffer(out_view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), device_ns=w[2] - w[1], posted=w[3])
+    return L.finish(rc, "shared_post_stress", out_view, ws, True, L.decode, ("posted",))
 
 
 # ---------------------------------------------------------------- remote atomics and put-with-signal
@@ -212,7 +197,7 @@ _OP_CS, _OP_FA = 0x11, 0x12
 
 def atomic_stream(qps, op: str, target_mr, fetch_mr, iters: int, add: int = 1, compare: int = 0, swap: int = 0,
                   chain: bool = False, target_stride: int = 0, window: int = 0, burst: int = 1, signal_every: int = 1,
-                  timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = 16384):
+                  timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = MAPPED["atomic_stream"].offset):
     """Device-posted 8-byte remote atomics: one warp per QP posts ``iters`` FETCH_AND_ADD (``op="fa"``: ``add``) or
     COMPARE_AND_SWAP (``op="cs"``: ``compare`` / ``swap``) work requests with the same windowed, bursted poster as
     :func:`rdma_stream`.  QP ``c`` targets the u64 at ``target_mr.addr + c * target_stride`` (``target_stride=0``: every
@@ -223,25 +208,18 @@ def atomic_stream(qps, op: str, target_mr, fetch_mr, iters: int, add: int = 1, c
     if op not in ("fa", "cs"):
         raise ValueError("op must be 'fa' or 'cs'")
     lib = N.load()
-    if not isinstance(qps, (list, tuple)):
-        qps = [qps]
+    qps, qp_arr = L.qp_array(qps)
     ctx = qps[0].ctx
     nq = len(qps)
     if fetch_mr.length < nq * iters * 8:
         raise ValueError(f"fetch_mr holds {fetch_mr.length} bytes; {nq} QPs x {iters} atomics need {nq * iters * 8}")
     ws = work_stream(ctx, stream)
-    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
-    out_addr, out_view = ctx.scratch(nq * 64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off, nq)
     m = 0xFFFFFFFFFFFFFFFF
     rc = lib.rn_k_atomic_stream(_stream_ptr(ws), qp_arr, nq, _OP_FA if op == "fa" else _OP_CS, int(chain), target_mr.addr,
                                 target_mr.rkey, target_stride, fetch_mr.addr, fetch_mr.lkey, add & m, compare & m, swap & m,
                                 iters, window, signal_every, burst, timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"atomic_stream launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_stream_out(out_view, nq, 8)
+    return L.finish(rc, "atomic_stream", out_view, ws, sync, parse_stream_out, nq, 8)
 
 
 def _fetch_sink(ctx):
@@ -254,7 +232,7 @@ def _fetch_sink(ctx):
 
 def put_signal(qp, src_mr, dst_mr, nbytes: int, sig_mr, sig_off: int = 0, fetch_mr=None, add: int = 1, iters: int = 1,
                window: int = 0, slot_stride: int = 0, nslots: int = 1, timeout_ms: int = 2000, stream=None,
-               sync: bool = True, scratch_off: int = 20480):
+               sync: bool = True, scratch_off: int = MAPPED["put_signal"].offset):
     """Device-posted put-with-signal: message ``i`` is an RDMA WRITE of ``nbytes`` from ``src_mr`` to ``dst_mr`` (slot
     ``i % nslots`` at ``slot_stride``) followed by a FETCH_AND_ADD of ``add`` on the remote u64 at
     ``sig_mr.addr + sig_off``, both published with one doorbell.  The atomic executes only after the WRITE has landed,
@@ -269,21 +247,16 @@ def put_signal(qp, src_mr, dst_mr, nbytes: int, sig_mr, sig_off: int = 0, fetch_
     if fetch_mr is None:
         fetch_mr = _fetch_sink(ctx)
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off)
     rc = lib.rn_k_put_signal(_stream_ptr(ws), qp.dev_ptr, src_mr.addr, src_mr.lkey, dst_mr.addr, dst_mr.rkey, nbytes,
                              slot_stride, nslots, sig_mr.addr + sig_off, sig_mr.rkey, fetch_mr.addr, fetch_mr.lkey,
                              max(fetch_mr.length // 8, 1), add & 0xFFFFFFFFFFFFFFFF, iters, window, timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"put_signal launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_stream_out(out_view, 1, nbytes)
+    return L.finish(rc, "put_signal", out_view, ws, sync, parse_stream_out, 1, nbytes)
 
 
 def put_inline(qps, values, dst_mr, nbytes: int, iters: int = 1, window: int = 0, burst: int = 1, signal_every: int = 1,
                slot_stride=None, nslots: int = 1, sig_mr=None, sig_off: int = 0, fetch_mr=None, add: int = 1,
-               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = 24576):
+               timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = MAPPED["put_inline"].offset):
     """Device-posted inline puts (DOCA ``p`` / ``p_signal``, ``nvshmem_p``): one warp per QP posts ``iters`` RDMA WRITEs
     whose ``nbytes`` (1..28) travel inside the WQE, with the windowed, bursted poster of :func:`rdma_stream`.  Message
     ``i`` of QP ``c`` (``m = c * iters + i``) reads its bytes into registers from row ``m % rows`` of ``values`` -- a CUDA
@@ -294,8 +267,7 @@ def put_inline(qps, values, dst_mr, nbytes: int, iters: int = 1, window: int = 0
     WRITE has landed, so a receiver may use :func:`signal_wait` unchanged.  Fetched values go to ``fetch_mr`` (default: the
     context's sink, see :func:`put_signal`).  ``window`` and ``burst`` count messages.  Returns a :class:`StreamResult`."""
     lib = N.load()
-    if not isinstance(qps, (list, tuple)):
-        qps = [qps]
+    qps, qp_arr = L.qp_array(qps)
     if not 1 <= nbytes <= 28:
         raise ValueError(f"inline puts carry 1..28 bytes, not {nbytes}")
     if not values.is_cuda or not values.is_contiguous():
@@ -312,20 +284,14 @@ def put_inline(qps, values, dst_mr, nbytes: int, iters: int = 1, window: int = 0
     if sig_mr is not None and fetch_mr is None:
         fetch_mr = _fetch_sink(ctx)
     ws = work_stream(ctx, stream)
-    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
-    out_addr, out_view = ctx.scratch(nq * 64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off, nq)
     sig = (sig_mr.addr + sig_off) if sig_mr is not None else 0
     rc = lib.rn_k_put_inline(_stream_ptr(ws), qp_arr, nq, values.data_ptr(), row_bytes, rows, dst_mr.addr, dst_mr.rkey, nbytes,
                              slot_stride, nslots, sig, sig_mr.rkey if sig_mr is not None else 0,
                              fetch_mr.addr if fetch_mr is not None else 0, fetch_mr.lkey if fetch_mr is not None else 0,
                              max(fetch_mr.length // 8, 1) if fetch_mr is not None else 1, add & 0xFFFFFFFFFFFFFFFF, iters, window,
                              signal_every, burst, timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"put_inline launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_stream_out(out_view, nq, nbytes)
+    return L.finish(rc, "put_inline", out_view, ws, sync, parse_stream_out, nq, nbytes)
 
 
 GATHER_VIA = {"poster": 0, "one_call": 1}
@@ -335,7 +301,7 @@ _OP_WRITE, _OP_SEND, _OP_READ = 0x08, 0x0A, 0x10
 def gather_stream(qps, opcode: int, mr0, mr1, remote_mr, nbytes: int, split: int, iters: int = 1, window: int = 0,
                   signal_every: int = 1, burst: int = 1, stride: int = 0, slot_stride: int = 0, nslots: int = 1,
                   via: str = "poster", timeout_ms: int = 2000, stream=None, sync: bool = True,
-                  scratch_off: int = 36864) -> StreamResult:
+                  scratch_off: int = MAPPED["gather_stream"].offset) -> StreamResult:
     """Device-posted two-entry work requests: one warp per QP posts ``iters`` messages of ``nbytes``, each one work
     request whose scatter-gather list is cut at ``split`` bytes.  Message ``i`` of QP ``c`` uses slot offset
     ``o = c * stride + (i % nslots) * slot_stride``: entry 0 is ``split`` bytes at ``mr0.addr + o``, entry 1 the other
@@ -354,27 +320,20 @@ def gather_stream(qps, opcode: int, mr0, mr1, remote_mr, nbytes: int, split: int
     if via not in GATHER_VIA:
         raise ValueError(f"via must be one of {sorted(GATHER_VIA)}")
     lib = N.load()
-    if not isinstance(qps, (list, tuple)):
-        qps = [qps]
+    qps, qp_arr = L.qp_array(qps)
     ctx = qps[0].ctx
     nq = len(qps)
     ws = work_stream(ctx, stream)
-    qp_arr = (C.c_uint64 * nq)(*[q.dev_ptr for q in qps])
-    out_addr, out_view = ctx.scratch(nq * 64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off, nq)
     rc = lib.rn_k_gather_stream(_stream_ptr(ws), qp_arr, nq, opcode, mr0.addr, mr0.lkey, mr1.addr, mr1.lkey,
                                 remote_mr.addr if remote_mr is not None else 0, remote_mr.rkey if remote_mr is not None else 0,
                                 stride, nbytes, split, slot_stride, nslots, iters, window, signal_every, burst, GATHER_VIA[via],
                                 timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"gather_stream launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_stream_out(out_view, nq, nbytes)
+    return L.finish(rc, "gather_stream", out_view, ws, sync, parse_stream_out, nq, nbytes)
 
 
 def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, stream=None, sync: bool = True,
-                check=None, scratch_off: int = 20544):
+                check=None, scratch_off: int = MAPPED["signal_wait"].offset):
     """Receiver side of :func:`put_signal`, on the GPU that holds the signal: waits until the u64 at ``signal`` (a
     tensor, a ``MemoryRegion`` or an ``(address, nbytes)`` pair; the word at its start) reaches each value ``1..until``
     in turn, with system-scope acquire loads and at most ``timeout_ms`` per arrival.  ``stamps`` (int64 tensor of at
@@ -385,7 +344,7 @@ def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, st
     lib = N.load()
     addr = signal.addr if hasattr(signal, "rkey") else _ptr_len(signal, 8)[0]
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off)
     cd = cs = cb = cst = 0
     if check is not None:
         d, s, cb, cst = check
@@ -394,16 +353,11 @@ def signal_wait(ctx, signal, until: int, stamps=None, timeout_ms: int = 2000, st
             raise ValueError("check slot_bytes must be a multiple of 16")
     rc = lib.rn_k_signal_wait(_stream_ptr(ws), addr, until, stamps.data_ptr() if stamps is not None else 0, out_addr,
                               timeout_ms, cd, cs, cb, cst)
-    if rc:
-        raise N.NativeError(f"signal_wait launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_signal_wait(out_view)
+    return L.finish(rc, "signal_wait", out_view, ws, sync, parse_signal_wait)
 
 
 def cq_watch(cq, n: int, dst, src, slot_stride: int, nslots: int, msg_bytes: int, piece: int, tail: int = 16384,
-             timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = 30720):
+             timeout_ms: int = 2000, stream=None, sync: bool = True, scratch_off: int = MAPPED["cq_watch"].offset):
     """Receiver-side check of a device send CQ that another kernel (the poster) consumes: waits for each of its first
     ``n`` CQEs in turn without consuming them (the CQ must hold ``n``), and the moment CQE ``k`` is visible compares the
     message it names -- slot ``wqe_counter % nslots`` of ``dst`` and ``src`` (tensors or ``(address, nbytes)`` pairs) at
@@ -412,47 +366,25 @@ def cq_watch(cq, n: int, dst, src, slot_stride: int, nslots: int, msg_bytes: int
     from ..api import _ptr_len
     ctx = cq.ctx
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off)
     rc = N.load().rn_k_cq_watch(_stream_ptr(ws), cq.dev_ptr, n, _ptr_len(dst, 1)[0], _ptr_len(src, 1)[0], slot_stride, nslots,
                                 msg_bytes, piece, tail, timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"cq_watch launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_cq_watch(out_view)
+    return L.finish(rc, "cq_watch", out_view, ws, sync, parse_cq_watch)
 
 
 def parse_cq_watch(view) -> dict:
     """Decode the record :func:`cq_watch` leaves in its scratch slot (for ``sync=False`` callers)."""
-    w = (C.c_int64 * 8).from_buffer(view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), seen=w[3], mismatches=w[4], error_cqes=w[5], device_ns=w[2] - w[1])
+    return L.decode(view, ("seen", "mismatches", "error_cqes"))
 
 
 def parse_signal_wait(view) -> dict:
     """Decode the record :func:`signal_wait` leaves in its scratch slot (for ``sync=False`` callers)."""
-    w = (C.c_int64 * 8).from_buffer(view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), seen=w[3], mismatches=w[4], device_ns=w[2] - w[1],
-                t_start_ns=w[1], t_end_ns=w[2])
-
-
-def _device_words(t, dtype, n: int, device: int, what: str) -> int:
-    """Address of ``t``, a contiguous CUDA tensor of ``dtype`` with at least ``n`` entries on GPU ``device``; ``ValueError``
-    otherwise.  The values are never read on the host (that would synchronise)."""
-    if not isinstance(t, torch.Tensor) or t.dtype != dtype:
-        raise ValueError(f"{what} must be a {dtype} tensor, not {getattr(t, 'dtype', type(t).__name__)}")
-    if not t.is_cuda or t.device.index != device:
-        raise ValueError(f"{what} must be on cuda:{device}, not {t.device}")
-    if not t.is_contiguous():
-        raise ValueError(f"{what} must be contiguous")
-    if t.numel() < n:
-        raise ValueError(f"{what} holds {t.numel()} entries; {n} are needed")
-    return t.data_ptr()
+    return L.decode(view, ("seen", "mismatches"))
 
 
 def read_records(qp, src_mr, dst_mr, rec_bytes: int, n: int, *, indices=None, src_off: int = 0, src_stride=None,
                  dst_off: int = 0, ready=None, window: int = 16, burst: int = 1, signal_every: int = 1, timeout_ms: int = 2000,
-                 stream=None, sync: bool = True, scratch_off: int = 40960):
+                 stream=None, sync: bool = True, scratch_off: int = MAPPED["read_records"].offset):
     """Pull ``n`` fixed-size records with device-posted RDMA READs and stamp an arrival word as each one lands.
 
     Record ``r`` is one READ of ``rec_bytes`` from ``src_mr.addr + src_off + j * src_stride`` (the remote side) into
@@ -481,25 +413,18 @@ def read_records(qp, src_mr, dst_mr, rec_bytes: int, n: int, *, indices=None, sr
         raise ValueError("src_off, src_stride and dst_off must be non-negative")
     if dst_off + n * rec_bytes > dst_mr.length:
         raise ValueError(f"{n} records of {rec_bytes} bytes at dst_off={dst_off} do not fit dst_mr ({dst_mr.length} bytes)")
-    idx_addr = 0 if indices is None else _device_words(indices, torch.int32, n, ctx.device, "indices")
-    ready_addr = 0 if ready is None else _device_words(ready, torch.int64, n, ctx.device, "ready")
+    idx_addr = 0 if indices is None else L.tensor_ptr(indices, torch.int32, ctx.device, "indices", n)
+    ready_addr = 0 if ready is None else L.tensor_ptr(ready, torch.int64, ctx.device, "ready", n)
     depth = min(qp.sq_depth, qp.scq.depth)
     window = depth if window <= 0 else min(int(window), depth)
     ws = work_stream(ctx, stream)
-    out_addr, out_view = ctx.scratch(64, offset=scratch_off)
+    out_addr, out_view = L.result(ctx, scratch_off)
     rc = N.load().rn_k_read_records(_stream_ptr(ws), qp.dev_ptr, dst_mr.addr + dst_off, dst_mr.lkey, src_mr.addr + src_off,
                                     src_mr.rkey, src_stride, rec_bytes, n, idx_addr, ready_addr, window, burst, signal_every,
                                     timeout_ms, out_addr)
-    if rc:
-        raise N.NativeError(f"read_records launch failed ({rc})")
-    if not sync:
-        return out_view, ws
-    ws.synchronize()
-    return parse_read_records(out_view)
+    return L.finish(rc, "read_records", out_view, ws, sync, parse_read_records)
 
 
 def parse_read_records(view) -> dict:
     """Decode the record :func:`read_records` leaves in its scratch slot (for ``sync=False`` callers)."""
-    w = (C.c_int64 * 8).from_buffer(view)
-    return dict(status=WAIT_STATUS.get(w[0], str(w[0])), done=w[3], device_ns=w[2] - w[1], t_start_ns=w[1], t_end_ns=w[2],
-                first_idx=w[4], last_idx=w[5], cons=w[6])
+    return L.decode(view, ("done", "first_idx", "last_idx", "cons"))

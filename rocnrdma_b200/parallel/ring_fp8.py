@@ -33,13 +33,11 @@ from typing import List, Optional
 import torch
 
 from .. import ops
-from ..ops import pack as P
-from ..ops.rdma import parse_recv
+from ..ops import launch as L, pack as P
+from ..ops.rdma import RECV_WORDS
 
 GUARD = 8                       # zero words behind the arrival words
-RESULT_BASE = 128 << 10         # mapped-scratch offset of the ring's result records: 4 KiB per device-scratch slot
-RESULT_SLOT_BYTES = 4096
-MAX_IN_PROCESS = 8              # one device-scratch slot per simulated rank
+MAX_IN_PROCESS = L.N_SLOTS      # one device-scratch slot per simulated rank
 MAX_QUEUE_DEPTH = 16384         # the deepest queue create_qp builds (a power of two; the doorbell index is 16 bits)
 
 
@@ -71,9 +69,8 @@ def schedule(rank: int, world: int) -> List[Step]:
     return steps
 
 
-# a launch's result words, by kind, decoded by the parser that owns their layout
-_PARSERS = {"pack": lambda v: vars(P._parse(v, 0, 0)), "reduce": lambda v: vars(P.parse_reduce(v)),
-            "unpack": P.parse_unpack, "recv": parse_recv}
+# the words of each kind of launch's result record, after the header
+_WORDS = {"pack": P.PACK_WORDS, "reduce": P.REDUCE_WORDS, "unpack": P.UNPACK_WORDS, "recv": RECV_WORDS}
 
 
 def _pow2(n: int) -> int:
@@ -144,16 +141,16 @@ class RingAllreduceFp8:
         if n_elems <= 0 or n_elems % (world * chunk_elems):
             raise ValueError(f"n_elems={n_elems} must be a multiple of world * chunk_elems = {world * chunk_elems}: "
                              "every shard is whole records")
-        if 2 * world + 3 > RESULT_SLOT_BYTES // 64:
-            raise ValueError(f"world={world}: {2 * world + 3} result records do not fit {RESULT_SLOT_BYTES} bytes")
+        if 2 * world + 3 > L.RING_SLOT_BYTES // L.RECORD_BYTES:
+            raise ValueError(f"world={world}: {2 * world + 3} result records do not fit {L.RING_SLOT_BYTES} bytes")
         self.ctx, self.n, self.chunk, self.rank, self.world = ctx, n_elems, chunk_elems, rank, world
         self.grid, self.timeout_ms, self.signal_every, self.engine_ctas = int(grid), int(timeout_ms), int(signal_every), int(engine_ctas)
         self.shard = n_elems // world
         self.R = self.shard // chunk_elems
         self.rec = P.record_bytes(chunk_elems)
         self.n_ids = 2 * (world - 1) * self.R
-        counter_bytes = P.counter_bytes(self.R + 3)       # the reduce's and the unpack's: R records and 3 words
-        if counter_bytes > P.SLOT_BYTES:
+        counter_bytes = L.counter_bytes(self.R + 3)       # the reduce's and the unpack's: R records and 3 words
+        if counter_bytes > L.SLOT_BYTES:
             raise ValueError(f"{self.R} records per shard need {counter_bytes} bytes of counters; a scratch slot holds 256 KiB")
         if self.R > max_records(world):
             raise ValueError(f"R={self.R} records per shard: the receive queue would need {_pow2(2 * self.n_ids)} entries, "
@@ -213,7 +210,7 @@ class RingAllreduceFp8:
 
     # ---------------------------------------------------------------- run
     def _res(self, i: int) -> int:
-        return RESULT_BASE + self.scratch_slot * RESULT_SLOT_BYTES + 64 * i
+        return L.ring_result_offset(self.scratch_slot, i)
 
     def _shard(self, t, s):
         s %= self.world
@@ -266,7 +263,7 @@ class RingAllreduceFp8:
         ``steps``: only these indices of :func:`schedule` (a caller that steps the ring from the host)."""
         out = x if out is None else out
         for t, what in ((x, "x"), (out, "out")):
-            P._check_bf16(t, self.n, self.ctx.device, what)
+            L.tensor_ptr(t, torch.bfloat16, self.ctx.device, what, self.n, exact=True, align=32)
         N, q, R, rec = self.world, self.rank, self.R, self.rec  # noqa: F841
         ms = self.main_stream
         if steps is None or 0 in steps:
@@ -324,7 +321,7 @@ class RingAllreduceFp8:
         """Decode the last run's result records (after :meth:`synchronize`)."""
         launches, received, posted = [], 0, 0
         for name, kind, view in self._views:
-            w = _PARSERS[kind](view)
+            w = L.decode(view, _WORDS[kind])
             launches.append(LaunchResult(name, w["status"], w["t_start_ns"], w["t_end_ns"]))
             posted += w.get("wqes", 0) + w.get("records_posted", 0) + w.get("records_forwarded", 0)
             received += w["seen"] if name == "receive" else 0

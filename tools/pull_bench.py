@@ -30,7 +30,7 @@ import torch  # noqa: E402
 
 import rocnrdma_b200 as rn  # noqa: E402
 from rocnrdma_b200 import ops, wire as W  # noqa: E402
-from rocnrdma_b200.ops import gemm_mx as MX  # noqa: E402
+from rocnrdma_b200.ops import gemm_mx as MX, launch as L  # noqa: E402
 
 
 def gpu_info():
@@ -42,11 +42,6 @@ def gpu_info():
 
 def _spread(xs):
     return {"min": round(min(xs), 3), "max": round(max(xs), 3), "runs": [round(x, 3) for x in xs]} if xs else None
-
-
-def _w(view):
-    import ctypes as C
-    return list((C.c_int64 * 8).from_buffer(view))
 
 
 def main():
@@ -142,10 +137,10 @@ def main():
                                                  timeout_ms=TMO, sync=False, stream=s_pull)
                         uv, _ = ops.unpack_fp8(ctx, land5, y5[kind], chunk, grid=64, timeout_ms=TMO, sync=False, stream=s_pull)
                         s_pull.synchronize()
-                    p, u = _w(pv), _w(uv)
-                    checks[f"k5_{kind}_words"] &= p[0] == 0 and p[3] == n_chunks and u[0] == 0
+                    p, u = ops.parse_read_records(pv), ops.parse_unpack(uv)
+                    checks[f"k5_{kind}_words"] &= p["status"] == "OK" and p["done"] == n_chunks and u["status"] == "OK"
                     if keep:
-                        res["k5_2^26"][kind].append((u[2] - p[1]) / 1e3)
+                        res["k5_2^26"][kind].append((u["t_end_ns"] - p["t_start_ns"]) / 1e3)
                 # K7
                 for kind in ("on_arrival", "after_pull"):
                     zero_words()
@@ -161,10 +156,10 @@ def main():
                         gv, _ = ops.gemm_mxfp8(ctx, a_op, b_op, y7[kind], grid=96, cta_group=1, timeout_ms=TMO, sync=False,
                                                stream=s_pull)
                         s_pull.synchronize()
-                    p, gw = _w(pv), _w(gv)
-                    checks[f"k7_{kind}_words"] &= p[0] == 0 and p[3] == n_panels and gw[0] == 0
+                    p, gw = ops.parse_read_records(pv), L.decode(gv)
+                    checks[f"k7_{kind}_words"] &= p["status"] == "OK" and p["done"] == n_panels and gw["status"] == "OK"
                     if keep:
-                        res["k7_4096^3_panels"][kind].append((gw[2] - p[1]) / 1e3)
+                        res["k7_4096^3_panels"][kind].append((gw["t_end_ns"] - p["t_start_ns"]) / 1e3)
             finally:
                 ctx.engine_stop()
             for kind in ("on_arrival", "after_pull"):       # the engine is gone: full-device work is safe again
