@@ -28,13 +28,18 @@
 //     NaN   amax is an fmaxf reduction, which drops NaN: a NaN stays in its own element, its neighbours quantise
 //           as if it were absent (an all-NaN block gets scale byte 0 and NaN codes)
 //     +-Inf e clamps to 127 (scale byte 254) and 2^-127 is 0.0 here: the Inf becomes NaN, its neighbours +-0
-//           (a finite sum that overflows fp32 in the reduce is such an Inf)
+//           (a finite sum that overflows fp32 in a reduce without error feedback is such an Inf)
 // Decode: scale byte 0x00 is 2^-127 (the OCP MX value, fp32 0x00400000), as in the block-scaled GEMM; 0xFF is Inf.
 // Error feedback (K3 and the reduce with a residual, EF = true): an fp32 residual of n_elems, read and written in place
 // by the thread that quantises the element.  K3 quantises v = x + r_in, the reduce v = (its sum) + r_in, the residual
 // added last; then r_out = v - d, d = code * ue8m0(scale byte) as the decoders make it, exact in fp32 wherever v and d
-// are finite (|d| <= 2|v|, same sign: Sterbenz), and 0 wherever either is not (NaN, a block holding Inf, an overflowing
-// sum), so one bad step cannot poison the residual for good.
+// are finite (|d| <= 2|v|, same sign: Sterbenz), and 0 wherever either is not (NaN, a block holding Inf), so one bad
+// step cannot poison the residual for good.  Every add of an EF kernel (K3's x + r_in; the reduce's addend + d0, + d1
+// and + r_in) saturates (ef_add): finite operands whose sum overflows give +-FLT_MAX instead of +-Inf.  The e = 120
+// saturation leaves up to FLT_MAX - 240 * 2^120 in the residual, and without this the next call's x + r_in, or a later
+// hop's sum of the records it enlarged, would overflow and turn a finite input into NaN.  So with error feedback finite
+// inputs always give finite records and residuals, and |r_out| <= FLT_MAX - 240 * 2^120.  A NaN or Inf operand, and a
+// decode that overflows (code 448 under scale byte 254), still propagate as above.
 //
 // No counterpart in the reference (it moves no payload: SURVEY.md section 3.2).
 #include <cuda_bf16.h>
@@ -162,6 +167,13 @@ __device__ __forceinline__ void st_bf16x32(__nv_bfloat16* dst, const float (&x)[
   st256_cs(dst + 16, o + 8);
 }
 
+// Error feedback's fp32 add: round to nearest, but a sum of finite operands that overflows is +-FLT_MAX, which is what
+// round-toward-zero gives there; with a NaN or Inf operand both give the same NaN or Inf.
+__device__ __forceinline__ float ef_add(float a, float b) {
+  const float s = __fadd_rn(a, b);
+  return isinf(s) ? __fadd_rz(a, b) : s;
+}
+
 // Error feedback after quantize_block32: v[i] becomes r_out = v - d, d = the block's decode as every decoder makes it
 // (mx_decode_block32).  The difference is exact where v and d are finite, and non-finite exactly where one of them is
 // not: then r_out = 0.
@@ -196,7 +208,7 @@ __device__ __forceinline__ void pack_group(const PackArgs& a, uint64_t first_til
     widen_bf16x32(w, x);
     if constexpr (EF) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) x[i] = __fadd_rn(x[i], __uint_as_float(rv[g][i]));
+      for (int i = 0; i < 32; ++i) x[i] = ef_add(x[i], __uint_as_float(rv[g][i]));
     }
     uint32_t q[8];
     const uint32_t scale = quantize_block32(x, q);
@@ -552,12 +564,14 @@ __device__ __forceinline__ void reduce_step(const ReduceArgs& a, uint64_t T0, ui
 #pragma unroll
     for (int s = 0; s < PMAX; ++s) {
       if (s < (int)a.n_src) {
-        mx_decode_block32(qv[g][s], e[g][s], [&](int i, float d) { x[i] = (!LOCAL && s == 0) ? d : __fadd_rn(x[i], d); });
+        mx_decode_block32(qv[g][s], e[g][s], [&](int i, float d) {
+          x[i] = (!LOCAL && s == 0) ? d : EF ? ef_add(x[i], d) : __fadd_rn(x[i], d);
+        });
       }
     }
     if constexpr (EF) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) x[i] = __fadd_rn(x[i], __uint_as_float(rv[g][i]));
+      for (int i = 0; i < 32; ++i) x[i] = ef_add(x[i], __uint_as_float(rv[g][i]));
     }
     if (a.out) st_bf16x32(a.out + block_off(T), x);
     if (a.out_rec) {

@@ -74,8 +74,9 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     ``direct``: ``staging_mr`` is the *peer's* buffer registered with this context (NVLink-mapped, ``ctx.reg_mr(tensor_on_the_peer)``):
     the kernel's own stores deliver the records and each one is announced by a zero-length RDMA_WRITE_IMM (needs ``with_imm``).
     ``residual``: error feedback, an fp32 CUDA tensor of ``src.numel()`` values (contiguous, 32-byte aligned) read and
-    written in place: the kernel quantises ``src + residual`` and leaves there what the records lost, ``v - decode``
-    (0 where either is not finite).  :func:`ref_pack_fp8` reproduces both bit for bit."""
+    written in place: the kernel quantises ``v = src + residual`` and leaves there what the records lost, ``v - decode``
+    (0 where either is not finite).  The add saturates: where finite operands overflow fp32, ``v`` is +-FLT_MAX, so
+    finite inputs always give finite records and residuals.  :func:`ref_pack_fp8` reproduces both bit for bit."""
     if direct and not (with_imm and qp is not None and dst_mr is not None):
         raise ValueError("direct mode announces records with RDMA_WRITE_IMM: pass qp, dst_mr and with_imm=True")
     assert src.dtype == torch.bfloat16 and src.is_contiguous()
@@ -173,6 +174,9 @@ def parse_unpack(view) -> dict:
 #   * decoding, scale byte 0x00 is 2^-127 (the OCP MX value, an fp32 denormal) and 0xFF is 2^128 == Inf.
 #   * at e = 120, the one exponent whose codes 248 and 256 would decode past fp32 max (to 2^128 = Inf), a scaled value
 #     above 240 in magnitude saturates to +-240, so every finite input decodes finite (NaN is kept).
+#   * error feedback (``residual=``) adds with _ef_add: finite operands whose fp32 sum overflows give +-FLT_MAX, not
+#     +-Inf, so that what the e = 120 saturation leaves in a residual (up to FLT_MAX - 240 * 2^120) cannot overflow the
+#     next add; NaN and Inf operands propagate.  Without a residual an overflowing sum is Inf.
 def _scale_exponent(amax: torch.Tensor) -> torch.Tensor:
     """e = smallest integer with amax / 2^e <= 448, clamped to [-127, 127], computed on the fp32 bit pattern of
     amax * (1/448) exactly as the kernels do (no log2 rounding): a value at or below 2^-127 (fp32 0x00400000) gives
@@ -219,6 +223,17 @@ def _quantized_records(x: torch.Tensor, chunk_elems: int) -> torch.Tensor:
     return out.reshape(-1)
 
 
+FLT_MAX = torch.finfo(torch.float32).max
+
+
+def _ef_add(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """Error feedback's fp32 add (``ef_add`` in pack_fp8.cu): ``a + b`` rounded to nearest, except that finite operands
+    whose sum overflows give +-FLT_MAX with the sign of the sum.  A NaN or Inf operand propagates as in ``a + b``."""
+    s = a + b
+    sat = torch.isinf(s) & torch.isfinite(a) & torch.isfinite(b)
+    return torch.where(sat, torch.copysign(torch.full_like(s, FLT_MAX), s), s)
+
+
 def _ef_residual(v: torch.Tensor, records: torch.Tensor, chunk_elems: int) -> torch.Tensor:
     """The residual error feedback keeps: ``v - d`` with ``d`` the decode of ``v``'s records, and 0 wherever that is
     not finite (``v`` or ``d`` is not).  For finite ``v`` and ``d`` the difference is exact in fp32, so ``d + r == v``."""
@@ -229,11 +244,11 @@ def _ef_residual(v: torch.Tensor, records: torch.Tensor, chunk_elems: int) -> to
 
 def ref_pack_fp8(src: torch.Tensor, chunk_elems: int, residual=None):
     """Reference chunk records (uint8) for a bf16 tensor; runs on CPU or GPU.  With ``residual`` (fp32, ``src.numel()``)
-    it quantises ``src + residual`` (one fp32 add) and returns ``(records, new residual)``, as
-    :func:`pack_fp8_write` does with ``residual=``."""
+    it quantises ``src + residual`` (one saturating fp32 add, :func:`_ef_add`) and returns ``(records, new residual)``,
+    as :func:`pack_fp8_write` does with ``residual=``."""
     if residual is None:
         return _quantized_records(src.float(), chunk_elems)
-    v = src.reshape(-1).float() + residual.reshape(-1).float().to(src.device)
+    v = _ef_add(src.reshape(-1).float(), residual.reshape(-1).float().to(src.device))
     recs = _quantized_records(v, chunk_elems)
     return recs, _ef_residual(v, recs, chunk_elems)
 
@@ -255,7 +270,9 @@ def _decode_records(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
 def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems: int, local=None, residual=None):
     """Reference of :func:`reduce_fp8`; runs on CPU or GPU.  Returns (bf16 sum, K3 records of the sum), and with
     ``residual`` (fp32, ``n_elems``) ``(bf16, records, new residual)``: the residual is added to the sum last, one fp32
-    add, and the bf16 output and the records both hold that value.
+    add, and the bf16 output and the records both hold that value.  With a residual every add saturates
+    (:func:`_ef_add`): finite operands whose sum overflows give +-FLT_MAX, so finite records and a finite addend give
+    finite records and residuals.
 
     The sum starts from ``local`` (bf16, exact in fp32) when given, else from source 0, and adds the other sources in
     source order, one fp32 add each: only the adds round.  The records quantise that fp32 sum with the rule of every
@@ -266,11 +283,12 @@ def ref_reduce_fp8(records: torch.Tensor, n_src: int, n_elems: int, chunk_elems:
         acc, first = local.reshape(-1).float().to(d.device), 0
     else:
         acc, first = d[0], 1
+    add = torch.add if residual is None else _ef_add
     for s in range(first, n_src):
-        acc = acc + d[s]
+        acc = add(acc, d[s])
     if residual is None:
         return acc.to(torch.bfloat16), _quantized_records(acc, chunk_elems)
-    acc = acc + residual.reshape(-1).float().to(acc.device)
+    acc = _ef_add(acc, residual.reshape(-1).float().to(acc.device))
     recs = _quantized_records(acc, chunk_elems)
     return acc.to(torch.bfloat16), recs, _ef_residual(acc, recs, chunk_elems)
 
@@ -282,7 +300,8 @@ def ref_allreduce_fp8(xs, chunk_elems: int, residuals=None):
     ``residuals``: the N ranks' fp32 error-feedback residuals of n elements each (``error_feedback=True``); then returns
     ``(out, new residuals)``.  Rank q quantises every shard once -- shard q in its pack, shard (q-1-k) mod N in reduce hop
     k -- and shard s of its residual is the error it made there: the pack and each hop quantise ``value + residual`` and
-    keep what the records lost (:func:`ref_pack_fp8`, :func:`ref_reduce_fp8`).
+    keep what the records lost (:func:`ref_pack_fp8`, :func:`ref_reduce_fp8`).  Every add of those steps saturates at
+    +-FLT_MAX, so finite inputs give a finite output and finite residuals on every run.
 
     Shard s (elements ``[s * n / N, (s + 1) * n / N)``) starts as ``ref_pack_fp8(xs[s])`` on rank s and is reduced with
     ``xs[s + 1], ..., xs[s - 1]`` (indices mod N) in ring order, one :func:`ref_reduce_fp8` hop each (the addend first,
@@ -372,6 +391,9 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
     ``residual``: error feedback, an fp32 CUDA tensor of ``n_elems`` (contiguous, 32-byte aligned) read and written in
     place.  It is added to the sum last, one fp32 add; ``out`` and the records hold that value, and the residual then
     holds what the records lost (0 where the value or its decode is not finite), as :func:`ref_reduce_fp8` computes it.
+    With a residual every add (the addend's, each source's and the residual's) saturates: finite operands whose sum
+    overflows give +-FLT_MAX, so finite inputs give finite records and residuals.  ``out`` is still that value rounded
+    to bf16, which is +-Inf above bf16's largest value.
     It needs ``out_mr``, and P = 1, or P = 2 with ``local`` (the variants a ring hop uses).
 
     Returns a :class:`ReduceResult`, or ``(result view, stream)`` with ``sync=False`` (decode with :func:`parse_reduce`)."""

@@ -23,7 +23,9 @@ from hop to hop because every posting launch waits for its flush.  DESIGN.md 3.4
 Error feedback (``error_feedback=True``): rank q quantises every shard exactly once per run -- shard q in the pack and
 shard (q-1-k) mod N in reduce hop k -- so one fp32 residual of n elements holds, in shard s, the error rank q made on
 shard s.  The pack and each hop quantise ``value + residual`` and write back what the records lost, in the same pass;
-summed over runs the output then equals the exact sum up to the last residual.  Nothing on the wire changes.
+summed over runs the output then equals the exact sum up to the last residual, while no add saturates.  Every add
+of those steps saturates at +-FLT_MAX, so finite inputs give a finite output and finite residuals on every run.
+Nothing on the wire changes.
 """
 from __future__ import annotations
 
@@ -127,7 +129,9 @@ class RingAllreduceFp8:
     ``error_feedback``: carry this rank's quantisation error from run to run in ``residual`` (fp32, ``n_elems``, zero at
     first), so that the bias of the fp8 rounding does not accumulate over the steps of a training loop.  ``residual`` is
     a public tensor: copy it out and back in between runs to checkpoint it, and :meth:`reset_residual` zeroes it.  After
-    a run that did not end OK it is undefined, as ``out`` is; reset it before the next run."""
+    a run that did not end OK it is undefined, as ``out`` is; reset it before the next run.  With error feedback every
+    fp32 add of the pack and the hops saturates at +-FLT_MAX, so finite inputs always give a finite output and a finite
+    residual, also at the top of the range (``ops.ref_allreduce_fp8`` with ``residuals=``)."""
 
     def __init__(self, ctx, n_elems: int, chunk_elems: int, rank: int, world: int, *, grid: int = 0,
                  timeout_ms: int = 2000, signal_every: int = 1, engine_ctas: int = 16, error_feedback: bool = False):

@@ -1,7 +1,8 @@
 """Error feedback in the fp8 pack, reduce and ring references, on the CPU.
 
 * Exactness: wherever the quantised value v is finite, ``decode(records) + r_out == v`` bit for bit, and ``r_out == 0``
-  wherever it is not -- on spread payloads and on the edge payload of test_ring_fp8_references.py (NaN, Inf, an
+  wherever it is not.  v is made with ``ef_add``, this file's saturating fp32 add (finite operands whose sum overflows
+  give +-FLT_MAX), which shares nothing with ``ops.pack``'s -- on spread payloads and on the edge payload of test_ring_fp8_references.py (NaN, Inf, an
   overflowing sum, the 448 and e = 120 boundaries, bf16 subnormals, bf16 max).  ``decode`` is that file's independent
   decoder, not ``ops.pack``'s.
 * A zero residual changes nothing but the sign of zero codes (-0 + 0 = +0).
@@ -23,6 +24,20 @@ def _f32_bits(t):
     return np.asarray(t, dtype=np.float32).view(np.uint32)
 
 
+FLT_MAX = float(np.finfo(np.float32).max)
+
+
+def ef_add(a, b):
+    """Error feedback's fp32 add: the exact sum (in fp64, which rounds to fp32 correctly for one add of fp32 operands)
+    clamped to [-FLT_MAX, FLT_MAX] when both operands are finite, then rounded to fp32.  A NaN or Inf operand
+    propagates as in an ordinary add."""
+    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
+    with np.errstate(over="ignore", invalid="ignore"):
+        s = a.astype(np.float64) + b.astype(np.float64)
+        s = np.where(np.isfinite(a) & np.isfinite(b), np.clip(s, -FLT_MAX, FLT_MAX), s)
+        return s.astype(np.float32)
+
+
 def _records_np(recs, n, chunk):
     """(codes [n / 32, 32], scale bytes [n / 32]) of K3 records."""
     r = recs.numpy().reshape(n // chunk, -1)
@@ -30,13 +45,18 @@ def _records_np(recs, n, chunk):
 
 
 def _check_identity(v, recs, r_out, chunk, label):
-    """decode(records) + r_out == v bit for bit where v is finite; r_out == 0 (+0) where it is not."""
+    """decode(records) + r_out == v bit for bit where v is finite; r_out == 0 (+0) where it is not.  A label that
+    starts with "spread" is a finite payload, and v must then be finite everywhere: with error feedback every add
+    saturates, so finite operands never make a non-finite v.  Any other payload must hold a non-finite v to check."""
     v = np.asarray(v, dtype=np.float32).reshape(-1)
     codes, sc = _records_np(recs, v.size, chunk)
     d = decode(codes, sc).reshape(-1)
     r = r_out.numpy().reshape(-1)
     fin = np.isfinite(v)
-    assert (~fin).any() or label.startswith("spread"), f"{label}: the payload has no non-finite value to check"
+    if label.startswith("spread"):
+        assert fin.all(), f"{label}: a finite payload gave a non-finite value"
+    else:
+        assert (~fin).any(), f"{label}: the payload has no non-finite value to check"
     with np.errstate(over="ignore", invalid="ignore"):
         back = d + r
     bad = np.flatnonzero(fin & (_f32_bits(back) != _f32_bits(v)))
@@ -68,18 +88,32 @@ def test_pack_residual_identity(kind):
         if kind == "edge":                                   # residuals that push blocks over the top and back
             r_in.view(-1, 32)[::97, 1] = 3.0e38
             r_in.view(-1, 32)[::89, 2] = float("nan")
+            xf = x.float()                                   # and ones whose sum with a top-of-range x overflows fp32
+            top = torch.isfinite(xf) & (xf.abs() >= 1e38)
+            r_in[top] = torch.copysign(torch.tensor(3.0e38), xf[top])
         recs, r_out = ops.ref_pack_fp8(x, CHUNK, residual=r_in)
-        with np.errstate(over="ignore", invalid="ignore"):
-            v = x.float().numpy() + r_in.numpy()
-        assert torch.equal(recs, ops.ref_pack_fp8(torch.from_numpy(v), CHUNK)), "the records quantise x + r_in"
+        # the records quantise x + r_in added with saturation: where both are finite and the sum overflows fp32 (bf16
+        # max plus 3e38), v is +-FLT_MAX, not +-Inf
+        v = ef_add(x.float().numpy(), r_in.numpy())
+        if kind == "edge":
+            with np.errstate(over="ignore", invalid="ignore"):
+                plain = x.float().numpy() + r_in.numpy()
+            assert (np.isinf(plain) & (np.abs(v) == FLT_MAX)).any(), "no add saturated: the rule is not exercised"
+        assert torch.equal(recs, ops.ref_pack_fp8(torch.from_numpy(v), CHUNK)), "the records quantise ef_add(x, r_in)"
         _check_identity(v, recs, r_out, CHUNK, f"{kind} pack rank {q}")
 
 
-@pytest.mark.parametrize("kind", ["spread", "edge"])
-@pytest.mark.parametrize("n_src,with_local", [(1, True), (1, False), (2, True)])
+# With an addend, the edge payload's "overflow" kind makes the addend's sum overflow fp32, and error feedback saturates
+# that add at +-FLT_MAX: those cases are "edge_saturating".  At P = 1 without the addend nothing saturates.
+REDUCE_IDENTITY_CASES = [(1, True, "spread"), (1, True, "edge_saturating"), (1, False, "spread"), (1, False, "edge"),
+                         (2, True, "spread"), (2, True, "edge_saturating")]
+
+
+@pytest.mark.parametrize("n_src,with_local,kind", REDUCE_IDENTITY_CASES)
 def test_reduce_residual_identity(kind, n_src, with_local):
-    """The residual is added last, after the addend and every source; the bf16 output is that value, rounded."""
-    xs = dict(_payloads())[kind]
+    """The residual is added last, after the addend and every source; the bf16 output is that value, rounded.  Every
+    add saturates (``ef_add``): where finite operands overflow fp32, v is +-FLT_MAX and quantises finite."""
+    xs = dict(_payloads())[kind.removesuffix("_saturating")]
     n = xs[0].numel()
     recs = torch.cat([ops.ref_pack_fp8(xs[s], CHUNK) for s in range(n_src)])
     local = xs[2] if with_local else None
@@ -90,8 +124,11 @@ def test_reduce_residual_identity(kind, n_src, with_local):
         dec = [decode(c, sc).reshape(-1) for c, sc in codes]
         v = local.float().numpy() if with_local else dec[0]
         for d in (dec if with_local else dec[1:]):
-            v = v + d
-        v = v + r_in.numpy()
+            v = ef_add(v, d)
+        v = ef_add(v, r_in.numpy())
+    saturated = np.abs(v) == np.float32(FLT_MAX)
+    assert saturated.any() == kind.endswith("_saturating"), "saturation where the case does not expect it, or none"
+    assert np.isfinite(decode(*_records_np(out, n, CHUNK)).reshape(-1)[saturated]).all(), "a saturated value decoded non-finite"
     assert_bits_equal(y, bf16_rne_bits(v), "out is v rounded to bf16")
     _check_identity(v, out, r_out, CHUNK, f"{kind} reduce P={n_src} local={with_local}")
 
@@ -113,18 +150,22 @@ def test_identity_at_the_boundaries(v):
 
 
 # ------------------------------------------------------------------ a zero residual
-@pytest.mark.parametrize("kind", ["spread", "edge"])
+@pytest.mark.parametrize("kind", ["spread", "edge_saturating"])
 def test_zero_residual_changes_only_the_sign_of_zero(kind):
-    xs = dict(_payloads())[kind]
+    """Except where a sum of finite values overflows: without a residual it is Inf (its code NaN, its block's other
+    codes +-0); with one it saturates to +-FLT_MAX and its block quantises finite.  Those blocks (the edge payload's
+    "overflow" kind) are exempt, and their records with the residual must decode finite."""
+    xs = dict(_payloads())[kind.removesuffix("_saturating")]
     x = xs[0]
     n = x.numel()
     zero = torch.zeros(n)
 
-    def same_up_to_zero_sign(a, b, what):
+    def same_up_to_zero_sign(a, b, what, exempt=None):
         ca, sa = _records_np(a, n, CHUNK)
         cb, sb = _records_np(b, n, CHUNK)
-        assert np.array_equal(sa, sb), f"{what}: scale bytes differ"
-        diff = ca != cb
+        keep = np.ones(len(sa), bool) if exempt is None else ~exempt
+        assert np.array_equal(sa[keep], sb[keep]), f"{what}: scale bytes differ"
+        diff = (ca != cb) & keep[:, None]
         assert np.all((ca[diff] & 0x7F) == 0) and np.all((cb[diff] & 0x7F) == 0), f"{what}: a nonzero code differs"
 
     recs, _ = ops.ref_pack_fp8(x, CHUNK, residual=zero)
@@ -132,7 +173,14 @@ def test_zero_residual_changes_only_the_sign_of_zero(kind):
     src = ops.ref_pack_fp8(xs[1], CHUNK)
     y0, rec0 = ops.ref_reduce_fp8(src, 1, n, CHUNK, local=xs[2])
     y1, rec1, _ = ops.ref_reduce_fp8(src, 1, n, CHUNK, local=xs[2], residual=zero)
-    same_up_to_zero_sign(rec1, rec0, "reduce")
+    loc, dec = xs[2].float().numpy(), decode(*_records_np(src, n, CHUNK)).reshape(-1)
+    with np.errstate(over="ignore", invalid="ignore"):
+        over = np.isinf(loc + dec) & np.isfinite(loc) & np.isfinite(dec)
+    exempt = over.reshape(-1, 32).any(axis=1)
+    assert exempt.any() == (kind != "spread"), "the edge payload's overflow kind must be exercised, spread must not"
+    same_up_to_zero_sign(rec1, rec0, "reduce", exempt)
+    d1 = decode(*_records_np(rec1, n, CHUNK))
+    assert np.isfinite(d1[exempt]).all(), "a saturated block decoded non-finite"
     assert torch.equal(y0.float(), y1.float()) or torch.equal(torch.isnan(y0), torch.isnan(y1))
 
 
@@ -140,14 +188,15 @@ def test_zero_residual_changes_only_the_sign_of_zero(kind):
 def ring_blocks_ef(xs, rs, trace=None):
     """The model's ring of one shard with error feedback.  ``xs[h]`` / ``rs[h]``: [B, 32] fp32, the input and the
     residual of the rank that quantises at hop h.  Returns (bf16 bits of the output, the new residuals per hop).
-    ``trace`` receives per hop (the rounded addend sum or None, the quantised value v)."""
+    ``trace`` receives per hop (the rounded addend sum or None, the quantised value v).  Both adds saturate
+    (``ef_add``)."""
     xs, rs = np.asarray(xs, np.float32), np.asarray(rs, np.float32)
     new = np.empty_like(rs)
     codes = sc = None
     for h in range(len(xs)):
         with np.errstate(over="ignore", invalid="ignore"):
-            a = xs[h] if h == 0 else xs[h] + decode(codes, sc)
-            v = a + rs[h]
+            a = xs[h] if h == 0 else ef_add(xs[h], decode(codes, sc))
+            v = ef_add(a, rs[h])
             codes, sc = encode(v)
             r = v - decode(codes, sc)
         new[h] = np.where(np.isfinite(r), r, np.float32(0))

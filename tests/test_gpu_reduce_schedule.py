@@ -36,29 +36,33 @@ pytestmark = pytest.mark.gpu
 TILE = P.TILE_ELEMS
 # (G tiles per step, PMAX sources, addend): pack_fp8.cu RN_REDUCE_VARIANTS, the entries with EF = false
 VARIANTS = ((4, 1, False), (4, 2, False), (2, 4, False), (1, 8, False), (2, 2, True), (1, 8, True))
+# ... and the entries with EF = true (a residual): P = 1 without the addend, P <= 2 with it, one tile per step
+EF_VARIANTS = ((1, 1, False), (1, 2, True))
 
 
 # ------------------------------------------------------------------ schedule model
-def variant_of(n_src, local):
-    """The variant rn_k_reduce_fp8 launches for P = ``n_src`` sources, with or without the addend."""
+def variant_of(n_src, local, ef=False):
+    """The variant rn_k_reduce_fp8 launches for P = ``n_src`` sources, with or without the addend, and with or without
+    a residual (``ef``; the host refuses other P with one)."""
     if local:
         pmax = 2 if n_src <= 2 else 8
     else:
         pmax = 1 if n_src == 1 else 2 if n_src <= 2 else 4 if n_src <= 4 else 8
-    return next(v for v in VARIANTS if v[1:] == (pmax, bool(local)))
+    return next(v for v in (EF_VARIANTS if ef else VARIANTS) if v[1:] == (pmax, bool(local)))
 
 
 class ReduceSchedule:
     """One launch of ``reduce_fp8``: ``steps[b]`` lists CTA b's steps in order, each as the list of its tiles in the
     flattened record-major order (tile T belongs to record T // tpc)."""
 
-    def __init__(self, chunk, n_rec, n_src, local=False, grid=0, ready=False, sms=H100_SMS):
+    def __init__(self, chunk, n_rec, n_src, local=False, grid=0, ready=False, sms=H100_SMS, ef=False):
         self.tpc, self.n_rec, self.n_src = chunk // TILE, n_rec, n_src
-        self.variant = variant_of(n_src, local)
+        self.variant = variant_of(n_src, local, ef)
         self.G, self.pmax = self.variant[0], self.variant[1]
         self.total = n_rec * self.tpc
         if grid <= 0:
             grid = sms if ready else 4 * sms
+        self.requested = grid
         self.grid = min(grid, self.total)
         G, g_, total = self.G, self.grid, self.total
         self.steps = [[[T0 + g * g_ for g in range(G) if T0 + g * g_ < total] for T0 in range(b, total, g_ * G)]

@@ -154,6 +154,22 @@ def test_reduce_schedule_variant_rule_and_grid_clamp():
     assert ReduceSchedule(8192, 5, 2, ready=True, grid=3).grid == 3
 
 
+def test_reduce_schedule_variants_are_the_kernels():
+    """VARIANTS and EF_VARIANTS are pack_fp8.cu's RN_REDUCE_VARIANTS (G, PMAX, LOCAL, EF), split by EF; a residual
+    takes P = 1 without the addend and P <= 2 with it, one tile per step."""
+    import re
+    from pathlib import Path
+    from test_gpu_reduce_schedule import EF_VARIANTS
+    src = (Path(__file__).resolve().parent.parent / "rocnrdma_b200" / "csrc" / "kernels" / "pack_fp8.cu").read_text()
+    body = re.search(r"#define RN_REDUCE_VARIANTS\(X\)(.*?)\n\n", src, re.S).group(1)
+    xs = [(int(g), int(p), l == "true", e == "true")
+          for g, p, l, e in re.findall(r"X\((\d+), (\d+), (true|false), (true|false)\)", body)]
+    assert {x[:3] for x in xs if not x[3]} == set(VARIANTS) and {x[:3] for x in xs if x[3]} == set(EF_VARIANTS)
+    assert variant_of(1, False, ef=True) == (1, 1, False)
+    assert variant_of(1, True, ef=True) == variant_of(2, True, ef=True) == (1, 2, True)
+    assert ReduceSchedule(3 * 8192, 7, 2, local=True, ready=True, ef=True).G == 1
+
+
 def test_reduce_schedule_hand_counted_walks():
     # tpc 3, grid 1, G 4: one CTA, four consecutive tiles per step
     s = ReduceSchedule(24576, 5, 2, grid=1)
