@@ -46,6 +46,7 @@ struct alignas(1024) Smem {
   uint8_t b[STAGES][B_STAGE];
   uint8_t sfa[STAGES][4][BM];                                  // scale bytes of the stage's four MX blocks, [block][row]
   uint8_t sfb[STAGES][4][BN];
+  uint32_t range[STAGES][4];                                   // per loader warp: bytes [min A, 255 - max A, min B, 255 - max B]
   alignas(8) uint64_t full[STAGES], empty[STAGES];
   volatile int abort;
 };
@@ -109,6 +110,71 @@ __device__ __forceinline__ uint32_t load_scales(const uint8_t* base, uint64_t re
   return v;
 }
 
+// [min, 255 - max] of the four scale bytes in w, reduced over the warp, in the low two bytes
+__device__ __forceinline__ uint32_t warp_byte_range(uint32_t w) {
+  const uint32_t lo = __vminu4(w, w >> 16), hi = __vmaxu4(w, w >> 16);
+  return __reduce_min_sync(0xffffffffu, min(lo & 0xff, (lo >> 8) & 0xff)) |
+         (255 - __reduce_max_sync(0xffffffffu, max(hi & 0xff, (hi >> 8) & 0xff))) << 8;
+}
+
+// acc += p * 2^(ea + eb) for the 64 accumulators of one MX block, with one rounding each (ea, eb: the scale bytes of the
+// accumulator's row and column, minus 127; byte 0 is 2^-127, byte 0xFF Inf).
+//   kInRange: every byte pair of the stage has ea + eb in [-149, 127] and no byte 0xFF, so the scale product sa * sb is
+//             exact in fp32 and fmaf(p, sa * sb, acc) is that one rounding.
+//   otherwise sa * sb may be Inf (0 * Inf = NaN where p = 0) or 0 while p * 2^(ea + eb) is an ordinary number.  Every p is
+//             a multiple of 2^-18 (a sum of e4m3 products) below 2^23 in magnitude, so p * lo with lo = min(sa, sb, 2^74)
+//             is exact and finite, and fmaf(p * lo, hi = max(sa, sb), acc) rounds once.  lo is capped so that p * lo
+//             never overflows: where the cap applies both scales exceed 2^74 and the true contribution, at least
+//             2^-18 * 2^150 in magnitude, rounds to +-Inf as the capped one does, while an accumulator that is already
+//             +-Inf stays so.  A byte 0xFF makes hi Inf: +-Inf, or NaN for p = 0.
+template <bool kInRange>
+__device__ __forceinline__ void mx_scale_add(float (&acc)[64], const float* p, const uint8_t* sfa, const uint8_t* sfb, uint32_t rl0,
+                                             uint32_t lane) {
+  const float sa0 = ue8m0(sfa[rl0]), sa1 = ue8m0(sfa[rl0 + 8]);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const uint32_t col = 8 * j + 2 * (lane & 3);
+    const uint16_t sb = *reinterpret_cast<const uint16_t*>(&sfb[col]);
+    const float sb0 = ue8m0(sb & 0xff), sb1 = ue8m0(sb >> 8);
+    const float cb0 = fminf(sb0, 0x1p74f), cb1 = fminf(sb1, 0x1p74f);      // min(sa, sb, 2^74) = min(sa, cb)
+    if constexpr (kInRange) {
+      acc[4 * j] = fmaf(p[4 * j], sa0 * sb0, acc[4 * j]);
+      acc[4 * j + 1] = fmaf(p[4 * j + 1], sa0 * sb1, acc[4 * j + 1]);
+      acc[4 * j + 2] = fmaf(p[4 * j + 2], sa1 * sb0, acc[4 * j + 2]);
+      acc[4 * j + 3] = fmaf(p[4 * j + 3], sa1 * sb1, acc[4 * j + 3]);
+    } else {
+      acc[4 * j] = fmaf(__fmul_rn(p[4 * j], fminf(sa0, cb0)), fmaxf(sa0, sb0), acc[4 * j]);
+      acc[4 * j + 1] = fmaf(__fmul_rn(p[4 * j + 1], fminf(sa0, cb1)), fmaxf(sa0, sb1), acc[4 * j + 1]);
+      acc[4 * j + 2] = fmaf(__fmul_rn(p[4 * j + 2], fminf(sa1, cb0)), fmaxf(sa1, sb0), acc[4 * j + 2]);
+      acc[4 * j + 3] = fmaf(__fmul_rn(p[4 * j + 3], fminf(sa1, cb1)), fmaxf(sa1, sb1), acc[4 * j + 3]);
+    }
+  }
+}
+
+// One stage: four 32-deep e4m3 MMAs (block k + 1's runs while block k is scaled, two partial register sets) and their
+// scaling into acc.
+template <bool kInRange>
+__device__ __forceinline__ void mx_stage(float (&acc)[64], float (&p0)[64], float (&p1)[64], uint64_t da, uint64_t db,
+                                         const uint8_t (&sfa)[4][BM], const uint8_t (&sfb)[4][BN], uint32_t rl0, uint32_t lane) {
+  wg_fence();
+  wgmma_e4m3_n128(p0, da, db, 0u);
+  wg_commit();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    float* p = (k & 1) ? p1 : p0;
+    if (k < 3) {
+      wg_fence();
+      wgmma_e4m3_n128((k & 1) ? p0 : p1, da + (uint64_t)(2 * (k + 1)), db + (uint64_t)(2 * (k + 1)), 0u);
+      wg_commit();
+      wg_wait<1>();
+    } else {
+      wg_wait<0>();
+    }
+    reg_fence<64>(p);
+    mx_scale_add<kInRange>(acc, p, sfa[k], sfb[k], rl0, lane);
+  }
+}
+
 template <int CTAS>
 __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const MxArgs& g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -133,17 +199,18 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
     reg_dealloc<40>();
     const uint32_t t = threadIdx.x;
     uint32_t stage = 0, phase = 0;
-    for (uint32_t tile = unit; tile < n_tiles && !s.abort; tile += n_units) {
+    // every exit is decided per warp (a vote), so the lanes stay together for the warp's scale-range reduction
+    for (uint32_t tile = unit; tile < n_tiles && !__any_sync(0xffffffffu, s.abort); tile += n_units) {
       const uint32_t m_blk = (tile / n_blks) * CTAS + rank, n_blk = tile % n_blks;
       const uint32_t ar = m_blk * BM, br = n_blk * BN;                       // rows of a tile never straddle records
       // wait for the record that holds rows ar.. (the scales travel in it too).  A tile that starts at or past row M -- the
       // pair kernel's second CTA when ceil(M / 128) is odd -- reads only zero-filled rows and neutral scales: no record
       // holds them, so there is nothing to wait for (and no arrival word to read).
-      if (ar < g.M && !wait_record(g.a_ready, ar / g.a_rows_per_rec, g.ready_timeout_ns, &s.abort)) break;
+      if (ar < g.M && !__all_sync(0xffffffffu, wait_record(g.a_ready, ar / g.a_rows_per_rec, g.ready_timeout_ns, &s.abort))) break;
       for (uint32_t kb = 0; kb < k_blks; ++kb) {
         const uint32_t sa = load_scales(g.a_s, g.a_rec_stride, g.a_rows_per_rec, g.M, ks, ar + t, kb);
         const uint32_t sb = load_scales(g.b_s, g.b_rec_stride, g.b_rows_per_rec, g.N, ks, br + t, kb);
-        if (!mbar_wait(&s.abort, &s.empty[stage], phase ^ 1, kWaitNs)) goto loader_done;
+        if (!__all_sync(0xffffffffu, mbar_wait(&s.abort, &s.empty[stage], phase ^ 1, kWaitNs))) goto loader_done;
         if (t == 0) {
           mbar_expect_tx(&s.full[stage], A_STAGE + B_STAGE);
           tma_load_3d(s.a[stage], &tmap_a, &s.full[stage], (int)(kb * BK), (int)(ar % g.a_rows_per_rec), (int)(ar / g.a_rows_per_rec));
@@ -157,7 +224,9 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
         }
 #pragma unroll
         for (int k = 0; k < 4; ++k) { s.sfa[stage][k][t] = (uint8_t)(sa >> (8 * k)); s.sfb[stage][k][t] = (uint8_t)(sb >> (8 * k)); }
-        mbar_arrive(&s.full[stage]);                                           // release: the scale bytes before the arrival
+        const uint32_t rng = warp_byte_range(sa) | warp_byte_range(sb) << 16;
+        if (lane == 0) s.range[stage][warp] = rng;
+        mbar_arrive(&s.full[stage]);                                           // release: the scale bytes and range before the arrival
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
@@ -178,33 +247,13 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
       for (uint32_t kb = 0; kb < k_blks; ++kb) {
         if (named_sync_or(2 + wg, 128, !mbar_wait(&s.abort, &s.full[stage], phase, kWaitNs))) { ok = false; break; }
         const uint64_t da = wg_desc(s.a[stage] + wg * 64 * BK), db = wg_desc(s.b[stage]);
-        wg_fence();
-        wgmma_e4m3_n128(p0, da, db, 0u);
-        wg_commit();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float* p = (k & 1) ? p1 : p0;
-          if (k < 3) {
-            wg_fence();
-            wgmma_e4m3_n128((k & 1) ? p0 : p1, da + (uint64_t)(2 * (k + 1)), db + (uint64_t)(2 * (k + 1)), 0u);
-            wg_commit();
-            wg_wait<1>();
-          } else {
-            wg_wait<0>();
-          }
-          reg_fence<64>(p);
-          const float sa0 = ue8m0(s.sfa[stage][k][rl0]), sa1 = ue8m0(s.sfa[stage][k][rl0 + 8]);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const uint32_t col = 8 * j + 2 * (lane & 3);
-            const uint16_t sb = *reinterpret_cast<const uint16_t*>(&s.sfb[stage][k][col]);
-            const float sb0 = ue8m0(sb & 0xff), sb1 = ue8m0(sb >> 8);
-            acc[4 * j] = fmaf(p[4 * j], sa0 * sb0, acc[4 * j]);
-            acc[4 * j + 1] = fmaf(p[4 * j + 1], sa0 * sb1, acc[4 * j + 1]);
-            acc[4 * j + 2] = fmaf(p[4 * j + 2], sa1 * sb0, acc[4 * j + 2]);
-            acc[4 * j + 3] = fmaf(p[4 * j + 3], sa1 * sb1, acc[4 * j + 3]);
-          }
-        }
+        // the stage's scale-byte range, the same for the whole warpgroup: one uniform branch per stage between the two scalings
+        const uint4 rw = *reinterpret_cast<const uint4*>(s.range[stage]);
+        const uint32_t r = __vminu4(__vminu4(rw.x, rw.y), __vminu4(rw.z, rw.w));
+        const bool in_range = (r & 0xff) + ((r >> 16) & 0xff) >= 105 && ((r >> 8) & 0xff) + (r >> 24) >= 129 &&
+                              ((r >> 8) & 0xff) != 0 && (r >> 24) != 0;
+        if (in_range) mx_stage<true>(acc, p0, p1, da, db, s.sfa[stage], s.sfb[stage], rl0, lane);
+        else mx_stage<false>(acc, p0, p1, da, db, s.sfa[stage], s.sfb[stage], rl0, lane);
         // every warp of the warpgroup has read this stage's scale bytes (wgmma.wait_group orders only the warp's own MMAs,
         // and the loaders rewrite the scales the moment the stage is released)
         named_sync(2 + wg, 128);

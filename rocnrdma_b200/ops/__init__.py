@@ -6,4 +6,4 @@ from .pack import (pack_fp8_write, unpack_fp8, ref_pack_fp8, ref_unpack_fp8, rec
                    PackResult, reduce_fp8, ref_reduce_fp8, parse_reduce, ReduceResult, parse_unpack, ref_allreduce_fp8)
 from .launch import result_offset  # noqa: F401
 from .gemm import gemm_send, GemmResult, panel_record_bytes, ref_fp8_panels, dequant_fp8_panels  # noqa: F401
-from .gemm_mx import gemm_mxfp8, MxOperand, MxResult, quantize_mx, dequantize_mx  # noqa: F401
+from .gemm_mx import gemm_mxfp8, MxOperand, MxResult, quantize_mx, dequantize_mx, ref_gemm_mxfp8  # noqa: F401

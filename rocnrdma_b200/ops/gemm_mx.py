@@ -112,3 +112,60 @@ def dequantize_mx(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
     rows, K = q.shape
     v = q.view(torch.float8_e4m3fn).float().reshape(rows, K // BLOCK, BLOCK)
     return (v * ue8m0(s)[..., None]).reshape(rows, K)
+
+
+def _add_rn32(acc: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """fp32 ``acc`` + fp64 ``x`` rounded once to fp32 (what ``fmaf`` does with an exact product).  The fp64 sum is made
+    round-to-odd first (two-sum error, then a step to the odd neighbour when it is inexact), which the final round to
+    nearest-even fp32 cannot round a second time: 53 bits is more than 24 + 2."""
+    a = acc.double()
+    s = a + x
+    bb = s - a
+    err = (a - (s - bb)) + (x - bb)
+    even = (s.view(torch.int64) & 1) == 0
+    fix = torch.isfinite(s) & (err != 0) & even
+    s = torch.where(fix, torch.nextafter(s, torch.where(err > 0, torch.inf, -torch.inf).to(s)), s)
+    return s.float()
+
+
+def ref_gemm_mxfp8(a_q: torch.Tensor, a_s: torch.Tensor, b_q: torch.Tensor, b_s: torch.Tensor) -> torch.Tensor:
+    """Bit-exact reference of ``gemm_mxfp8``'s arithmetic over every pair of scale bytes: bf16 ``C[M, N]`` from e4m3
+    bytes ``a_q [M, K]`` / ``b_q [N, K]`` and UE8M0 scale bytes ``a_s [M, K/32]`` / ``b_s [N, K/32]``, computed in fp64 on
+    the operands' device, with each MX block added into an fp32 accumulator in k order with one rounding.
+
+    For every output:
+
+    * the MX blocks are taken in k order, into an fp32 accumulator that starts at +0;
+    * a block's partial ``p`` is the exact sum of its 32 e4m3 products (fp64 holds it exactly: products span
+      2^-18 .. 2^17.6; a NaN code makes it NaN; it is -0 only when every product is -0);
+    * its contribution is ``x = p * 2^(ea + eb)`` with ``ea``, ``eb`` the row's and column's scale bytes minus 127 (byte 0 is
+      2^-127, as in every decoder).  A byte 0xFF in either operand makes ``x = p * Inf``: +-Inf, or NaN where p = 0;
+    * ``acc = fl32(acc + x)``: one rounding of the exact sum per block, over the whole range of ``ea + eb`` (-254 .. 254);
+    * the output is ``acc`` rounded to nearest-even bf16.
+
+    The kernel follows this rule only where the tensor core forms ``p`` exactly.  Its internal accumulator width is not
+    measured (at least 11 bits, DESIGN.md), so a bit-for-bit comparison needs data whose block partials fit in 11
+    significant bits; elsewhere compare against a bound."""
+    M, K = a_q.shape
+    Nn = b_q.shape[0]
+    kb = K // BLOCK
+    assert b_q.shape[1] == K and tuple(a_s.shape) == (M, kb) and tuple(b_s.shape) == (Nn, kb)
+    A = a_q.view(torch.float8_e4m3fn).double().reshape(M, kb, BLOCK)
+    B = b_q.view(torch.float8_e4m3fn).double().reshape(Nn, kb, BLOCK)
+    ea, eb = a_s.to(torch.int32) - 127, b_s.to(torch.int32) - 127
+    a_inf, b_inf = a_s == 255, b_s == 255
+    # sign bits and nonzero indicators of the codes (a NaN code counts as nonzero: its partial is NaN anyway)
+    na, nb = ((a_q & 0x80) != 0).double().reshape(M, kb, BLOCK), ((b_q & 0x80) != 0).double().reshape(Nn, kb, BLOCK)
+    za, zb = ((a_q & 0x7F) != 0).double().reshape(M, kb, BLOCK), ((b_q & 0x7F) != 0).double().reshape(Nn, kb, BLOCK)
+    acc = torch.zeros(M, Nn, dtype=torch.float32, device=a_q.device)
+    for k in range(kb):
+        p = A[:, k] @ B[:, k].T
+        # IEEE sign of an exact zero sum: -0 only when all 32 products are -0 (zero, with signs that differ)
+        opposite = na[:, k] @ (1 - nb[:, k]).T + (1 - na[:, k]) @ nb[:, k].T
+        nonzero = za[:, k] @ zb[:, k].T
+        neg_zero = (opposite == BLOCK) & (nonzero == 0)
+        p = torch.where(p == 0, torch.where(neg_zero, -0.0, 0.0).to(p), p)
+        x = p * torch.exp2((ea[:, k, None] + eb[None, :, k]).double())
+        x = torch.where(a_inf[:, k, None] | b_inf[None, :, k], p * torch.inf, x)
+        acc = _add_rn32(acc, x)
+    return acc.to(torch.bfloat16)

@@ -336,15 +336,19 @@ def _mx_operand(kind, q, s):
 
 @pytest.mark.parametrize("cta_group", [1, 2])
 @pytest.mark.parametrize("kind,M,N,K", [("plain", 200, 136, 160), ("plain", 130, 72, 96), ("plain", 64, 300, 32), ("plain", 700, 520, 256),
-                                        ("panel", 300, 136, 160), ("panel", 130, 264, 224), ("chunk", 256, 200, 160), ("chunk", 384, 72, 96)])
+                                        ("panel", 300, 136, 160), ("panel", 130, 264, 224), ("chunk", 256, 200, 160), ("chunk", 384, 72, 96),
+                                        ("b_panel", 200, 300, 160), ("b_panel", 130, 264, 224), ("b_chunk", 96, 256, 160), ("b_chunk", 300, 384, 96)])
 def test_k7_exact_integer_gemm_rounds_to_nearest_even(ctx, kind, M, N, K, cta_group):
+    """kind: where A lives (plain, K4 panel records, K3 chunk records), or b_*: B in records (a ragged N: a short last
+    panel record) with A plain."""
     g = _gen(M + N + K + cta_group)
     aq, as_ = _mx_exact_operand(M, K, g)
     bq, bs = _mx_exact_operand(N, K, g)
     ref = _mx_exact_ref(aq, as_, bq, bs)
     pad = torch.full((M + 1, N), 7.0, device="cuda", dtype=torch.bfloat16)
     c = pad[:M]
-    r = ops.gemm_mxfp8(ctx, _mx_operand(kind, aq, as_), MX.MxOperand.from_tensors(bq, bs), c, cta_group=cta_group)
+    a_kind, b_kind = (kind, "plain") if not kind.startswith("b_") else ("plain", kind[2:])
+    r = ops.gemm_mxfp8(ctx, _mx_operand(a_kind, aq, as_), _mx_operand(b_kind, bq, bs), c, cta_group=cta_group)
     assert r.ok, r.status
     assert _bits_equal(c, ref), _mismatch(c, ref)
     assert torch.all(pad[M] == 7.0), "the epilogue wrote past the last row"
