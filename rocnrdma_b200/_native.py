@@ -132,10 +132,13 @@ _SIGS = {
     "rn_gemm_timeline": (i32, [C.POINTER(C.c_uint64)]),
     "rn_k_gemm_send": (i32, [u64, i32, u64, u64, u64, u32, u32, u32, u64, u64, u32, u64, u32, u32, u32, u32, u32, u32, u32, u64, u64, u64]),
     "rn_k_gemm_mxfp8": (i32, [u64, i32, u64, u64, u32, u64, u64, u64, u32, u64, u64, u32, u32, u32, u64, u32, u64, u64, u64]),
+    "rn_k_gemm_mxfp8_ordered": (i32, [u64, i32, u64, u64, u32, u64, u64, u64, u32, u64, u64, u32, u32, u32, u64, u32, u64, u64, u64,
+                                      u64]),
     "rn_k_shared_post_stress": (i32, [u64, u64, i32, u64, u32, u64, u32, u32, u64, u64, u64]),
     "rn_k_recv_consume": (i32, [u64, u64, u32, u32, u64, u64, u64, u64, u32, u32]),
     "rn_hca_enable_peer": (i32, [vp, i32]),
     "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64, u64, u64, u64, u32, u64, u32, u32, u32, u32]),
+    "rn_k_relay_records": (i32, [u64, u64, u64, u32, u32, u64, u64, u32, u64, u32, u64, u32, u32, u64, u64, u64]),
     "rn_k_reduce_fp8": (i32, [u64, i32, u64, u32, u64, u64, u64, u64, u32, u64, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64,
                               u32, u64]),
     "rn_k_rdma_stream": (i32, [u64, C.POINTER(u64), u32, u32, u64, u32, u64, u32, u64, u32, u32, u32, u32, u32, u64, u32, u64, u64, u32]),

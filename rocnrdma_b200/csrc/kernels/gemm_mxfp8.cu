@@ -17,7 +17,8 @@
 //                  shared memory (layout [MX block][row])
 //   warpgroups 1-2 each owns 64 rows of the tile: MMA, scaling, then bounds-checked bf16 stores from registers
 // gemm_mxfp8_kernel runs one CTA per tile; gemm_mxfp8_pair_kernel a 2-CTA cluster per 256 x 128 tile, each CTA loading
-// half of the B tile and multicasting it to both (half the B traffic per FLOP).
+// half of the B tile and multicasting it to both (half the B traffic per FLOP); gemm_mxfp8_ordered_kernel is the single-CTA
+// kernel walking A record by record in a given order (tile_coords).
 // No counterpart in the reference.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -175,8 +176,29 @@ __device__ __forceinline__ void mx_stage(float (&acc)[64], float (&p0)[64], floa
   }
 }
 
-template <int CTAS>
-__device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const MxArgs& g) {
+// Tile `tile` of a CTA's walk -> its 128-row block of A and 128-column block of B.
+//   row order (ORDERED = false): m-block tile / n_blks (of the pair kernel, the rank-th of the cluster's two), n-block tile % n_blks
+//   ORDERED: record by record in the order a_order gives, each record's bpr = rows_per_rec / 128 m-blocks in row order:
+//            rec = a_order[tile / (bpr * n_blks)], m-block rec * bpr + (tile % (bpr * n_blks)) / n_blks, n-block tile % n_blks.
+//            An entry past the last record is taken as n_rec: its tiles start at row M, read only zero-filled rows and
+//            neutral scales, and store nothing.
+// The loaders and the consumers walk with this one mapping.
+template <int CTAS, bool ORDERED>
+__device__ __forceinline__ void tile_coords(uint32_t tile, uint32_t n_blks, uint32_t rank, const int32_t* a_order, uint32_t bpr,
+                                            uint32_t n_rec, uint32_t& m_blk, uint32_t& n_blk) {
+  if constexpr (ORDERED) {
+    const uint32_t per_rec = bpr * n_blks;
+    const uint32_t rec = min((uint32_t)__ldg(a_order + tile / per_rec), n_rec);
+    m_blk = rec * bpr + (tile % per_rec) / n_blks;
+  } else {
+    m_blk = (tile / n_blks) * CTAS + rank;
+  }
+  n_blk = tile % n_blks;
+}
+
+template <int CTAS, bool ORDERED = false>
+__device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const MxArgs& g,
+                                        const int32_t* a_order = nullptr) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -185,6 +207,8 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
   const uint32_t m_tiles = (g.M + CTAS * BM - 1) / (CTAS * BM), n_blks = (g.N + BN - 1) / BN, k_blks = (g.K + BK - 1) / BK;
   const uint32_t n_tiles = m_tiles * n_blks, n_units = gridDim.x / CTAS, unit = blockIdx.x / CTAS;
   const uint32_t ks = g.K / 32;
+  // ORDERED: A is n_rec whole records of bpr 128-row blocks (the host checks M % rows_per_rec == 0, rows_per_rec % 128 == 0)
+  const uint32_t bpr = ORDERED ? g.a_rows_per_rec / BM : 0u, n_rec = ORDERED ? g.M / g.a_rows_per_rec : 0u;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) { mbar_init(&s.full[i], 1 + 128); mbar_init(&s.empty[i], 2 * CTAS); }
@@ -201,7 +225,8 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
     uint32_t stage = 0, phase = 0;
     // every exit is decided per warp (a vote), so the lanes stay together for the warp's scale-range reduction
     for (uint32_t tile = unit; tile < n_tiles && !__any_sync(0xffffffffu, s.abort); tile += n_units) {
-      const uint32_t m_blk = (tile / n_blks) * CTAS + rank, n_blk = tile % n_blks;
+      uint32_t m_blk, n_blk;
+      tile_coords<CTAS, ORDERED>(tile, n_blks, rank, a_order, bpr, n_rec, m_blk, n_blk);
       const uint32_t ar = m_blk * BM, br = n_blk * BN;                       // rows of a tile never straddle records
       // wait for the record that holds rows ar.. (the scales travel in it too).  A tile that starts at or past row M -- the
       // pair kernel's second CTA when ceil(M / 128) is odd -- reads only zero-filled rows and neutral scales: no record
@@ -240,7 +265,8 @@ __device__ __forceinline__ void mx_body(const CUtensorMap& tmap_a, const CUtenso
     uint32_t stage = 0, phase = 0;
     float acc[64], p0[64], p1[64];
     for (uint32_t tile = unit; tile < n_tiles; tile += n_units) {
-      const uint32_t m_blk = (tile / n_blks) * CTAS + rank, n_blk = tile % n_blks;
+      uint32_t m_blk, n_blk;
+      tile_coords<CTAS, ORDERED>(tile, n_blks, rank, a_order, bpr, n_rec, m_blk, n_blk);
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       bool ok = true;
@@ -298,6 +324,13 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
 gemm_mxfp8_pair_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ MxArgs g) {
   mx_body<2>(tmap_a, tmap_b, g);
 }
+// The single-CTA kernel walking A's records in the order a_order gives (tile_coords), so that a receiver multiplies the
+// records it holds first.  The pair kernel has no ordered walk.
+__global__ void __launch_bounds__(kThreads, 1) gemm_mxfp8_ordered_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                                                                         const __grid_constant__ CUtensorMap tmap_b,
+                                                                         const __grid_constant__ MxArgs g, const int32_t* a_order) {
+  mx_body<1, true>(tmap_a, tmap_b, g, a_order);
+}
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -331,9 +364,12 @@ int make_map3(CUtensorMap* m, const void* base, uint64_t rows, uint64_t K, uint6
 // a_q / b_q: fp8 e4m3 bytes; a_s / b_s: UE8M0 scale bytes (one per 32 elements of K); *_rows_per_rec / *_rec_stride
 // describe operands that live inside K3 chunk records or K4 panel records (rows_per_rec = rows and any stride for a
 // plain matrix).  K % 32 == 0, K % 16 == 0 for the TMA row stride; M and N are free (bf16 C rows of N elements).
-RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s, uint32_t a_rows_per_rec, uint64_t a_rec_stride, uint64_t b_q,
-                           uint64_t b_s, uint32_t b_rows_per_rec, uint64_t b_rec_stride, uint64_t c, uint32_t M, uint32_t N, uint32_t K,
-                           uint64_t out_dev, uint32_t cta_group, uint64_t done_dev, uint64_t a_ready_dev, uint64_t ready_timeout_ms) {
+// a_order (rn_k_gemm_mxfp8_ordered; 0 here): int32 record ids of A, a permutation of its M / a_rows_per_rec records, walked
+// in that order by the single-CTA kernel.  It needs whole records of whole 128-row blocks and refuses cta_group 2.
+static int launch_mx(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s, uint32_t a_rows_per_rec, uint64_t a_rec_stride, uint64_t b_q,
+                     uint64_t b_s, uint32_t b_rows_per_rec, uint64_t b_rec_stride, uint64_t c, uint32_t M, uint32_t N, uint32_t K,
+                     uint64_t out_dev, uint32_t cta_group, uint64_t done_dev, uint64_t a_ready_dev, uint64_t ready_timeout_ms,
+                     uint64_t a_order) {
   if (!M || !N || !K || (K % 32) || (K % 16)) return -22;
   if ((a_q | b_q) & 15 || (c & 1)) return -22;
   if (!a_rows_per_rec) a_rows_per_rec = M;
@@ -341,6 +377,7 @@ RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s
   if ((a_rows_per_rec < M && a_rows_per_rec % BM) || (b_rows_per_rec < N && b_rows_per_rec % BN)) return -22;   // tiles must not straddle records
   if ((a_rows_per_rec < M && (a_rec_stride % 16 || a_rec_stride < (uint64_t)a_rows_per_rec * K)) ||
       (b_rows_per_rec < N && (b_rec_stride % 16 || b_rec_stride < (uint64_t)b_rows_per_rec * K))) return -22;
+  if (a_order && (cta_group == 2 || (a_order & 3) || a_rows_per_rec % BM || M % a_rows_per_rec)) return -22;
   if (a_rows_per_rec >= M) a_rec_stride = (uint64_t)M * K;
   if (b_rows_per_rec >= N) b_rec_stride = (uint64_t)N * K;
   CUtensorMap ma, mb;
@@ -363,7 +400,7 @@ RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s
   const size_t smem = sizeof(Smem) + 1024;
   // cta_group: 2 = 2-CTA cluster per 256 x 128 tile, 1 = one CTA per 128 x 128 tile, 0 = the cluster when the matrix has more
   // than one 128-row block (a cluster tile hanging over the last rows computes zeros: correct, wasted)
-  if ((cta_group == 2 || (cta_group == 0 && M > BM)) && grid >= 2) {
+  if (!a_order && (cta_group == 2 || (cta_group == 0 && M > BM)) && grid >= 2) {
     rc = make_map3(&mb, (const void*)b_q, N, K, b_rows_per_rec, b_rec_stride >= 16 ? (b_rec_stride + 15) / 16 * 16 : 16, BN / 2);
     if (rc) return rc;
     const uint32_t n_tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN);
@@ -378,10 +415,33 @@ RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s
   if (rc) return rc;
   const uint32_t n_tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
   if ((uint32_t)grid > n_tiles) grid = (int)n_tiles;
+  if (a_order) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_mxfp8_ordered_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return -(int)e - 1000;
+    gemm_mxfp8_ordered_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(ma, mb, g, (const int32_t*)a_order);
+    return (int)cudaGetLastError();
+  }
   cudaError_t e = cudaFuncSetAttribute(gemm_mxfp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return -(int)e - 1000;
   gemm_mxfp8_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(ma, mb, g);
   return (int)cudaGetLastError();
+}
+
+RN_API int rn_k_gemm_mxfp8(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s, uint32_t a_rows_per_rec, uint64_t a_rec_stride, uint64_t b_q,
+                           uint64_t b_s, uint32_t b_rows_per_rec, uint64_t b_rec_stride, uint64_t c, uint32_t M, uint32_t N, uint32_t K,
+                           uint64_t out_dev, uint32_t cta_group, uint64_t done_dev, uint64_t a_ready_dev, uint64_t ready_timeout_ms) {
+  return launch_mx(stream, grid, a_q, a_s, a_rows_per_rec, a_rec_stride, b_q, b_s, b_rows_per_rec, b_rec_stride, c, M, N, K, out_dev,
+                   cta_group, done_dev, a_ready_dev, ready_timeout_ms, 0);
+}
+
+// rn_k_gemm_mxfp8 with a_order (launch_mx): nonzero, 4-byte aligned, one int32 per record of A.
+RN_API int rn_k_gemm_mxfp8_ordered(uint64_t stream, int grid, uint64_t a_q, uint64_t a_s, uint32_t a_rows_per_rec, uint64_t a_rec_stride,
+                                   uint64_t b_q, uint64_t b_s, uint32_t b_rows_per_rec, uint64_t b_rec_stride, uint64_t c, uint32_t M,
+                                   uint32_t N, uint32_t K, uint64_t out_dev, uint32_t cta_group, uint64_t done_dev, uint64_t a_ready_dev,
+                                   uint64_t ready_timeout_ms, uint64_t a_order) {
+  if (!a_order) return -22;
+  return launch_mx(stream, grid, a_q, a_s, a_rows_per_rec, a_rec_stride, b_q, b_s, b_rows_per_rec, b_rec_stride, c, M, N, K, out_dev,
+                   cta_group, done_dev, a_ready_dev, ready_timeout_ms, a_order);
 }
 
 extern "C" __attribute__((visibility("default"))) void rn_preload_gemm_mx() {
@@ -390,5 +450,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_gemm_mx() {
   cudaFuncSetAttribute(gemm_mxfp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Smem) + 1024));
   cudaFuncGetAttributes(&at, gemm_mxfp8_pair_kernel);
   cudaFuncSetAttribute(gemm_mxfp8_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Smem) + 1024));
+  cudaFuncGetAttributes(&at, gemm_mxfp8_ordered_kernel);
+  cudaFuncSetAttribute(gemm_mxfp8_ordered_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Smem) + 1024));
   encode_tiled();
 }

@@ -11,6 +11,8 @@
 //  unpack_fp8_kernel       consumer: optionally waits for each record's arrival (receive
 //                          CQE carrying the chunk id as immediate), then fp8 -> bf16; <true> also
 //                          forwards each record unchanged, from where it landed, as soon as it is seen.
+//  relay_records_kernel    one thread that forwards given records, in a given order, each once its arrival word is set
+//                          (the forwarding unpack's per-record gate without the unpack: a ring all-gather's hop).
 //  reduce_fp8_kernel       the sum of P sources of records (plus a bf16 addend) as each record's sources land,
 //                          as bf16 and / or re-quantised records; the CTA that completes a record of the sum
 //                          posts its RDMA WRITE(_IMM), as K3 does.
@@ -362,6 +364,17 @@ __device__ __forceinline__ bool step_gate(uint64_t T0, uint32_t stride, uint64_t
   return good;
 }
 
+// Pass record r on unchanged: one RDMA WRITE (WRITE_IMM carrying imm) of rec bytes from src_va + r * rec to
+// remote_va + r * rec, after one fence of the poster's scope that releases the record to the wire.  The caller has
+// acquired the record (its arrival word, or stream order).  The forwarding unpack's and the relay's per-record post.
+__device__ __forceinline__ void forward_record(QpDev* qp, uint32_t with_imm, uint64_t src_va, uint32_t lkey, uint64_t remote_va,
+                                               uint32_t rkey, uint64_t rec, uint32_t r, uint32_t imm, uint32_t signal_every,
+                                               unsigned long long* acc, unsigned long long* out, uint64_t timeout_ns) {
+  fence_scope(poster_sys(qp));
+  post_record(qp, with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, src_va + (uint64_t)r * rec, lkey, remote_va + (uint64_t)r * rec,
+              rkey, (uint32_t)rec, imm, signal_every, acc, out, timeout_ns);
+}
+
 struct UnpackArgs {
   const uint8_t* staging;    // records, back to back
   __nv_bfloat16* dst;
@@ -434,12 +447,9 @@ __global__ void __launch_bounds__(kPackThreads, FWD ? 3 : 0) unpack_fp8_kernel(U
         // poster's scope and posts it.  32-bit divisions: the host keeps total tiles below 2^32.
         if (!step_gate<G, true>(T0, stride, total, tiles_per_chunk, [&](uint32_t r) {
               if (a.ready && !wait_word(a.ready + r, abort_flag, a.out, a.timeout_ns)) return false;
-              if (atomicExch(&a.arrived[r], 1u) == 0u) {
-                fence_scope(poster_sys(a.fwd_qp));
-                post_record(a.fwd_qp, a.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.fwd_src_va + (uint64_t)r * rec,
-                            a.fwd_lkey, a.fwd_remote_va + (uint64_t)r * rec, a.fwd_rkey, (uint32_t)rec, a.imm_base + r,
-                            a.signal_every, a.acc, a.out, a.timeout_ns);
-              }
+              if (atomicExch(&a.arrived[r], 1u) == 0u)
+                forward_record(a.fwd_qp, a.with_imm, a.fwd_src_va, a.fwd_lkey, a.fwd_remote_va, a.fwd_rkey, rec, r,
+                               a.imm_base + r, a.signal_every, a.acc, a.out, a.timeout_ns);
               return true;
             }))
           break;
@@ -496,6 +506,48 @@ __global__ void __launch_bounds__(kPackThreads, FWD ? 3 : 0) unpack_fp8_kernel(U
     a.out[3] = seen;
     for (uint32_t c = 0; c <= a.n_chunks + 2; ++c) a.arrived[c] = 0;   // self-clean (the claim flags included)
   }
+}
+
+// ---- relay: pass records on, in a given order, each as soon as its arrival word is set -- the forwarding unpack's
+// per-record gate without the unpack (a ring all-gather's hop, whose receiver reads the records where they land).
+struct RelayArgs {
+  QpDev* qp;
+  const int32_t* ids;        // record ids, in posting order
+  uint32_t n_ids, n_rec;     // ids must lie below n_rec: the records src and dst hold
+  const unsigned long long* ready;   // n_rec arrival words (nullptr: the records are in place)
+  uint64_t src_va, remote_va;        // record r: src_va + r * rec -> remote_va + r * rec
+  uint32_t lkey, rkey;
+  uint64_t rec;
+  uint32_t with_imm, post_only, signal_every;   // WRITE_IMM carries r
+  unsigned int* abort_flag;  // wait_word's (self-cleaned)
+  unsigned long long* acc;   // post_record's [max WQE index + 1, records posted, ~first post time]
+  unsigned long long* out;   // [status, t_start, t_end, records_posted, t_first_post, 0, 0, 0]
+  uint64_t timeout_ns;
+};
+
+// One thread: for each id r in order, wait for ready[r], then post record r (forward_record); then one flush, waited for
+// unless post_only.  A word that never comes ends the kernel TIMEOUT within timeout_ns, and neither that record nor any
+// after it is posted; an id out of range ends it -22 the same way.
+__global__ void __launch_bounds__(32) relay_records_kernel(RelayArgs a) {
+  if (threadIdx.x != 0) return;
+  const unsigned long long t_start = globaltimer_ns();
+  bool bad_id = false;
+#pragma unroll 1
+  for (uint32_t i = 0; i < a.n_ids; ++i) {
+    const uint32_t r = (uint32_t)a.ids[i];
+    if (r >= a.n_rec) { bad_id = true; break; }
+    if (a.ready && !wait_word(a.ready + r, a.abort_flag, a.out, a.timeout_ns)) break;
+    forward_record(a.qp, a.with_imm, a.src_va, a.lkey, a.remote_va, a.rkey, a.rec, r, r, a.signal_every, a.acc, a.out,
+                   a.timeout_ns);
+  }
+  unsigned long long first;
+  const unsigned long long posted = flush_records(a.qp, a.post_only, a.timeout_ns, a.n_ids, a.acc, a.out, first);
+  if (bad_id) a.out[0] = (unsigned long long)(long long)-22;
+  a.out[1] = t_start;
+  a.out[2] = globaltimer_ns();
+  a.out[3] = posted;
+  a.out[4] = posted ? first : 0;
+  *a.abort_flag = 0;
 }
 
 // ---- reduce: the sum of P sources of K3 records (plus an optional bf16 addend) as bf16 and / or as K3 records, each
@@ -730,6 +782,26 @@ RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t
   return (int)cudaGetLastError();
 }
 
+// ids_dev: n_ids int32 record ids below n_rec, in posting order; ready_dev: n_rec arrival words, or 0.  Record r goes
+// from src_va + r * rec_bytes to remote_va + r * rec_bytes.  counters_dev: 8 + 24 bytes of zeroed device memory, cleaned
+// by the kernel.  flags: bit 0 RDMA_WRITE_IMM (immediate = record id), bit 1 post_only.
+RN_API int rn_k_relay_records(uint64_t stream, uint64_t qp_dev, uint64_t ids_dev, uint32_t n_ids, uint32_t n_rec,
+                              uint64_t ready_dev, uint64_t src_va, uint32_t lkey, uint64_t remote_va, uint32_t rkey,
+                              uint64_t rec_bytes, uint32_t flags, uint32_t signal_every, uint64_t counters_dev,
+                              uint64_t out_dev, uint64_t timeout_ms) {
+  if (!qp_dev || !ids_dev || !counters_dev || !n_ids || !n_rec || !rec_bytes || rec_bytes >= (1ull << 32)) return -22;
+  RelayArgs a;
+  a.qp = (QpDev*)qp_dev; a.ids = (const int32_t*)ids_dev; a.n_ids = n_ids; a.n_rec = n_rec;
+  a.ready = (const unsigned long long*)ready_dev; a.src_va = src_va; a.remote_va = remote_va; a.lkey = lkey; a.rkey = rkey;
+  a.rec = rec_bytes; a.with_imm = flags & 1u; a.post_only = (flags >> 1) & 1u; a.signal_every = signal_every ? signal_every : 1;
+  a.abort_flag = (unsigned int*)counters_dev;
+  a.acc = acc_after(counters_dev, 1);
+  a.out = clear_record(out_dev);
+  a.timeout_ns = timeout_ns(timeout_ms);
+  relay_records_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
 // counters_dev: >= (n_rec + 3) * 4 bytes (rounded up to 8) + 24 of zero-initialised device memory, cleaned by the kernel.
 // flags: bit 0 RDMA_WRITE_IMM (immediate = record id), bit 1 post_only.  residual: n_elems fp32 of error feedback (0: none);
 // it needs out_rec, and P = 1, or P = 2 with the addend.
@@ -771,6 +843,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_pack() {
   cudaFuncGetAttributes(&at, pack_fp8_write_kernel<true>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<false>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<true>);
+  cudaFuncGetAttributes(&at, relay_records_kernel);
 #define RN_PRELOAD(G, PMAX, LOCAL, EF) cudaFuncGetAttributes(&at, reduce_fp8_kernel<G, PMAX, LOCAL, EF>);
   RN_REDUCE_VARIANTS(RN_PRELOAD)
 #undef RN_PRELOAD

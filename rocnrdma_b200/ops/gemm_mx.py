@@ -69,7 +69,7 @@ class MxResult:
 
 
 def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, stream=None, sync: bool = True, scratch_slot: int = L.SLOT["gemm_mxfp8"],
-               cta_group: int = 0, a_ready=None, timeout_ms: int = 2000):
+               cta_group: int = 0, a_ready=None, timeout_ms: int = 2000, a_order=None, result_off=None):
     """``c[M,N] (bf16) = dequant(a)[M,K] @ dequant(b)[N,K].T`` with the block scales applied by the tensor core.
     Any M and N; K a multiple of 32 (one MX block) and of 16 bytes.
     ``cta_group``: 2 = CTA-pair kernel (256 x 128 per 2-CTA cluster, B multicast: half the B traffic per FLOP), 1 = single-CTA kernel
@@ -79,7 +79,15 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
     kernel starts a tile only once the word of the record it reads is nonzero, so the product overlaps the transfer record
     by record.  ``ops.recv_consume(..., stamps=a_ready)`` produces exactly these words when every record arrives by
     RDMA_WRITE_IMM with its index as the immediate: the chunk id for K3 records, the panel id for K4 records.  Launch with
-    a ``grid`` that leaves SMs for whatever produces the records (a persistent kernel spinning on all SMs would starve it)."""
+    a ``grid`` that leaves SMs for whatever produces the records (a persistent kernel spinning on all SMs would starve it).
+    ``a_order``: an int32 CUDA tensor with one entry per record of ``a``, a permutation of the record ids.  The
+    single-CTA kernel then walks its tiles record by record in that order (each record's 128-row blocks in row order,
+    every column block of a row block before the next), so that with ``a_ready`` it starts on the records that land
+    first.  C does not depend on the order.  It needs ``a`` in whole records of whole 128-row blocks (M a multiple of
+    ``rows_per_rec``, ``rows_per_rec`` a multiple of 128) and refuses ``cta_group=2``; with 0 it runs the single-CTA
+    kernel.  An entry outside the record ids leaves that record's rows of C unwritten.
+    ``result_off``: where in the mapped scratch the kernel writes its result words (default: the record of
+    ``scratch_slot``)."""
     import os
     if os.environ.get("RN_MX_CTA_GROUP"):
         cta_group = int(os.environ["RN_MX_CTA_GROUP"])
@@ -87,12 +95,20 @@ def gemm_mxfp8(ctx, a: MxOperand, b: MxOperand, c: torch.Tensor, grid: int = 0, 
     assert b.K == K and c.dtype == torch.bfloat16 and tuple(c.shape) == (M, Nn) and c.is_contiguous()
     ready_addr = 0 if a_ready is None else L.tensor_ptr(a_ready, torch.int64, ctx.device,
                                                         "a_ready (one word per record of a)", -(-M // (a.rows_per_rec or M)))
+    if a_order is not None:
+        rpr = a.rows_per_rec or M
+        if cta_group == 2:
+            raise ValueError("a_order walks the single-CTA kernel: cta_group=2 (the CTA-pair kernel) has no ordered walk")
+        if rpr % PANEL_ROWS or M % rpr:
+            raise ValueError(f"a_order needs a in whole records of whole 128-row blocks: M={M}, rows_per_rec={rpr}")
+        order_addr = L.tensor_ptr(a_order, torch.int32, ctx.device, "a_order (one id per record of a)", M // rpr, exact=True)
     lib = N.load()
     ws = work_stream(ctx, stream)
-    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot))
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
     done = L.counters(ctx, 1, scratch_slot)          # zeroed device counter, cleaned by the kernel
-    rc = lib.rn_k_gemm_mxfp8(_stream_ptr(ws), grid, a.q_ptr, a.s_ptr, a.rows_per_rec, a.rec_stride, b.q_ptr, b.s_ptr, b.rows_per_rec,
-                             b.rec_stride, c.data_ptr(), M, Nn, K, out_addr, cta_group, done, ready_addr, timeout_ms)
+    args = (_stream_ptr(ws), grid, a.q_ptr, a.s_ptr, a.rows_per_rec, a.rec_stride, b.q_ptr, b.s_ptr, b.rows_per_rec,
+            b.rec_stride, c.data_ptr(), M, Nn, K, out_addr, cta_group, done, ready_addr, timeout_ms)
+    rc = lib.rn_k_gemm_mxfp8(*args) if a_order is None else lib.rn_k_gemm_mxfp8_ordered(*args, order_addr)
     return L.finish(rc, "gemm_mxfp8", out_view, ws, sync, _parse, M, Nn, K)
 
 

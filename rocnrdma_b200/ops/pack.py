@@ -66,9 +66,11 @@ def _parse(view, n_elems, wire) -> PackResult:
 def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chunk_elems: int = 1 << 20,
                    with_imm: bool = False, signal_every: int = 1, grid: int = 0, timeout_ms: int = 2000,
                    stream=None, sync: bool = True, scratch_slot: int = SLOT["pack"], post_only: bool = False, direct: bool = False,
-                   result_off=None, residual=None):
+                   result_off=None, residual=None, staging_off: int = 0):
     """Pack ``src`` (bf16) into fp8 chunk records in ``staging_mr`` and, if ``qp`` is given,
     RDMA-write every record to the same offset of ``dst_mr`` from inside the kernel.
+    ``staging_off``: the records start that many bytes into ``staging_mr`` (a multiple of 64), and land at the same
+    offset of ``dst_mr``.
     ``result_off``: where in the mapped scratch the kernel writes its result words (default: the record of
     ``scratch_slot``, see :func:`~rocnrdma_b200.ops.launch.result_offset`).
     ``direct``: ``staging_mr`` is the *peer's* buffer registered with this context (NVLink-mapped, ``ctx.reg_mr(tensor_on_the_peer)``):
@@ -84,7 +86,10 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     if n % TILE_ELEMS or chunk_elems % TILE_ELEMS or n % chunk_elems:
         raise ValueError(f"n_elems and chunk_elems must be multiples of {TILE_ELEMS}, n_elems of chunk_elems")
     wire = staging_bytes(n, chunk_elems)
-    if staging_mr.length < wire or (dst_mr is not None and dst_mr.length < wire):
+    staging_off = int(staging_off)
+    if staging_off < 0 or staging_off % 64:
+        raise ValueError(f"staging_off={staging_off}: a non-negative multiple of 64")
+    if staging_mr.length < staging_off + wire or (dst_mr is not None and dst_mr.length < staging_off + wire):
         raise ValueError("staging / destination region too small for the records")
     res_addr = 0 if residual is None else L.tensor_ptr(residual, torch.float32, ctx.device, "residual", n, exact=True, align=32)
     lib = N.load()
@@ -92,9 +97,9 @@ def pack_fp8_write(ctx, src: torch.Tensor, staging_mr, qp=None, dst_mr=None, chu
     # [n_chunks] groups packed per record ; CTAs done
     counters = L.counters(ctx, n // chunk_elems + 1, scratch_slot)
     out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
-    rc = lib.rn_k_pack_fp8_write(_stream_ptr(ws), grid, src.data_ptr(), staging_mr.addr, n, chunk_elems,
-                                 qp.dev_ptr if qp is not None else 0, staging_mr.addr, staging_mr.lkey,
-                                 dst_mr.addr if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
+    rc = lib.rn_k_pack_fp8_write(_stream_ptr(ws), grid, src.data_ptr(), staging_mr.addr + staging_off, n, chunk_elems,
+                                 qp.dev_ptr if qp is not None else 0, staging_mr.addr + staging_off, staging_mr.lkey,
+                                 dst_mr.addr + staging_off if dst_mr is not None else 0, dst_mr.rkey if dst_mr is not None else 0,
                                  int(with_imm) | (2 if post_only else 0) | (4 if direct else 0), signal_every, counters, out_addr, timeout_ms,
                                  res_addr)
     return L.finish(rc, "pack_fp8_write", out_view, ws, sync, None if qp is None else _parse, n, wire)
@@ -163,6 +168,57 @@ def unpack_fp8(ctx, staging: torch.Tensor, dst: torch.Tensor, chunk_elems: int =
 def parse_unpack(view) -> dict:
     """Decode the record :func:`unpack_fp8` leaves in the mapped scratch (for ``sync=False`` callers)."""
     return L.decode(view, UNPACK_WORDS)
+
+
+# ------------------------------------------------------------------ relay
+RELAY_WORDS = ("records_posted", "t_first_post_ns")
+
+
+def relay_records(qp, src_mr, dst_mr, rec_bytes: int, ids, *, ready=None, with_imm: bool = True, signal_every: int = 1,
+                  post_only: bool = False, timeout_ms: int = 2000, stream=None, sync: bool = True,
+                  scratch_slot: int = SLOT["unpack"], result_off=None):
+    """Pass records on unchanged, in a given order, each as soon as it has landed: one thread on the GPU that does the
+    forwarding unpack's per-record step without the unpack.
+
+    ``src_mr`` and ``dst_mr`` hold records of ``rec_bytes`` back to back; record r goes from ``src_mr.addr + r *
+    rec_bytes`` to ``dst_mr.addr + r * rec_bytes``.  ``ids`` (int32 CUDA tensor) lists the record ids in posting order.
+    For each id r the kernel waits for ``ready[r]`` (int64 CUDA tensor, one arrival word per record of ``src_mr``, as
+    ``recv_consume`` sets them; None: the records are in place), then posts one RDMA WRITE, or WRITE_IMM with immediate
+    r when ``with_imm``.  Then it posts one flush and waits for it, unless ``post_only``.  A word still 0 after
+    ``timeout_ms`` ends the kernel ``TIMEOUT``: that record and every later one are never posted.  An id outside the
+    records ends it with status ``-22`` the same way.  Nothing else may post to ``qp`` while the relay runs.
+
+    Its counters are the last 32 bytes of ``scratch_slot``, so it can run beside a launch that keeps its counters at the
+    start of the same slot (the unpack's, the GEMM's).  Returns a dict with ``records_posted`` and ``t_first_post_ns``,
+    or ``(result view, stream)`` with ``sync=False`` (decode with :func:`parse_relay`)."""
+    rec_bytes = int(rec_bytes)
+    if rec_bytes <= 0 or rec_bytes % 64 or rec_bytes >= 1 << 32:
+        raise ValueError(f"rec_bytes={rec_bytes}: a positive multiple of 64 below 2**32")
+    n_rec = min(src_mr.length, dst_mr.length) // rec_bytes
+    if n_rec == 0:
+        raise ValueError(f"src_mr ({src_mr.length} bytes) and dst_mr ({dst_mr.length} bytes) must hold a record of {rec_bytes}")
+    if not isinstance(ids, torch.Tensor) or ids.dim() != 1 or ids.numel() == 0:
+        raise ValueError("ids must be a non-empty 1-D int32 tensor of record ids")
+    ctx = qp.ctx
+    ids_addr = L.tensor_ptr(ids, torch.int32, ctx.device, "ids", 1)
+    if ids.numel() >= 1 << 32:
+        raise ValueError(f"{ids.numel()} ids: at most 2**32 - 1")
+    ready_addr = 0 if ready is None else L.tensor_ptr(ready, torch.int64, ctx.device, "ready", n_rec)
+    lib = N.load()
+    ws = work_stream(ctx, stream)
+    nb = L.counter_bytes(1)                 # abort flag ; post_record's three words
+    L.counters(ctx, 1, scratch_slot)        # checks the slot
+    counters = ctx.dev_scratch(nb, offset=(scratch_slot + 1) * L.SLOT_BYTES - nb)
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
+    rc = lib.rn_k_relay_records(_stream_ptr(ws), qp.dev_ptr, ids_addr, ids.numel(), min(n_rec, (1 << 32) - 1), ready_addr,
+                                src_mr.addr, src_mr.lkey, dst_mr.addr, dst_mr.rkey, rec_bytes,
+                                int(with_imm) | (2 if post_only else 0), signal_every, counters, out_addr, timeout_ms)
+    return L.finish(rc, "relay_records", out_view, ws, sync, parse_relay)
+
+
+def parse_relay(view) -> dict:
+    """Decode the record :func:`relay_records` leaves in the mapped scratch (for ``sync=False`` callers)."""
+    return L.decode(view, RELAY_WORDS)
 
 
 # ------------------------------------------------------------------ bit-exact references
@@ -329,6 +385,16 @@ def ref_allreduce_fp8(xs, chunk_elems: int, residuals=None):
                 _, recs = ref_reduce_fp8(recs, 1, m, chunk_elems, local=xs[q].reshape(-1)[part])
         out[part] = ref_unpack_fp8(recs, m, chunk_elems).to(out.device)
     return (out, new) if ef else out
+
+
+def ref_allgather_fp8(shards, chunk_elems: int):
+    """Reference of the fp8 ring all-gather (:class:`~rocnrdma_b200.parallel.allgather_fp8.RingAllgatherFp8`), bit for
+    bit; runs on CPU or GPU.  ``shards``: the N ranks' bf16 tensors of the same number of elements, a multiple of
+    ``chunk_elems``.  Returns ``(bf16 gathered, gathered records)``: shard s's K3 records (:func:`ref_pack_fp8`) at record
+    ``s * R``, and their dequantisation (:func:`ref_unpack_fp8`) at element ``s * n``.  Every rank holds both."""
+    recs = torch.cat([ref_pack_fp8(x.reshape(-1), chunk_elems) for x in shards])
+    n = sum(x.numel() for x in shards)
+    return ref_unpack_fp8(recs, n, chunk_elems), recs
 
 
 # ------------------------------------------------------------------ reduce

@@ -72,7 +72,8 @@ def schedule(rank: int, world: int) -> List[Step]:
 
 
 # the words of each kind of launch's result record, after the header
-_WORDS = {"pack": P.PACK_WORDS, "reduce": P.REDUCE_WORDS, "unpack": P.UNPACK_WORDS, "recv": RECV_WORDS}
+_WORDS = {"pack": P.PACK_WORDS, "reduce": P.REDUCE_WORDS, "unpack": P.UNPACK_WORDS, "recv": RECV_WORDS,
+          "relay": P.RELAY_WORDS, "gemm": ()}
 
 
 def _pow2(n: int) -> int:
@@ -113,7 +114,103 @@ class RingResult:
         return [l.device_ns for l in self.launches if l.name != "receive"]
 
 
-class RingAllreduceFp8:
+class _RingPlan:
+    """What the GPU-driven ring plans share: linking (the receive queue and the next rank's landing region), the consumer
+    stream that receives and stamps every record a run brings, recovery after a failed run, and the result.  A plan
+    sets ``n_recv`` (receives per run), ``n_ids`` (arrival words, ids ``[0, n_ids)``), ``landing`` / ``landing_mr``,
+    ``words`` and the streams."""
+    WAITERS = 1                 # waiting launches of a rank beside its compute grid: the consumer
+
+    # ---------------------------------------------------------------- links
+    def _attach(self, send_qp, recv_qp, remote_landing, scratch_slot: int, grid: int, in_process: bool):
+        depth = recv_qp.rq_depth
+        cq_depth = recv_qp.rcq.depth
+        if depth < 2 * self.n_recv or cq_depth < 2 * self.n_recv:
+            raise ValueError(f"the receive queue ({depth}) and its CQ ({cq_depth}) must hold 2 * {self.n_recv} entries: "
+                             f"{self.n_recv} receives per run, and those a failed run leaves behind")
+        if remote_landing.length < self.landing.numel():
+            raise ValueError("the next rank's landing region is smaller than this plan's")
+        self.send_qp, self.recv_qp, self.remote_landing = send_qp, recv_qp, remote_landing
+        self.scratch_slot, self.grid, self.in_process = scratch_slot, grid, in_process
+
+    def connect(self, group=None, sq_depth: int = 256):
+        """One process per GPU: create this rank's queue pair and connect it through ``parallel.peer.connect_ring``.
+        Its send queue goes to the next rank, its receive queue takes the previous rank's records.  Collective."""
+        import torch.distributed as dist
+        from .peer import connect_ring
+        if dist.get_rank(group) != self.rank or dist.get_world_size(group) != self.world:
+            raise ValueError("the process group's rank and world size differ from the plan's")
+        grid = self.grid or _default_grid(self.ctx, self.engine_ctas, 1, self.WAITERS)
+        _check_budget(self.ctx, self.engine_ctas, 1, grid, self.WAITERS)
+        depth = _pow2(2 * self.n_recv)
+        scq = self.ctx.create_cq(2 * sq_depth)
+        rcq = self.ctx.create_cq(depth)
+        qp = self.ctx.create_qp(scq, rcq, sq_depth, depth)
+        _, remote = connect_ring(self.ctx, qp, [self.landing_mr], group)
+        self._attach(qp, qp, next(iter(remote.values())), 0, grid, in_process=False)
+
+    # ---------------------------------------------------------------- run
+    def _res(self, i: int) -> int:
+        return L.ring_result_offset(self.scratch_slot, i)
+
+    def _shard(self, t, s):
+        s %= self.world
+        return t[s * self.shard:(s + 1) * self.shard]
+
+    def start_consumer(self):
+        """Enqueue the consumer stream: clear the words, then receive and stamp this run's ``n_recv`` records."""
+        if self.send_qp is None:
+            raise RuntimeError("link the plan first: link_in_process(plans) or plan.connect()")
+        if self._failed and not self.in_process:
+            raise RuntimeError("a failed run leaves receive completions behind that only a new connection clears: "
+                               "build new plans and connect them")
+        if self._rq_backlog > self.n_recv:
+            raise RuntimeError(f"{self._rq_backlog} receive WQEs are left from failed runs: link new plans")
+        cs = self.consumer_stream
+        kw = dict(timeout_ms=self.timeout_ms, stream=cs, sync=False)
+        views = []
+        if self._stale_cqes:
+            # completions of a failed run's late records: reap them before this run's words are cleared
+            views.append(("drain", "recv", ops.recv_consume(self.recv_qp, self._stale_cqes, 0, None, scratch_off=self._res(self._DRAIN), **kw)[0]))
+        with torch.cuda.stream(cs):
+            self.words.zero_()
+        self._cleared.record(cs)
+        fresh = self.n_recv - self._rq_backlog
+        views.append(("receive", "recv", ops.recv_consume(self.recv_qp, fresh, self.n_ids, self.words, scratch_off=self._res(0),
+                                                  prepost_mr=self.landing_mr, prepost_bytes=0, **kw)[0]))
+        if self._rq_backlog:
+            # the receive WQEs a failed run left posted take the rest of this run's records
+            views.append(("receive", "recv", ops.recv_consume(self.recv_qp, self._rq_backlog, self.n_ids, self.words,
+                                                      scratch_off=self._res(self._DRAIN + 1), **kw)[0]))
+        self._stale_cqes = self._rq_backlog = 0
+        self._views = views
+
+    def _streams(self):
+        return (self.consumer_stream, self.main_stream)
+
+    def synchronize(self):
+        for s in self._streams():
+            s.synchronize()
+
+    def result(self) -> RingResult:
+        """Decode the last run's result records (after :meth:`synchronize`)."""
+        launches, received, posted = [], 0, 0
+        for name, kind, view in self._views:
+            w = L.decode(view, _WORDS[kind])
+            launches.append(LaunchResult(name, w["status"], w["t_start_ns"], w["t_end_ns"]))
+            posted += w.get("wqes", 0) + w.get("records_posted", 0) + w.get("records_forwarded", 0)
+            received += w["seen"] if name == "receive" else 0
+        bad = next((l for l in launches if l.status != "OK"), None)
+        starts = [l.t_start_ns for l in launches if l.t_start_ns > 0]
+        ends = [l.t_end_ns for l in launches if l.t_end_ns > 0]
+        total = max(ends) - min(starts) if starts and ends else 0
+        if bad is not None:
+            self._failed = True
+        return RingResult(self.rank, bad.status if bad else "OK", bad.name if bad else None, launches, total, received,
+                          posted)
+
+
+class RingAllreduceFp8(_RingPlan):
     """One rank's plan of the fp8 ring all-reduce of ``n_elems`` bf16 elements over ``world`` ranks.
 
     Everything is allocated and registered here, before any engine runs (DESIGN.md 3.2): the send staging (R records),
@@ -153,6 +250,7 @@ class RingAllreduceFp8:
         self.R = self.shard // chunk_elems
         self.rec = P.record_bytes(chunk_elems)
         self.n_ids = 2 * (world - 1) * self.R
+        self.n_recv = self.n_ids
         counter_bytes = L.counter_bytes(self.R + 3)       # the reduce's and the unpack's: R records and 3 words
         if counter_bytes > L.SLOT_BYTES:
             raise ValueError(f"{self.R} records per shard need {counter_bytes} bytes of counters; a scratch slot holds 256 KiB")
@@ -183,43 +281,9 @@ class RingAllreduceFp8:
         self._stale_cqes = 0            # receive completions a failed run left unreaped (in-process accounting)
         self._rq_backlog = 0            # receive WQEs a failed run left posted
         self._failed = False
-
-    # ---------------------------------------------------------------- links
-    def _attach(self, send_qp, recv_qp, remote_landing, scratch_slot: int, grid: int, in_process: bool):
-        depth = recv_qp.rq_depth
-        cq_depth = recv_qp.rcq.depth
-        if depth < 2 * self.n_ids or cq_depth < 2 * self.n_ids:
-            raise ValueError(f"the receive queue ({depth}) and its CQ ({cq_depth}) must hold 2 * {self.n_ids} entries: "
-                             f"2(N-1)R = {self.n_ids} receives per run, and those a failed run leaves behind")
-        if remote_landing.length < self.n_ids * self.rec:
-            raise ValueError("the next rank's landing region is smaller than this plan's")
-        self.send_qp, self.recv_qp, self.remote_landing = send_qp, recv_qp, remote_landing
-        self.scratch_slot, self.grid, self.in_process = scratch_slot, grid, in_process
-
-    def connect(self, group=None, sq_depth: int = 256):
-        """One process per GPU: create this rank's queue pair and connect it through ``parallel.peer.connect_ring``.
-        Its send queue goes to the next rank, its receive queue takes the previous rank's records.  Collective."""
-        import torch.distributed as dist
-        from .peer import connect_ring
-        if dist.get_rank(group) != self.rank or dist.get_world_size(group) != self.world:
-            raise ValueError("the process group's rank and world size differ from the plan's")
-        grid = self.grid or _default_grid(self.ctx, self.engine_ctas, 1)
-        _check_budget(self.ctx, self.engine_ctas, 1, grid)
-        depth = _pow2(2 * self.n_ids)
-        scq = self.ctx.create_cq(2 * sq_depth)
-        rcq = self.ctx.create_cq(depth)
-        qp = self.ctx.create_qp(scq, rcq, sq_depth, depth)
-        _, remote = connect_ring(self.ctx, qp, [self.landing_mr], group)
-        self._attach(qp, qp, next(iter(remote.values())), 0, grid, in_process=False)
+        self._DRAIN = 2 * world + 1     # result records of the drain and of the backlog's receive
 
     # ---------------------------------------------------------------- run
-    def _res(self, i: int) -> int:
-        return L.ring_result_offset(self.scratch_slot, i)
-
-    def _shard(self, t, s):
-        s %= self.world
-        return t[s * self.shard:(s + 1) * self.shard]
-
     @property
     def error_feedback(self) -> bool:
         return self.residual is not None
@@ -233,34 +297,6 @@ class RingAllreduceFp8:
 
     def _slot(self, m):
         return self.landing[m * self.R * self.rec:(m + 1) * self.R * self.rec], self.words[m * self.R:(m + 1) * self.R]
-
-    def start_consumer(self):
-        """Enqueue the consumer stream: clear the words, then receive and stamp this run's 2(N-1)R records."""
-        if self.send_qp is None:
-            raise RuntimeError("link the plan first: link_in_process(plans) or plan.connect()")
-        if self._failed and not self.in_process:
-            raise RuntimeError("a failed run leaves receive completions behind that only a new connection clears: "
-                               "build new plans and connect them")
-        if self._rq_backlog > self.n_ids:
-            raise RuntimeError(f"{self._rq_backlog} receive WQEs are left from failed runs: link new plans")
-        cs = self.consumer_stream
-        kw = dict(timeout_ms=self.timeout_ms, stream=cs, sync=False)
-        views = []
-        if self._stale_cqes:
-            # completions of a failed run's late records: reap them before this run's words are cleared
-            views.append(("drain", "recv", ops.recv_consume(self.recv_qp, self._stale_cqes, 0, None, scratch_off=self._res(2 * self.world + 1), **kw)[0]))
-        with torch.cuda.stream(cs):
-            self.words.zero_()
-        self._cleared.record(cs)
-        fresh = self.n_ids - self._rq_backlog
-        views.append(("receive", "recv", ops.recv_consume(self.recv_qp, fresh, self.n_ids, self.words, scratch_off=self._res(0),
-                                                  prepost_mr=self.landing_mr, prepost_bytes=0, **kw)[0]))
-        if self._rq_backlog:
-            # the receive WQEs a failed run left posted take the rest of this run's records
-            views.append(("receive", "recv", ops.recv_consume(self.recv_qp, self._rq_backlog, self.n_ids, self.words,
-                                                      scratch_off=self._res(2 * self.world + 2), **kw)[0]))
-        self._stale_cqes = self._rq_backlog = 0
-        self._views = views
 
     def enqueue_main(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, steps=None):
         """Enqueue this rank's main stream (after :meth:`start_consumer`): K3, the N-1 reduce hops and the N unpacks.
@@ -317,60 +353,42 @@ class RingAllreduceFp8:
         self.synchronize()
         return self.result()
 
-    def synchronize(self):
-        self.consumer_stream.synchronize()
-        self.main_stream.synchronize()
-
-    def result(self) -> RingResult:
-        """Decode the last run's result records (after :meth:`synchronize`)."""
-        launches, received, posted = [], 0, 0
-        for name, kind, view in self._views:
-            w = L.decode(view, _WORDS[kind])
-            launches.append(LaunchResult(name, w["status"], w["t_start_ns"], w["t_end_ns"]))
-            posted += w.get("wqes", 0) + w.get("records_posted", 0) + w.get("records_forwarded", 0)
-            received += w["seen"] if name == "receive" else 0
-        bad = next((l for l in launches if l.status != "OK"), None)
-        starts = [l.t_start_ns for l in launches if l.t_start_ns > 0]
-        ends = [l.t_end_ns for l in launches if l.t_end_ns > 0]
-        total = max(ends) - min(starts) if starts and ends else 0
-        if bad is not None:
-            self._failed = True
-        return RingResult(self.rank, bad.status if bad else "OK", bad.name if bad else None, launches, total, received,
-                          posted)
-
 
 def _sms(ctx) -> int:
     return torch.cuda.get_device_properties(ctx.device).multi_processor_count
 
 
-def _default_grid(ctx, engine_ctas: int, ranks: int) -> int:
-    return max(1, min(64, (_sms(ctx) - engine_ctas) // ranks - 1))
+def _default_grid(ctx, engine_ctas: int, ranks: int, waiters: int = 1) -> int:
+    return max(1, min(64, (_sms(ctx) - engine_ctas) // ranks - waiters))
 
 
-def _check_budget(ctx, engine_ctas: int, ranks: int, grid: int):
-    need = engine_ctas + ranks * (grid + 1)
+def _check_budget(ctx, engine_ctas: int, ranks: int, grid: int, waiters: int = 1):
+    """``waiters``: the one-CTA waiting launches of a rank beside its grid (the consumer, and a plan's relay)."""
+    need = engine_ctas + ranks * (grid + waiters)
     if need > _sms(ctx):
-        raise ValueError(f"SM budget: engine {engine_ctas} + {ranks} ranks x (grid {grid} + consumer 1) = {need} CTAs, "
+        others = "consumer 1" if waiters == 1 else f"consumer and relay {waiters}"
+        raise ValueError(f"SM budget: engine {engine_ctas} + {ranks} ranks x (grid {grid} + {others}) = {need} CTAs, "
                          f"above the device's {_sms(ctx)} SMs; every waiting kernel must be resident as a whole")
 
 
-def link_in_process(plans: List[RingAllreduceFp8], sq_depth: int = 256, rq_depth: Optional[int] = None):
+def link_in_process(plans: List[_RingPlan], sq_depth: int = 256, rq_depth: Optional[int] = None):
     """Simulate N ranks in one context: connect the send QP of rank q to the receive QP of rank q+1 for every q, and
     give rank q device-scratch slot q.  Call before the engine starts."""
     N = len(plans)
     if N < 2 or any(p.world != N or p.rank != i for i, p in enumerate(plans)):
         raise ValueError("plans must be ranks 0..N-1 of one world of N >= 2")
     ctx = plans[0].ctx
-    if any(p.ctx is not ctx or (p.n, p.chunk) != (plans[0].n, plans[0].chunk) for p in plans):
-        raise ValueError("in-process plans share one context, n_elems and chunk_elems")
+    if any(type(p) is not type(plans[0]) or p.ctx is not ctx or (p.n, p.chunk) != (plans[0].n, plans[0].chunk) for p in plans):
+        raise ValueError("in-process plans are of one kind and share one context, n_elems and chunk_elems")
     if N > MAX_IN_PROCESS:
         raise ValueError(f"{N} in-process ranks: the device scratch has {MAX_IN_PROCESS} slots, one per rank")
-    grid = plans[0].grid or _default_grid(ctx, plans[0].engine_ctas, N)
-    _check_budget(ctx, plans[0].engine_ctas, N, grid)
-    depth = rq_depth if rq_depth is not None else _pow2(2 * plans[0].n_ids)
-    if depth < 2 * plans[0].n_ids:
-        raise ValueError(f"rq_depth={depth}: the receive queue and its CQ must hold 2 * {plans[0].n_ids} entries: "
-                         f"2(N-1)R receives per run, and those a failed run leaves behind")
+    waiters = plans[0].WAITERS
+    grid = plans[0].grid or _default_grid(ctx, plans[0].engine_ctas, N, waiters)
+    _check_budget(ctx, plans[0].engine_ctas, N, grid, waiters)
+    depth = rq_depth if rq_depth is not None else _pow2(2 * plans[0].n_recv)
+    if depth < 2 * plans[0].n_recv:
+        raise ValueError(f"rq_depth={depth}: the receive queue and its CQ must hold 2 * {plans[0].n_recv} entries: "
+                         f"{plans[0].n_recv} receives per run, and those a failed run leaves behind")
     send, recv = [], []
     for _ in range(N):
         send.append(ctx.create_qp(ctx.create_cq(2 * sq_depth), ctx.create_cq(64), sq_depth, 16))
@@ -387,11 +405,17 @@ def run_in_process(plans: List[RingAllreduceFp8], xs, outs=None, sync: bool = Tr
     enqueued (a rank that never contributes; its receives are still posted).  Returns one :class:`RingResult` per rank
     with ``sync``."""
     outs = outs or [None] * len(plans)
+    return _run_ranks(plans, [lambda p=p, x=x, o=o: p.enqueue_main(x, o) for p, x, o in zip(plans, xs, outs)], sync, skip)
+
+
+def _run_ranks(plans: List[_RingPlan], enqueues, sync: bool, skip):
+    """Every consumer, then ``enqueues[q]()`` for every rank q not in ``skip``; with ``sync`` wait, and record what a
+    failed run leaves in each receive queue for the next run to reap.  Returns one :class:`RingResult` per rank."""
     for p in plans:
         p.start_consumer()
-    for p, x, o in zip(plans, xs, outs):
+    for p, enqueue in zip(plans, enqueues):
         if p.rank not in skip:
-            p.enqueue_main(x, o)
+            enqueue()
     if not sync:
         return None
     for p in plans:
@@ -402,5 +426,5 @@ def run_in_process(plans: List[RingAllreduceFp8], xs, outs=None, sync: bool = Tr
     for q, p in enumerate(plans):
         arrivals = res[(q - 1) % N].posted
         p._stale_cqes = max(0, arrivals - res[q].received)
-        p._rq_backlog = max(0, p.n_ids - arrivals)
+        p._rq_backlog = max(0, p.n_recv - arrivals)
     return res
