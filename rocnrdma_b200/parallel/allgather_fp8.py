@@ -109,8 +109,12 @@ class RingAllgatherFp8(_RingPlan):
         self.compute_stream = torch.cuda.Stream(device=dev)
         self._cleared, self._own_set, self._done = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
         with torch.cuda.stream(self.consumer_stream):
-            self.words.fill_(1)             # loads the fill kernel now (step 2 and the consumer's clear): a first load
-            self.words.zero_()              # later would wait for the engine
+            # load the fill kernels now (step 2 and the consumer's clear): a first load later would wait for the engine.
+            # Step 2 fills one slot's words, and where they start picks torch's kernel (a slot whose words are not 16-
+            # or 32-byte aligned gets a narrower one), so fill every slot as step 2 does.
+            for s in range(world):
+                self._slot(s)[1].fill_(1)
+            self.words.zero_()
         self._cleared.record(self.consumer_stream)
         torch.cuda.synchronize(dev)
         self.send_qp = self.recv_qp = self.remote_landing = None

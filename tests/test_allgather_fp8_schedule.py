@@ -161,3 +161,66 @@ def test_ref_allgather_is_each_shard_packed_and_unpacked(N, chunk):
         want = P.ref_pack_fp8(x, chunk)
         assert torch.equal(recs[s * rb:(s + 1) * rb], want)
         assert torch.equal(out[s * n:(s + 1) * n].view(torch.int16), P.ref_unpack_fp8(want, n, chunk).view(torch.int16))
+
+
+# ------------------------------------------------------------------ the ordered K7 inside the gather (test_gpu_allgather_fp8_shapes.py)
+@pytest.mark.parametrize("N", [2, 3, 5, 8])
+def test_gather_schedule_walk_is_the_ordered_walk(N):
+    """Every rank's model walk is ``_ordered_walk`` of its arrival order, and its CTAs' strided shares cover it once."""
+    from test_gpu_allgather_fp8_shapes import OrderedGatherSchedule
+    for K, rows_per_rec, R, Nb, grid in [(64, 128, 2, 200, 7), (4096, 512, 1, 4096, 0), (32, 256, 3, 1, 1),
+                                         (160, 256, 2, 391, 300)]:
+        for q in range(N):
+            s = OrderedGatherSchedule(N, q, K, rows_per_rec, R, Nb, grid)
+            order = [sl * R + r for sl in AG.arrival_slots(q, N) for r in range(R)]
+            assert s.order == order
+            assert s.coords() == _ordered_walk(order, rows_per_rec // 128, -(-Nb // 128), N * R)
+            assert sorted(t for ts in s.tiles for t in ts) == list(range(s.n_tiles))
+            assert s.place(s.walk[0][0]) == 0 and s.place(s.walk[-1][0]) == N - 1
+
+
+def test_gather_schedule_hand_counted_walks():
+    from test_gpu_allgather_fp8_shapes import OrderedGatherSchedule
+    # N 2, rank 1, two 128-row blocks a record, two column blocks, grid 3: records 1 then 0, four tiles each
+    s = OrderedGatherSchedule(2, 1, 64, 256, 1, 200, 3)
+    assert s.walk == [(1, 2, 0), (1, 2, 1), (1, 3, 0), (1, 3, 1), (0, 0, 0), (0, 0, 1), (0, 1, 0), (0, 1, 1)]
+    assert s.tiles == [[0, 3, 6], [1, 4, 7], [2, 5]]
+    f = s.facts()
+    assert f == {"multi_block_records": True, "cta_crosses_slots": True, "cta_starts_remote": False,
+                 "record_shared": True, "ragged_n": True, "odd_n": False, "partial_k": True, "mid_ring_entry": True,
+                 "clamped_grid": False}
+    # N 3, rank 0, one tile a record, grid 7 clamped to 3: each CTA one record, in the arrival order 0, 2, 1
+    s = OrderedGatherSchedule(3, 0, 4096, 128, 1, 1, 7)
+    assert s.grid == 3 and s.tiles == [[0], [1], [2]] and s.walk == [(0, 0, 0), (2, 2, 0), (1, 1, 0)]
+    assert [s.place(r) for r, _, _ in s.walk] == [0, 1, 2]
+    f = s.facts()
+    assert f["clamped_grid"] and f["cta_starts_remote"] and not f["cta_crosses_slots"] and not f["record_shared"]
+    assert not f["mid_ring_entry"] and not f["partial_k"] and f["odd_n"] and f["ragged_n"]
+    # N 4, rank 2, R 2, grid 1: one CTA walks slots 2, 1, 0, 3, every record of a slot before the next slot
+    s = OrderedGatherSchedule(4, 2, 512, 128, 2, 128, 1)
+    assert [r for r, _, _ in s.walk] == [4, 5, 2, 3, 0, 1, 6, 7] and s.tiles == [list(range(8))]
+    f = s.facts()
+    assert f["cta_crosses_slots"] and not f["cta_starts_remote"] and not f["record_shared"]
+    assert not f["mid_ring_entry"] and not f["ragged_n"] and not f["partial_k"]       # k_blks 4: every tile from stage 0
+    assert OrderedGatherSchedule(4, 2, 384, 128, 2, 128, 1).facts()["mid_ring_entry"]   # k_blks 3: the second from stage 3
+
+
+def test_gather_geometry_cases_cover_every_fact_and_parameter():
+    """The GPU geometry cases: each claims facts of both walks, the same on every rank; together they cover every fact,
+    N = 2..8, Nb from 1 to 4096, grids 1, 3, 7, the default and one above the tile count, and signal_every 1, 3, 8."""
+    from test_gpu_allgather_fp8_shapes import GEMM_FACTS, GEOMETRY_CASES, UNPACK_FACTS, case_facts, gather_grid
+    seen_k, seen_u = set(), set()
+    for (N, K, rows_per_rec, R, Nb, grid, sig), k, u in GEOMETRY_CASES:
+        assert k and u, "every case claims facts"
+        assert (rows_per_rec * K) % P.TILE_ELEMS == 0 and rows_per_rec % 128 == 0 and K % 32 == 0
+        for q in range(N):
+            assert case_facts(N, K, rows_per_rec, R, Nb, grid, rank=q) == (k, u), (N, K, rows_per_rec, R, Nb, grid, q)
+        assert 16 + N * (gather_grid(N, grid) + 2) <= 132, "SM budget"
+        seen_k |= k
+        seen_u |= u
+    assert seen_k == set(GEMM_FACTS) and seen_u == set(UNPACK_FACTS)
+    cases = [c for c, _, _ in GEOMETRY_CASES]
+    assert {c[0] for c in cases} == set(range(2, 9))
+    assert min(c[4] for c in cases) == 1 and max(c[4] for c in cases) == 4096
+    assert {1, 3, 7, 0} <= {c[5] for c in cases}
+    assert {1, 3, 8} <= {c[6] for c in cases}

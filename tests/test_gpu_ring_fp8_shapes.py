@@ -95,9 +95,10 @@ REDUCE_FACTS = ("multi_tile_run", "boundary_in_step", "step_completes_two", "rec
                 "waits_on_a_later_record")
 
 
-def ring_grid(N, grid):
-    """The grid every launch of an in-process ring of N ranks gets (``link_in_process``): ``grid``, or the default."""
-    return grid or max(1, min(64, (H100_SMS - ENGINE_CTAS) // N - 1))
+def ring_grid(N, grid, waiters=1):
+    """The grid every launch of an in-process ring of N ranks gets (``link_in_process``): ``grid``, or the default
+    beside ``waiters`` one-CTA waiting launches per rank (the consumer, and the all-gather's relay)."""
+    return grid or max(1, min(64, (H100_SMS - ENGINE_CTAS) // N - waiters))
 
 
 def case_facts(N, tpc, R, grid):
@@ -191,8 +192,8 @@ def _check(plans, results, wqe_growth, outs, wants):
         _bf16_equal_up_to_nan(got[0], want)
 
 
-def _sm_budget(N, grid):
-    need = ENGINE_CTAS + N * (ring_grid(N, grid) + 1)
+def _sm_budget(N, grid, waiters=1):
+    need = ENGINE_CTAS + N * (ring_grid(N, grid, waiters) + waiters)
     assert need <= H100_SMS
     return need
 
