@@ -29,7 +29,7 @@ from typing import List
 import torch
 
 from .. import ops
-from ..ops import launch as L, pack as P
+from ..ops import launch as L
 from ..ops.gemm_mx import PANEL_ROWS, MxOperand
 from .ring_fp8 import GUARD, MAX_QUEUE_DEPTH, _pow2, _RingPlan, _run_ranks, link_in_process  # noqa: F401
 
@@ -70,44 +70,28 @@ class RingAllgatherFp8(_RingPlan):
 
     def __init__(self, ctx, shard_elems: int, chunk_elems: int, rank: int, world: int, *, grid: int = 0,
                  timeout_ms: int = 2000, signal_every: int = 1, engine_ctas: int = 16):
-        shard_elems, chunk_elems, rank, world = int(shard_elems), int(chunk_elems), int(rank), int(world)
-        if world < 2:
-            raise ValueError(f"world={world}: a ring needs at least 2 ranks")
-        if not 0 <= rank < world:
-            raise ValueError(f"rank={rank} outside [0, {world})")
-        if chunk_elems <= 0 or chunk_elems % P.TILE_ELEMS:
-            raise ValueError(f"chunk_elems={chunk_elems}: a positive multiple of {P.TILE_ELEMS}")
+        super().__init__(ctx, chunk_elems, rank, world, grid, timeout_ms, signal_every, engine_ctas)
+        shard_elems, world, chunk_elems = int(shard_elems), self.world, self.chunk
         if shard_elems <= 0 or shard_elems % chunk_elems:
             raise ValueError(f"shard_elems={shard_elems} must be a multiple of chunk_elems = {chunk_elems}: "
                              "every shard is whole records")
-        self.ctx, self.n, self.chunk, self.rank, self.world = ctx, shard_elems, chunk_elems, rank, world
-        self.grid, self.timeout_ms, self.signal_every, self.engine_ctas = int(grid), int(timeout_ms), int(signal_every), int(engine_ctas)
-        self.shard = shard_elems
+        self.n = self.shard = shard_elems
         self.R = shard_elems // chunk_elems
-        self.rec = P.record_bytes(chunk_elems)
-        self.n_ids = world * self.R                 # records of the landing region, and arrival words
-        self.n_recv = (world - 1) * self.R          # records received per run
         if self.R > max_records(world):
-            raise ValueError(f"R={self.R} records per shard: the receive queue would need {_pow2(2 * self.n_recv)} entries, "
-                             f"above {MAX_QUEUE_DEPTH}; at world={world} R may be at most {max_records(world)}")
+            raise ValueError(f"R={self.R} records per shard: the receive queue would need "
+                             f"{_pow2(2 * (world - 1) * self.R)} entries, above {MAX_QUEUE_DEPTH}; at world={world} R "
+                             f"may be at most {max_records(world)}")
         # the unpack's counters from the bottom of the plan's scratch slot, the relay's 32 bytes at its top
         if L.counter_bytes(self.R + 3) + L.counter_bytes(1) > L.SLOT_BYTES:
             raise ValueError(f"{self.R} records per shard need more counters than a scratch slot holds")
-        self._DRAIN = world + 3                     # result records: 0 receive, 1 pack, 2 relay, 3.. compute, then these two
-        if self._DRAIN + 2 > L.RING_SLOT_BYTES // L.RECORD_BYTES:
-            raise ValueError(f"world={world}: {self._DRAIN + 2} result records do not fit {L.RING_SLOT_BYTES} bytes")
+        # landing slot s holds shard s; result records: 0 receive, 1 pack, 2 relay, 3.. compute
+        self._allocate(world * self.R, (world - 1) * self.R, world + 3)
         dev = ctx.device
-        self.landing = torch.zeros(self.n_ids * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")
-        self.words_full = torch.zeros(self.n_ids + GUARD, dtype=torch.int64, device=f"cuda:{dev}")
-        self.words = self.words_full[:self.n_ids]
-        order = [s * self.R + r for s in arrival_slots(rank, world) for r in range(self.R)]
+        order = [s * self.R + r for s in arrival_slots(self.rank, world) for r in range(self.R)]
         self.a_order = torch.tensor(order, dtype=torch.int32, device=f"cuda:{dev}")   # K7's walk: every record, as it lands
         self.relay_ids = self.a_order[:self.n_recv]                                    # the relay's: all but slot q+1
-        self.landing_mr = ctx.reg_mr(self.landing)
-        self.consumer_stream = torch.cuda.Stream(device=dev)
-        self.main_stream = torch.cuda.Stream(device=dev)
         self.compute_stream = torch.cuda.Stream(device=dev)
-        self._cleared, self._own_set, self._done = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
+        self._own_set, self._done = torch.cuda.Event(), torch.cuda.Event()
         with torch.cuda.stream(self.consumer_stream):
             # load the fill kernels now (step 2 and the consumer's clear): a first load later would wait for the engine.
             # Step 2 fills one slot's words, and where they start picks torch's kernel (a slot whose words are not 16-
@@ -117,16 +101,6 @@ class RingAllgatherFp8(_RingPlan):
             self.words.zero_()
         self._cleared.record(self.consumer_stream)
         torch.cuda.synchronize(dev)
-        self.send_qp = self.recv_qp = self.remote_landing = None
-        self.scratch_slot = None
-        self.in_process = False
-        self._views = []
-        self._stale_cqes = 0            # receive completions a failed run left unreaped (in-process accounting)
-        self._rq_backlog = 0            # receive WQEs a failed run left posted
-        self._failed = False
-
-    def _slot(self, s):
-        return self.landing[s * self.R * self.rec:(s + 1) * self.R * self.rec], self.words[s * self.R:(s + 1) * self.R]
 
     def _streams(self):
         return (self.consumer_stream, self.main_stream, self.compute_stream)
@@ -204,12 +178,7 @@ class RingAllgatherFp8(_RingPlan):
         may be ``out``'s shard ``rank`` (in place).  With ``sync`` waits and returns a :class:`RingResult`.  Ranks
         simulated in one process must all be enqueued before any is waited for: use :func:`run_in_process`."""
         self._check_run(x, out)
-        self.start_consumer()
-        self.enqueue_main(x, out)
-        if not sync:
-            return None
-        self.synchronize()
-        return self.result()
+        return self._run(lambda: self.enqueue_main(x, out), sync)
 
     def run_gemm(self, x: torch.Tensor, b: MxOperand, c: torch.Tensor, sync: bool = True):
         """The all-gather GEMM of a column-parallel layer: ``c[world * rows, Nb] = dequant(gathered A) @ dequant(b).T``,
@@ -217,12 +186,7 @@ class RingAllgatherFp8(_RingPlan):
         lands, the records this rank holds first.  ``chunk_elems`` must be a multiple of ``128 * K``.  The gathered
         records stay in :meth:`records`."""
         self._check_gemm(x, b, c)
-        self.start_consumer()
-        self.enqueue_gemm(x, b, c)
-        if not sync:
-            return None
-        self.synchronize()
-        return self.result()
+        return self._run(lambda: self.enqueue_gemm(x, b, c), sync)
 
 
 def run_in_process(plans: List[RingAllgatherFp8], xs, outs, sync: bool = True, skip=()):

@@ -115,11 +115,52 @@ class RingResult:
 
 
 class _RingPlan:
-    """What the GPU-driven ring plans share: linking (the receive queue and the next rank's landing region), the consumer
-    stream that receives and stamps every record a run brings, recovery after a failed run, and the result.  A plan
-    sets ``n_recv`` (receives per run), ``n_ids`` (arrival words, ids ``[0, n_ids)``), ``landing`` / ``landing_mr``,
-    ``words`` and the streams."""
+    """What the GPU-driven ring plans share: the arguments both check, the landing region, its arrival words and the
+    streams, linking (the receive queue and the next rank's landing region), the consumer stream that receives and
+    stamps every record a run brings, recovery after a failed run, and the result.  A plan calls
+    ``_RingPlan.__init__``, sets ``shard`` and ``R``, then calls :meth:`_allocate`."""
     WAITERS = 1                 # waiting launches of a rank beside its compute grid: the consumer
+
+    def __init__(self, ctx, chunk_elems: int, rank: int, world: int, grid: int, timeout_ms: int, signal_every: int,
+                 engine_ctas: int):
+        chunk_elems, rank, world = int(chunk_elems), int(rank), int(world)
+        if world < 2:
+            raise ValueError(f"world={world}: a ring needs at least 2 ranks")
+        if not 0 <= rank < world:
+            raise ValueError(f"rank={rank} outside [0, {world})")
+        if chunk_elems <= 0 or chunk_elems % P.TILE_ELEMS:
+            raise ValueError(f"chunk_elems={chunk_elems}: a positive multiple of {P.TILE_ELEMS}")
+        self.ctx, self.chunk, self.rank, self.world = ctx, chunk_elems, rank, world
+        self.grid, self.timeout_ms, self.signal_every, self.engine_ctas = int(grid), int(timeout_ms), int(signal_every), int(engine_ctas)
+        self.rec = P.record_bytes(chunk_elems)
+
+    def _allocate(self, n_ids: int, n_recv: int, n_results: int):
+        """Check the result records, then allocate and register the landing region of ``n_ids`` records, its arrival
+        words with guard words behind them, and the consumer and main streams.  ``n_recv``: records received per run;
+        ``n_results``: result records of a run before the two a failed run's recovery takes."""
+        if n_results + 2 > L.RING_SLOT_BYTES // L.RECORD_BYTES:
+            raise ValueError(f"world={self.world}: {n_results + 2} result records do not fit {L.RING_SLOT_BYTES} bytes")
+        self._DRAIN = n_results         # result records of the drain and of the backlog's receive
+        self.n_ids, self.n_recv = n_ids, n_recv
+        dev = self.ctx.device
+        self.landing = torch.zeros(n_ids * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")
+        self.words_full = torch.zeros(n_ids + GUARD, dtype=torch.int64, device=f"cuda:{dev}")
+        self.words = self.words_full[:n_ids]
+        self.landing_mr = self.ctx.reg_mr(self.landing)
+        self.consumer_stream = torch.cuda.Stream(device=dev)
+        self.main_stream = torch.cuda.Stream(device=dev)
+        self._cleared = torch.cuda.Event()
+        self.send_qp = self.recv_qp = self.remote_landing = None
+        self.scratch_slot = None
+        self.in_process = False
+        self._views = []
+        self._stale_cqes = 0            # receive completions a failed run left unreaped (in-process accounting)
+        self._rq_backlog = 0            # receive WQEs a failed run left posted
+        self._failed = False
+
+    def _slot(self, m):
+        """Landing slot ``m``: its R records and their arrival words."""
+        return self.landing[m * self.R * self.rec:(m + 1) * self.R * self.rec], self.words[m * self.R:(m + 1) * self.R]
 
     # ---------------------------------------------------------------- links
     def _attach(self, send_qp, recv_qp, remote_landing, scratch_slot: int, grid: int, in_process: bool):
@@ -188,6 +229,15 @@ class _RingPlan:
     def _streams(self):
         return (self.consumer_stream, self.main_stream)
 
+    def _run(self, enqueue, sync: bool):
+        """Start the consumer, ``enqueue()`` this rank's other streams, and with ``sync`` wait and return the result."""
+        self.start_consumer()
+        enqueue()
+        if not sync:
+            return None
+        self.synchronize()
+        return self.result()
+
     def synchronize(self):
         for s in self._streams():
             s.synchronize()
@@ -232,56 +282,32 @@ class RingAllreduceFp8(_RingPlan):
 
     def __init__(self, ctx, n_elems: int, chunk_elems: int, rank: int, world: int, *, grid: int = 0,
                  timeout_ms: int = 2000, signal_every: int = 1, engine_ctas: int = 16, error_feedback: bool = False):
-        n_elems, chunk_elems, rank, world = int(n_elems), int(chunk_elems), int(rank), int(world)
-        if world < 2:
-            raise ValueError(f"world={world}: a ring needs at least 2 ranks")
-        if not 0 <= rank < world:
-            raise ValueError(f"rank={rank} outside [0, {world})")
-        if chunk_elems <= 0 or chunk_elems % P.TILE_ELEMS:
-            raise ValueError(f"chunk_elems={chunk_elems}: a positive multiple of {P.TILE_ELEMS}")
+        super().__init__(ctx, chunk_elems, rank, world, grid, timeout_ms, signal_every, engine_ctas)
+        n_elems, world, chunk_elems = int(n_elems), self.world, self.chunk
         if n_elems <= 0 or n_elems % (world * chunk_elems):
             raise ValueError(f"n_elems={n_elems} must be a multiple of world * chunk_elems = {world * chunk_elems}: "
                              "every shard is whole records")
-        if 2 * world + 3 > L.RING_SLOT_BYTES // L.RECORD_BYTES:
-            raise ValueError(f"world={world}: {2 * world + 3} result records do not fit {L.RING_SLOT_BYTES} bytes")
-        self.ctx, self.n, self.chunk, self.rank, self.world = ctx, n_elems, chunk_elems, rank, world
-        self.grid, self.timeout_ms, self.signal_every, self.engine_ctas = int(grid), int(timeout_ms), int(signal_every), int(engine_ctas)
+        self.n = n_elems
         self.shard = n_elems // world
         self.R = self.shard // chunk_elems
-        self.rec = P.record_bytes(chunk_elems)
-        self.n_ids = 2 * (world - 1) * self.R
-        self.n_recv = self.n_ids
         counter_bytes = L.counter_bytes(self.R + 3)       # the reduce's and the unpack's: R records and 3 words
         if counter_bytes > L.SLOT_BYTES:
             raise ValueError(f"{self.R} records per shard need {counter_bytes} bytes of counters; a scratch slot holds 256 KiB")
         if self.R > max_records(world):
-            raise ValueError(f"R={self.R} records per shard: the receive queue would need {_pow2(2 * self.n_ids)} entries, "
-                             f"above {MAX_QUEUE_DEPTH}; at world={world} R may be at most {max_records(world)}")
+            raise ValueError(f"R={self.R} records per shard: the receive queue would need {_pow2(4 * (world - 1) * self.R)} "
+                             f"entries, above {MAX_QUEUE_DEPTH}; at world={world} R may be at most {max_records(world)}")
+        # result records: 0 receive, 1.. the 2N launches of schedule()
+        self._allocate(2 * (world - 1) * self.R, 2 * (world - 1) * self.R, 2 * world + 1)
         dev = ctx.device
         self.staging = torch.zeros(self.R * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")
-        self.landing = torch.zeros(self.n_ids * self.rec, dtype=torch.uint8, device=f"cuda:{dev}")
-        self.words_full = torch.zeros(self.n_ids + GUARD, dtype=torch.int64, device=f"cuda:{dev}")
-        self.words = self.words_full[:self.n_ids]
         self.residual = torch.zeros(n_elems, dtype=torch.float32, device=f"cuda:{dev}") if error_feedback else None
         self.staging_mr = ctx.reg_mr(self.staging)
-        self.landing_mr = ctx.reg_mr(self.landing)
-        self.consumer_stream = torch.cuda.Stream(device=dev)
-        self.main_stream = torch.cuda.Stream(device=dev)
-        self._cleared = torch.cuda.Event()
         with torch.cuda.stream(self.consumer_stream):
             self.words.zero_()              # loads the fill kernel now: a first load later would wait for the engine
             if self.residual is not None:
                 self.residual.zero_()       # and reset_residual()'s
         self._cleared.record(self.consumer_stream)
         torch.cuda.synchronize(dev)
-        self.send_qp = self.recv_qp = self.remote_landing = None
-        self.scratch_slot = None
-        self.in_process = False
-        self._views = []
-        self._stale_cqes = 0            # receive completions a failed run left unreaped (in-process accounting)
-        self._rq_backlog = 0            # receive WQEs a failed run left posted
-        self._failed = False
-        self._DRAIN = 2 * world + 1     # result records of the drain and of the backlog's receive
 
     # ---------------------------------------------------------------- run
     @property
@@ -294,9 +320,6 @@ class RingAllreduceFp8(_RingPlan):
             raise RuntimeError("this plan has no residual: build it with error_feedback=True")
         with torch.cuda.stream(self.main_stream):
             self.residual.zero_()
-
-    def _slot(self, m):
-        return self.landing[m * self.R * self.rec:(m + 1) * self.R * self.rec], self.words[m * self.R:(m + 1) * self.R]
 
     def enqueue_main(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, steps=None):
         """Enqueue this rank's main stream (after :meth:`start_consumer`): K3, the N-1 reduce hops and the N unpacks.
@@ -346,12 +369,7 @@ class RingAllreduceFp8(_RingPlan):
         ``sync`` waits and returns a :class:`RingResult`.  Ranks simulated in one process must all be enqueued before
         any is waited for: use :func:`run_in_process`.  After a run that did not end OK the contents of ``out`` are
         undefined, as with NCCL, and so is ``residual`` with error feedback."""
-        self.start_consumer()
-        self.enqueue_main(x, out)
-        if not sync:
-            return None
-        self.synchronize()
-        return self.result()
+        return self._run(lambda: self.enqueue_main(x, out), sync)
 
 
 def _sms(ctx) -> int:
