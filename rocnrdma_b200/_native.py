@@ -131,6 +131,8 @@ _SIGS = {
     "rn_k_pack_fp8_write": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64, u64]),
     "rn_gemm_timeline": (i32, [C.POINTER(C.c_uint64)]),
     "rn_k_gemm_send": (i32, [u64, i32, u64, u64, u64, u32, u32, u32, u64, u64, u32, u64, u32, u32, u32, u32, u32, u32, u32, u64, u64, u64]),
+    "rn_k_gemm_reduce_send": (i32, [u64, i32, u64, u64, u32, u32, u32, u64, u64, u64, u32, u64, u32, u64, u32, u64, u64, u32, u64,
+                                    u64, u32, u64, u32, u32, u32, u32, u32, u64, u64, u64]),
     "rn_k_gemm_mxfp8": (i32, [u64, i32, u64, u64, u32, u64, u64, u64, u32, u64, u64, u32, u32, u32, u64, u32, u64, u64, u64]),
     "rn_k_gemm_mxfp8_ordered": (i32, [u64, i32, u64, u64, u32, u64, u64, u64, u32, u64, u64, u32, u32, u32, u64, u32, u64, u64, u64,
                                       u64]),

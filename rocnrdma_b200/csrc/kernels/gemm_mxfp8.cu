@@ -27,6 +27,7 @@
 
 #include "../hca/post.cuh"
 #include "mx_scale.cuh"
+#include "record_wait.cuh"
 #include "sm90.cuh"
 
 using namespace rn;
@@ -69,24 +70,6 @@ struct MxArgs {
   const unsigned long long* a_ready;
   uint64_t ready_timeout_ns;
 };
-// bounded wait for a record's arrival word; the acquire orders it before the loads of the record, the proxy fence extends
-// that to the async proxy (TMA reads the record)
-__device__ __forceinline__ bool wait_record(const unsigned long long* ready, uint32_t rec, uint64_t timeout_ns, volatile int* abort) {
-  if (!ready) return true;
-  unsigned long long v, t0 = 0;
-  for (unsigned n = 0;; ++n) {
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ready + rec) : "memory");
-    if (v) break;
-    if (*abort) return false;
-    if ((n & 63) == 63) {
-      if (!t0) t0 = globaltimer_ns();
-      else if (globaltimer_ns() - t0 > timeout_ns) { *abort = 1; return false; }
-      __nanosleep(200);
-    }
-  }
-  asm volatile("fence.proxy.async;" ::: "memory");
-  return true;
-}
 // Result words live in host memory: one atomic per CTA there (the first version's atomicMax of the end time) is a PCIe
 // round trip each -- one per CTA, serialised, cost ~150 us per launch, more than a 4096^3 product.  Count in device memory,
 // let the last CTA write.

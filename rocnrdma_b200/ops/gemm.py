@@ -136,3 +136,141 @@ def parse(view, M, Nn, K) -> GemmResult:
                     M=M, N=Nn, K=K)
     r.stream_k = bool(r.stream_k)
     return r
+
+
+# ------------------------------------------------------------------ K4 with a landed addend
+RS_WORDS = ("records_posted", "t_first_post_ns", "t_compute_end_ns", "records_added")
+
+
+@dataclass
+class ReduceSendResult:
+    status: str
+    t_start_ns: int
+    t_end_ns: int
+    records_posted: int
+    t_first_post_ns: int
+    t_compute_end_ns: int
+    records_added: int
+
+    @property
+    def ok(self) -> bool:
+        return self.status == "OK"
+
+    @property
+    def device_ns(self) -> int:
+        return self.t_end_ns - self.t_start_ns
+
+
+def parse_reduce_send(view) -> ReduceSendResult:
+    """Decode the record :func:`gemm_reduce_send` leaves in the mapped scratch (for ``sync=False`` callers)."""
+    return L.decode_as(ReduceSendResult, view, RS_WORDS)
+
+
+def _host_ids(t, what: str, n: int, device: int, host) -> list:
+    L.tensor_ptr(t, torch.int32, device, what, n, exact=True, align=4)
+    return [int(v) for v in (t.tolist() if host is None else host)]
+
+
+def gemm_reduce_send(ctx, a: torch.Tensor, b: torch.Tensor, *, walk, add_ids, send_ids, qp, staging_mr=None, dst_mr=None,
+                     landing=None, ready=None, out=None, ids_host=None, with_imm: bool = True, signal_every: int = 1,
+                     post_only: bool = False, cta_group: int = 1, group_m: int = 0, direct: bool = False,
+                     plain_stores: bool = False, stream_k: bool = False, grid: int = 0, timeout_ms: int = 2000, stream=None,
+                     sync: bool = True, scratch_slot: int = L.SLOT["gemm_send"], result_off=None):
+    """K4 with a landed addend: one hop of a reduce-scatter of ``a @ b.T``, in one launch.
+
+    ``a`` [M, K] and ``b`` [Nb, K] are contiguous bf16, M a multiple of 128, Nb of 32, K of 8.  The P = M / 128 m-blocks
+    of ``a`` are computed in the order ``walk`` gives (int32 [P], a permutation of 0..P-1); the tile raster runs over
+    walk positions, ``group_m`` of them advancing together across Nb.  Walk position p's 128 x Nb panel, accumulated in
+    fp32, then:
+
+    * adds landed record ``add_ids[p]`` of ``landing`` (uint8 CUDA tensor of fp8 panel records, ``panel_record_bytes(Nb)``
+      apart) once its arrival word ``ready[add_ids[p]]`` (int64) is set, or nothing for -1.  The gate runs after the
+      tile's MMAs, so the tile computes while its record is on the wire.  Each element is ``acc + code * 2^(byte - 127)``,
+      one fp32 multiply and one fp32 add, the bits of :func:`~rocnrdma_b200.ops.reduce_fp8` with an fp32 ``local``;
+    * becomes staging record ``send_ids[p]``: quantised by the fp8 epilogue's rule into ``staging_mr`` at ``id * rec`` and
+      posted by the CTA that finishes it, as one RDMA WRITE (WRITE_IMM with immediate ``id`` when ``with_imm``) to the same
+      offset of ``dst_mr``; or, for -1, the j-th such position stores bf16 rows ``[128 j, 128 j + 128)`` of ``out``
+      (contiguous bf16 [128 * #(-1), Nb]), rounded to nearest even.
+
+    The last CTA posts a flush and waits for it unless ``post_only``.  A word still 0 after ``timeout_ms`` raises a
+    grid-wide flag that ends every other wait too, so a failed launch ends ``TIMEOUT`` within about one timeout; a panel
+    that is not finished is never posted, and fewer posted records than ``send_ids`` holds is ``TIMEOUT``.
+
+    ``walk``, ``add_ids`` and ``send_ids`` are int32 tensors on the context's device.  They are checked on the host from
+    ``ids_host`` (three lists) when given, else by reading them back (which waits for the stream that wrote them).
+    Refused: ids out of range, a walk entry that repeats, a send id used twice, ``cta_group`` other than 1, ``direct``,
+    ``plain_stores`` and ``stream_k``.  With ``ids_host`` the kernel still reads the tensors, and nothing compares the
+    two: lists that differ from the tensors leave the tensors' ids unchecked (out-of-range TMA coordinates and record
+    offsets).  Pass ``ids_host`` only with the values the tensors hold, as ``RingReduceScatterFp8`` does with the ids it
+    built them from.  Returns a :class:`ReduceSendResult`, or ``(view, stream)``
+    with ``sync=False`` (decode with :func:`parse_reduce_send`)."""
+    dev = ctx.device
+    if cta_group != 1:
+        raise ValueError(f"cta_group={cta_group}: the walk runs on the single-CTA tile (cta_group=1)")
+    if direct or plain_stores or stream_k:
+        raise ValueError("gemm_reduce_send has no direct, plain_stores or stream_k variant")
+    for t, what in ((a, "a"), (b, "b")):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16 or t.dim() != 2 or not t.is_contiguous():
+            raise ValueError(f"{what} must be a contiguous 2-D bf16 tensor")
+        L.tensor_ptr(t, torch.bfloat16, dev, what, t.numel(), align=16)
+    M, K = a.shape
+    Nn, K2 = b.shape
+    if K != K2:
+        raise ValueError(f"a has K={K}, b has K={K2}")
+    if M <= 0 or M % BM or Nn <= 0 or Nn % 32 or K <= 0 or K % 8:
+        raise ValueError(f"shape ({M},{Nn},{K}): M must be a multiple of {BM}, Nb of 32 and K of 8")
+    if qp is None:
+        raise ValueError("gemm_reduce_send posts its records and flushes: pass qp")
+    P, rec = M // BM, panel_record_bytes(Nn)
+    hw, ha, hs = ids_host if ids_host is not None else (None, None, None)
+    walk_l = _host_ids(walk, "walk", P, dev, hw)
+    add_l = _host_ids(add_ids, "add_ids", P, dev, ha)
+    send_l = _host_ids(send_ids, "send_ids", P, dev, hs)
+    if sorted(walk_l) != list(range(P)):
+        raise ValueError(f"walk must hold every m-block 0..{P - 1} once")
+    n_land = 0
+    if landing is not None:
+        if not isinstance(landing, torch.Tensor) or landing.dtype != torch.uint8:
+            raise ValueError("landing must be a uint8 tensor of fp8 panel records")
+        L.tensor_ptr(landing, torch.uint8, dev, "landing", landing.numel(), align=16)
+        n_land = landing.numel() // rec
+    if any(i < -1 or i >= n_land for i in add_l):
+        raise ValueError(f"add_ids must lie in [-1, {n_land}): landing holds {n_land} records of {rec} bytes")
+    if n_land and any(i >= 0 for i in add_l):
+        if ready is None:
+            raise ValueError("an addend needs its arrival words: pass ready")
+        L.tensor_ptr(ready, torch.int64, dev, "ready", n_land, align=8)
+    sends = [i for i in send_l if i >= 0]
+    n_staging = 0 if staging_mr is None else staging_mr.length // rec
+    if any(i < -1 for i in send_l) or any(i >= n_staging for i in sends):
+        raise ValueError(f"send_ids must lie in [-1, {n_staging}): staging_mr holds {n_staging} records of {rec} bytes")
+    if len(set(sends)) != len(sends):
+        raise ValueError("a send id may be used once")
+    if sends and (dst_mr is None or dst_mr.length < (max(sends) + 1) * rec):
+        raise ValueError("dst_mr must hold every posted record at its id's offset")
+    if sends and staging_mr.addr % 16:
+        raise ValueError("staging_mr must be 16-byte aligned")
+    out_rows = BM * (P - len(sends))
+    if out_rows:
+        if out is None or out.dtype != torch.bfloat16 or tuple(out.shape) != (out_rows, Nn) or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous bf16 [{out_rows}, {Nn}] tensor: one 128-row block per send id -1")
+        L.tensor_ptr(out, torch.bfloat16, dev, "out", out.numel(), align=16)
+        lo, hi = out.data_ptr(), out.data_ptr() + out.numel() * 2
+        for t in (a, landing):
+            if t is not None and lo < t.data_ptr() + t.numel() * t.element_size() and t.data_ptr() < hi:
+                raise ValueError("out must not overlap a or landing")
+    if group_m == 0:
+        group_m = next(g for g in (4, 2, 1) if P % g == 0)
+    lib = N.load()
+    ws = work_stream(ctx, stream)
+    counters = L.counters(ctx, P + 3, scratch_slot)      # per m-block ; CTAs done ; abort flag ; records added
+    out_addr, out_view = L.result(ctx, L.result_offset(scratch_slot, result_off))
+    rc = lib.rn_k_gemm_reduce_send(
+        _stream_ptr(ws), grid, a.data_ptr(), b.data_ptr(), M, Nn, K, walk.data_ptr(), add_ids.data_ptr(),
+        send_ids.data_ptr(), len(sends), staging_mr.addr if staging_mr is not None else 0, n_staging,
+        landing.data_ptr() if landing is not None else 0, n_land, ready.data_ptr() if ready is not None else 0,
+        out.data_ptr() if out_rows else 0, out_rows, qp.dev_ptr, staging_mr.addr if staging_mr is not None else 0,
+        staging_mr.lkey if staging_mr is not None else 0, dst_mr.addr if dst_mr is not None else 0,
+        dst_mr.rkey if dst_mr is not None else 0, signal_every, int(with_imm) | (2 if post_only else 0), cta_group, group_m,
+        counters, out_addr, timeout_ms)
+    return L.finish(rc, "gemm_reduce_send", out_view, ws, sync, parse_reduce_send)

@@ -518,3 +518,24 @@ def reduce_fp8(ctx, records: torch.Tensor, n_src: int, n_elems: int, chunk_elems
                              dst_mr.rkey if dst_mr is not None else 0, int(with_imm) | (2 if post_only else 0), signal_every,
                              counters, res_addr, timeout_ms, imm_base, res_ptr)
     return L.finish(rc, "reduce_fp8", res_view, ws, sync, parse_reduce, hbm)
+
+
+def ref_reduce_scatter_fp8(xs, chunk_elems: int):
+    """Reference of the fp8 ring reduce-scatter (:class:`~rocnrdma_b200.parallel.reduce_scatter_fp8.RingReduceScatterFp8`),
+    bit for bit; runs on CPU or GPU.  ``xs``: the N ranks' tensors of n elements each, bf16 (``run``) or fp32 partials
+    (``run_gemm``, whose records are one 128-row panel each: ``chunk_elems = 128 * Nb``).  Returns the list of the N
+    ranks' bf16 shards, rank s's being the reduction of elements ``[s * n / N, (s + 1) * n / N)``.
+
+    Shard s starts as :func:`ref_pack_fp8` of rank s+1's part and is reduced with the parts of ranks s+2, ..., s (indices
+    mod N), in that order, one :func:`ref_reduce_fp8` hop each (the addend first, then the decoded records, one fp32 add).
+    The last hop's bf16 sum is the output: unlike the all-reduce, nothing is quantised after it."""
+    N = len(xs)
+    m = xs[0].numel() // N
+    out = []
+    for s in range(N):
+        part = slice(s * m, (s + 1) * m)
+        recs = ref_pack_fp8(xs[(s + 1) % N].reshape(-1)[part], chunk_elems)
+        for h in range(2, N + 1):
+            y, recs = ref_reduce_fp8(recs, 1, m, chunk_elems, local=xs[(s + h) % N].reshape(-1)[part])
+        out.append(y)
+    return out

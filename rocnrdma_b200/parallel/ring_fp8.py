@@ -35,7 +35,7 @@ from typing import List, Optional
 import torch
 
 from .. import ops
-from ..ops import launch as L, pack as P
+from ..ops import gemm as G, launch as L, pack as P
 from ..ops.rdma import RECV_WORDS
 
 GUARD = 8                       # zero words behind the arrival words
@@ -73,7 +73,7 @@ def schedule(rank: int, world: int) -> List[Step]:
 
 # the words of each kind of launch's result record, after the header
 _WORDS = {"pack": P.PACK_WORDS, "reduce": P.REDUCE_WORDS, "unpack": P.UNPACK_WORDS, "recv": RECV_WORDS,
-          "relay": P.RELAY_WORDS, "gemm": ()}
+          "relay": P.RELAY_WORDS, "gemm": (), "gemm_rs": G.RS_WORDS}
 
 
 def _pow2(n: int) -> int:
