@@ -129,6 +129,8 @@ _SIGS = {
     "rn_pack_record_bytes": (u64, [u64]),
     "rn_pack_tile_elems": (u32, []),
     "rn_k_pack_fp8_write": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u32, u64, u32, u32, u32, u64, u64, u64, u64]),
+    "rn_k_pack_fp8_scatter": (i32, [u64, i32, u64, u64, u64, u32, u32, u32, C.POINTER(u64), C.POINTER(u64), C.POINTER(u32),
+                                    u64, u32, u64, u64, u32, u32, u64, u64, u64]),
     "rn_gemm_timeline": (i32, [C.POINTER(C.c_uint64)]),
     "rn_k_gemm_send": (i32, [u64, i32, u64, u64, u64, u32, u32, u32, u64, u64, u32, u64, u32, u32, u32, u32, u32, u32, u32, u64, u64, u64]),
     "rn_k_gemm_reduce_send": (i32, [u64, i32, u64, u64, u32, u32, u32, u64, u64, u64, u32, u64, u32, u64, u32, u64, u64, u32, u64,
@@ -138,6 +140,7 @@ _SIGS = {
                                       u64]),
     "rn_k_shared_post_stress": (i32, [u64, u64, i32, u64, u32, u64, u32, u32, u64, u64, u64]),
     "rn_k_recv_consume": (i32, [u64, u64, u32, u32, u64, u64, u64, u64, u32, u32]),
+    "rn_k_recv_consume_qps": (i32, [u64, C.POINTER(u64), C.POINTER(u32), u32, u32, u32, u64, u64, u64, u64, u32]),
     "rn_hca_enable_peer": (i32, [vp, i32]),
     "rn_k_unpack_fp8": (i32, [u64, i32, u64, u64, u64, u32, u64, u64, u64, u64, u64, u64, u64, u32, u64, u32, u32, u32, u32]),
     "rn_k_relay_records": (i32, [u64, u64, u64, u32, u32, u64, u64, u32, u64, u32, u64, u32, u32, u64, u64, u64]),

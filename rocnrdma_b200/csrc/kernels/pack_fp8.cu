@@ -8,6 +8,9 @@
 //                          chunks i+1.. are still being packed.  The kernel ends only when
 //                          the last CQE has been seen: its device time is the whole
 //                          pack+transfer pipeline.
+//  pack_fp8_scatter_kernel K3 of an all-to-all: every shard of x in one launch, in phase order, each record posted
+//                          to its own rank's queue pair as it completes; the own shard's records stay in place and
+//                          get their arrival words stamped.
 //  unpack_fp8_kernel       consumer: optionally waits for each record's arrival (receive
 //                          CQE carrying the chunk id as immediate), then fp8 -> bf16; <true> also
 //                          forwards each record unchanged, from where it landed, as soon as it is seen.
@@ -315,6 +318,87 @@ __global__ void __launch_bounds__(kPackThreads) pack_fp8_write_kernel(PackArgs a
     a.out[4] = first;
     a.out[5] = t_pack_end;
     a.counters[a.n_chunks] = 0;
+  }
+}
+
+// ---- scatter: K3 of an all-to-all.  x holds `world` shards of `p.n_elems` elements, R = p.n_chunks records each; shard
+// d goes to rank d.  One launch packs every shard, in phase order: phase j is shard (rank + j) mod world, so phase 0 is
+// the own shard and at each phase every rank of a mesh sends to one peer.  Record r of shard d != rank is packed into the
+// send staging at (d R + r) * rec and posted on qps[d] to remote_va[d] + (rank R + r) * rec -- slot `rank` of rank d's
+// landing region -- with immediate rank R + r, as soon as it is complete.  The own shard's records are written into the
+// plan's own landing slot (`own`) and nothing is posted for them: their arriver stamps own_words[r] with the same
+// st.release.gpu the receive consumer uses, so a reader gated on the words starts on them while the pack still runs.
+constexpr int kMaxScatter = 8;
+struct ScatterArgs {
+  PackArgs p;                // src, staging, n_elems (one shard), chunk_elems, n_chunks (R), staging_va, lkey, with_imm,
+                             // post_only, signal_every, counters ([world R] groups per record ; CTAs done), out,
+                             // timeout_ns; acc: 3 words per destination.  p.qp, p.rkey, p.remote_va, p.direct and
+                             // p.residual are unused.
+  QpDev* qps[kMaxScatter];   // qps[d]: the send QP to rank d (qps[rank] unused)
+  uint64_t remote_va[kMaxScatter];   // rank d's landing region
+  uint32_t rkey[kMaxScatter];
+  uint8_t* own;              // this rank's landing slot `rank`: R records
+  unsigned long long* own_words;     // its R arrival words
+  uint32_t rank, world;
+  unsigned long long* counts;        // second result record: word d = records posted to rank d
+};
+
+__global__ void __launch_bounds__(kPackThreads) pack_fp8_scatter_kernel(ScatterArgs a) {
+  const unsigned long long t_start = globaltimer_ns();
+  const uint32_t tiles_per_chunk = a.p.chunk_elems / kTileElems;
+  const uint64_t rec = record_bytes(a.p.chunk_elems);
+  const uint32_t G = tiles_per_chunk % 4 == 0 ? 4 : (tiles_per_chunk % 2 == 0 ? 2 : 1);   // as pack_fp8_write_kernel<false>
+  const uint32_t R = a.p.n_chunks, groups_per_chunk = tiles_per_chunk / G;
+  const uint64_t groups_per_shard = (uint64_t)R * groups_per_chunk, n_groups = groups_per_shard * a.world;
+  for (uint64_t grp = blockIdx.x; grp < n_groups; grp += gridDim.x) {
+    const uint32_t d = (uint32_t)((a.rank + grp / groups_per_shard) % a.world);
+    const uint64_t first_tile = grp % groups_per_shard * G;
+    const uint32_t chunk = (uint32_t)(first_tile / tiles_per_chunk);
+    PackArgs p = a.p;
+    p.src = a.p.src + (uint64_t)d * a.p.n_elems;
+    p.staging = d == a.rank ? a.own : a.p.staging + (uint64_t)d * R * rec;
+    if (G == 4) pack_group<4, false>(p, first_tile, tiles_per_chunk, rec);
+    else if (G == 2) pack_group<2, false>(p, first_tile, tiles_per_chunk, rec);
+    else pack_group<1, false>(p, first_tile, tiles_per_chunk, rec);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      fence_gpu();   // release this group's record bytes (all threads, via the barrier) before the count
+      unsigned int* count = &a.p.counters[(uint64_t)d * R + chunk];
+      if (d == a.rank) {
+        // complete_run posts when its queue pair is non-null: the own slot has none, so it gets the words as its
+        // stand-in, and its "post" is the arrival stamp behind a gpu-scope fence
+        complete_run(count, 1, groups_per_chunk, nullptr, reinterpret_cast<const QpDev*>(a.own_words), false, [&] {
+          asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(a.own_words + chunk), "l"(globaltimer_ns()) : "memory");
+        });
+      } else {
+        QpDev* qp = a.qps[d];
+        complete_run(count, 1, groups_per_chunk, nullptr, qp, poster_sys(qp), [&] {
+          post_record(qp, a.p.with_imm ? OP_RDMA_WRITE_IMM : OP_RDMA_WRITE, a.p.staging_va + ((uint64_t)d * R + chunk) * rec,
+                      a.p.lkey, a.remote_va[d] + ((uint64_t)a.rank * R + chunk) * rec, a.rkey[d], (uint32_t)rec,
+                      a.rank * R + chunk, a.p.signal_every, a.p.acc + 3 * d, a.p.out, a.p.timeout_ns);
+        });
+      }
+    }
+  }
+  // ---- the CTA that finishes last flushes every destination's queue pair
+  if (last_cta(&a.p.counters[(uint64_t)a.world * R])) {
+    const unsigned long long t_pack_end = globaltimer_ns();
+    fence_gpu();
+    unsigned long long total = 0, first_all = ~0ull;
+    for (uint32_t d = 0; d < a.world; ++d) {
+      if (d == a.rank) continue;
+      unsigned long long first;
+      const unsigned long long posted = flush_records(a.qps[d], a.p.post_only, a.p.timeout_ns, R, a.p.acc + 3 * d, a.p.out, first);
+      a.counts[d] = posted;
+      total += posted;
+      if (posted && first < first_all) first_all = first;
+    }
+    a.p.out[1] = t_start;
+    a.p.out[2] = globaltimer_ns();
+    a.p.out[3] = total;
+    a.p.out[4] = total ? first_all : 0;
+    a.p.out[5] = t_pack_end;
+    a.p.counters[(uint64_t)a.world * R] = 0;
   }
 }
 
@@ -752,6 +836,42 @@ RN_API int rn_k_pack_fp8_write(uint64_t stream, int grid, uint64_t src, uint64_t
   return (int)cudaGetLastError();
 }
 
+// src: world shards of shard_elems bf16; staging: world * R records (shard d's at d * R; the own shard's are unused),
+// registered at staging_va / lkey; own: R records, own_words: R arrival words.  qps_host / remote_va_host / rkeys_host:
+// world entries, entry `rank` ignored.  counters_dev: >= (world * R + 1) * 4 bytes (rounded up to 8) + 24 * world of
+// zeroed device memory, cleaned by the kernel.  out_dev: two result records.  flags: bit 0 RDMA_WRITE_IMM, bit 1 post_only.
+RN_API int rn_k_pack_fp8_scatter(uint64_t stream, int grid, uint64_t src, uint64_t staging, uint64_t shard_elems,
+                                 uint32_t chunk_elems, uint32_t rank, uint32_t world, const uint64_t* qps_host,
+                                 const uint64_t* remote_va_host, const uint32_t* rkeys_host, uint64_t staging_va,
+                                 uint32_t lkey, uint64_t own, uint64_t own_words, uint32_t flags, uint32_t signal_every,
+                                 uint64_t counters_dev, uint64_t out_dev, uint64_t timeout_ms) {
+  if (world < 2 || world > (uint32_t)kMaxScatter || rank >= world || !own_words || !shard_elems) return -22;
+  if ((src | staging | own) & 31) return -22;                  // 256-bit loads, 128-bit stores
+  ScatterArgs a;
+  for (uint32_t d = 0; d < world; ++d) {
+    a.qps[d] = d == rank ? nullptr : (QpDev*)qps_host[d];
+    if (d != rank && !a.qps[d]) return -22;
+    a.remote_va[d] = remote_va_host[d];
+    a.rkey[d] = rkeys_host[d];
+  }
+  if (shard_elems % chunk_elems) return -22;
+  if (int rc = launch_setup(world * shard_elems, chunk_elems, out_dev, timeout_ms, 4, grid, a.p.timeout_ns)) return rc;
+  a.counts = clear_record(out_dev + 64);
+  a.p.src = (const __nv_bfloat16*)src; a.p.staging = (uint8_t*)staging; a.p.n_elems = shard_elems;
+  a.p.chunk_elems = chunk_elems; a.p.n_chunks = (uint32_t)(shard_elems / chunk_elems); a.p.qp = nullptr;
+  a.p.staging_va = staging_va; a.p.lkey = lkey; a.p.rkey = 0; a.p.remote_va = 0;
+  a.p.with_imm = flags & 1u; a.p.post_only = (flags >> 1) & 1u; a.p.direct = 0;
+  a.p.signal_every = signal_every ? signal_every : 1;
+  a.p.counters = (unsigned int*)counters_dev;
+  a.p.acc = acc_after(counters_dev, (uint64_t)world * a.p.n_chunks + 1);
+  a.p.out = (unsigned long long*)out_dev;
+  a.p.residual = nullptr;
+  a.own = (uint8_t*)own; a.own_words = (unsigned long long*)own_words;
+  a.rank = rank; a.world = world;
+  pack_fp8_scatter_kernel<<<grid, kPackThreads, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
 // arrived_dev: >= (n_chunks + 3) * 4 bytes of zeroed device memory, and with fwd_qp (rounded up to 8) + 24 more.
 // fwd_flags: bit 0 RDMA_WRITE_IMM (immediate = imm_base + record id), bit 1 post_only.
 RN_API int rn_k_unpack_fp8(uint64_t stream, int grid, uint64_t staging, uint64_t dst, uint64_t n_elems,
@@ -841,6 +961,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_pack() {
   cudaFuncAttributes at;
   cudaFuncGetAttributes(&at, pack_fp8_write_kernel<false>);
   cudaFuncGetAttributes(&at, pack_fp8_write_kernel<true>);
+  cudaFuncGetAttributes(&at, pack_fp8_scatter_kernel);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<false>);
   cudaFuncGetAttributes(&at, unpack_fp8_kernel<true>);
   cudaFuncGetAttributes(&at, relay_records_kernel);

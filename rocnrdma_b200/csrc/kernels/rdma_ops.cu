@@ -290,6 +290,60 @@ RN_API int rn_k_recv_consume(uint64_t stream, uint64_t qp_dev, uint32_t n, uint3
   return (int)cudaGetLastError();
 }
 
+// The consumer of a mesh: up to kMaxRecvQps receive QPs, one per source, that share one receive CQ.  The kernel first
+// posts prepost[i] zero-length receive WQEs on qps[i] (RDMA_WRITE_IMM ignores the buffer), then takes `n` completions
+// from the shared CQ and stamps each by its immediate, as recv_consume_kernel does.  recv_wait ignores the QP number of
+// a receive completion and the engine claims the CQ's producer index atomically, so completions of every QP arrive on
+// the one CQ in the order the engine claimed them.  out: as recv_consume_kernel's.
+constexpr int kMaxRecvQps = 7;
+struct RecvQpsArgs {
+  QpDev* qps[kMaxRecvQps];
+  uint32_t prepost[kMaxRecvQps];
+  uint32_t nqp, n, max_imm;
+  uint64_t prepost_addr;
+  uint32_t prepost_lkey;
+  unsigned long long* stamps;
+  unsigned long long* out;
+  unsigned long long timeout_ns;
+};
+
+__global__ void __launch_bounds__(32, 1) recv_consume_qps_kernel(RecvQpsArgs a) {
+  if (threadIdx.x != 0) return;
+  const unsigned long long t0 = globaltimer_ns();
+  for (uint32_t q = 0; q < a.nqp; ++q)
+    for (uint32_t i = 0; i < a.prepost[q]; ++i) post_recv(a.qps[q], a.prepost_addr, a.prepost_lkey, 0);
+  unsigned long long bytes = 0;
+  uint32_t seen = 0;
+  int status = WAIT_OK;
+  while (seen < a.n) {
+    uint32_t imm = 0;
+    long long got = recv_wait(a.qps[0], &imm, a.timeout_ns);
+    if (got < 0) { status = (int)got; break; }
+    if (a.stamps && imm < a.max_imm)
+      asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(a.stamps + imm), "l"(globaltimer_ns()) : "memory");
+    bytes += (unsigned long long)got;
+    ++seen;
+  }
+  a.out[0] = (unsigned long long)(long long)status;
+  a.out[1] = t0; a.out[2] = globaltimer_ns(); a.out[3] = seen; a.out[4] = bytes;
+}
+// qps_host / prepost_host: nqp (1..7) queue pairs and the receive WQEs to post on each.  The caller guarantees that
+// they share one receive CQ.
+RN_API int rn_k_recv_consume_qps(uint64_t stream, const uint64_t* qps_host, const uint32_t* prepost_host, uint32_t nqp,
+                                 uint32_t n, uint32_t max_imm, uint64_t stamps_dev, uint64_t out_dev, uint64_t timeout_ms,
+                                 uint64_t prepost_addr, uint32_t prepost_lkey) {
+  RecvQpsArgs a;
+  if (!copy_qps(a.qps, qps_host, nqp)) return -22;
+  for (uint32_t i = 0; i < nqp; ++i) a.prepost[i] = prepost_host[i];
+  a.nqp = nqp; a.n = n; a.max_imm = max_imm;
+  a.prepost_addr = prepost_addr; a.prepost_lkey = prepost_lkey;
+  a.stamps = (unsigned long long*)stamps_dev;
+  a.out = clear_record(out_dev);
+  a.timeout_ns = timeout_ns(timeout_ms);
+  recv_consume_qps_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
 // ---------------------------------------------------------------- remote atomics (device-posted)
 // One warp per QP, posting CS / FA work requests with the exclusive Poster exactly like rdma_stream_kernel: bursts
 // share one reservation and one doorbell, the window bounds the outstanding WQEs.  Op i of CTA c targets the word at
@@ -920,6 +974,7 @@ extern "C" __attribute__((visibility("default"))) void rn_preload_rdma_ops() {
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, rdma_stream_kernel);
   cudaFuncGetAttributes(&a, recv_consume_kernel);
+  cudaFuncGetAttributes(&a, recv_consume_qps_kernel);
   cudaFuncGetAttributes(&a, shared_post_stress_kernel);
   cudaFuncGetAttributes(&a, write_read_kernel);
   cudaFuncGetAttributes(&a, atomic_stream_kernel);

@@ -2,6 +2,7 @@
 the receive-side unpack, the reduction of several sources' records, and the bit-exact PyTorch references of all three."""
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 
 import torch
@@ -221,7 +222,87 @@ def parse_relay(view) -> dict:
     return L.decode(view, RELAY_WORDS)
 
 
-# ------------------------------------------------------------------ bit-exact references
+# ------------------------------------------------------------------ scatter
+MAX_SCATTER = 8                 # ranks of one pack_fp8_scatter launch (pack_fp8.cu kMaxScatter)
+SCATTER_WORDS = PACK_WORDS
+
+
+def pack_fp8_scatter(ctx, x: torch.Tensor, rank: int, world: int, staging_mr, own: torch.Tensor, own_words: torch.Tensor,
+                     qps, dst_mrs, chunk_elems: int = 1 << 20, *, with_imm: bool = True, signal_every: int = 1,
+                     post_only: bool = False, residual=None, grid: int = 0, timeout_ms: int = 2000, stream=None,
+                     sync: bool = True, scratch_slot: int = SLOT["pack"], result_off=None):
+    """K3 of an all-to-all: pack ``world`` shards of ``x`` (bf16, shard d = ``x[d * n:(d + 1) * n]``, R = n /
+    ``chunk_elems`` records each) in one launch and post shard d to rank d as its records complete.
+
+    Shards are packed in phase order: phase j is shard ``(rank + j) % world``, phase 0 the own shard.  Record r of shard
+    d != ``rank`` is packed into ``staging_mr`` at record ``d * R + r`` and posted on ``qps[d]`` to ``dst_mrs[d]`` at
+    record ``rank * R + r`` -- slot ``rank`` of rank d's landing region -- as an RDMA WRITE_IMM with immediate ``rank * R
+    + r`` (WRITE without ``with_imm``).  The own shard's R records are written into ``own`` (uint8, R records: this rank's
+    landing slot) and nothing is posted for them; the CTA that completes record r stamps ``own_words[r]`` (int64, R words)
+    with a release store, as the receive consumer stamps landed records, so a reader gated on those words starts on
+    them while the pack still runs.  ``qps[rank]`` and ``dst_mrs[rank]`` are ignored (None is fine).
+
+    The last CTA posts one flush on every destination's queue pair and waits for them unless ``post_only``; the status is
+    ``TIMEOUT`` when fewer than R records went to some destination.  There is no error feedback: an all-to-all quantises
+    every value once, so ``residual`` is refused.  The counters sit at the top of ``scratch_slot`` (as the relay's), so the
+    pack runs beside a launch that keeps its counters at the start of the same slot.  Two result records at
+    ``result_off`` (default: the first two ring records of ``scratch_slot``): the first is K3's (``wqes`` = records
+    posted in all), word d of the second the records posted to rank d.  Returns ``(PackResult, counts)`` or, with
+    ``sync=False``, ``(view, stream)`` (decode with :func:`parse_scatter`)."""
+    if residual is not None:
+        raise ValueError("pack_fp8_scatter has no error feedback: an all-to-all quantises every value once, so there is "
+                         "no error to carry into a later call")
+    rank, world, chunk_elems = int(rank), int(world), int(chunk_elems)
+    if not 2 <= world <= MAX_SCATTER or not 0 <= rank < world:
+        raise ValueError(f"rank={rank}, world={world}: 2..{MAX_SCATTER} ranks")
+    dev = ctx.device
+    L.tensor_ptr(x, torch.bfloat16, dev, "x", 1, align=32)
+    total = x.numel()
+    n = total // world
+    if total % world or n % TILE_ELEMS or chunk_elems <= 0 or chunk_elems % TILE_ELEMS or n % chunk_elems:
+        raise ValueError(f"x holds {total} elements: {world} shards of a multiple of chunk_elems={chunk_elems}, itself a "
+                         f"multiple of {TILE_ELEMS}")
+    R, rec = n // chunk_elems, record_bytes(chunk_elems)
+    L.tensor_ptr(own, torch.uint8, dev, "own", R * rec, exact=True, align=32)
+    L.tensor_ptr(own_words, torch.int64, dev, "own_words", R, exact=True)
+    if staging_mr.length < world * R * rec:
+        raise ValueError(f"staging_mr holds {staging_mr.length} bytes; {world} shards of {R} records need {world * R * rec}")
+    if staging_mr.addr & 31:
+        raise ValueError("staging_mr must be 32-byte aligned")
+    if len(qps) != world or len(dst_mrs) != world:
+        raise ValueError(f"qps and dst_mrs: one entry per rank ({world})")
+    peers = [d for d in range(world) if d != rank]
+    if any(qps[d] is None or dst_mrs[d] is None for d in peers):
+        raise ValueError("every other rank needs a queue pair and a landing region")
+    if any(dst_mrs[d].length < (rank + 1) * R * rec for d in peers):
+        raise ValueError(f"a destination's landing region cannot hold slot {rank} ({R} records of {rec} bytes)")
+    U64, U32 = C.c_uint64 * world, C.c_uint32 * world
+    qp_arr = U64(*[0 if d == rank else qps[d].dev_ptr for d in range(world)])
+    va_arr = U64(*[0 if d == rank else dst_mrs[d].addr for d in range(world)])
+    rk_arr = U32(*[0 if d == rank else dst_mrs[d].rkey for d in range(world)])
+    lib = N.load()
+    ws = work_stream(ctx, stream)
+    # [world R] groups packed per record ; CTAs done ; then post_record's three words per destination
+    nb = L.counter_bytes(world * R + 1) + 24 * (world - 1)
+    L.counters(ctx, 1, scratch_slot)        # checks the slot
+    if nb > L.SLOT_BYTES:
+        raise ValueError(f"{world} shards of {R} records need {nb} bytes of counters; a scratch slot holds {L.SLOT_BYTES}")
+    counters = ctx.dev_scratch(nb, offset=(scratch_slot + 1) * L.SLOT_BYTES - nb)
+    off = L.ring_result_offset(scratch_slot, 0) if result_off is None else L.scratch_offset(result_off, 2)
+    out_addr, out_view = L.result(ctx, off, 2)
+    rc = lib.rn_k_pack_fp8_scatter(_stream_ptr(ws), grid, x.data_ptr(), staging_mr.addr, n, chunk_elems, rank, world,
+                                   qp_arr, va_arr, rk_arr, staging_mr.addr, staging_mr.lkey, own.data_ptr(),
+                                   own_words.data_ptr(), int(with_imm) | (2 if post_only else 0), signal_every, counters,
+                                   out_addr, timeout_ms)
+    return L.finish(rc, "pack_fp8_scatter", out_view, ws, sync, parse_scatter, total, world * R * rec - R * rec)
+
+
+def parse_scatter(view, n_elems: int = 0, wire: int = 0):
+    """Decode the two records :func:`pack_fp8_scatter` leaves: ``(PackResult, counts)``, ``counts[d]`` the records posted
+    to rank d (0 for the own rank)."""
+    counts = list((C.c_int64 * 8).from_buffer(view, L.RECORD_BYTES))
+    return _parse(view, n_elems, wire), counts
+
 # Non-finite rule (the kernels' behaviour, which these references reproduce bit for bit):
 #   * the block amax ignores NaN (the kernels reduce with fmaxf), so a NaN stays in its own element and its
 #     finite neighbours quantise as if it were absent;
@@ -395,6 +476,19 @@ def ref_allgather_fp8(shards, chunk_elems: int):
     recs = torch.cat([ref_pack_fp8(x.reshape(-1), chunk_elems) for x in shards])
     n = sum(x.numel() for x in shards)
     return ref_unpack_fp8(recs, n, chunk_elems), recs
+
+
+def ref_alltoall_fp8(xs, chunk_elems: int):
+    """Reference of the fp8 all-to-all (:class:`~rocnrdma_b200.parallel.alltoall_fp8.AllToAllFp8`), bit for bit; runs on
+    CPU or GPU.  ``xs``: the N ranks' bf16 tensors of N equal shards each, shard d going to rank d.  Returns ``(outs,
+    records)``, one entry per rank q: ``records[q]`` is what lands on rank q, slot s holding :func:`ref_pack_fp8` of rank
+    s's shard q, and ``outs[q]`` its dequantisation (:func:`ref_unpack_fp8`), shard s at element ``s * n``, as
+    ``torch.distributed.all_to_all_single`` lays it out with equal splits."""
+    N = len(xs)
+    m = xs[0].numel() // N
+    records = [torch.cat([ref_pack_fp8(xs[s].reshape(-1)[q * m:(q + 1) * m], chunk_elems) for s in range(N)])
+               for q in range(N)]
+    return [ref_unpack_fp8(r, N * m, chunk_elems) for r in records], records
 
 
 # ------------------------------------------------------------------ reduce

@@ -1,6 +1,7 @@
 """K1 / K2 / K6 wrappers: GPU-initiated RDMA streams and verification helpers."""
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 from typing import List
 
@@ -174,10 +175,36 @@ def recv_consume(qp, n: int, max_imm: int = 0, stamps=None, timeout_ms: int = 20
 
 
 RECV_WORDS = ("seen", "bytes")
+MAX_RECV_QPS = 7                # queue pairs of one recv_consume_qps launch (rdma_ops.cu kMaxRecvQps)
 
 
 def parse_recv(view) -> dict:
     return L.decode(view, RECV_WORDS)
+
+
+def recv_consume_qps(qps, n: int, prepost, prepost_mr, max_imm: int = 0, stamps=None, timeout_ms: int = 2000,
+                     stream=None, sync: bool = True, scratch_off: int = MAPPED["recv_consume"].offset):
+    """:func:`recv_consume` over several receive queue pairs that share one receive CQ (a mesh's receiver: one QP per
+    source).  The kernel first posts ``prepost[i]`` zero-length receive WQEs on ``qps[i]`` (``prepost_mr`` gives their
+    address and lkey; RDMA_WRITE_IMM ignores the buffer), then takes ``n`` completions from the shared CQ, whichever QP
+    they belong to, and with ``stamps`` stamps %globaltimer into word ``imm`` of each one whose immediate is below
+    ``max_imm``.  1..7 queue pairs.  Returns ``dict(status, seen, bytes, ...)``, or ``(view, stream)`` with
+    ``sync=False`` (decode with :func:`parse_recv`)."""
+    qps, qp_arr = L.qp_array(qps)
+    if not 1 <= len(qps) <= MAX_RECV_QPS:
+        raise ValueError(f"{len(qps)} queue pairs: recv_consume_qps takes 1..{MAX_RECV_QPS}")
+    if any(q.rcq is not qps[0].rcq for q in qps):
+        raise ValueError("recv_consume_qps: the queue pairs must share one receive CQ")
+    prepost = [int(k) for k in prepost]
+    if len(prepost) != len(qps) or any(k < 0 or k > q.rq_depth for k, q in zip(prepost, qps)):
+        raise ValueError("prepost: one count per queue pair, each between 0 and its receive queue's depth")
+    ctx = qps[0].ctx
+    ws = work_stream(ctx, stream)
+    out_addr, out_view = L.result(ctx, scratch_off)
+    rc = N.load().rn_k_recv_consume_qps(_stream_ptr(ws), qp_arr, (C.c_uint32 * len(qps))(*prepost), len(qps), n, max_imm,
+                                        stamps.data_ptr() if stamps is not None else 0, out_addr, timeout_ms,
+                                        prepost_mr.addr, prepost_mr.lkey)
+    return L.finish(rc, "recv_consume_qps", out_view, ws, sync, parse_recv)
 
 
 def shared_post_stress(qp, src_mr, dst_mr, ctas: int = 64, per_cta: int = 64, timeout_ms: int = 3000, stream=None):

@@ -129,3 +129,28 @@ def connect_ring(ctx, qp, mrs, group=None, describe=None, connect=None):
     remote = (connect or connect_to)(ctx, qp, infos[nxt])
     dist.barrier(group=group)           # everybody is mapped before anybody starts writing
     return nxt, remote
+
+
+def connect_mesh(ctx, send_qps, recv_qps, mrs, group=None, describe=None, connect=None):
+    """All ranks call this: the full mesh of an all-to-all.  ``send_qps[d]`` and ``recv_qps[s]`` are this rank's queue
+    pairs to rank d and from rank s (entry ``rank`` of each is ignored).  Every rank publishes one description per
+    receive QP, with ``mrs``, and connects its send QP for rank d to rank d's receive QP for this rank.  Returns ``{d:
+    {rkey: RemoteMR}}``: what this rank may write to on each peer.  ``describe`` / ``connect`` as in
+    :func:`connect_ring`."""
+    import torch.distributed as dist
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    if len(send_qps) != world or len(recv_qps) != world:
+        raise ValueError(f"send_qps and recv_qps: one entry per rank ({world})")
+    mine = {s: (describe or describe_local)(ctx, recv_qps[s], mrs, rank) for s in range(world) if s != rank}
+    infos: List[Optional[Dict[int, PeerInfo]]] = [None] * world
+    dist.all_gather_object(infos, mine, group=group)
+    remote: Dict[int, Dict[int, RemoteMR]] = {}
+    for d in range(world):
+        if d == rank:
+            continue
+        info = (infos[d] or {}).get(rank)
+        if info is None or info.rank != d:
+            raise RuntimeError(f"rank {rank}: rendezvous returned no description of rank {d}'s receive queue pair for it")
+        remote[d] = (connect or connect_to)(ctx, send_qps[d], info)
+    dist.barrier(group=group)           # everybody is mapped before anybody starts writing
+    return remote

@@ -73,7 +73,7 @@ def schedule(rank: int, world: int) -> List[Step]:
 
 # the words of each kind of launch's result record, after the header
 _WORDS = {"pack": P.PACK_WORDS, "reduce": P.REDUCE_WORDS, "unpack": P.UNPACK_WORDS, "recv": RECV_WORDS,
-          "relay": P.RELAY_WORDS, "gemm": (), "gemm_rs": G.RS_WORDS}
+          "relay": P.RELAY_WORDS, "gemm": (), "gemm_rs": G.RS_WORDS, "scatter": P.SCATTER_WORDS}
 
 
 def _pow2(n: int) -> int:
@@ -104,6 +104,7 @@ class RingResult:
     total_ns: int = 0
     received: int = 0           # arrivals the consumer saw
     posted: int = 0             # records this rank posted to the next one
+    posted_to: List[int] = field(default_factory=list)    # an all-to-all's: records posted to each rank
 
     @property
     def ok(self) -> bool:
@@ -216,6 +217,12 @@ class _RingPlan:
         with torch.cuda.stream(cs):
             self.words.zero_()
         self._cleared.record(cs)
+        self._receive(views, kw)
+        self._stale_cqes = self._rq_backlog = 0
+        self._views = views
+
+    def _receive(self, views, kw):
+        """Enqueue the receives of this run's ``n_recv`` records, the backlog's WQEs included."""
         fresh = self.n_recv - self._rq_backlog
         views.append(("receive", "recv", ops.recv_consume(self.recv_qp, fresh, self.n_ids, self.words, scratch_off=self._res(0),
                                                   prepost_mr=self.landing_mr, prepost_bytes=0, **kw)[0]))
@@ -223,8 +230,13 @@ class _RingPlan:
             # the receive WQEs a failed run left posted take the rest of this run's records
             views.append(("receive", "recv", ops.recv_consume(self.recv_qp, self._rq_backlog, self.n_ids, self.words,
                                                       scratch_off=self._res(self._DRAIN + 1), **kw)[0]))
-        self._stale_cqes = self._rq_backlog = 0
-        self._views = views
+
+    def _reap(self, res: List[RingResult]):
+        """After a run of every rank in one process: record what the run left in this rank's receive queue for the next
+        run to reap -- completions nobody reaped, and receive WQEs no record took."""
+        arrivals = res[(self.rank - 1) % self.world].posted
+        self._stale_cqes = max(0, arrivals - res[self.rank].received)
+        self._rq_backlog = max(0, self.n_recv - arrivals)
 
     def _streams(self):
         return (self.consumer_stream, self.main_stream)
@@ -439,10 +451,6 @@ def _run_ranks(plans: List[_RingPlan], enqueues, sync: bool, skip):
     for p in plans:
         p.synchronize()
     res = [p.result() for p in plans]
-    # what a failed run leaves in each receive queue: completions nobody reaped, and receive WQEs no record took
-    N = len(plans)
-    for q, p in enumerate(plans):
-        arrivals = res[(q - 1) % N].posted
-        p._stale_cqes = max(0, arrivals - res[q].received)
-        p._rq_backlog = max(0, p.n_recv - arrivals)
+    for p in plans:
+        p._reap(res)
     return res

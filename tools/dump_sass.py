@@ -5,8 +5,8 @@ lib = os.path.join(root, "rocnrdma_b200", "lib", "librocnrdma_b200.so")
 out = os.path.join(root, "profiles", "sass")
 os.makedirs(out, exist_ok=True)
 txt = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
-want = ["engine_kernel", "gemm_mxfp8_pair_kernel", "gemm_mxfp8_ordered_kernel", "gemm_mxfp8_kernel", "gemm_send2_kernel", "gemm_send_kernel", "gemm_reduce_send_kernel", "pack_fp8_write_kernel", "unpack_fp8_kernelILb0", "unpack_fp8_kernelILb1", "reduce_fp8_kernel", "relay_records_kernel",
-        "rdma_stream_kernel", "shared_post_stress_kernel", "recv_consume_kernel"]
+want = ["engine_kernel", "gemm_mxfp8_pair_kernel", "gemm_mxfp8_ordered_kernel", "gemm_mxfp8_kernel", "gemm_send2_kernel", "gemm_send_kernel", "gemm_reduce_send_kernel", "pack_fp8_write_kernel", "pack_fp8_scatter_kernel", "unpack_fp8_kernelILb0", "unpack_fp8_kernelILb1", "reduce_fp8_kernel", "relay_records_kernel",
+        "rdma_stream_kernel", "shared_post_stress_kernel", "recv_consume_kernel", "recv_consume_qps_kernel"]
 summary = {}
 for m in re.finditer(r"\t\tFunction : (\S+)\n(.*?)(?=\n\t\tFunction : |\Z)", txt, re.S):
     mangled, body = m.group(1), m.group(2)
