@@ -452,24 +452,34 @@ a = [torch.randint(-2, 3, (M, K), generator=g).to(torch.bfloat16) for _ in range
 b = [torch.randint(-2, 3, (Nb, K), generator=g).to(torch.bfloat16) for _ in range(N)]
 outs = [torch.zeros(M // N, Nb, dtype=torch.bfloat16, device="cuda") for _ in range(N)]
 ad, bd = [t.cuda() for t in a], [t.cuda() for t in b]
+xs = [torch.randint(-64, 65, (M * Nb,), generator=g).to(torch.bfloat16) for _ in range(N)]
+xd = [t.cuda() for t in xs]
 torch.cuda.synchronize()
 ctx.engine_start(ctas=16, idle_timeout_ms=5000)
 try:
-    res = RS.run_gemm_in_process(plans, ad, bd, outs)
+    if {kind!r} == "run":
+        res = RS.run_in_process(plans, xd, [o.reshape(-1) for o in outs])
+    else:
+        res = RS.run_gemm_in_process(plans, ad, bd, outs)
 finally:
     ctx.engine_stop()
-want = ops.ref_reduce_scatter_fp8([(x.float() @ y.float().T).reshape(-1) for x, y in zip(a, b)], 128 * Nb)
+if {kind!r} == "run":
+    want = ops.ref_reduce_scatter_fp8(xs, 128 * Nb)
+else:
+    want = ops.ref_reduce_scatter_fp8([(x.float() @ y.float().T).reshape(-1) for x, y in zip(a, b)], 128 * Nb)
 print("statuses", *[r.status for r in res])
 print("exact", all(torch.equal(o.cpu().reshape(-1).view(torch.int16), w.view(torch.int16)) for o, w in zip(outs, want)))
 ctx.close()
 """
 
 
-@pytest.mark.parametrize("N,R", [(2, 3), (3, 1)])
-def test_first_run_of_a_fresh_process(N, R):
-    """The first run_gemm of a new process: every kernel a run uses is loaded before the engine starts."""
+@pytest.mark.parametrize("N,R,kind", [(2, 3, "run_gemm"), (3, 1, "run_gemm"), (2, 3, "run"), (3, 1, "run")],
+                         ids=["2-3", "3-1", "run-2-3", "run-3-1"])
+def test_first_run_of_a_fresh_process(N, R, kind):
+    """The first run_gemm, or the first run, of a new process: every kernel a run uses is loaded before the engine
+    starts."""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    p = subprocess.run([sys.executable, "-c", _FIRST_RUN.format(root=root, N=N, R=R)], capture_output=True, text=True,
-                       timeout=300, cwd=root)
+    p = subprocess.run([sys.executable, "-c", _FIRST_RUN.format(root=root, N=N, R=R, kind=kind)], capture_output=True,
+                       text=True, timeout=300, cwd=root)
     assert p.returncode == 0, p.stderr[-3000:]
     assert f"statuses {' '.join(['OK'] * N)}" in p.stdout and "exact True" in p.stdout, p.stdout

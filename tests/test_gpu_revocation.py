@@ -21,6 +21,7 @@ def _require_dmabuf():
 
 
 def _victim():
+    torch.cuda.empty_cache()    # no free cached segment can be split to serve it, whatever earlier tests left behind
     x = torch.empty(BIG, dtype=torch.uint8, device="cuda:0")
     x.fill_(7)
     torch.cuda.synchronize()
